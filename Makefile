@@ -4,7 +4,7 @@
 #   make oracle     -> oracle only
 NVCC      ?= nvcc
 CXX       := g++
-ARCH      := -gencode arch=compute_100a,code=sm_100a
+ARCH      := -gencode arch=compute_90a,code=sm_90a
 NVFLAGS   := -std=c++17 -O3 -lineinfo $(ARCH) -Xcompiler -fPIC,-fopenmp -Xptxas -v
 CSRC      := rpt_b200/csrc
 OBJDIR    := build/obj
@@ -48,7 +48,7 @@ $(LIB): $(OBJDIR)/kernels_f32.o $(OBJDIR)/kernels_vx.o $(OBJDIR)/kernels_f64.o $
 	@mkdir -p rpt_b200/lib
 	$(NVCC) -shared $(ARCH) -o $@ $^ -Xcompiler -fopenmp -lgomp -cudart shared
 
-# -march=x86-64-v3: AVX2 hosts (this container and the GPU boxes); no FMA contraction so
+# -march=x86-64-v3: AVX2 hosts; no FMA contraction so
 # the f64 arithmetic rounds like the reference's
 $(ORACLE): oracle/oracle.cpp include/rpt_b200.h
 	@mkdir -p oracle/_build
@@ -66,7 +66,7 @@ HOSTEMU := tests/hostemu/_build/libhostemu.so
 hostemu: $(HOSTEMU)
 $(HOSTEMU): tests/hostemu/hostemu.cu $(CSRC)/kdbuild.cpp $(CSRC)/bvhbuild.cpp $(HDRS)
 	@mkdir -p $(dir $@)
-	nvcc -std=c++17 -O2 -DRPTB_HOST_EMU -DRPTB_BUILD_BVH8=1 -DRPTB_BUILD_BVH4=1 -gencode arch=compute_100a,code=sm_100a -Xcompiler -fPIC,-fopenmp,-ffp-contract=off -shared -Xlinker -Bsymbolic -o $@ tests/hostemu/hostemu.cu $(CSRC)/kdbuild.cpp $(CSRC)/bvhbuild.cpp -lgomp
+	nvcc -std=c++17 -O2 -DRPTB_HOST_EMU -DRPTB_BUILD_BVH8=1 -DRPTB_BUILD_BVH4=1 -gencode arch=compute_90a,code=sm_90a -Xcompiler -fPIC,-fopenmp,-ffp-contract=off -shared -Xlinker -Bsymbolic -o $@ tests/hostemu/hostemu.cu $(CSRC)/kdbuild.cpp $(CSRC)/bvhbuild.cpp -lgomp
 
 clean:
 	rm -rf build $(LIB) $(ORACLE) tests/hostemu/_build

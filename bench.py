@@ -4,8 +4,9 @@ Msamples/s = path segments, i.e. trace_ray invocations, per second).
 
     python bench.py --gpus N --steps K --warmup W            # this repo's CUDA path
     python bench.py --impl reference --gpus N --steps K ...  # the reference's CPU path
-                                                             # (rpt-restated C++ oracle: the
-                                                             # reference is Rust, no rustc here)
+                                                             # (rpt-restated C++ oracle)
+    python bench.py ... --dump-outputs DIR                   # also write the last timed step's
+                                                             # image(s) as DIR/<name>.npy (float32)
 
 A "step" is one pass of Renderer::sample over one batch: the BASELINE configs[1] workload,
 Cornell box 800x800, 512 spp per GPU, max_bounces 6.  At N GPUs the image gets 512*N spp and every
@@ -56,6 +57,9 @@ def parse_args():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-secondary", action="store_true", help="skip the dragon / glass strong-scaling block")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the image of the last timed step (and of each secondary render) as "
+                         "DIR/<name>.npy, float32, height x width x 3 -- for comparing two builds output for output")
     return ap.parse_args()
 
 
@@ -163,27 +167,16 @@ def measured_peaks():
     if os.path.exists(path):
         try:
             d = json.load(open(path))
-            return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)", float(d.get("sm_max_mhz", 1965.0))
+            return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)", 1965.0
-
-
-def ncu_record(workload_name: str):
-    """Per-launch figures of the dominant kernel from the committed `ncu --set full` capture of this round
-    (profiles/ncu_kernels.json, written by tools/ncu_kernels_json.py): dram bytes, warp and thread instructions and
-    the segments the captured launch traced -- the per-segment ratios are properties of the kernel."""
-    try:
-        rec = json.load(open(os.path.join(ROOT, "profiles", "ncu_kernels.json"))).get(workload_name)
-        return rec if isinstance(rec, dict) else None
-    except Exception:
-        return None
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3)"
 
 
 # ------------------------------------------------------------------ CPU arm -----------
 def host_cores():
-    """Threads this process may really use: the scheduler affinity, capped by the cgroup CPU quota (a GPU box
-    reports 128 CPUs and grants 16 of them)."""
+    """Threads this process may really use: the scheduler affinity, capped by the cgroup CPU quota (a container
+    may see 128 CPUs and be granted 16 of them)."""
     try:
         aff = len(os.sched_getaffinity(0))
     except AttributeError:
@@ -288,7 +281,7 @@ def run_native(args):
     stream = torch.cuda.Stream(dev)
     raw = stream.cuda_stream
     K, W = args.steps, args.warmup
-    peak, peak_src, sm_max_mhz = measured_peaks()
+    peak, peak_src = measured_peaks()
 
     def barrier():
         if world > 1:
@@ -384,6 +377,9 @@ def run_native(args):
         step_ms = sum(step_max)
         kern_ms = sum(kern_max)
         image_mean = float(job.image.mean().item())
+        # what the timed path hands its caller: the assembled image of the last timed step (every workload is at most
+        # 1920x1080, so the headline image and the two secondary ones stay under 64 MB of float32 together)
+        dumps = {"image": job.image.cpu().numpy().reshape(cfg.height, cfg.width, 3)} if args.dump_outputs else {}
 
         # ---- e2e: the public call with HOST buffers, copies inside the timed region -----
         e2e = None
@@ -441,9 +437,8 @@ def run_native(args):
                 sj.render(spp=probe_spp)             # warm-up of the plain kernel
                 sj.assemble()
                 # ... and one un-timed render at the full size: the first full-size launch of a process is slower than the
-                # ones after it (measured, tools/gpu_fullspp_repeat.py, two processes alike: dragon 1 688 / 1 709 then 1 821 /
-                # 1 851, glass 20 787 / 20 562 then 21 233 / 21 209 Msamples/s; it is also the first launch that needs the
-                # full set of chunk sums in scratch)
+                # ones after it (tools/gpu_fullspp_repeat.py; it is also the first launch that needs the full set of chunk
+                # sums in scratch)
                 sj.render()
                 sj.assemble()
                 stream.synchronize()
@@ -478,9 +473,10 @@ def run_native(args):
                                  "algorithmic_bytes_per_launch": bytes_all / world, "bytes_model": BYTES_MODEL,
                                  "per_ray": {"bvh_nodes": ctr["bvh_node_visits"] / max(ctr["rays"], 1), "bvh_tris": ctr["bvh_tri_tests"] / max(ctr["rays"], 1),
                                              "objects": ctr["object_tests"] / max(ctr["rays"], 1)},
-                                 "traffic": (lambda rec: None if not rec else rec["dram_bytes"] * segs / world / max(rec["segments"], 1))(ncu_record(scfg.name)),
                                  "note": "counters from a %d-spp pass of the counting variant of the same kernel, scaled by segments" % probe_spp},
                 }
+                if args.dump_outputs:
+                    dumps["secondary_" + scfg.name] = sj.image.cpu().numpy().reshape(scfg.height, scfg.width, 3)
                 sj.close()
 
     if rank == 0:
@@ -488,35 +484,12 @@ def run_native(args):
         bytes_all = algorithmic_bytes(total, npix)  # summed over ranks (each writes its own pixels)
         kern_s = kern_ms / 1e3 / K
         achieved_hbm = bytes_all / world / kern_s / 1e9  # per GPU
-        rec = ncu_record(cfg.name)
-        sm_mhz = (clocks or {}).get("sm_mhz") or sm_max_mhz
-        segs_per_gpu = total["segments"] / world
-        hbm_view = {"achieved_algorithmic_gbs": achieved_hbm, "peak": peak, "unit": "GB/s", "frac_algorithmic": achieved_hbm / peak,
+        roofline = {"bound": "hbm", "achieved": achieved_hbm, "peak": peak, "unit": "GB/s", "frac": achieved_hbm / peak,
                     "peak_source": peak_src, "algorithmic_bytes_per_launch": bytes_all / world, "bytes_model": BYTES_MODEL,
                     "counters_per_step": total}
-        if rec:
-            traffic = rec["dram_bytes"] * segs_per_gpu / max(rec["segments"], 1)
-            hbm_view["dram_frac"] = traffic / kern_s / 1e9 / peak
-        else:
-            traffic = None
-        cache_resident = flat.host_bytes() < (32 << 20)
-        if cache_resident and rec:
-            # a scene that lives in L1/L2 is bound by instruction issue, not by HBM: thread-instructions per second against
-            # 148 SMs x 128 FP32 lanes x the SM clock sampled during the run (the per-segment instruction count is the
-            # kernel's, from this round's ncu capture)
-            tinst = rec["thread_inst"] * segs_per_gpu / max(rec["segments"], 1)
-            ach = tinst / kern_s / 1e9
-            pk = 148 * 128 * sm_mhz * 1e6 / 1e9
-            roofline = {"bound": "issue", "achieved": ach, "peak": pk, "unit": "Gthread-inst/s", "frac": ach / pk, "traffic": traffic,
-                        "peak_source": "148 SMs x 128 lanes x %.0f MHz (median SM clock during the timed region)" % sm_mhz,
-                        "thread_inst_per_segment": rec["thread_inst"] / max(rec["segments"], 1),
-                        "lanes_per_warp_inst": rec["thread_inst"] / max(rec["inst"], 1),
-                        "note": "the whole scene is cache resident (%d B): the HBM view below counts bytes L1/L2 serve" % flat.host_bytes(),
-                        "hbm": hbm_view}
-        else:
-            roofline = {"bound": "hbm", "achieved": achieved_hbm, "peak": peak, "unit": "GB/s", "frac": achieved_hbm / peak, "traffic": traffic,
-                        "peak_source": peak_src, "algorithmic_bytes_per_launch": bytes_all / world, "bytes_model": BYTES_MODEL,
-                        "counters_per_step": total}
+        if flat.host_bytes() < (32 << 20):
+            roofline["note"] = ("the whole scene is cache resident (%d B): the bytes counted here are served by L1/L2, "
+                                "so this is not an HBM bound" % flat.host_bytes())
         roofline["kernel"] = ("rptb::render_kernel<float,16,false,FEAT> (megakernel: one launch per step, + chunk resolve)" if engine_used != 2 else
                               "rptb::wf_trace_kernel (+ wf_shade_kernel; wavefront engine: the duration is the whole step's kernels)")
         line = {
@@ -539,6 +512,10 @@ def run_native(args):
         }
         if secondary:
             line["secondary"] = secondary
+        if args.dump_outputs:
+            os.makedirs(args.dump_outputs, exist_ok=True)
+            for name, arr in dumps.items():
+                np.save(os.path.join(args.dump_outputs, name + ".npy"), np.ascontiguousarray(arr, dtype=np.float32))
         if world == 1 and not args.no_cpu_baseline:
             res = cpu_arm(cfg, 8, 1, budget_s=12.0)
             line["cpu_baseline"] = {k: res[k] for k in ("value", "unit", "cores", "cores_affinity", "cgroup_cpu_quota", "kind", "sample")}
@@ -556,7 +533,7 @@ def main():
     # to stdout when NCCL_DEBUG is set), so fd 1 is pointed at stderr for the whole run and the JSON
     # line goes to the saved descriptor.
     if args.impl == "native" and args.gpus > 1 and "WORLD_SIZE" not in os.environ:
-        # convenience: re-launch under torchrun exactly like the driver does
+        # convenience: re-launch itself under torchrun, one process per GPU
         cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node", str(args.gpus),
                "--master-addr", "127.0.0.1", "--master-port", str(free_port()), os.path.abspath(__file__)] + sys.argv[1:]
         return subprocess.call(cmd)

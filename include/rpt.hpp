@@ -1,6 +1,6 @@
 // rpt.hpp -- header-only C++ host mirror of rpt's public builder API over the C ABI of
-// rpt_b200.h, for compiled hosts (the reference is a compiled Rust crate; no rustc exists
-// in this build image, see INTEGRATION.md).  Same names and argument meaning as:
+// rpt_b200.h, for compiled hosts (the reference is a compiled Rust crate; its Rust side
+// here is never compiled, see INTEGRATION.md).  Same names and argument meaning as:
 //
 //   Scene / SceneAdd            src/scene.rs:7-41        Object            src/object.rs:10-32
 //   Material::{diffuse,...}     src/material.rs:28-106   Light             src/light.rs:7-19

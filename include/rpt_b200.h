@@ -1,5 +1,5 @@
 /*
- * rpt_b200.h -- C ABI of the B200-native path-tracing core that stands where
+ * rpt_b200.h -- C ABI of the H100-native path-tracing core that stands where
  * rpt's private `Renderer::sample` stands today.
  *
  * Every entry point cites the reference interface it replaces.  Citations are
@@ -45,7 +45,7 @@ typedef enum rptb_status {
     RPTB_OK = 0,
     RPTB_ERR_BAD_ARG = -1,   /* null pointer, out-of-range index, bad enum   */
     RPTB_ERR_CUDA = -2,      /* a CUDA runtime call failed (message has it)  */
-    RPTB_ERR_NO_DEVICE = -3, /* no usable sm_100 device / extension missing  */
+    RPTB_ERR_NO_DEVICE = -3, /* no usable sm_90 device / extension missing   */
     RPTB_ERR_OOM = -4,       /* host or device allocation failed             */
     RPTB_ERR_UNSUPPORTED = -5
 } rptb_status;

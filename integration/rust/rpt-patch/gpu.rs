@@ -1,5 +1,5 @@
-//! `rpt::gpu` -- puts librpt_b200.so behind `Renderer::sample`.  UNVERIFIED SOURCE (no rustc in the image
-//! it was written in); see ../README.md and the repository's INTEGRATION.md.
+//! `rpt::gpu` -- puts librpt_b200.so behind `Renderer::sample`.  UNVERIFIED SOURCE (never
+//! compiled); see ../README.md and the repository's INTEGRATION.md.
 //!
 //! The crate's shapes are type-erased (`Object.shape: Box<dyn Shape>`, src/object.rs:12), so the flattening
 //! needs one addition to the `Shape` trait: `describe`, implemented by every shape of the crate

@@ -1,8 +1,8 @@
-"""rpt_b200 -- B200-native path-tracing core behind rpt's Renderer/Scene/Camera/Material API.
+"""rpt_b200 -- H100-native path-tracing core behind rpt's Renderer/Scene/Camera/Material API.
 
 Host mirror of the reference API: rpt_b200.api (re-exported here).  The hot path --
 everything under Renderer::sample (ekzhang/rpt src/renderer.rs:117-220) -- runs in
-rpt_b200/lib/librpt_b200.so (CUDA, sm_100a) behind the C ABI of include/rpt_b200.h.
+rpt_b200/lib/librpt_b200.so (CUDA, sm_90a) behind the C ABI of include/rpt_b200.h.
 """
 from .api import (Buffer, Camera, Cube, DeviceScene, Environment, Filter, FlatScene, Hdri, KdTree, Light, Material, Mesh,
                   MonomialSurface, monomial_surface,

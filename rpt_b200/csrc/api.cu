@@ -43,8 +43,8 @@ int parse_stl_bytes(const void* data, size_t len, std::vector<double>& tris, std
 
 using namespace rptb;
 
-// What RPTB_ACCEL_AUTO means when the environment does not say.  Measured on one B200 (tools/gpu_accel.py,
-// profiles/raw/accel_table.json): teapot 5.8 -> 16.5 Gsamples/s, dragon proxy 0.145 -> 0.89 Gsamples/s, same images.
+// What RPTB_ACCEL_AUTO means when the environment does not say (tools/gpu_accel.py compares the two): the BVH
+// renders the same images several times faster on the teapot and the dragon proxy.
 #ifndef RPTB_ACCEL_DEFAULT
 #define RPTB_ACCEL_DEFAULT RPTB_ACCEL_BVH
 #endif
@@ -331,10 +331,9 @@ bool use_wavefront(const rptb_scene* s, const rptb_render_params* p) {
     if (s->features & F_EXT) return false;  // kd-trees over shapes / MonomialSurface: megakernel only
     if (p->engine == RPTB_ENGINE_WAVEFRONT) return true;
     if (p->engine == RPTB_ENGINE_MEGAKERNEL) return false;
-    // measured on one B200 with the reference-shaped kd-trees: the megakernel wins while traversal is cheap
-    // (teapot: 2 487 nodes, 5.8 vs 2.3 Gsamples/s), the wavefront wins once it dominates (dragon proxy: 823 k
-    // nodes, 45 vs 145 Msamples/s).  Through the BVH a ray costs ~25 node visits and ~3 triangle tests on
-    // either mesh and the megakernel wins on both (dragon proxy 892 vs 670 Msamples/s, teapot 16.5 vs 3.2 G).
+    // measured with the reference-shaped kd-trees: the megakernel wins while traversal is cheap (teapot:
+    // 2 487 nodes), the wavefront wins once it dominates (dragon proxy: 823 k nodes).  Through the BVH a ray
+    // costs ~25 node visits and ~3 triangle tests on either mesh and the megakernel wins on both.
     if (s->features & F_BVH) return false;
     return s->has_tree && s->tree_nodes >= 50000 && s->sampled_lights <= 8;
 }
@@ -404,8 +403,8 @@ int render_launch(rptb_scene* s, const rptb_camera* cam, const rptb_render_param
             if (rc != RPTB_OK) return rc;
             a.ks = s->sampled_lights;
             // RPTB_VX=1 selects the vertex-at-once schedule (integrator_vx.cuh) where it has ray slots for the scene's lights.
-            // Measured on one B200 (profiles/r02_vx_vs_slot.md): it loses to the slot schedule on every BASELINE config but
-            // glass (+8 %), so the slot schedule stays the default.  A counting pass over the reference-shaped kd-trees
+            // Measured before the port to the H100: it lost to the slot schedule on every BASELINE config but glass, so the
+            // slot schedule stays the default.  A counting pass over the reference-shaped kd-trees
             // (collect_stats = 2) is always the slot engine's.
             static const bool vx_on = getenv("RPTB_VX") != nullptr && std::strcmp(getenv("RPTB_VX"), "1") == 0;
             if (vx_on && vx_supported(a.ks) && p->collect_stats != 2) CU(launch_render_vx_f32(s->view32, a, (int)p->collect_stats, s->features, stream, launches));

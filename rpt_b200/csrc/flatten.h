@@ -616,8 +616,8 @@ inline int flatten_scene(const rptb_scene_desc* d, HostScene& hs, std::string& e
     if (has_mono) hs.features |= F_MONO;
     // small scenes: the uniform tables also ride in the kernel parameters (scene_dev.cuh, SmallTables)
     // ... but only when what a ray actually walks (objects + lights + one-leaf triangles) stays within
-    // ~1 KB: the constant cache in front of parameter space is tiny.  Measured: sphere scene (0.6 KB)
-    // 9.2 -> 10.6 Gsamples/s; Cornell (2.1 KB walked per ray) 5.08 -> 4.40 -- so Cornell stays on L1.
+    // ~1 KB: the constant cache in front of parameter space is tiny.  Measured: the sphere scene (0.6 KB)
+    // got faster, Cornell (2.1 KB walked per ray) slower -- so Cornell stays on L1.
     const size_t walked = d->nobjects * sizeof(ObjectRec<float>) + d->nlights * sizeof(LightRec<float>) + hs.small_tris.size() * sizeof(float4);
     hs.small_ok = d->nobjects <= (uint32_t)SMALL_OBJECTS && d->nlights <= (uint32_t)SMALL_LIGHTS && d->nmeshes <= (uint32_t)SMALL_MESHES &&
                   hs.small_tris.size() <= (size_t)3 * SMALL_TRIS && walked <= 1024 && !(hs.features & F_EXT);

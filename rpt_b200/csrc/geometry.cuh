@@ -921,8 +921,8 @@ RPTB_D bool group_intersect(const SceneView<R>& sv, const GroupRec<R>& g, Vec3<R
                 if constexpr (!M<R>::literal) {
                     // f32 only (the f64 gate calls every child, like the reference): a ray that misses the
                     // child's bounding box cannot hit the child, so skip the change of space, the three
-                    // reciprocals and the slab test of the instance's own root (profiles/
-                    // r01_render_kernel_fractal_teapots.md: ~40 children tested per ray, most of them missed)
+                    // reciprocals and the slab test of the instance's own root (fractal_teapots: ~40 children
+                    // tested per ray, most of them missed)
                     const float4 bl = ldg(g.child_box + 2 * c), bh = ldg(g.child_box + 2 * c + 1);
                     const R x1 = ((R)bl.x - o.x) * inv.x, x2 = ((R)bh.x - o.x) * inv.x;
                     const R y1 = ((R)bl.y - o.y) * inv.y, y2 = ((R)bh.y - o.y) * inv.y;

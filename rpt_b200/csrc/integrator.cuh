@@ -8,7 +8,7 @@
 //   Renderer::sample_lights src/renderer.rs:177-204
 //   Renderer::get_closest_hit src/renderer.rs:211-220
 //
-// B200 design: one thread owns one pixel for all `iterations` samples and sums them
+// Design: one thread owns one pixel for all `iterations` samples and sums them
 // in sample order, so the image is bit-reproducible and independent of how pixel
 // tiles are sharded over GPUs (no atomics on the film).  A warp covers an 8x4 pixel
 // block, a CTA a 16x8 tile; tiles are dealt round-robin to shards.  The recursion
@@ -27,9 +27,9 @@
 namespace rptb {
 
 constexpr int RENDER_THREADS = 128;  // 4 warps: a 16x8 pixel tile
-// Resident CTAs/SM each instantiation is compiled for (register cap = 65536 / (128 * blocks)).
-// Measured, Msamples/s: full-feature kernel (glass) 5 -> 20.1 G, 6 -> 19.1 G;
-// feature-free kernel (Cornell) 4 -> 4060, 5 -> 4586, 6 -> 4784, 7 -> 4838, 8 -> 4927.
+// Resident CTAs/SM each instantiation is compiled for (register cap = 65536 / (128 * blocks); the
+// H100 has the same 64 K registers per SM as the GPU these were tuned on, not yet re-tuned on it).
+// Measured: the full-feature kernel (glass) is fastest at 5, the feature-free kernel (Cornell) at 8.
 #ifndef RPTB_MIN_BLOCKS
 #define RPTB_MIN_BLOCKS 5
 #endif
@@ -37,14 +37,14 @@ constexpr int RENDER_THREADS = 128;  // 4 warps: a 16x8 pixel tile
 #define RPTB_MIN_BLOCKS_LITE 8
 #endif
 #ifndef RPTB_MIN_BLOCKS_TREE
-#define RPTB_MIN_BLOCKS_TREE 8   // F_TREE only (teapot: 5 -> 5230, 6 -> 5426, 8 -> 5816 Msamples/s)
+#define RPTB_MIN_BLOCKS_TREE 8   // F_TREE only (teapot: fastest of 5 / 6 / 8)
 #endif
 #ifndef RPTB_MIN_BLOCKS_GLASS
-#define RPTB_MIN_BLOCKS_GLASS 5  // F_TRANSP | F_HDRI, no trees (glass: flat, 19.2-19.4 G for 5/6/8)
+#define RPTB_MIN_BLOCKS_GLASS 5  // F_TRANSP | F_HDRI, no trees (glass: flat across 5 / 6 / 8)
 #endif
 #ifndef RPTB_MIN_BLOCKS_BVH
 #define RPTB_MIN_BLOCKS_BVH 8    // F_BVH: the node loop is latency bound at 5-6 lanes, more resident warps help more than the spills of the 64-register
-                                 // build hurt (r02j, Msamples/s for 6 / 7 / 8: teapot 16 527 / 16 870 / 16 971, dragon-proxy 1 666 / 1 750 / 1 798, knot 901 / 961 / 999)
+                                 // build hurt (8 beat 6 and 7 on teapot, dragon-proxy and knot)
 #endif
 #ifndef RPTB_MIN_BLOCKS_EXT
 #define RPTB_MIN_BLOCKS_EXT 4    // F_EVERY (two nested traversal stacks in local memory): not tuned on hardware yet
@@ -206,11 +206,11 @@ RPTB_D void render_thread(const SceneView<R>& sv, const RenderArgs<R>& a, const 
 
     while (true) {
         const bool light_slot = slot < Ks;
-        // (Measured and dropped, gpurun r02u: moving the generator of a lane that is certain to regenerate in this slot --
+        // (Measured and dropped: moving the generator of a lane that is certain to regenerate in this slot --
         // ST_FINISH, or a vertex that is dead or at max_bounces -- to its next sample HERE, so that the sample's first
         // Philox block is computed with everybody else's refill instead of on demand by the one lane in five that starts a
-        // sample: bit-identical images, cornell 5 243 -> 5 040, sphere 11 557 -> 11 098, teapot 18 656 -> 18 233, glass
-        // 20 343 -> 19 452 Msamples/s.  The extra state test at the top of every slot costs more than the refills it merges.)
+        // sample: bit-identical images, slower on every config.  The extra state test at the top of every slot costs more
+        // than the refills it merges.)
         {   // converged here: the lanes that are short of draws for this slot compute their Philox blocks together
             uint32_t need = 0;
             if (status == ST_VERTEX && !dead) {

@@ -19,7 +19,7 @@ cudaError_t launch_render_impl(const SceneView<R>& sv, const RenderArgs<R>& args
         // (MAXD sizes the f64 gate's level stack; the f32 path composes the clamps forward and has no depth limit of its own)
         if (args.max_bounces <= 16 || !M<R>::literal) {
             // pick the instantiation compiled for exactly the features this scene has (tree scenes do not
-            // take the parameter-space tables: teapot 5762 without vs 5181 Msamples/s with)
+            // take the parameter-space tables: measured slower with them)
             const int base = features & F_ALL;
             const bool small = (features & F_SMALL) != 0;
             // kd-trees over whole shapes and MonomialSurface live in one extra instantiation (F_EVERY), so

@@ -153,12 +153,10 @@ struct Rng<double> {
 //   BUF_PAIR  two draws enter a 4-entry FIFO, the other two wait in s0/s1           (6 words)
 //   BUF_FOUR  a 4-entry FIFO, refilled when empty                                    (4 words)
 //   BUF_EIGHT an 8-entry FIFO; a block enters whenever four entries are free          (8 words)
-// Measured on one B200 (gpurun r02r/r02s, Msamples/s at 64-100 spp; PAIR / FOUR / EIGHT):
-//   sphere 10 595 / 10 515 / 11 619, cornell 4 670 / 4 705 / 5 214, glass 19 620 / 20 631 / 20 359,
-//   teapot 17 253 / 18 802 / 17 201, monomial_glass 7 232 / 6 873 / 7 006.
-// (Two more were tried and dropped -- the current block in a 4-entry FIFO plus the whole next block beside it, handed
-// over at the draw that empties the FIFO or at the next draw after: cornell 5 081 and 5 233, within 2 % of EIGHT; the
-// shared-memory ring below with four-word blocks: cornell 4 481.  profiles/r02_rng_buffering.md has the table.)
+// No one of them was fastest on every scene when they were compared (before the port to the H100; not re-measured
+// there).  (Two more were tried and dropped -- the current block in a 4-entry FIFO plus the whole next block beside it,
+// handed over at the draw that empties the FIFO or at the next draw after, and the shared-memory ring below: neither
+// beat EIGHT.)
 // EIGHT keeps ensure() -- the converged point -- the place where nearly every block is computed (a lane holds >= 4
 // draws after it, and few slots draw more); FOUR is the smallest in registers, which is what the 64-register kernels of
 // the mesh scenes (F_BVH, 8 CTAs per SM) want.  The megakernel picks per instantiation (integrator.cuh, MegaRng).
@@ -302,7 +300,7 @@ struct RngF32 : RngBuf<BUF> {
         this->clear();
     }
     template <class W>
-    RPTB_HD void ensure(unsigned, uint32_t) { RngBuf<BUF>::ensure(); }  // (topping up to the slot's expected draws instead was measured too: Cornell 4 841 vs 5 673)
+    RPTB_HD void ensure(unsigned, uint32_t) { RngBuf<BUF>::ensure(); }  // (topping up to the slot's expected draws instead was measured too, and was slower)
     RPTB_HD void ensure() { RngBuf<BUF>::ensure(); }
     RPTB_HD void bind(uint32_t*, uint32_t) {}
     RPTB_HD float gen() { return (float)(this->next32() >> 8) * (1.0f / 16777216.0f); }
@@ -328,21 +326,19 @@ struct Rng<float> : RngF32<RPTB_FIFO_MODE> {};
 // as Rng<float> (high word of every 64-bit draw), buffered in an
 // 8-entry ring per thread that lives in SHARED memory on the device (entry i of thread t at ring[i * stride + t]:
 // one bank per lane, no conflicts; a ring in registers would need shuffling moves per draw and four more live
-// registers in a kernel that already spills).  What this buys (ncu, Cornell, round 2): with the 4-entry register FIFO
-// a slot that drew more than the FIFO held refilled it inside whatever rejection loop it was in -- the ~60-instruction
-// Philox block ran at 7.4 of 32 lanes and was 27 % of the kernel's warp instructions.  ensure() tops a lane up to
+// registers in a kernel that already spills).  What this buys: with the 4-entry register FIFO a slot that drew more
+// than the FIFO held refilled it inside whatever rejection loop it was in -- the ~60-instruction Philox block ran on a
+// few lanes of the warp at a time.  ensure() tops a lane up to
 // what it is about to draw where the warp is converged, and all lanes that need a block compute it together.
 constexpr uint32_t RNG_RING = 8;
 #ifndef RPTB_RNG_FILL
 #define RPTB_RNG_FILL 0
 #endif
 #ifndef RPTB_RNG_FIFO
-// 1 = the slot engine keeps a register FIFO (RngF32), 0 = it draws from the ring below.  Measured on one B200 with
-// everything else equal, Msamples/s, FIFO / ring topped up / ring topped up on demand -- while a block still was two
-// draws (gpurun r02h): cornell 5 676 / 5 252 / 4 919, glass 20 553 / 14 676 / 15 590, sphere 9 284 / 9 638 / 8 908; with
-// four-word blocks (r02r): cornell 5 214 / 4 347 / 4 481, glass 20 359 / 17 374 / 19 432 -- the ring does raise the
-// lanes per Philox instruction (7.4 -> 11.2, ncu) but its shared-memory traffic and vote loops cost more than that saves,
-// so the FIFO is the default and the ring is what the vertex-at-once engine (integrator_vx.cuh) uses.
+// 1 = the slot engine keeps a register FIFO (RngF32), 0 = it draws from the ring below.  The ring raises the lanes per
+// Philox instruction, but its shared-memory traffic and vote loops cost more than that saves (measured with everything
+// else equal, before the port to the H100), so the FIFO is the default and the ring is what the vertex-at-once engine
+// (integrator_vx.cuh) uses.
 #define RPTB_RNG_FIFO 1
 #endif
 struct RngRing {

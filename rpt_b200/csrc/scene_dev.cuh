@@ -41,14 +41,13 @@ enum : int {
     F_BVH = 64 /* f32 only: meshes are traversed through their BVH (MeshRec::bvh_*) instead of the reference-shaped kd-tree */
 };
 
-// Two experiments of round 2 on the mesh configs, both measured slower than what they were meant to improve and
-// therefore off (one B200, Msamples/s, teapot / dragon-proxy / dragon-knot; gpurun r02h, r02i):
-//   RPTB_BVH_PREFETCH  prefetch.global.L1 of both children's lines once their boxes are hit: 13 586 / 1 450 / 781 against
-//                      14 982 / 1 635 / 887 without -- the loop is latency bound, but the extra requests cost more than
-//                      the early lines save
+// Two experiments on the mesh configs (teapot / dragon-proxy / dragon-knot), both measured slower than what they were
+// meant to improve and therefore off (measured before the port to the H100; not re-measured there):
+//   RPTB_BVH_PREFETCH  prefetch.global.L1 of both children's lines once their boxes are hit -- the loop is latency bound,
+//                      but the extra requests cost more than the early lines save
 //   RPTB_COOP_MAX      the warp's rays that enter a mesh are traversed by groups of eight lanes over the eight-wide tree
-//                      when there are at most this many of them (closest_hit_coop): always 3 370 / 744 / 331; at most 4:
-//                      14 271 / 1 269 / 720; at most 8: 13 902 / 1 231 / 711.  0 = never, and the code is compiled out
+//                      when there are at most this many of them (closest_hit_coop): slower at every limit tried.
+//                      0 = never, and the code is compiled out
 #ifndef RPTB_BVH_PREFETCH
 #define RPTB_BVH_PREFETCH 0
 #endif
@@ -122,9 +121,8 @@ struct __align__(16) Bvh4Node {
     int4 _pad;
 };
 #ifndef RPTB_BVH4
-#define RPTB_BVH4 0  // 1: meshes with a BVH are traversed through the four-wide tree.  Measured (gpurun r02p, one B200, Msamples/s, binary / four-wide
-                     // at 8, 6, 5 CTAs per SM): teapot 17 002 / 12 707 / 14 153 / 14 115, dragon 1 796 / 1 439 / 1 449 / 1 408, dragon_knot
-                     // 1 002 / 850 / 794 / 760, fractal_teapots 644 / 594 / 580 / 584 -- 0.45x the dependent fetches (tests/test_hostemu.py) but
+#define RPTB_BVH4 0  // 1: meshes with a BVH are traversed through the four-wide tree.  Measured slower than the binary tree on every mesh
+                     // config at 8, 6 and 5 CTAs per SM (before the port to the H100): 0.45x the dependent fetches (tests/test_hostemu.py) but
                      // 24 slab FMAs + a sorting network per step whether one child is hit or four: the loop is bound by issue slots at 5-6
                      // active lanes, not by the fetch latency alone, so the binary tree stays the default.
 #endif
@@ -204,7 +202,7 @@ struct EnvRec {
 };
 
 // A small scene's warp-uniform tables, carried IN the kernel parameters (constant bank, up to 32 KB per
-// launch on sm_100): every lane of a warp walks scene.objects / scene.lights in lock step and tests
+// launch on sm_90): every lane of a warp walks scene.objects / scene.lights in lock step and tests
 // the same few triangles of one-leaf meshes, so these reads are uniform -- from parameter space they
 // are constant-cache broadcasts that need no LSU slot, no L1 tag look-up and no address registers.
 // Divergent accesses (the object / material of a lane's own hit) keep using the global copies.
@@ -279,11 +277,10 @@ inline void sample_chunks(uint32_t iterations, uint32_t& nchunks, uint32_t& chun
     nchunks = (iterations + chunk - 1u) / chunk;
     if (nchunks < 1u) nchunks = 1u;
 }
-// groups so that tiles * groups is about 10 waves of resident CTAs (148 SMs x 8 CTAs).  Measured on
-// Cornell 800x800x512 (5 000 tiles, 8 CTAs/SM): 1 group 4964, 2 -> 5047, 3 -> 5075, 4 -> 5036,
-// 8 -> 4931 Msamples/s: more CTAs shorten the grid's tail, longer runs per thread shorten the warp's.
+// groups so that tiles * groups is about 10 waves of resident CTAs (H100: 132 SMs x 8 CTAs): more CTAs
+// shorten the grid's tail, longer runs per thread shorten the warp's.  The image does not depend on it.
 inline void sample_groups(uint32_t ntiles, uint32_t nchunks, uint32_t& ngroups, uint32_t& chunks_per_group) {
-    const uint32_t want = ntiles ? (12000u + ntiles - 1u) / ntiles : 1u;
+    const uint32_t want = ntiles ? (10560u + ntiles - 1u) / ntiles : 1u;
     ngroups = want < 1u ? 1u : (want > nchunks ? nchunks : want);
     chunks_per_group = (nchunks + ngroups - 1u) / ngroups;
     ngroups = (nchunks + chunks_per_group - 1u) / chunks_per_group;

@@ -5,7 +5,7 @@
 // get_closest_hit varies by two orders of magnitude between the rays of a warp (a ray
 // that misses the mesh AABB costs nothing, one that grazes the dragon visits > 1000
 // triangles).  In the megakernel a lane is tied to its pixel, so a warp's trace takes as
-// long as its slowest ray: ncu measured 7.7 of 32 lanes active on the dragon proxy.
+// long as its slowest ray: on the dragon proxy about a quarter of the lanes are active.
 // Here the rays of all paths go through a PERSISTENT TRACE KERNEL whose lanes fetch a new
 // ray the moment theirs is finished (Aila & Laine's persistent while-while with dynamic
 // fetch), while a SHADE KERNEL advances every path by one vertex per step:
@@ -32,7 +32,7 @@ namespace rptb {
 constexpr int WF_THREADS = 128;
 constexpr int WF_MAX_SHADOW = 8;
 #ifndef WF_TRACE_MIN_BLOCKS
-#define WF_TRACE_MIN_BLOCKS 8  // resident CTAs/SM the trace kernel is compiled for (64 registers; latency bound: measured best of 7/8/10)
+#define WF_TRACE_MIN_BLOCKS 8  // resident CTAs/SM the trace kernel is compiled for (64 registers; latency bound: 8 measured best of 7/8/10)
 #endif  // sampled (non-ambient) lights per scene the wavefront engine handles
 
 struct __align__(16) WfRay {
@@ -522,8 +522,8 @@ __global__ void __launch_bounds__(WF_THREADS, WF_TRACE_MIN_BLOCKS) wf_trace_kern
         }
         // ---- one round of the kd traversal: descend to a leaf, test it, pop ---------------
         // ("while-while".  A finer-grained "if-if" schedule -- a few node steps, then one 4-triangle
-        // batch per loop iteration -- was measured on the dragon proxy and lost: 101 vs 143 Msamples/s,
-        // +35 % instructions for +1.5 active lanes.)
+        // batch per loop iteration -- was measured on the dragon proxy and lost: a third more instructions
+        // for one or two more active lanes.)
         if (BVH && have && trav) {
             // ---- one round of the BVH traversal (geometry.cuh, bvh_intersect) -----------------
             bool mesh_done = false;

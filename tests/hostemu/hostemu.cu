@@ -6,7 +6,7 @@
 // with a single-lane warp policy) compiled for the HOST with RPTB_HOST_EMU, over the very arrays
 // rptb_scene_create would upload (flatten.h), so that their control flow -- kd traversal, the kd-tree of
 // shapes, MonomialSurface, Transformed, finalize_hit, shape_sample -- can be checked against the oracle
-// in the build container, which has no GPU.  It proves nothing about the kernels' scheduling, fast-math
+// on a machine without a GPU.  It proves nothing about the kernels' scheduling, fast-math
 // or memory behaviour; the `-m gpu` parity tests through the C ABI stay the gate.
 //
 // Built by `make hostemu` with nvcc (host pass) and -ffp-contract=off so Real = double rounds like the

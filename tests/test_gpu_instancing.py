@@ -193,7 +193,7 @@ def test_cpp_host_mirror_builds_the_same_kd_trees_of_shapes(gpu_ok, tmp_path):
 @pytest.mark.parametrize("name", ["fractal_spheres", "fractal_teapots", "monomial_glass"])
 def test_gpu_matches_committed_golden(gpu_ok, name):
     """The f64 gate reproduces the committed oracle fixtures of the row-N4 scenes (tests/golden,
-    tools/make_golden.py) -- this test needs no oracle on the GPU box."""
+    tools/make_golden.py) -- this test needs no oracle on the GPU machine."""
     import os
     g = np.load(os.path.join(os.path.dirname(__file__), "golden", f"{name}_render.npz"))
     cfg = util.golden_config(name)

@@ -239,7 +239,7 @@ def test_flatten_kdtree_of_shapes_shares_meshes_and_keeps_child_order():
 
 
 def test_bench_arms_share_one_config_and_count_real_cores():
-    """bench.py: the CPU arm's `config` is the GPU arm's (the driver compares them), the core count honours the cgroup
+    """bench.py: the CPU arm's `config` is the GPU arm's (so the two lines can be compared), the core count honours the cgroup
     quota, and the bytes model adds the BVH counters."""
     import importlib.util
     import os

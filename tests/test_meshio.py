@@ -153,20 +153,20 @@ def test_stl_errors():
         api.parse_stl_native(truncated)
 
 
-REF = "/root/reference/examples"
+GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
 
-@pytest.mark.skipif(not os.path.exists(REF + "/cylinder.stl"), reason="reference assets only exist in the build container")
 def test_reference_assets_parse():
-    """examples/cylinder.rs and examples/lego.rs inputs: 364 binary facets; the LEGO .obj/.mtl pair cut
+    """Inputs of the reference's examples/cylinder.rs and examples/lego.rs, stored in tests/golden/reference_assets.zip:
+    cylinder.stl as shipped (364 binary facets), LEGO.Creator_Plane.mtl as shipped and the first 7 102 lines of
+    LEGO.Creator_Plane.obj (every face there indexes earlier vertices; four material runs).  The .obj/.mtl pair is cut
     at every change of `usemtl`."""
-    data = open(REF + "/cylinder.stl", "rb").read()
-    tris = api.parse_stl_native(data)
+    z = zipfile.ZipFile(os.path.join(GOLDEN, "reference_assets.zip"))
+    tris = api.parse_stl_native(z.read("cylinder.stl"))
     assert tris.shape == (364, 18) and np.isfinite(tris).all()
     assert np.array_equal(tris[:, 9:12], tris[:, 15:18])
-    z = zipfile.ZipFile(REF + "/lego.zip")
-    obj = z.read("LEGO.Creator_Plane/LEGO.Creator_Plane.obj")
-    mtl = z.read("LEGO.Creator_Plane/LEGO.Creator_Plane.mtl")
+    obj = z.read("LEGO.Creator_Plane.obj")
+    mtl = z.read("LEGO.Creator_Plane.mtl")
     objects = api.load_obj_with_mtl(io.BytesIO(obj), io.BytesIO(mtl), build=False)
     runs, last = 0, None
     open_faces = False

@@ -1,8 +1,8 @@
 """Convert the reference's example OBJ input into a compact binary fixture.
 
-Run in the build container (the reference checkout does not exist on the GPU box):
+Run with a checkout of the reference (ekzhang/rpt) at hand:
 
-    python tools/make_assets.py
+    RPT_REFERENCE=/path/to/rpt python tools/make_assets.py
 
 teapot.obj (examples/teapot.rs:16) is parsed with rpt_b200.api.parse_obj -- the mirror
 of src/io.rs:27-73 -- and stored as an (n, 18) float64 triangle array
@@ -23,7 +23,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 from rpt_b200.api import parse_obj  # noqa: E402
 
-REF = os.environ.get("RPT_REFERENCE", "/root/reference")
+REF = os.environ.get("RPT_REFERENCE", "")
 
 
 def pegasus():

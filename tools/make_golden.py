@@ -1,7 +1,7 @@
-"""Generate tests/golden/*.npz from the CPU oracle (run in the build container).
+"""Generate tests/golden/*_render.npz and *_hits.npz from the CPU oracle (no GPU needed).
 
-The reference holds no golden vectors for this path (SURVEY 8c) and cannot be run here
-(no rustc), so these fixtures pin the ORACLE against regressions; they are not outputs
+The reference holds no golden vectors for this path (SURVEY 8c) and is not built by this
+project (it is Rust), so these fixtures pin the ORACLE against regressions; they are not outputs
 of rpt itself.  Regenerate only when the oracle is deliberately changed:
 
     python tools/make_golden.py

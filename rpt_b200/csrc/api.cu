@@ -273,7 +273,7 @@ int scene_bind_device(HostScene& hs, rptb_scene* s, bool release) {
     s->arena.stream = s->stream;
     ArenaPut put{s->arena};
     if (!bind_scene(hs, put, release, s->view32, s->view64, s->f32_bytes)) CU(put.error);
-    s->features = hs.features | (hs.flat_ok ? (int)F_FLAT : 0);
+    s->features = kernel_features(hs);
     s->has_tree = hs.has_tree;
     s->tree_nodes = hs.tree_nodes;
     s->sampled_lights = hs.sampled_lights;
@@ -294,8 +294,6 @@ int flatten_desc(const rptb_scene_desc* d, HostScene& hs) {
     std::string err;
     const int rc = flatten_scene(d, hs, err, resolve_accel(d->accel) == RPTB_ACCEL_BVH);
     if (rc != RPTB_OK) return fail(rc, "%s", err.c_str());
-    if (getenv("RPTB_NO_SMALL") != nullptr) hs.small_ok = false;
-    if (getenv("RPTB_NO_FLAT") != nullptr) hs.flat_ok = false;  // A/B: the scan over scene.objects instead of the packed table
     return RPTB_OK;
 }
 
@@ -419,7 +417,7 @@ int render_launch(rptb_scene* s, const rptb_camera* cam, const rptb_render_param
         a.counters = want_counters ? s->counters : nullptr;
         const int rc = ensure_partial(s, a);
         if (rc != RPTB_OK) return rc;
-        CU(launch_render_f64(s->view64, a, (int)p->collect_stats, F_ALL | (s->features & F_EXT), stream, launches));
+        CU(launch_render_f64(s->view64, a, (int)p->collect_stats, s->features, stream, launches));
     }
     return RPTB_OK;
 }
@@ -590,7 +588,7 @@ int rptb_scene_create_multi(const rptb_scene_desc* desc, const int* devices, int
             std::memset(&s->view64, 0, sizeof(s->view64));
             reps.push_back(s);
             rc = scene_bind_device(hs, s, i + 1 == ndevices);
-            s->features = hs.features | (hs.flat_ok ? (int)F_FLAT : 0);
+            s->features = kernel_features(hs);
             s->has_tree = hs.has_tree;
             s->tree_nodes = hs.tree_nodes;
             s->sampled_lights = hs.sampled_lights;

@@ -675,15 +675,23 @@ inline int flatten_scene(const rptb_scene_desc* d, HostScene& hs, std::string& e
     // ... but only when what a ray actually walks (objects + lights + one-leaf triangles) stays within
     // ~1 KB: the constant cache in front of parameter space is tiny.  Measured: the sphere scene (0.6 KB)
     // got faster, Cornell (2.1 KB walked per ray) slower -- so Cornell stays on L1.
-    // The packed primitive table (F_FLAT, 704 B for Cornell) lives in global memory only.  Measured on one H100 80GB HBM3
+    // The packed primitive table (F_FLAT, 608 B for Cornell) lives in global memory only.  Measured on one H100 80GB HBM3
     // at a 400 W power limit, megakernel time at the bench size (Cornell 800x800, 512 spp, max_bounces 6): 253.3 ms with
     // the object scan, 238.6 ms with the table through L1, 243.9 ms with the same table in kernel-parameter space.
     const size_t walked = d->nobjects * sizeof(ObjectRec<float>) + d->nlights * sizeof(LightRec<float>) + hs.small_tris.size() * sizeof(float4);
     hs.small_ok = d->nobjects <= (uint32_t)SMALL_OBJECTS && d->nlights <= (uint32_t)SMALL_LIGHTS && d->nmeshes <= (uint32_t)SMALL_MESHES &&
                   hs.small_tris.size() <= (size_t)3 * SMALL_TRIS && walked <= 1024 && !(hs.features & F_EXT);
     build_flat_table(hs);
+    // A/B switches, read when a scene is created: RPTB_NO_SMALL keeps the tables out of kernel-parameter space, RPTB_NO_FLAT
+    // traces a flat scene through the scan over scene.objects instead of the packed table (which is still built)
+    if (getenv("RPTB_NO_SMALL") != nullptr) hs.small_ok = false;
+    if (getenv("RPTB_NO_FLAT") != nullptr) hs.flat_ok = false;
     return RPTB_OK;
 }
+
+// The feature bits the launchers dispatch on (launch.h) once bind_scene has run: what the scene has (hs.features, F_SMALL
+// included), plus F_FLAT when it is traced through the packed primitive table.
+inline int kernel_features(const HostScene& hs) { return hs.features | (hs.flat_ok ? (int)F_FLAT : 0); }
 
 // Hands every array to `put` (which returns where the kernels will find it) and fills the SceneViews.
 // Put:  template <class T> bool operator()(std::vector<T>& host, const T** where);   uint64_t bytes() const;

@@ -6,11 +6,6 @@ namespace rptb {
 
 bool vx_supported(uint32_t sampled_lights) { return sampled_lights <= VX_MAX_SHADOW; }
 
-template <bool STATS, int FEAT>
-static void vx_launch(const SceneView<float>& sv, const RenderArgs<float>& args, dim3 grid, size_t smem, cudaStream_t stream) {
-    render_kernel_vx<STATS, FEAT><<<grid, RENDER_THREADS, smem, stream>>>(sv, args);
-}
-
 cudaError_t launch_render_vx_f32(const SceneView<float>& sv, const RenderArgs<float>& args, int stats, int features,
                                  cudaStream_t stream, uint32_t* launches) {
     uint32_t nl = 0;
@@ -22,21 +17,12 @@ cudaError_t launch_render_vx_f32(const SceneView<float>& sv, const RenderArgs<fl
     if (args.ntiles_mine > 0) {
         const dim3 grid(args.ntiles_mine, args.ngroups);
         const size_t smem = sizeof(uint32_t) * vx_shared_words(args.ks + 1u);
-        const int base = features & F_ALL;
-        const bool small = (features & F_SMALL) != 0, ext = (features & F_EXT) != 0, bvh = (features & F_BVH) != 0;
-        // the same feature-specialised variants as the slot engine (launch_impl.cuh); no MAXD: there is no level stack
-        if (stats == 1 && bvh) vx_launch<true, F_EVERY | F_BVH>(sv, args, grid, smem, stream);
-        else if (stats) vx_launch<true, F_EVERY>(sv, args, grid, smem, stream);
-        else if (ext && bvh) vx_launch<false, F_EVERY | F_BVH>(sv, args, grid, smem, stream);
-        else if (ext) vx_launch<false, F_EVERY>(sv, args, grid, smem, stream);
-        else if (bvh && base == F_TREE) vx_launch<false, F_TREE | F_BVH>(sv, args, grid, smem, stream);
-        else if (bvh) vx_launch<false, F_ALL | F_BVH>(sv, args, grid, smem, stream);
-        else if (base == 0 && small) vx_launch<false, F_SMALL>(sv, args, grid, smem, stream);
-        else if (base == 0) vx_launch<false, 0>(sv, args, grid, smem, stream);
-        else if (base == F_TREE) vx_launch<false, F_TREE>(sv, args, grid, smem, stream);
-        else if (base == (F_TRANSP | F_HDRI) && small) vx_launch<false, F_TRANSP | F_HDRI | F_SMALL>(sv, args, grid, smem, stream);
-        else if (base == (F_TRANSP | F_HDRI)) vx_launch<false, F_TRANSP | F_HDRI>(sv, args, grid, smem, stream);
-        else vx_launch<false, F_ALL>(sv, args, grid, smem, stream);
+        // the same feature-specialised variants as the slot engine (launch.h); no MAXD: there is no level stack
+        const bool found = visit(RenderVariantsVx{}, pick_render_vx(features, stats), [&](auto v) {
+            using T = decltype(v);
+            render_kernel_vx<T::stats, T::feat><<<grid, RENDER_THREADS, smem, stream>>>(sv, args);
+        });
+        if (!found) return cudaErrorInvalidValue;
         nl++;
         if (args.nchunks > 1) {
             resolve_chunks_kernel<float><<<args.ntiles_mine, RENDER_THREADS, 0, stream>>>(args);

@@ -1,5 +1,7 @@
 // launch_impl.cuh -- templated bodies of the launchers declared in launch.h.
 #pragma once
+#include <type_traits>
+
 #include "integrator.cuh"
 #include "launch.h"
 
@@ -16,43 +18,12 @@ cudaError_t launch_render_impl(const SceneView<R>& sv, const RenderArgs<R>& args
     }
     if (args.ntiles_mine > 0) {
         const dim3 grid(args.ntiles_mine, args.ngroups), block(RENDER_THREADS);
-        // (MAXD sizes the f64 gate's level stack; the f32 path composes the clamps forward and has no depth limit of its own)
-        if (args.max_bounces <= 16 || !M<R>::literal) {
-            // pick the instantiation compiled for exactly the features this scene has (tree scenes do not
-            // take the parameter-space tables: measured slower with them)
-            const int base = features & F_ALL;
-            const bool small = (features & F_SMALL) != 0;
-            const bool flat = (features & F_FLAT) != 0;  // closest_hit walks the packed primitive table
-            // kd-trees over whole shapes and MonomialSurface live in one extra instantiation (F_EVERY), so
-            // the variants tuned for the BASELINE scenes carry none of that code
-            const bool ext = (features & F_EXT) != 0;
-            // counting passes: stats == 1 counts what the product path traverses (the BVH when the scene has one),
-            // stats == 2 walks the reference-shaped kd-trees (the algorithmic work of SURVEY 8d)
-            const bool count_bvh = !M<R>::literal && stats == 1 && (features & F_BVH);
-            if (count_bvh) render_kernel<R, 16, true, F_EVERY | F_BVH><<<grid, block, 0, stream>>>(sv, args);
-            else if (stats) render_kernel<R, 16, true, F_EVERY><<<grid, block, 0, stream>>>(sv, args);
-            else if (!M<R>::literal && ext && (features & F_BVH)) render_kernel<R, 16, false, F_EVERY | F_BVH><<<grid, block, 0, stream>>>(sv, args);
-            else if (ext) render_kernel<R, 16, false, F_EVERY><<<grid, block, 0, stream>>>(sv, args);
-            else if constexpr (M<R>::literal) render_kernel<R, 16, false><<<grid, block, 0, stream>>>(sv, args);  // the f64 gate is not specialised
-            else if ((features & F_BVH) && base == F_TREE) render_kernel<R, 16, false, F_TREE | F_BVH><<<grid, block, 0, stream>>>(sv, args);
-            else if (features & F_BVH) render_kernel<R, 16, false, F_ALL | F_BVH><<<grid, block, 0, stream>>>(sv, args);
-            // (the glass variant keeps the scan: its two transformed spheres are cheaper from parameter space than the table
-            // is through L1 -- 43.7 against 44.0 ms at 256 spp on one H100 80GB HBM3 at a 400 W power limit)
-            else if (base == 0 && flat && small) render_kernel<R, 16, false, F_FLAT | F_SMALL><<<grid, block, 0, stream>>>(sv, args);
-            else if (base == 0 && flat) render_kernel<R, 16, false, F_FLAT><<<grid, block, 0, stream>>>(sv, args);
-            else if (base == 0 && small) render_kernel<R, 16, false, F_SMALL><<<grid, block, 0, stream>>>(sv, args);
-            else if (base == 0) render_kernel<R, 16, false, 0><<<grid, block, 0, stream>>>(sv, args);
-            else if (base == F_TREE) render_kernel<R, 16, false, F_TREE><<<grid, block, 0, stream>>>(sv, args);
-            else if (base == (F_TRANSP | F_HDRI) && small) render_kernel<R, 16, false, F_TRANSP | F_HDRI | F_SMALL><<<grid, block, 0, stream>>>(sv, args);
-            else if (base == (F_TRANSP | F_HDRI)) render_kernel<R, 16, false, F_TRANSP | F_HDRI><<<grid, block, 0, stream>>>(sv, args);
-            else render_kernel<R, 16, false><<<grid, block, 0, stream>>>(sv, args);
-        } else {
-            // f64 gate, deep paths (max_bounces > 16): the level stack sized for MAX_BOUNCES_SUPPORTED
-            if constexpr (M<R>::literal) {
-                if (stats) render_kernel<R, (int)MAX_BOUNCES_SUPPORTED, true, F_EVERY><<<grid, block, 0, stream>>>(sv, args);
-                else render_kernel<R, (int)MAX_BOUNCES_SUPPORTED, false, F_EVERY><<<grid, block, 0, stream>>>(sv, args);
-            }
-        }
+        using List = std::conditional_t<M<R>::literal, RenderVariantsF64, RenderVariantsF32>;
+        const bool found = visit(List{}, pick_render(features, stats, M<R>::literal, args.max_bounces), [&](auto v) {
+            using T = decltype(v);
+            render_kernel<R, T::maxd, T::stats, T::feat><<<grid, block, 0, stream>>>(sv, args);
+        });
+        if (!found) return cudaErrorInvalidValue;
         nl++;
         if (args.nchunks > 1) {
             resolve_chunks_kernel<R><<<args.ntiles_mine, RENDER_THREADS, 0, stream>>>(args);
@@ -69,25 +40,16 @@ cudaError_t launch_closest_hit_impl(const SceneView<R>& sv, const double* rays, 
                                     cudaStream_t stream) {
     if (n == 0) return cudaSuccess;
     const unsigned grid = (unsigned)((n + 127) / 128);
-    // stats == 1: counters of the structure the product path traverses; stats == 2: the reference-shaped kd-trees
-    // (with the lane-group traversal compiled in, a scene with a BVH is queried the way it is rendered)
-    if constexpr (!M<R>::literal && RPTB_COOP_MAX > 0) {
-        if (stats != 2 && (features & F_BVH)) {
-            if (stats) closest_hit_coop_kernel<true, F_EVERY | F_BVH><<<grid, 128, 0, stream>>>(sv, rays, n, tmin, out_t, out_obj, out_n, counters);
-            else closest_hit_coop_kernel<false, F_EVERY | F_BVH><<<grid, 128, 0, stream>>>(sv, rays, n, tmin, out_t, out_obj, out_n, counters);
-            return cudaGetLastError();
-        }
-    }
-    if constexpr (!M<R>::literal) {
-        if (!stats && (features & F_FLAT)) {  // the table the megakernel walks for this scene
-            closest_hit_kernel<R, false, F_FLAT><<<grid, 128, 0, stream>>>(sv, rays, n, tmin, out_t, out_obj, out_n, counters);
-            return cudaGetLastError();
-        }
-    }
-    if (!M<R>::literal && stats == 1 && (features & F_BVH)) closest_hit_kernel<R, true, F_EVERY | F_BVH><<<grid, 128, 0, stream>>>(sv, rays, n, tmin, out_t, out_obj, out_n, counters);
-    else if (stats) closest_hit_kernel<R, true, F_EVERY><<<grid, 128, 0, stream>>>(sv, rays, n, tmin, out_t, out_obj, out_n, counters);
-    else if (!M<R>::literal && (features & F_BVH)) closest_hit_kernel<R, false, F_EVERY | F_BVH><<<grid, 128, 0, stream>>>(sv, rays, n, tmin, out_t, out_obj, out_n, counters);
-    else closest_hit_kernel<R, false, F_EVERY><<<grid, 128, 0, stream>>>(sv, rays, n, tmin, out_t, out_obj, out_n, counters);
+    using List = std::conditional_t<M<R>::literal, HitVariantsF64, HitVariantsF32>;
+    const bool found = visit(List{}, pick_closest_hit(features, stats, M<R>::literal), [&](auto v) {
+        using T = decltype(v);
+        // with the lane-group traversal compiled in, a scene with a BVH is queried the way it is rendered
+        if constexpr (!M<R>::literal && RPTB_COOP_MAX > 0 && (T::feat & F_BVH) != 0)
+            closest_hit_coop_kernel<T::stats, T::feat><<<grid, 128, 0, stream>>>(sv, rays, n, tmin, out_t, out_obj, out_n, counters);
+        else
+            closest_hit_kernel<R, T::stats, T::feat><<<grid, 128, 0, stream>>>(sv, rays, n, tmin, out_t, out_obj, out_n, counters);
+    });
+    if (!found) return cudaErrorInvalidValue;
     return cudaGetLastError();
 }
 

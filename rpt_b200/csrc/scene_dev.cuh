@@ -227,7 +227,7 @@ struct SmallTables<float> {
 //   MESH        1 word:  q0, the plane the run's k triangles share bitwise (one plane test for all of them);
 //               k x 2 words: q1, q2 of each triangle (tri48 without its q0)
 // Every word is read by the whole warp at once; a ray walks the table with no dependent ObjectRec -> MeshRec -> tri48 loads.
-// Cornell's table is 44 words (704 B) against the ~2.2 KB of records and triangles the scan reads per ray.
+// Cornell's table is 38 words (608 B) against the ~2.2 KB of records and triangles the scan reads per ray.
 enum : uint32_t { FLAT_TF = 0x100u };
 
 template <class R>

@@ -26,7 +26,10 @@ def lib():
         L.hostemu_scene_destroy.argtypes = [C.c_void_p]
         L.hostemu_scene_features.argtypes = [C.c_void_p]
         L.hostemu_closest_hit.argtypes = [C.c_void_p, dp, C.c_uint64, C.c_double, C.c_uint32, dp, capi.c_i32_p, dp,
-                                          C.POINTER(capi.Stats)]
+                                          capi.c_u32_p, dp, C.POINTER(capi.Stats)]
+        L.hostemu_flat_table.restype = None
+        L.hostemu_flat_table.argtypes = [C.c_void_p, C.POINTER(C.c_uint64), capi.c_u32_p, C.POINTER(C.c_float), C.POINTER(C.c_float)]
+        L.hostemu_pick_variant.argtypes = [C.c_int, C.c_int, C.c_int, C.c_uint32, C.c_uint32, capi.c_i32_p]
         L.hostemu_render.argtypes = [C.c_void_p, C.POINTER(capi.Camera), C.POINTER(capi.RenderParams), C.c_int, dp, C.POINTER(capi.Stats)]
         L.hostemu_occluded.argtypes = [C.c_void_p, dp, dp, C.c_uint64, C.c_double, C.c_uint32, C.c_int, capi.c_i32_p]
         L.hostemu_bvh_check.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(C.c_uint64)]
@@ -37,6 +40,16 @@ def lib():
         L.hostemu_illuminate.argtypes = [C.c_void_p, C.c_uint32, dp, C.c_uint64, C.c_uint64, C.c_uint32, dp, dp, dp]
         _lib = L
     return _lib
+
+
+ENGINE_RENDER, ENGINE_VX, ENGINE_CLOSEST_HIT = 0, 1, 2
+
+
+def pick_variant(engine, features, stats, precision, max_bounces):
+    """The kernel variant the launchers pick (launch.h): ((STATS, FEAT, MAXD), whether it is compiled)."""
+    out = (C.c_int32 * 3)()
+    compiled = lib().hostemu_pick_variant(engine, features, stats, precision, max_bounces, out)
+    return (bool(out[0]), int(out[1]), int(out[2])), bool(compiled)
 
 
 def draws(seed, pixel, sample, n, ensure_every=0):
@@ -85,8 +98,9 @@ class EmuScene:
         rays = np.ascontiguousarray(rays, dtype=np.float64).reshape(-1, 6)
         tmax = np.ascontiguousarray(np.broadcast_to(np.asarray(tmax, dtype=np.float64), (rays.shape[0],)))
         out = np.empty(rays.shape[0], np.int32)
-        lib().hostemu_occluded(self.handle, rays.ctypes.data_as(dp), tmax.ctypes.data_as(dp), rays.shape[0], t_min, precision,
-                               1 if use_bvh else 0, out.ctypes.data_as(capi.c_i32_p))
+        if lib().hostemu_occluded(self.handle, rays.ctypes.data_as(dp), tmax.ctypes.data_as(dp), rays.shape[0], t_min, precision,
+                                  1 if use_bvh else 0, out.ctypes.data_as(capi.c_i32_p)) < 0:
+            raise RuntimeError("occluded: the variant the launchers pick is not compiled")
         return out
 
     def bvh_check(self, mesh: int = 0):
@@ -121,15 +135,38 @@ class EmuScene:
         return t, tri, dict(zip(("nodes4", "empty_slots", "visits2", "visits4", "tris2", "tris4"), [int(v) for v in info]))
 
     def closest_hit(self, rays, t_min=1e-12, precision=capi.PRECISION_F64):
+        t, obj, nrm, _, _, st = self.closest_hit_detail(rays, t_min, precision)
+        return t, obj, nrm, st
+
+    def closest_hit_detail(self, rays, t_min=1e-12, precision=capi.PRECISION_F64):
+        """closest_hit plus Hit::aux (the triangle or cube face hit) and the barycentrics (v, w) as (n, 2)."""
         rays = np.ascontiguousarray(rays, dtype=np.float64).reshape(-1, 6)
         n = rays.shape[0]
         t = np.empty(n)
         obj = np.empty(n, np.int32)
         nrm = np.empty((n, 3))
+        aux = np.empty(n, np.uint32)
+        bvw = np.empty((n, 2))
         st = capi.Stats()
-        lib().hostemu_closest_hit(self.handle, rays.ctypes.data_as(dp), n, t_min, precision, t.ctypes.data_as(dp),
-                                  obj.ctypes.data_as(capi.c_i32_p), nrm.ctypes.data_as(dp), C.byref(st))
-        return t, obj, nrm, st.as_dict()
+        if lib().hostemu_closest_hit(self.handle, rays.ctypes.data_as(dp), n, t_min, precision, t.ctypes.data_as(dp),
+                                     obj.ctypes.data_as(capi.c_i32_p), nrm.ctypes.data_as(dp), aux.ctypes.data_as(capi.c_u32_p),
+                                     bvw.ctypes.data_as(dp), C.byref(st)) < 0:
+            raise RuntimeError("closest_hit: the variant the launchers pick is not compiled")
+        return t, obj, nrm, aux, bvw, st.as_dict()
+
+    def flat_table(self):
+        """The packed primitive table as built (scene_dev.cuh): (words as uint32 (nwords, 4), flat_ok, inverse-transform
+        rows of every f32 object record as float32 (nobjects, 3, 4), tri48 of every mesh's triangles as float32
+        (ntris over all meshes, 3, 4), meshes in order)."""
+        info = (C.c_uint64 * 4)()
+        lib().hostemu_flat_table(self.handle, info, None, None, None)
+        nwords, ok, nobj, ntris = (int(v) for v in info)
+        words = np.zeros((nwords, 4), np.uint32)
+        inv = np.zeros((nobj, 3, 4), np.float32)
+        tri48 = np.zeros((ntris, 3, 4), np.float32)
+        fp = C.POINTER(C.c_float)
+        lib().hostemu_flat_table(self.handle, info, words.ctypes.data_as(capi.c_u32_p), inv.ctypes.data_as(fp), tri48.ctypes.data_as(fp))
+        return words, bool(ok), inv, tri48
 
     def illuminate(self, light, pos, seed=0, precision=capi.PRECISION_F64):
         pos = np.ascontiguousarray(pos, dtype=np.float64).reshape(-1, 3)

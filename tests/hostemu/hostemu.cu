@@ -17,6 +17,7 @@
 #include <cstring>
 #include <new>
 #include <string>
+#include <type_traits>
 
 #include "../../rpt_b200/csrc/flatten.h"
 #include "../../rpt_b200/csrc/integrator.cuh"
@@ -56,7 +57,7 @@ void occluded(const SceneView<R>& sv, const double* rays, const double* tmax, ui
 
 template <class R, int FEAT>
 void closest_hits(const SceneView<R>& sv, const double* rays, uint64_t n, double tmin, double* out_t, int32_t* out_obj,
-                  double* out_n, rptb_stats* stats) {
+                  double* out_n, uint32_t* out_aux, double* out_bvw, rptb_stats* stats) {
     unsigned long long nv = 0, tt = 0, ot = 0, bn = 0, bt = 0;
 #pragma omp parallel for schedule(static) reduction(+ : nv, tt, ot, bn, bt)
     for (int64_t i = 0; i < (int64_t)n; i++) {  // body of closest_hit_kernel (integrator.cuh)
@@ -69,6 +70,11 @@ void closest_hits(const SceneView<R>& sv, const double* rays, uint64_t n, double
         closest_hit<R, true, FEAT>(sv, o, d, (R)tmin, false, h, ts);
         out_obj[i] = h.obj;
         out_t[i] = h.obj >= 0 ? (double)h.t : (double)INFINITY;
+        if (out_aux) out_aux[i] = h.aux;  // which triangle / cube face: on a flat polygon the normal does not tell
+        if (out_bvw) {
+            out_bvw[2 * i] = (double)h.bv;
+            out_bvw[2 * i + 1] = (double)h.bw;
+        }
         if (out_n) {
             Vec3<R> nn = {(R)0, (R)0, (R)0};
             if (h.obj >= 0) nn = finalize_hit<R, FEAT>(sv, sv.objects[h.obj], o, d, h).n;
@@ -167,58 +173,42 @@ void run_grid_vx(const SceneView<float>& sv, const RenderArgs<float>& a) {
     }
 }
 
-// launch_render_vx_f32's dispatch (kernels_vx.cu).  Returns the FEAT it ran, tagged with bit 30.
+// launch_render_vx_f32's dispatch (kernels_vx.cu, through launch.h).  Returns the FEAT it ran, -1 if that variant is not
+// compiled.
 inline int run_render_vx(const SceneView<float>& sv, const RenderArgs<float>& a, int stats, int features) {
-    const int base = features & F_ALL;
-    const bool small = (features & F_SMALL) != 0, ext = (features & F_EXT) != 0, bvh = (features & F_BVH) != 0;
-    int f;
-    if (stats == 1 && bvh) { run_grid_vx<true, F_EVERY | F_BVH>(sv, a); f = F_EVERY | F_BVH; }
-    else if (stats) { run_grid_vx<true, F_EVERY>(sv, a); f = F_EVERY; }
-    else if (ext && bvh) { run_grid_vx<false, F_EVERY | F_BVH>(sv, a); f = F_EVERY | F_BVH; }
-    else if (ext) { run_grid_vx<false, F_EVERY>(sv, a); f = F_EVERY; }
-    else if (bvh && base == F_TREE) { run_grid_vx<false, F_TREE | F_BVH>(sv, a); f = F_TREE | F_BVH; }
-    else if (bvh) { run_grid_vx<false, F_ALL | F_BVH>(sv, a); f = F_ALL | F_BVH; }
-    else if (base == 0 && small) { run_grid_vx<false, F_SMALL>(sv, a); f = F_SMALL; }
-    else if (base == 0) { run_grid_vx<false, 0>(sv, a); f = 0; }
-    else if (base == F_TREE) { run_grid_vx<false, F_TREE>(sv, a); f = F_TREE; }
-    else if (base == (F_TRANSP | F_HDRI) && small) { run_grid_vx<false, F_TRANSP | F_HDRI | F_SMALL>(sv, a); f = F_TRANSP | F_HDRI | F_SMALL; }
-    else if (base == (F_TRANSP | F_HDRI)) { run_grid_vx<false, F_TRANSP | F_HDRI>(sv, a); f = F_TRANSP | F_HDRI; }
-    else { run_grid_vx<false, F_ALL>(sv, a); f = F_ALL; }
-    return f;
+    const Variant v = pick_render_vx(features, stats);
+    if (!visit(RenderVariantsVx{}, v, [&](auto t) { using T = decltype(t); run_grid_vx<T::stats, T::feat>(sv, a); })) return -1;
+    return v.feat;
 }
 
-// The instantiation launch_render_impl (launch_impl.cuh) would launch for these features -- keep in step with it.
-// Returns the FEAT it ran.
+// launch_render_impl's dispatch (launch_impl.cuh, through launch.h).  Returns the FEAT it ran, -1 if that variant is not
+// compiled.
 template <class R>
-int run_render(const SceneView<R>& sv, const RenderArgs<R>& a, int stats, int features) {  // launch_render_impl's dispatch
-    const int base = features & F_ALL;
-    const bool small = (features & F_SMALL) != 0, ext = (features & F_EXT) != 0;
-    if constexpr (M<R>::literal)
-        if (a.max_bounces > 16) {  // f64 gate only: the level stack sized for MAX_BOUNCES_SUPPORTED (the f32 path has no stack)
-            if (stats) run_grid<R, (int)MAX_BOUNCES_SUPPORTED, true, F_EVERY>(sv, a);
-            else run_grid<R, (int)MAX_BOUNCES_SUPPORTED, false, F_EVERY>(sv, a);
-            return F_EVERY;
-        }
-    if constexpr (!M<R>::literal)
-        if (stats == 1 && (features & F_BVH)) { run_grid<R, 16, true, F_EVERY | F_BVH>(sv, a); return F_EVERY | F_BVH; }
-    if (stats) { run_grid<R, 16, true, F_EVERY>(sv, a); return F_EVERY; }
-    if constexpr (!M<R>::literal)
-        if (ext && (features & F_BVH)) { run_grid<R, 16, false, F_EVERY | F_BVH>(sv, a); return F_EVERY | F_BVH; }
-    if (ext) { run_grid<R, 16, false, F_EVERY>(sv, a); return F_EVERY; }
-    if constexpr (M<R>::literal) {
-        run_grid<R, 16, false, F_ALL>(sv, a);
-        return F_ALL;
-    } else {
-        if ((features & F_BVH) && base == F_TREE) { run_grid<R, 16, false, F_TREE | F_BVH>(sv, a); return F_TREE | F_BVH; }
-        if (features & F_BVH) { run_grid<R, 16, false, F_ALL | F_BVH>(sv, a); return F_ALL | F_BVH; }
-        if (base == 0 && small) { run_grid<R, 16, false, F_SMALL>(sv, a); return F_SMALL; }
-        if (base == 0) { run_grid<R, 16, false, 0>(sv, a); return 0; }
-        if (base == F_TREE) { run_grid<R, 16, false, F_TREE>(sv, a); return F_TREE; }
-        if (base == (F_TRANSP | F_HDRI) && small) { run_grid<R, 16, false, F_TRANSP | F_HDRI | F_SMALL>(sv, a); return F_TRANSP | F_HDRI | F_SMALL; }
-        if (base == (F_TRANSP | F_HDRI)) { run_grid<R, 16, false, F_TRANSP | F_HDRI>(sv, a); return F_TRANSP | F_HDRI; }
-        run_grid<R, 16, false, F_ALL>(sv, a);
-        return F_ALL;
-    }
+int run_render(const SceneView<R>& sv, const RenderArgs<R>& a, int stats, int features) {
+    using List = std::conditional_t<M<R>::literal, RenderVariantsF64, RenderVariantsF32>;
+    const Variant v = pick_render(features, stats, M<R>::literal, a.max_bounces);
+    if (!visit(List{}, v, [&](auto t) { using T = decltype(t); run_grid<R, T::maxd, T::stats, T::feat>(sv, a); })) return -1;
+    return v.feat;
+}
+
+// launch_closest_hit_impl's choice for rptb_closest_hit without counters (the any-hit queries take the same walk); the
+// emulation always counts.  Returns the FEAT it ran, -1 if that variant is not compiled.
+template <class R>
+int run_closest_hits(const SceneView<R>& sv, int features, const double* rays, uint64_t n, double tmin, double* out_t,
+                     int32_t* out_obj, double* out_n, uint32_t* out_aux, double* out_bvw, rptb_stats* stats) {
+    using List = std::conditional_t<M<R>::literal, HitVariantsF64, HitVariantsF32>;
+    const Variant v = pick_closest_hit(features, 0, M<R>::literal);
+    if (!visit(List{}, v, [&](auto t) { closest_hits<R, decltype(t)::feat>(sv, rays, n, tmin, out_t, out_obj, out_n, out_aux, out_bvw, stats); }))
+        return -1;
+    return v.feat;
+}
+
+template <class R>
+int run_occluded(const SceneView<R>& sv, int features, const double* rays, const double* tmax, uint64_t n, double tmin, int32_t* out) {
+    using List = std::conditional_t<M<R>::literal, HitVariantsF64, HitVariantsF32>;
+    const Variant v = pick_closest_hit(features, 0, M<R>::literal);
+    if (!visit(List{}, v, [&](auto t) { occluded<R, decltype(t)::feat>(sv, rays, tmax, n, tmin, out); })) return -1;
+    return v.feat;
 }
 
 template <class R>
@@ -288,7 +278,7 @@ hostemu_scene* hostemu_scene_create(const rptb_scene_desc* desc, char* err, size
     InPlace put;
     uint64_t f32_bytes = 0;
     bind_scene(s->hs, put, false, s->v32, s->v64, f32_bytes);
-    s->features = s->hs.features;
+    s->features = kernel_features(s->hs);
     return s;
 }
 
@@ -296,14 +286,58 @@ void hostemu_scene_destroy(hostemu_scene* s) { delete s; }
 
 int hostemu_scene_features(const hostemu_scene* s) { return s->features; }
 
-// precision: 0 = Real float, 1 = Real double (rptb_precision)
+// precision: 0 = Real float, 1 = Real double (rptb_precision).  out_aux (n) and out_bvw (n x 2) may be null: the hit
+// triangle or cube face, and the barycentrics (v, w) of a triangle hit.  Returns the FEAT of the walk, -1 if it is not
+// compiled.
 int hostemu_closest_hit(const hostemu_scene* s, const double* rays, uint64_t n, double t_min, uint32_t precision,
-                        double* out_t, int32_t* out_object, double* out_normal, rptb_stats* stats) {
-    // like launch_closest_hit_impl: f32 goes through the BVH when the scene has one
-    if (precision == RPTB_PRECISION_F64) closest_hits<double, F_EVERY>(s->v64, rays, n, t_min, out_t, out_object, out_normal, stats);
-    else if (s->features & F_BVH) closest_hits<float, F_EVERY | F_BVH>(s->v32, rays, n, t_min, out_t, out_object, out_normal, stats);
-    else closest_hits<float, F_EVERY>(s->v32, rays, n, t_min, out_t, out_object, out_normal, stats);
-    return 0;
+                        double* out_t, int32_t* out_object, double* out_normal, uint32_t* out_aux, double* out_bvw, rptb_stats* stats) {
+    if (precision == RPTB_PRECISION_F64)
+        return run_closest_hits<double>(s->v64, s->features, rays, n, t_min, out_t, out_object, out_normal, out_aux, out_bvw, stats);
+    return run_closest_hits<float>(s->v32, s->features, rays, n, t_min, out_t, out_object, out_normal, out_aux, out_bvw, stats);
+}
+
+// The packed primitive table (scene_dev.cuh, F_FLAT) as built, whether or not the scene is traced through it, and what it
+// was built from.  info = {words, flat_ok, objects, triangles over all meshes}; each pointer may be null:
+// words (4 x info[0] 32-bit words), inv (12 floats per object: the f32 ObjectRec's inverse-transform rows),
+// tri48 (12 floats per triangle, the meshes in order).
+void hostemu_flat_table(const hostemu_scene* s, uint64_t* info, uint32_t* words, float* inv, float* tri48) {
+    const HostScene& hs = s->hs;
+    uint64_t ntris = 0;
+    for (const HostMesh& hm : hs.meshes) ntris += hm.tri48.size() / 3;
+    info[0] = hs.flat.size();
+    info[1] = hs.flat_ok ? 1u : 0u;
+    info[2] = hs.t32.objects.size();
+    info[3] = ntris;
+    if (words && !hs.flat.empty()) std::memcpy(words, hs.flat.data(), hs.flat.size() * sizeof(float4));
+    if (inv)
+        for (size_t i = 0; i < hs.t32.objects.size(); i++) std::memcpy(inv + 12 * i, hs.t32.objects[i].inv, 12 * sizeof(float));
+    if (tri48)
+        for (const HostMesh& hm : hs.meshes) {
+            if (!hm.tri48.empty()) std::memcpy(tri48, hm.tri48.data(), hm.tri48.size() * sizeof(float4));
+            tri48 += 4 * hm.tri48.size();
+        }
+}
+
+// The variant the launchers pick (launch.h).  engine: 0 = render_kernel (slot engine), 1 = render_kernel_vx, 2 =
+// closest_hit_kernel.  out = {STATS, FEAT, MAXD}; returns 1 if that variant is in the list of compiled ones, else 0.
+int hostemu_pick_variant(int engine, int features, int stats, uint32_t precision, uint32_t max_bounces, int32_t* out) {
+    const bool f64 = precision == RPTB_PRECISION_F64;
+    Variant v;
+    bool compiled;
+    if (engine == 0) {
+        v = pick_render(features, stats, f64, max_bounces);
+        compiled = f64 ? RenderVariantsF64::has(v) : RenderVariantsF32::has(v);
+    } else if (engine == 1) {
+        v = pick_render_vx(features, stats);
+        compiled = RenderVariantsVx::has(v);
+    } else {
+        v = pick_closest_hit(features, stats, f64);
+        compiled = f64 ? HitVariantsF64::has(v) : HitVariantsF32::has(v);
+    }
+    out[0] = v.stats ? 1 : 0;
+    out[1] = v.feat;
+    out[2] = v.maxd;
+    return compiled ? 1 : 0;
 }
 
 // Structural check of the BVH of mesh `mesh`: out = {nodes, leaves, largest leaf, depth, distinct triangles
@@ -317,7 +351,7 @@ int hostemu_render(const hostemu_scene* s, const rptb_camera* cam, const rptb_re
     if (!s || !cam || !p || !out_rgb || p->width == 0 || p->height == 0 || p->iterations == 0 ||
         p->max_bounces > MAX_BOUNCES_SUPPORTED)
         return -1;
-    if (p->precision == RPTB_PRECISION_F64) return render_impl<double>(s->v64, cam, p, F_ALL | (s->features & F_EXT), s->hs.sampled_lights, out_rgb, stats);
+    if (p->precision == RPTB_PRECISION_F64) return render_impl<double>(s->v64, cam, p, s->features, s->hs.sampled_lights, out_rgb, stats);
     int feats = s->features;
     if ((feats & F_EXT) && !ext_bvh) feats &= ~F_BVH;
     return render_impl<float>(s->v32, cam, p, feats, s->hs.sampled_lights, out_rgb, stats);
@@ -453,13 +487,12 @@ int hostemu_bvh_check(const hostemu_scene* s, uint32_t mesh, uint64_t* out) {
     return 0;
 }
 
-// precision as above; use_bvh: take the BVH where the scene has one (f32 only)
+// precision as above; use_bvh: take the BVH where the scene has one (f32 only).  Returns the FEAT of the walk, -1 if it
+// is not compiled.
 int hostemu_occluded(const hostemu_scene* s, const double* rays, const double* tmax, uint64_t n, double t_min, uint32_t precision,
                      int use_bvh, int32_t* out) {
-    if (precision == RPTB_PRECISION_F64) occluded<double, F_EVERY>(s->v64, rays, tmax, n, t_min, out);
-    else if (use_bvh && (s->features & F_BVH)) occluded<float, F_EVERY | F_BVH>(s->v32, rays, tmax, n, t_min, out);
-    else occluded<float, F_EVERY>(s->v32, rays, tmax, n, t_min, out);
-    return 0;
+    if (precision == RPTB_PRECISION_F64) return run_occluded<double>(s->v64, s->features, rays, tmax, n, t_min, out);
+    return run_occluded<float>(s->v32, use_bvh ? s->features : s->features & ~(int)F_BVH, rays, tmax, n, t_min, out);
 }
 
 int hostemu_illuminate(const hostemu_scene* s, uint32_t light, const double* pos, uint64_t n, uint64_t seed, uint32_t precision,

@@ -26,7 +26,10 @@ def soup(rng, n, spread=1.0):
     return np.stack([api.Triangle.from_vertices(*t) for t in v])
 
 
-def random_scene(seed):
+def random_scene(seed, table_only=False):
+    """table_only: only what the packed primitive table holds (spheres, cubes, one-leaf meshes, planes; no kd-tree of a
+    mesh or of shapes, no monomial) and no transparent material, so that the f32 megakernel walks the table too.  The
+    default scenes are those of the seeds before the option existed."""
     rng = np.random.default_rng(seed)
     scene = api.Scene()
     mats = [api.Material.diffuse(api.hex_color(0x8090A0)), api.Material.specular(api.hex_color(0xC04020), 0.3),
@@ -36,11 +39,14 @@ def random_scene(seed):
     mesh_small = api.Mesh(soup(rng, 6, 0.5))       # one leaf
     makers = [lambda: api.sphere(), lambda: api.cube(), lambda: mesh_big, lambda: mesh_small,
               lambda: api.monomial_surface(rng.uniform(0.5, 2.5), 4.0)]
+    if table_only:
+        makers = [lambda: api.sphere(), lambda: api.cube(), lambda: mesh_small, lambda: api.Mesh(soup(rng, 3, 0.4))]
+        mats = mats[:3] + mats[4:]
     for _ in range(rng.integers(3, 7)):
         shape = makers[rng.integers(0, len(makers))]()
         shape = random_xf(rng, shape) if rng.random() < 0.8 else shape
         scene.add(api.Object(shape).material(mats[rng.integers(0, len(mats))]))
-    if rng.random() < 0.7:                         # a kd-tree over 20-40 transformed shapes
+    if rng.random() < 0.7 and not table_only:      # a kd-tree over 20-40 transformed shapes
         kids = [random_xf(rng, makers[rng.integers(0, len(makers))]()) for _ in range(rng.integers(20, 40))]
         group = api.KdTree(kids)
         scene.add(api.Object(group if rng.random() < 0.5 else random_xf(rng, group)).material(mats[rng.integers(0, 3)]))

@@ -120,10 +120,9 @@ RPTB_D Frame<R> local_to_world(Vec3<R> n) {
     return f;
 }
 
-// PIT sample of the Beckmann microfacet normal (material.rs:244-254)
+// PIT sample of the Beckmann microfacet angle (material.rs:247-250): one draw
 template <class R, class RNG>
-RPTB_D Vec3<R> beckmann_sample(R m2, Vec3<R> n, RNG& rng) {
-    R sin_t, cos_t;
+RPTB_D void beckmann_angle(R m2, RNG& rng, R& sin_t, R& cos_t) {
     const R u = rng.gen();
     if (M<R>::literal) {
         const double theta = atan(sqrt(m2 * -log((double)u)));
@@ -135,6 +134,13 @@ RPTB_D Vec3<R> beckmann_sample(R m2, Vec3<R> n, RNG& rng) {
         cos_t = M<R>::sqrt(c2);
         sin_t = M<R>::sqrt(M<R>::max((R)1 - c2, (R)0));
     }
+}
+
+// PIT sample of the Beckmann microfacet normal (material.rs:244-254)
+template <class R, class RNG>
+RPTB_D Vec3<R> beckmann_sample(R m2, Vec3<R> n, RNG& rng) {
+    R sin_t, cos_t;
+    beckmann_angle(m2, rng, sin_t, cos_t);
     R x, y;
     unit_circle(rng, x, y);
     return local_to_world(n).apply(x * sin_t, y * sin_t, cos_t);
@@ -156,6 +162,15 @@ RPTB_D R beckmann_pdf(R m2, Vec3<R> n, Vec3<R> h) {
 }
 
 // Material::sample_f (material.rs:224-313).  Returns false for `None` (TIR ends the path).
+//
+// The lobes are sampled in one pass.  The Beckmann lobes (reflection, and transmission on a transparent material) draw
+// the microfacet angle and then a UnitCircle pair, the diffuse lobe draws a UnitDisc pair; both are rejection from
+// [-1,1]^2 and differ only in accepting `< 1` or `<= 1`, so one loop serves both and a warp whose lanes chose different
+// lobes runs it once, for as many tries as its slowest lane needs, instead of once per lobe.  One frame maps the local
+// sample to world space.  Every lane takes the draws, in the order, and the source arithmetic of rng.cuh's unit_circle /
+// unit_disc and of the lobes written one after the other.  The compiler may still fuse multiply-adds differently in the
+// two forms, so the rounding is a property of each kernel and not of the source: the Cornell and glass images at the
+// bench size are bit-identical to the two-loop form's; the F_BVH kernels keep that form (below).
 template <class R, int FEAT = F_ALL, class RNG>
 RPTB_D bool sample_f(const MaterialRec<R>& m, Vec3<R> n, Vec3<R> wo, RNG& rng, Vec3<R>& wi_out, R& pdf_out) {
     constexpr bool TR = (FEAT & F_TRANSP) != 0;
@@ -168,23 +183,66 @@ RPTB_D bool sample_f(const MaterialRec<R>& m, Vec3<R> n, Vec3<R> wo, RNG& rng, V
     const R eta_t = wo_dot_n > (R)0 ? m.index : (R)1 / m.index;
 
     Vec3<R> wi;
-    if (gen_bool(rng, f)) {
-        const Vec3<R> h = beckmann_sample(m2, n, rng);
-        wi = -(wo - ((R)2 * dot(h, wo)) * h);  // -glm::reflect_vec(wo, h)
-    } else if (!TR || !m.transparent) {
-        R x, y;
-        unit_disc(rng, x, y);
-        const R z = M<R>::sqrt(M<R>::literal ? ((R)1 - x * x - y * y) : M<R>::max((R)1 - x * x - y * y, (R)0));
-        wi = local_to_world(n).apply(x, y, z);
+    if constexpr ((FEAT & F_BVH) != 0) {
+        // The kernels that traverse a BVH keep the lobes one after the other.  With the one-pass form their compiled
+        // rounding differed from this form's (the dragon proxy's image changed in ~1 % of its pixels at 1024 spp); the
+        // instruction that differs has not been found, and these kernels were not faster with it.
+        if (gen_bool(rng, f)) {
+            const Vec3<R> h = beckmann_sample(m2, n, rng);
+            wi = -(wo - ((R)2 * dot(h, wo)) * h);  // -glm::reflect_vec(wo, h)
+        } else if (!TR || !m.transparent) {
+            R x, y;
+            unit_disc(rng, x, y);
+            const R z = M<R>::sqrt(M<R>::literal ? ((R)1 - x * x - y * y) : M<R>::max((R)1 - x * x - y * y, (R)0));
+            wi = local_to_world(n).apply(x, y, z);
+        } else {
+            const Vec3<R> h = beckmann_sample(m2, n, rng);
+            const R cos_to = dot(h, wo);
+            const Vec3<R> wo_perp = wo - h * cos_to;
+            const Vec3<R> wi_perp = -wo_perp / eta_t;
+            const R sin2_ti = length2(wi_perp);
+            if (sin2_ti > (R)1) return false;
+            const R cos_ti = M<R>::sqrt((R)1 - sin2_ti);
+            wi = (-signum(cos_to) * cos_ti) * h + wi_perp;
+        }
     } else {
-        const Vec3<R> h = beckmann_sample(m2, n, rng);
-        const R cos_to = dot(h, wo);
-        const Vec3<R> wo_perp = wo - h * cos_to;
-        const Vec3<R> wi_perp = -wo_perp / eta_t;
-        const R sin2_ti = length2(wi_perp);
-        if (sin2_ti > (R)1) return false;
-        const R cos_ti = M<R>::sqrt((R)1 - sin2_ti);
-        wi = (-signum(cos_to) * cos_ti) * h + wi_perp;
+        const bool reflect = gen_bool(rng, f);
+        const bool beckmann = reflect || (TR && m.transparent);  // else the diffuse lobe
+        R sin_t = (R)0, cos_t = (R)0;
+        if (beckmann) beckmann_angle(m2, rng, sin_t, cos_t);
+        R x1, x2, sum;
+        while (true) {  // UnitCircle (beckmann) or UnitDisc
+            x1 = uniform_pm1<R>(rng);
+            x2 = uniform_pm1<R>(rng);
+            sum = x1 * x1 + x2 * x2;
+            if (beckmann ? sum < (R)1 : sum <= (R)1) break;
+        }
+        R lx, ly, lz;
+        if (beckmann) {  // von Neumann's map of the pair onto the circle, scaled to the microfacet angle
+            const R diff = x1 * x1 - x2 * x2;
+            lx = diff / sum * sin_t;
+            ly = (R)2 * x1 * x2 / sum * sin_t;
+            lz = cos_t;
+        } else {
+            lx = x1;
+            ly = x2;
+            lz = M<R>::sqrt(M<R>::literal ? ((R)1 - x1 * x1 - x2 * x2) : M<R>::max((R)1 - x1 * x1 - x2 * x2, (R)0));
+        }
+        const Vec3<R> v = local_to_world(n).apply(lx, ly, lz);  // beckmann: the microfacet normal h; diffuse: wi
+
+        if (reflect) {
+            wi = -(wo - ((R)2 * dot(v, wo)) * v);  // -glm::reflect_vec(wo, h)
+        } else if (!TR || !m.transparent) {
+            wi = v;
+        } else {
+            const R cos_to = dot(v, wo);
+            const Vec3<R> wo_perp = wo - v * cos_to;
+            const Vec3<R> wi_perp = -wo_perp / eta_t;
+            const R sin2_ti = length2(wi_perp);
+            if (sin2_ti > (R)1) return false;
+            const R cos_ti = M<R>::sqrt((R)1 - sin2_ti);
+            wi = (-signum(cos_to) * cos_ti) * v + wi_perp;
+        }
     }
 
     R p = (R)0;

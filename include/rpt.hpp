@@ -256,6 +256,46 @@ private:
     uint32_t batches_ = 0;
 };
 
+// The same Buffer kept in device memory (rptb_buffer) on every GPU of a scene: Renderer::sample adds an entry
+// without a copy to the host, and image() / variance() cost O(width*height) however many entries it holds.
+// Owns its device memory; it may outlive the Renderer that made it.
+class DeviceBuffer {
+public:
+    DeviceBuffer(rptb_scene* scene, uint32_t w, uint32_t h, Filter f = {}) : width_(w), height_(h) {
+        if (rptb_buffer_create(scene, w, h, f.radius, &handle_) != RPTB_OK) throw std::runtime_error(rptb_last_error());
+    }
+    ~DeviceBuffer() { if (handle_) rptb_buffer_destroy(handle_); }
+    DeviceBuffer(const DeviceBuffer&) = delete;
+    DeviceBuffer& operator=(const DeviceBuffer&) = delete;
+    DeviceBuffer(DeviceBuffer&& o) noexcept : width_(o.width_), height_(o.height_), handle_(o.handle_) { o.handle_ = nullptr; }
+
+    void add_samples(const std::vector<double>& rgb) {  // :32-40
+        if (rgb.size() != (size_t)width_ * height_ * 3) throw std::invalid_argument("Invalid sample dimension");
+        check(rptb_buffer_add_samples(handle_, rgb.data()));
+    }
+    std::vector<uint8_t> image() const {  // :43-56
+        std::vector<uint8_t> out((size_t)width_ * height_ * 3);
+        check(rptb_buffer_image(handle_, out.data()));
+        return out;
+    }
+    double variance() const {  // :59-73; NaN with fewer than two entries
+        double v = 0;
+        check(rptb_buffer_variance(handle_, &v));
+        return v;
+    }
+    std::vector<double> sums() const {  // per-pixel sums over the entries, row-major
+        std::vector<double> out((size_t)width_ * height_ * 3);
+        check(rptb_buffer_sums(handle_, out.data(), nullptr));
+        return out;
+    }
+    rptb_buffer* handle() const { return handle_; }
+
+private:
+    static void check(int rc) { if (rc != RPTB_OK) throw std::runtime_error(rptb_last_error()); }
+    uint32_t width_, height_;
+    rptb_buffer* handle_ = nullptr;
+};
+
 // Renderer (src/renderer.rs:18-115); `sample` is the seam into the CUDA library.
 class Renderer {
 public:
@@ -291,22 +331,52 @@ public:
     }
     void sample(uint32_t iterations, Buffer& buffer) {  // :117-129
         ensure_scene();
-        rptb_render_params p{};
-        p.width = width_; p.height = height_; p.iterations = iterations; p.max_bounces = max_bounces_;
-        p.exposure_value = ev_; p.seed = seed_; p.first_sample = next_sample_; p.shard_count = 1;
-        rptb_camera c{};
-        const Vec3* src[3] = {&camera_.eye, &camera_.direction, &camera_.up};
-        double* dst[3] = {c.eye, c.direction, c.up};
-        for (int i = 0; i < 3; i++) { dst[i][0] = src[i]->x; dst[i][1] = src[i]->y; dst[i][2] = src[i]->z; }
-        c.fov = camera_.fov; c.aperture = camera_.aperture; c.focal_distance = camera_.focal_distance;
+        const rptb_render_params p = params(iterations);
+        const rptb_camera c = camera();
         std::vector<double> colors((size_t)width_ * height_ * 3);
         if (rptb_render_samples(handle_, &c, &p, colors.data(), &stats) != RPTB_OK) throw std::runtime_error(rptb_last_error());
         next_sample_ += iterations;
         buffer.add_samples(colors);
     }
+
+    // The device-resident Buffer: one for this renderer's size and filter on its GPUs, the entry added on the device.
+    DeviceBuffer device_buffer() {
+        ensure_scene();
+        return DeviceBuffer(handle_, width_, height_, filter_);
+    }
+    void sample(uint32_t iterations, DeviceBuffer& buffer) {  // :117-129, without the copy to the host
+        ensure_scene();
+        const rptb_render_params p = params(iterations);
+        const rptb_camera c = camera();
+        if (rptb_sample_into(handle_, &c, &p, buffer.handle(), nullptr) != RPTB_OK) throw std::runtime_error(rptb_last_error());
+        next_sample_ += iterations;
+    }
+    void iterative_render(uint32_t interval, DeviceBuffer& buffer, const std::function<void(uint32_t, const DeviceBuffer&)>& cb) {
+        uint32_t iteration = 0;
+        while (iteration < num_samples_) {
+            const uint32_t steps = std::min(num_samples_ - iteration, interval);
+            sample(steps, buffer);
+            iteration += steps;
+            cb(iteration, buffer);
+        }
+    }
     rptb_stats stats{};
 
 private:
+    rptb_render_params params(uint32_t iterations) const {
+        rptb_render_params p{};
+        p.width = width_; p.height = height_; p.iterations = iterations; p.max_bounces = max_bounces_;
+        p.exposure_value = ev_; p.seed = seed_; p.first_sample = next_sample_; p.shard_count = 1;
+        return p;
+    }
+    rptb_camera camera() const {
+        rptb_camera c{};
+        const Vec3* src[3] = {&camera_.eye, &camera_.direction, &camera_.up};
+        double* dst[3] = {c.eye, c.direction, c.up};
+        for (int i = 0; i < 3; i++) { dst[i][0] = src[i]->x; dst[i][1] = src[i]->y; dst[i][2] = src[i]->z; }
+        c.fov = camera_.fov; c.aperture = camera_.aperture; c.focal_distance = camera_.focal_distance;
+        return c;
+    }
     static rptb_material to_c(const Material& m) {
         rptb_material r{};
         r.color[0] = m.color.x; r.color[1] = m.color.y; r.color[2] = m.color.z;

@@ -13,6 +13,7 @@
  *   Camera                                     src/camera.rs:8-26
  *   KdTree<Triangle> (= Mesh)                  src/kdtree.rs:99-119,226-233, src/shape/mesh.rs:7-22,102
  *   Buffer::image / variance, color_bytes      src/buffer.rs:43-93, src/color.rs:17-23
+ *   Buffer (device-resident) / add_samples     src/buffer.rs:6-40
  *
  * All structs are plain-old-data; all pointers are caller-owned host memory
  * unless the name says `_device`.  Values cross the boundary as `double`
@@ -384,6 +385,36 @@ int rptb_film_variance(const double* batches, uint32_t nbatches, uint64_t npixel
  * the entries, width*height*3 doubles).  out_rgb8 = width*height*3 bytes.    */
 int rptb_film_resolve(const double* sums, uint32_t nbatches, uint32_t width, uint32_t height,
                       uint32_t box_radius, int device, uint8_t* out_rgb8);
+
+/* ---- Buffer on the device: src/buffer.rs:6-93 -------------------------------------------------------------
+ * Replaces: Buffer::new(width, height, Filter::Box(box_radius)) (src/buffer.rs:17-29), kept in device memory on
+ * every replica of `scene`: per pixel the running sum of its entries in double, added in entry order (the
+ * sequential sum np.sum(batches, axis=0) computes, bit for bit), and one streaming (Welford) M2 summed over the
+ * three channels.  Replica i of n holds the 16x8 tiles t with t % n == i.  image / variance / sums gather the
+ * replicas on the first device and cost O(width*height) however many entries were added; their results are the
+ * same bits for any device count.  The buffer owns its memory: it and its scene may be destroyed in either order.
+ * A buffer is used from one thread at a time (calls on it are serialised internally).                        */
+typedef struct rptb_buffer rptb_buffer; /* opaque */
+int rptb_buffer_create(rptb_scene* scene, uint32_t width, uint32_t height, uint32_t box_radius, rptb_buffer** out);
+void rptb_buffer_destroy(rptb_buffer* buffer);
+/* Replaces: Renderer::sample(iterations, &mut Buffer) (src/renderer.rs:117-129): renders params->iterations samples
+ * and adds ONE entry per pixel -- the mean times 2^exposure_value, exactly what rptb_render_samples writes (the
+ * f32 path's float widened to double) -- to `buffer`, on the device.  The render is not copied to the host; with
+ * stats == NULL the call returns once the work is enqueued.  width/height must be the buffer's and `scene` must have
+ * the device list of the scene the buffer was created on (else RPTB_ERR_BAD_ARG); shard_count > 1 is
+ * RPTB_ERR_UNSUPPORTED (a buffer holds the whole image); compact_out is ignored.                              */
+int rptb_sample_into(rptb_scene* scene, const rptb_camera* camera, const rptb_render_params* params,
+                     rptb_buffer* buffer, rptb_stats* stats /* nullable, forces sync */);
+/* Replaces: Buffer::add_samples (src/buffer.rs:32-40) of a host entry: width*height*3 doubles, row-major.      */
+int rptb_buffer_add_samples(rptb_buffer* buffer, const double* rgb);
+/* Replaces: Buffer::image (src/buffer.rs:43-56,75-93): width*height*3 bytes, the bytes rptb_film_resolve gives
+ * for the same sums.  No entry yet: RPTB_ERR_BAD_ARG, "Pixel found with no samples" (src/buffer.rs:89).       */
+int rptb_buffer_image(rptb_buffer* buffer, uint8_t* out_rgb8);
+/* Replaces: Buffer::variance (src/buffer.rs:59-73): the mean over pixels of M2 / (entries - 1), reduced in a
+ * fixed order.  NaN with fewer than two entries, as in the reference.                                        */
+int rptb_buffer_variance(rptb_buffer* buffer, double* out);
+/* The per-pixel sums (width*height*3 doubles, row-major) and the entry count (out_entries nullable).        */
+int rptb_buffer_sums(rptb_buffer* buffer, double* out_sums, uint32_t* out_entries);
 
 #ifdef __cplusplus
 }

@@ -207,6 +207,12 @@ pub struct RptbScene {
     _private: [u8; 0],
 }
 
+/// Opaque `rptb_buffer`: `Buffer` (src/buffer.rs:6-93) kept in device memory.
+#[repr(C)]
+pub struct RptbBuffer {
+    _private: [u8; 0],
+}
+
 extern "C" {
     pub fn rptb_last_error() -> *const c_char;
     pub fn rptb_device_count() -> c_int;
@@ -267,6 +273,22 @@ extern "C" {
         out_rgb8: *mut u8,
     ) -> c_int;
     pub fn rptb_film_variance(batches: *const f64, nbatches: u32, npixels: u64, device: c_int, out: *mut f64) -> c_int;
+    /// `Buffer::new(width, height, Filter::Box(box_radius))` on every GPU of `scene`; it may outlive the scene.
+    pub fn rptb_buffer_create(scene: *mut RptbScene, width: u32, height: u32, box_radius: u32, out: *mut *mut RptbBuffer) -> c_int;
+    pub fn rptb_buffer_destroy(buffer: *mut RptbBuffer);
+    /// `Renderer::sample(iterations, &mut buffer)` (src/renderer.rs:117-129) with the entry added on the device;
+    /// with `stats` null it returns once the work is enqueued.
+    pub fn rptb_sample_into(
+        scene: *mut RptbScene,
+        camera: *const RptbCamera,
+        params: *const RptbRenderParams,
+        buffer: *mut RptbBuffer,
+        stats: *mut RptbStats, // nullable
+    ) -> c_int;
+    pub fn rptb_buffer_add_samples(buffer: *mut RptbBuffer, rgb: *const f64) -> c_int; // width * height * 3, row-major
+    pub fn rptb_buffer_image(buffer: *mut RptbBuffer, out_rgb8: *mut u8) -> c_int;
+    pub fn rptb_buffer_variance(buffer: *mut RptbBuffer, out: *mut f64) -> c_int; // NaN below two entries
+    pub fn rptb_buffer_sums(buffer: *mut RptbBuffer, out_sums: *mut f64, out_entries: *mut u32) -> c_int;
 }
 
 /// The thread-local message of the last failing call.

@@ -13,6 +13,7 @@ LIB_PATH = os.environ.get("RPTB_LIB") or os.path.join(_HERE, "lib", "librpt_b200
 
 # ---- enums (include/rpt_b200.h) ------------------------------------------------
 OK = 0
+ERR_BAD_ARG, ERR_CUDA, ERR_NO_DEVICE, ERR_OOM, ERR_UNSUPPORTED = -1, -2, -3, -4, -5
 SHAPE_SPHERE, SHAPE_PLANE, SHAPE_CUBE, SHAPE_MESH, SHAPE_MONOMIAL, SHAPE_GROUP = 0, 1, 2, 3, 4, 5
 LIGHT_POINT, LIGHT_AMBIENT, LIGHT_DIRECTIONAL, LIGHT_OBJECT = 0, 1, 2, 3
 ENV_COLOR, ENV_HDRI = 0, 1
@@ -231,6 +232,14 @@ SYMBOLS = [
     ("rptb_film_variance", C.c_int, [c_double_p, C.c_uint32, C.c_uint64, C.c_int, c_double_p]),
     ("rptb_film_resolve", C.c_int,
      [c_double_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_int, c_u8_p]),
+    ("rptb_buffer_create", C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(C.c_void_p)]),
+    ("rptb_buffer_destroy", None, [C.c_void_p]),
+    ("rptb_sample_into", C.c_int,
+     [C.c_void_p, C.POINTER(Camera), C.POINTER(RenderParams), C.c_void_p, C.POINTER(Stats)]),
+    ("rptb_buffer_add_samples", C.c_int, [C.c_void_p, c_double_p]),
+    ("rptb_buffer_image", C.c_int, [C.c_void_p, c_u8_p]),
+    ("rptb_buffer_variance", C.c_int, [C.c_void_p, c_double_p]),
+    ("rptb_buffer_sums", C.c_int, [C.c_void_p, c_double_p, c_u32_p]),
 ]
 
 _lib = None

@@ -14,6 +14,7 @@ API, so scene scripts and tests read like the reference's examples:
     load_obj                    src/io.rs:27-73,151-200
     Renderer                    src/renderer.rs:18-115
     Buffer / Filter             src/buffer.rs:6-108
+    DeviceBuffer                src/buffer.rs:6-93, kept on the GPU (rptb_buffer)
     hex_color / color_bytes     src/color.rs:10-23
 
 Everything below `Renderer.sample` (src/renderer.rs:117-129) is *not* here:
@@ -871,6 +872,68 @@ class Buffer:
         return float(out.value)
 
 
+class DeviceBuffer:
+    """src/buffer.rs:6-93 kept in device memory (rptb_buffer): per pixel the running sum of its entries and a
+    streaming variance, on every GPU of the scene it was made for.  Renderer.sample adds an entry without
+    copying the render to the host, and image() / variance() cost O(width * height) however many entries it
+    holds.  The numbers are those of the host Buffer over the same entries: sums() is np.sum(batches, axis=0)
+    bit for bit, image() gives the same bytes, variance() agrees to rounding (Welford instead of two passes)."""
+
+    def __init__(self, scene: DeviceScene, width: int, height: int, filter: Optional[Filter] = None):
+        self.width, self.height = int(width), int(height)
+        self.filter = filter or Filter()
+        self.devices = list(scene.devices)
+        self.entries = 0  # entries per pixel: add_samples and Renderer.sample calls
+        self.handle = C.c_void_p()
+        capi.check(capi.lib().rptb_buffer_create(scene.handle, self.width, self.height, self.filter.radius,
+                                                 C.byref(self.handle)), "rptb_buffer_create")
+
+    def add_samples(self, samples) -> None:  # :32-40
+        samples = np.ascontiguousarray(np.asarray(samples, dtype=np.float64).reshape(-1, 3))
+        assert samples.shape[0] == self.width * self.height, "Invalid sample dimension"
+        capi.check(capi.lib().rptb_buffer_add_samples(self.handle, samples.ctypes.data_as(capi.c_double_p)),
+                   "rptb_buffer_add_samples")
+        self.entries += 1
+
+    def sums(self) -> np.ndarray:
+        """(width * height, 3) per-pixel sums over the entries, row-major."""
+        out = np.empty((self.width * self.height, 3), np.float64)
+        n = C.c_uint32(0)
+        capi.check(capi.lib().rptb_buffer_sums(self.handle, out.ctypes.data_as(capi.c_double_p), C.byref(n)),
+                   "rptb_buffer_sums")
+        assert n.value == self.entries
+        return out
+
+    def image(self) -> np.ndarray:
+        """:43-56 -> (height, width, 3) uint8."""
+        out = np.empty((self.height, self.width, 3), np.uint8)
+        capi.check(capi.lib().rptb_buffer_image(self.handle, out.ctypes.data_as(capi.c_u8_p)), "rptb_buffer_image")
+        return out
+
+    def variance(self) -> float:
+        """:59-73.  NaN with fewer than two entries, like the reference."""
+        out = C.c_double(0.0)
+        capi.check(capi.lib().rptb_buffer_variance(self.handle, C.byref(out)), "rptb_buffer_variance")
+        return float(out.value)
+
+    def close(self) -> None:
+        if self.handle:
+            capi.lib().rptb_buffer_destroy(self.handle)
+            self.handle = C.c_void_p()
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *a):
+        self.close()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
 # ---------------------------------------------------------------- renderer ----
 class Renderer:
     """src/renderer.rs:18-115.  Builder methods carry the reference's names; the
@@ -968,11 +1031,26 @@ class Renderer:
             self._dev_scene.close()
             self._dev_scene = None
 
+    def device_buffer(self) -> DeviceBuffer:
+        """A DeviceBuffer of this renderer's size and filter on the GPUs of its device scene."""
+        return DeviceBuffer(self.device_scene(), self._width, self._height, self._filter)
+
     # ---- the seam: Renderer::sample (:117-129) ---------------------------------
-    def sample(self, iterations: int, buffer: Buffer, collect_stats: int = 0) -> None:
+    def sample(self, iterations: int, buffer, collect_stats: int = 0, want_stats: bool = True) -> None:
+        """Adds one entry of `iterations` samples per pixel to `buffer`.  A host Buffer gets the image through
+        host memory; a DeviceBuffer gets it on the device, and the call returns once the work is enqueued unless
+        `want_stats` (then last_stats is filled, which waits for the render)."""
         ds = self.device_scene()
         p = self.params(iterations, self._next_sample, collect_stats=collect_stats)
         cam = self.camera.to_c()
+        if isinstance(buffer, DeviceBuffer):
+            stats = capi.Stats()
+            capi.check(capi.lib().rptb_sample_into(ds.handle, C.byref(cam), C.byref(p), buffer.handle,
+                                                   C.byref(stats) if want_stats else None), "rptb_sample_into")
+            self._next_sample += int(iterations)
+            buffer.entries += 1
+            self.last_stats = stats.as_dict() if want_stats else None
+            return
         colors = np.empty((self._width * self._height, 3), np.float64)
         stats = capi.Stats()
         capi.check(
@@ -989,11 +1067,16 @@ class Renderer:
         self.sample(self._num_samples, buffer)
         return buffer.image()
 
-    def iterative_render(self, callback_interval: int, callback: Callable[[int, Buffer], None]) -> None:  # :103-115
-        buffer = Buffer(self._width, self._height, self._filter, self._first_device())
+    def iterative_render(self, callback_interval: int, callback: Callable[[int, Buffer], None],
+                         buffer: Optional[DeviceBuffer] = None) -> None:  # :103-115
+        """`buffer`: a DeviceBuffer (Renderer.device_buffer()) to accumulate into on the device; None keeps a
+        host Buffer.  The callback receives whichever it is."""
+        device = buffer is not None
+        if buffer is None:
+            buffer = Buffer(self._width, self._height, self._filter, self._first_device())
         iteration = 0
         while iteration < self._num_samples:
             steps = min(self._num_samples - iteration, callback_interval)
-            self.sample(steps, buffer)
+            self.sample(steps, buffer, want_stats=not device)
             iteration += steps
             callback(iteration, buffer)

@@ -31,6 +31,15 @@ cudaError_t launch_film_resolve(const double* sums, uint32_t nbatches, uint32_t 
                                 uint32_t radius, uint8_t* out, cudaStream_t stream);
 cudaError_t launch_convert_f64_to_f32(const double* in, float* out, size_t n, cudaStream_t stream);
 cudaError_t launch_film_variance(const double* batches, uint32_t nbatches, uint64_t npixels, double* out_sum, cudaStream_t stream);
+cudaError_t launch_buffer_accumulate(const float* in32, const double* in64, bool rowmajor, uint32_t n, uint64_t nelem,
+                                     uint32_t width, uint32_t height, uint32_t shard_index, uint32_t shard_count,
+                                     double* sums, double* m2, cudaStream_t stream);
+cudaError_t launch_buffer_scatter(const double* sums, const double* m2, uint64_t nelem, uint32_t width, uint32_t height,
+                                  uint32_t shard_index, uint32_t shard_count, double* row_sums, double* row_m2,
+                                  cudaStream_t stream);
+uint32_t buffer_variance_blocks(uint64_t npixels);
+cudaError_t launch_buffer_variance(const double* m2, uint64_t npixels, uint32_t n, double* partial, double* out_sum,
+                                   cudaStream_t stream);
 int parse_obj_text(const char* text, size_t len, std::vector<double>& tris, std::string& err);
 struct ObjGroup {
     rptb_material material;
@@ -526,6 +535,141 @@ void destroy_replica(rptb_scene* s) {
         pool_scene_gone(s->device);  // counted by scene_bind_device right before the stream was made
     }
     delete s;
+}
+
+}  // namespace
+
+// ---- the device-resident Buffer (src/buffer.rs:6-93) ------------------------------------------------------------
+// One part per replica of the scene it was created on, each holding that replica's own 16x8 tiles in the compact
+// tile-major layout (film.cu): 3 running sums and one Welford M2 per pixel, in double.  The buffer owns its memory
+// (cudaMalloc, so destroy hands it back to the driver), its streams and its events, so it and its scene may be
+// destroyed in either order.  `done` is recorded behind every accumulate -- on the scene's stream (rptb_sample_into)
+// or on the part's own (rptb_buffer_add_samples) -- and every later operation on the part waits for it.
+struct BufferPart {
+    int device = 0;
+    uint32_t tiles = 0;          // tiles t with t % nparts == this part's index
+    double* sums = nullptr;      // tiles * 128 * 3
+    double* m2 = nullptr;        // tiles * 128
+    double* upload = nullptr;    // a host entry, row-major width*height*3 (first add_samples allocates it)
+    cudaStream_t stream = nullptr;
+    cudaEvent_t done = nullptr;
+};
+
+struct rptb_buffer {
+    uint32_t width = 0, height = 0, radius = 0;
+    uint32_t entries = 0;
+    std::vector<BufferPart> parts;
+    // on parts[0]'s device, allocated by the first image / variance / sums: the image gathered row-major
+    double* row_sums = nullptr;  // width*height*3
+    double* row_m2 = nullptr;    // width*height
+    double* gather = nullptr;    // one other part's sums + M2, copied over
+    double* partial = nullptr;   // variance block partials, then the total
+    uint8_t* rgb8 = nullptr;
+    std::mutex lock;
+};
+
+namespace {
+
+uint32_t buffer_tiles(uint32_t width, uint32_t height, uint32_t index, uint32_t nparts) {
+    const uint32_t ntiles = ((width + 15u) / 16u) * ((height + 7u) / 8u);
+    return ntiles > index ? (ntiles - index + nparts - 1u) / nparts : 0u;
+}
+
+void buffer_free(rptb_buffer* b) {
+    for (size_t i = 0; i < b->parts.size(); i++) {
+        BufferPart& q = b->parts[i];
+        DeviceGuard g(q.device);
+        if (q.done) cudaEventSynchronize(q.done);  // an accumulate may still run on the scene's stream
+        if (q.stream) cudaStreamSynchronize(q.stream);
+        cudaFree(q.sums);
+        cudaFree(q.m2);
+        cudaFree(q.upload);
+        if (i == 0) {
+            cudaFree(b->row_sums);
+            cudaFree(b->row_m2);
+            cudaFree(b->gather);
+            cudaFree(b->partial);
+            cudaFree(b->rgb8);
+        }
+        if (q.done) cudaEventDestroy(q.done);
+        if (q.stream) cudaStreamDestroy(q.stream);
+    }
+    delete b;
+}
+
+int buffer_part_alloc(BufferPart& q) {
+    CU(cudaStreamCreateWithFlags(&q.stream, cudaStreamNonBlocking));
+    CU(cudaEventCreateWithFlags(&q.done, cudaEventDisableTiming));
+    if (q.tiles) {
+        const size_t nelem = (size_t)q.tiles * 128u;
+        CU(cudaMalloc((void**)&q.sums, nelem * 3 * sizeof(double)));
+        CU(cudaMalloc((void**)&q.m2, nelem * sizeof(double)));
+        CU(cudaMemsetAsync(q.sums, 0, nelem * 3 * sizeof(double), q.stream));  // sums() of an empty buffer reads zero
+        CU(cudaMemsetAsync(q.m2, 0, nelem * sizeof(double), q.stream));
+    }
+    CU(cudaEventRecord(q.done, q.stream));
+    return RPTB_OK;
+}
+
+// Brings every part's sums and/or M2 to parts[0]'s device in row-major order, on parts[0]'s stream (the caller has
+// made that device current).  Other parts are copied with cudaMemcpyPeerAsync, which needs no peer access.
+int buffer_gather(rptb_buffer* b, bool want_sums, bool want_m2) {
+    BufferPart& q0 = b->parts[0];
+    const uint32_t nparts = (uint32_t)b->parts.size();
+    const size_t npix = (size_t)b->width * b->height;
+    if (!b->row_sums) {
+        uint32_t most = 0;
+        for (uint32_t i = 1; i < nparts; i++) most = std::max(most, b->parts[i].tiles);
+        CU(cudaMalloc((void**)&b->row_sums, npix * 3 * sizeof(double)));
+        CU(cudaMalloc((void**)&b->row_m2, npix * sizeof(double)));
+        if (most) CU(cudaMalloc((void**)&b->gather, (size_t)most * 128u * 4u * sizeof(double)));
+        CU(cudaMalloc((void**)&b->partial, (buffer_variance_blocks(npix) + 1) * sizeof(double)));
+        CU(cudaMalloc((void**)&b->rgb8, npix * 3));
+    }
+    double* rs = want_sums ? b->row_sums : nullptr;
+    double* rm = want_m2 ? b->row_m2 : nullptr;
+    CU(cudaStreamWaitEvent(q0.stream, q0.done, 0));
+    CU(launch_buffer_scatter(q0.sums, q0.m2, (uint64_t)q0.tiles * 128u, b->width, b->height, 0, nparts, rs, rm, q0.stream));
+    for (uint32_t i = 1; i < nparts; i++) {
+        const BufferPart& q = b->parts[i];
+        if (!q.tiles) continue;
+        const size_t nelem = (size_t)q.tiles * 128u;
+        CU(cudaStreamWaitEvent(q0.stream, q.done, 0));
+        if (want_sums) CU(cudaMemcpyPeerAsync(b->gather, q0.device, q.sums, q.device, nelem * 3 * sizeof(double), q0.stream));
+        if (want_m2) CU(cudaMemcpyPeerAsync(b->gather + nelem * 3, q0.device, q.m2, q.device, nelem * sizeof(double), q0.stream));
+        CU(launch_buffer_scatter(b->gather, b->gather + nelem * 3, nelem, b->width, b->height, i, nparts, rs, rm, q0.stream));
+    }
+    return RPTB_OK;
+}
+
+// Enqueues replica `index` of `nparts`'s share of one rptb_sample_into on the replica's own stream: render its
+// tiles into the compact out32/out64 scratch, then add them to the buffer part as entry `n`.  No host synchronise.
+int sample_part(rptb_scene* r, const rptb_camera* cam, const rptb_render_params* p, uint32_t index, uint32_t nparts,
+                uint32_t n, BufferPart& q, bool want_stats, uint32_t* launches) {
+    DeviceGuard g(r->device);
+    if (!g.ok) return fail(RPTB_ERR_CUDA, "cudaSetDevice(%d) failed", r->device);
+    int rc = wait_busy(r, r->stream);
+    if (rc != RPTB_OK) return rc;
+    rptb_render_params qp = *p;
+    qp.shard_index = index;
+    qp.shard_count = nparts;
+    const uint64_t nelem = (uint64_t)q.tiles * 128u;
+    rc = ensure_out(r, nelem ? nelem * 3 : 1);
+    if (rc != RPTB_OK) return rc;
+    CU(cudaStreamWaitEvent(r->stream, q.done, 0));  // an add_samples on the part's own stream
+    if (want_stats) CU(cudaEventRecord(r->ev0, r->stream));
+    rc = render_launch(r, cam, &qp, r->out32, r->out64, r->stream, want_stats, true, launches);
+    if (rc != RPTB_OK) return rc;
+    if (want_stats) CU(cudaEventRecord(r->ev1, r->stream));
+    const bool f32 = p->precision == RPTB_PRECISION_F32;
+    CU(launch_buffer_accumulate(f32 ? r->out32 : nullptr, f32 ? nullptr : r->out64, false, n, nelem, p->width, p->height,
+                                index, nparts, q.sums, q.m2, r->stream));
+    (*launches)++;
+    CU(cudaEventRecord(q.done, r->stream));
+    // the scratch is read until the accumulate has run: later calls on any stream order themselves behind it
+    CU(cudaEventRecord(r->busy, r->stream));
+    r->busy_pending = true;
+    return RPTB_OK;
 }
 
 }  // namespace
@@ -1052,6 +1196,162 @@ int rptb_film_resolve(const double* sums, uint32_t nbatches, uint32_t width, uin
     CUC(launch_film_resolve(d_in, nbatches, width, height, box_radius, d_out, 0));
     CUC(cudaMemcpy(out_rgb8, d_out, nvals, cudaMemcpyDeviceToHost));
     cleanup();
+    return RPTB_OK;
+}
+
+int rptb_buffer_create(rptb_scene* s, uint32_t width, uint32_t height, uint32_t box_radius, rptb_buffer** out) {
+    if (!s || !out) return fail(RPTB_ERR_BAD_ARG, "null argument");
+    *out = nullptr;
+    if (width == 0 || height == 0) return fail(RPTB_ERR_BAD_ARG, "empty image %ux%u", width, height);
+    if ((uint64_t)width * height > 0x7FFFFFFFull / 4) return fail(RPTB_ERR_UNSUPPORTED, "image too large");
+    rptb_buffer* b = new (std::nothrow) rptb_buffer();
+    if (!b) return fail(RPTB_ERR_OOM, "host allocation failed");
+    b->width = width;
+    b->height = height;
+    b->radius = box_radius;
+    const uint32_t nparts = 1u + (uint32_t)s->peers.size();
+    b->parts.resize(nparts);
+    int rc = RPTB_OK;
+    for (uint32_t i = 0; rc == RPTB_OK && i < nparts; i++) {
+        BufferPart& q = b->parts[i];
+        q.device = i == 0 ? s->device : s->peers[i - 1]->device;
+        q.tiles = buffer_tiles(width, height, i, nparts);
+        DeviceGuard g(q.device);
+        rc = g.ok ? buffer_part_alloc(q) : fail(RPTB_ERR_CUDA, "cudaSetDevice(%d) failed", q.device);
+    }
+    if (rc != RPTB_OK) {
+        const std::string keep = g_error;
+        buffer_free(b);
+        g_error = keep;
+        return rc;
+    }
+    *out = b;
+    return RPTB_OK;
+}
+
+void rptb_buffer_destroy(rptb_buffer* b) {
+    if (b) buffer_free(b);
+}
+
+int rptb_sample_into(rptb_scene* s, const rptb_camera* cam, const rptb_render_params* p, rptb_buffer* b, rptb_stats* stats) {
+    if (!b) return fail(RPTB_ERR_BAD_ARG, "null argument");
+    int rc = check_params(s, cam, p);
+    if (rc != RPTB_OK) return rc;
+    if (p->shard_count > 1)
+        return fail(RPTB_ERR_UNSUPPORTED, "shard_count %u: a buffer holds the whole image (shard with rptb_render_samples_device)", p->shard_count);
+    if (p->width != b->width || p->height != b->height)
+        return fail(RPTB_ERR_BAD_ARG, "render is %ux%u but the buffer is %ux%u", p->width, p->height, b->width, b->height);
+    const uint32_t nparts = 1u + (uint32_t)s->peers.size();
+    bool same = nparts == b->parts.size();
+    for (uint32_t i = 0; same && i < nparts; i++) same = (i == 0 ? s->device : s->peers[i - 1]->device) == b->parts[i].device;
+    if (!same) return fail(RPTB_ERR_BAD_ARG, "the buffer was created on a scene with another device list");
+    std::lock_guard<std::mutex> bl(b->lock);
+    if (b->entries == UINT32_MAX) return fail(RPTB_ERR_UNSUPPORTED, "too many entries");
+    const uint32_t n = b->entries + 1;
+    // every replica's share is enqueued before any is waited for, so the devices run concurrently
+    std::vector<std::unique_lock<std::mutex>> locks;
+    std::vector<uint32_t> launches(nparts, 0);
+    for (uint32_t i = 0; i < nparts; i++) {
+        rptb_scene* r = i == 0 ? s : s->peers[i - 1];
+        locks.emplace_back(r->lock);
+        rc = sample_part(r, cam, p, i, nparts, n, b->parts[i], stats != nullptr, &launches[i]);
+        if (rc != RPTB_OK) return nparts > 1 ? fail(rc, "device %d: %s", r->device, g_error.c_str()) : rc;
+    }
+    b->entries = n;
+    if (!stats) return RPTB_OK;
+    std::memset(stats, 0, sizeof(*stats));
+    for (uint32_t i = 0; i < nparts; i++) {
+        rptb_scene* r = i == 0 ? s : s->peers[i - 1];
+        DeviceGuard g(r->device);
+        DeviceCounters c;
+        CU(cudaMemcpyAsync(&c, r->counters, sizeof(c), cudaMemcpyDeviceToHost, r->stream));
+        CU(cudaStreamSynchronize(r->stream));
+        r->busy_pending = false;
+        rptb_stats st;
+        std::memset(&st, 0, sizeof(st));
+        read_stats(c, &st);
+        float ms = 0;
+        CU(cudaEventElapsedTime(&ms, r->ev0, r->ev1));
+        stats->segments += st.segments; stats->rays += st.rays;
+        stats->node_visits += st.node_visits; stats->tri_tests += st.tri_tests;
+        stats->mesh_hits += st.mesh_hits; stats->env_lookups += st.env_lookups;
+        stats->object_tests += st.object_tests;
+        stats->bvh_node_visits += st.bvh_node_visits; stats->bvh_tri_tests += st.bvh_tri_tests;
+        stats->gpu_ms = std::max(stats->gpu_ms, (double)ms);  // the devices run concurrently
+        stats->launches += launches[i];
+    }
+    stats->engine = use_wavefront(s, p) ? RPTB_ENGINE_WAVEFRONT : RPTB_ENGINE_MEGAKERNEL;
+    return RPTB_OK;
+}
+
+int rptb_buffer_add_samples(rptb_buffer* b, const double* rgb) {
+    if (!b || !rgb) return fail(RPTB_ERR_BAD_ARG, "null argument");
+    std::lock_guard<std::mutex> bl(b->lock);
+    if (b->entries == UINT32_MAX) return fail(RPTB_ERR_UNSUPPORTED, "too many entries");
+    const uint32_t n = b->entries + 1, nparts = (uint32_t)b->parts.size();
+    const size_t nvals = (size_t)b->width * b->height * 3;
+    for (uint32_t i = 0; i < nparts; i++) {
+        BufferPart& q = b->parts[i];
+        DeviceGuard g(q.device);
+        if (!g.ok) return fail(RPTB_ERR_CUDA, "cudaSetDevice(%d) failed", q.device);
+        if (!q.upload) CU(cudaMalloc((void**)&q.upload, nvals * sizeof(double)));
+        CU(cudaStreamWaitEvent(q.stream, q.done, 0));
+        // pageable source: the call returns once the bytes are staged, `rgb` may be reused afterwards
+        CU(cudaMemcpyAsync(q.upload, rgb, nvals * sizeof(double), cudaMemcpyHostToDevice, q.stream));
+        CU(launch_buffer_accumulate(nullptr, q.upload, true, n, (uint64_t)q.tiles * 128u, b->width, b->height, i, nparts,
+                                    q.sums, q.m2, q.stream));
+        CU(cudaEventRecord(q.done, q.stream));
+    }
+    b->entries = n;
+    return RPTB_OK;
+}
+
+int rptb_buffer_image(rptb_buffer* b, uint8_t* out_rgb8) {
+    if (!b || !out_rgb8) return fail(RPTB_ERR_BAD_ARG, "null argument");
+    std::lock_guard<std::mutex> bl(b->lock);
+    if (b->entries == 0) return fail(RPTB_ERR_BAD_ARG, "Pixel found with no samples");  // buffer.rs:89
+    BufferPart& q0 = b->parts[0];
+    DeviceGuard g(q0.device);
+    int rc = buffer_gather(b, true, false);
+    if (rc != RPTB_OK) return rc;
+    const size_t nvals = (size_t)b->width * b->height * 3;
+    CU(launch_film_resolve(b->row_sums, b->entries, b->width, b->height, b->radius, b->rgb8, q0.stream));
+    CU(cudaMemcpyAsync(out_rgb8, b->rgb8, nvals, cudaMemcpyDeviceToHost, q0.stream));
+    CU(cudaStreamSynchronize(q0.stream));
+    return RPTB_OK;
+}
+
+int rptb_buffer_variance(rptb_buffer* b, double* out) {
+    if (!b || !out) return fail(RPTB_ERR_BAD_ARG, "null argument");
+    std::lock_guard<std::mutex> bl(b->lock);
+    if (b->entries < 2) {  // n - 1 = 0: the reference divides by it
+        *out = NAN;
+        return RPTB_OK;
+    }
+    BufferPart& q0 = b->parts[0];
+    DeviceGuard g(q0.device);
+    int rc = buffer_gather(b, false, true);
+    if (rc != RPTB_OK) return rc;
+    const uint64_t npix = (uint64_t)b->width * b->height;
+    double* total = b->partial + buffer_variance_blocks(npix);
+    CU(launch_buffer_variance(b->row_m2, npix, b->entries, b->partial, total, q0.stream));
+    double sum = 0.0;
+    CU(cudaMemcpyAsync(&sum, total, sizeof(double), cudaMemcpyDeviceToHost, q0.stream));
+    CU(cudaStreamSynchronize(q0.stream));
+    *out = sum / (double)npix;
+    return RPTB_OK;
+}
+
+int rptb_buffer_sums(rptb_buffer* b, double* out_sums, uint32_t* out_entries) {
+    if (!b || !out_sums) return fail(RPTB_ERR_BAD_ARG, "null argument");
+    std::lock_guard<std::mutex> bl(b->lock);
+    BufferPart& q0 = b->parts[0];
+    DeviceGuard g(q0.device);
+    int rc = buffer_gather(b, true, false);
+    if (rc != RPTB_OK) return rc;
+    CU(cudaMemcpyAsync(out_sums, b->row_sums, (size_t)b->width * b->height * 3 * sizeof(double), cudaMemcpyDeviceToHost, q0.stream));
+    CU(cudaStreamSynchronize(q0.stream));
+    if (out_entries) *out_entries = b->entries;
     return RPTB_OK;
 }
 

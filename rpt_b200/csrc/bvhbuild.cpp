@@ -158,8 +158,11 @@ std::unique_ptr<Node> build(std::vector<Prim>& prims, uint32_t first, uint32_t c
 // Round a box outward and pad it: the f32 triangle test works on o + t d evaluated in float, which can
 // land a few ulps outside the exact triangle, and the slab test evaluates (b - o)/d as b*(1/d) - o*(1/d), whose
 // rounding error is ~6e-8 |o| in space whatever the box.  The pad therefore scales with the larger of the box's own
-// coordinate and the MESH's extent (g_root_mag, set per build): it covers ray origins out to ~60 mesh extents from
-// the local origin on every box, including boxes that hug a coordinate plane (where |b| alone would give no pad).
+// coordinate and the MESH's extent (g_root_mag, set per build), including boxes that hug a coordinate plane (where
+// |b| alone would give no pad).  Measured against a scan of every triangle (tests/test_hostemu_placement.py): the BVH
+// returns every hit well inside a triangle from ray origins up to 1e3 mesh extents away.  At 1e5 extents, where t itself
+// is resolved to ~1 % of the mesh, 0.8 % of those hits differ -- the same with a pad 100x smaller, so there it is the
+// rounding of t, not the boxes, that decides.
 float g_root_mag = 0.0f;
 #pragma omp threadprivate(g_root_mag)
 void pad(const Box& b, float* lo, float* hi) {

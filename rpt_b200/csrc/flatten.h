@@ -457,6 +457,47 @@ void fill_tables(const rptb_scene_desc* d, Tables<R>& t) {
     }
 }
 
+// ObjectRec::err_mag.  A hit is computed on object-space coordinates (M^-1 o, the tri48 plane word pn . v1, q0.w - pn . o),
+// which round relative to the object's own extent, and the rounding reaches world space through the transform's linear
+// part L.  So the f32 path's restart offset (offset_origin) is sized from max(|world coordinates|, err_mag) with
+// err_mag = ||L||_inf * (largest |coordinate| of the object's bounds in its own space) / 8: offset_origin's 32 ulp of it are
+// 4 ulp of the object-space magnitude, what the chain M^-1 o, pn . o, q0.w - pn . o and the plane word rounds
+// (tests/test_hostemu_placement.py measures the choice).  A mesh whose vertices sit far
+// from its local origin and are pulled back by its transform (scanned, CAD and georeferenced files) has world
+// coordinates ~1 but object-space ones ~1e4: the world term alone leaves its restarted rays re-hitting their own face.
+// Without a transform the object-space coordinates are the world ones: 0.  A kd-tree of shapes: its children's terms.
+inline double object_err_mag(const rptb_scene_desc* d, const rptb_object& o, const std::vector<HostMesh>& meshes,
+                             const std::vector<HostGroup>& groups) {
+    double mag = 0.0, inner = 0.0;
+    switch (o.kind) {
+        case RPTB_SHAPE_SPHERE: mag = 1.0; break;
+        case RPTB_SHAPE_CUBE: mag = 0.5; break;
+        case RPTB_SHAPE_MONOMIAL: mag = std::fmax(1.0, std::fabs(o.monomial_height)); break;
+        case RPTB_SHAPE_PLANE: {
+            const double len = std::sqrt(o.plane_normal[0] * o.plane_normal[0] + o.plane_normal[1] * o.plane_normal[1] +
+                                         o.plane_normal[2] * o.plane_normal[2]);
+            mag = len > 0.0 ? std::fabs(o.plane_value) / len : 0.0;
+            break;
+        }
+        case RPTB_SHAPE_MESH:
+            for (int a = 0; a < 3; a++) mag = std::fmax(mag, std::fmax(std::fabs(meshes[o.mesh].bmin[a]), std::fabs(meshes[o.mesh].bmax[a])));
+            break;
+        case RPTB_SHAPE_GROUP: {
+            const HostGroup& g = groups[o.mesh];
+            for (int a = 0; a < 3; a++) mag = std::fmax(mag, std::fmax(std::fabs(g.bmin[a]), std::fabs(g.bmax[a])));
+            const rptb_group& dg = d->groups[o.mesh];
+            for (uint64_t i = 0; i < dg.nchildren; i++) inner = std::fmax(inner, object_err_mag(d, dg.children[i], meshes, groups));
+            break;
+        }
+        default: break;
+    }
+    if (!o.has_transform) return inner;
+    double norm = 0.0;  // ||L||_inf: the largest absolute row sum of the linear part
+    for (int r = 0; r < 3; r++)
+        norm = std::fmax(norm, std::fabs(o.transform[r]) + std::fabs(o.transform[4 + r]) + std::fabs(o.transform[8 + r]));
+    return norm * std::fmax(mag, inner) / 8.0;
+}
+
 // f32 bounds must contain what f32 arithmetic makes of the contents: widen by one ulp outward
 inline void widen_bounds(const double* lo, const double* hi, float* flo, float* fhi) {
     for (int k = 0; k < 3; k++) {
@@ -637,6 +678,7 @@ inline int flatten_scene(const rptb_scene_desc* d, HostScene& hs, std::string& e
         a.root_is_leaf = b.root_is_leaf = (hg.nodes32[0].word & 3u) == 3u;
         for (uint64_t c = 0; c < d->groups[i].nchildren; c++) has_mono |= d->groups[i].children[c].kind == RPTB_SHAPE_MONOMIAL;
     }
+    for (uint32_t i = 0; i < d->nobjects; i++) hs.t32.objects[i].err_mag = (float)object_err_mag(d, d->objects[i], hs.meshes, hs.groups);
     for (uint32_t i = 0; i < d->nobjects; i++) has_mono |= d->objects[i].kind == RPTB_SHAPE_MONOMIAL;
     for (uint32_t i = 0; i < d->nlights; i++)
         if (d->lights[i].kind == RPTB_LIGHT_OBJECT) has_mono |= d->lights[i].object.kind == RPTB_SHAPE_MONOMIAL;

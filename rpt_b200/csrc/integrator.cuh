@@ -407,7 +407,8 @@ RPTB_D void render_thread(const SceneView<R>& sv, const RenderArgs<R>& a, const 
                     wo = -M<R>::normalize(rd);
                     mat_id = ob.material;
                     const MaterialRec<R> mat = sv.materials[mat_id];
-                    err_scale = M<R>::literal ? (R)0 : M<R>::max(max_abs3(pos), max_abs3(ro));
+                    // the world coordinates involved, and the object-space ones mapped to world (ObjectRec::err_mag)
+                    err_scale = M<R>::literal ? (R)0 : M<R>::max(M<R>::max(max_abs3(pos), max_abs3(ro)), ob.err_mag);
                     color = mat.emittance * mat_color(mat);
                     // opaque surface seen from its back: bsdf == 0 for every wi (material.rs:130-133),
                     // so neither the lights nor the bounce can contribute (f32 only; f64 stays literal)

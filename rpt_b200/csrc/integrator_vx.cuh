@@ -410,7 +410,7 @@ RPTB_D void render_thread_vx(const SceneView<float>& sv, const RenderArgs<float>
                 wo = -M<R>::normalize(rd);
                 mat_id = ob.material;
                 const MaterialRec<R> mat = sv.materials[mat_id];
-                err_scale = M<R>::max(max_abs3(pos), max_abs3(ro));
+                err_scale = M<R>::max(M<R>::max(max_abs3(pos), max_abs3(ro)), ob.err_mag);
                 color = mat.emittance * mat_color(mat);
                 // opaque surface seen from its back: bsdf == 0 for every wi (material.rs:130-133)
                 dead = !mat.transparent && M<R>::signbit(dot(n, wo));

@@ -162,7 +162,7 @@ struct ObjectRec {
     R plane_n[3];     // PLANE: normal.  MONOMIAL: plane_n[0] = exp
     R plane_v;        // PLANE: value.   MONOMIAL: height
     R plane_unit[3];  // normalize(plane normal), precomputed
-    R _pad;
+    R err_mag;  // f32: world size of the rounding of the object-space arithmetic (flatten.h, object_err_mag); 0 in f64
 };
 
 // KdTree<Box<dyn Bounded>> (src/kdtree.rs:99-104 over shapes): the tree's refs index `children`, each a

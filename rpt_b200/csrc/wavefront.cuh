@@ -307,7 +307,7 @@ __global__ void __launch_bounds__(WF_THREADS) wf_shade_kernel(const SceneView<fl
         const Vec3<R> n = sf.n, ng = sf.ng;
         const Vec3<R> wo = -M<R>::normalize(rd);
         const MaterialRec<R> mat = sv.materials[ob.material];
-        const R err_scale = M<R>::max(max_abs3(pos), max_abs3(ro));
+        const R err_scale = M<R>::max(M<R>::max(max_abs3(pos), max_abs3(ro)), ob.err_mag);
         color = mat.emittance * mat_color(mat);
         const bool dead = !mat.transparent && M<R>::signbit(dot(n, wo));
         rng.ensure();

@@ -61,6 +61,9 @@ class Case:
     ev: float = 0.0
     env: Dict[str, str] = field(default_factory=dict)
     wavefront: bool = False        # also rendered through ENGINE_WAVEFRONT on the GPU (kd-tree scenes)
+    base: str = ""                 # PLACEMENTS: the case whose world geometry this one shares ("" = none)
+    degrades: bool = False         # PLACEMENTS: f32 agreement below the base's by design, or the oracle's own image moves
+    base_slack: float = 0.0        # PLACEMENTS: measured shortfall of the f32 agreement below the base's floor
 
 
 @contextlib.contextmanager
@@ -258,4 +261,154 @@ CASES: Dict[str, Case] = {
     "lights_lens": Case(_lights, 37, 23, 20, 3, A, F_FLAT, 0.999, 0.999),
     "smooth_kd": Case(_smooth(False), 32, 32, 16, 3, K, F_TREE, 0.999, 0.999, wavefront=True),
     "smooth_glass_bvh": Case(_smooth(True), 32, 32, 16, 4, B, F_ALL | F_BVH, 0.995, 0.995),
+}
+
+
+# ------------------------------------------------------------------------------------------------ placements ------
+# The same world geometry placed where the f32 path's magnitude-dependent rules are stretched: meshes whose vertices
+# sit far from their own origin and are pulled back by the object's transform (scanned, CAD and georeferenced files
+# arrive like this), scenes scaled by 1e-3 and 1e3, a small instance seen from far away, a scene far from the world
+# origin.  Each case either has its base's world geometry exactly, or is its base scaled uniformly with the point
+# lights' intensities times s^2, so that the oracle's image is the base's.
+def moved(make, m: np.ndarray, s: float = 1.0):
+    """make() with every shape, point light and the camera mapped by the 4x4 similarity m of uniform scale s."""
+    def moved_make():
+        scene, cam = make()
+        seen = set()
+        for o in list(scene.objects) + [l.object for l in scene.lights if l.object is not None]:
+            if id(o) not in seen:
+                seen.add(id(o))
+                o.shape = o.shape.transform(m)
+        for l in scene.lights:
+            if l.kind == capi.LIGHT_POINT:
+                l.vec = (m @ np.append(l.vec, 1.0))[:3]
+                l.color = l.color * s * s
+        cam.eye = (m @ np.append(cam.eye, 1.0))[:3]
+        cam.focal_distance *= s
+        cam.aperture *= s
+        return scene, cam
+    return moved_make
+
+
+def _translation(v) -> np.ndarray:
+    m = np.eye(4)
+    m[:3, 3] = v
+    return m
+
+
+def _teapot_at(d: float, group: bool = False):
+    """A specular teapot on a diffuse floor under a point light, its vertices shifted by d along x in object space and
+    pulled back by translate(-d) (d = 0: the unshifted mesh, no extra transform).  group: the teapot is the one child
+    of a kd-tree of shapes."""
+    def make():
+        tris = scenes.teapot_triangles().copy()
+        tris[:, 0:9:3] += d
+        mesh = api.Mesh(tris)
+        shape = (mesh.translate(api.vec3(-d, 0.0, 0.0)) if d else mesh).scale(api.vec3(0.5, 0.5, 0.5)).translate(api.vec3(0.0, -1.0, 0.0))
+        scene = api.Scene()
+        scene.add(api.Object(api.KdTree([shape]) if group else shape).material(api.Material.specular(api.hex_color(0xCC4422), 0.3)))
+        scene.add(api.Object(api.plane(api.vec3(0, 1, 0), -1.0)).material(api.Material.diffuse(api.hex_color(0xAAAAAA))))
+        scene.add(api.Light.Ambient(api.vec3(0.02, 0.02, 0.02)))
+        scene.add(api.Light.Point(api.vec3(60.0, 60.0, 60.0), api.vec3(0.0, 5.0, 5.0)))
+        return scene, api.Camera.default()
+    return make
+
+
+def _quad_plane_at(d: float):
+    """A diffuse floor quad (two triangles, one leaf) whose vertices sit at d along x and z in object space, and a back
+    wall plane(n, -2 + d) translated back by -d n; a red ball and a point light: the packed primitive table's mesh and
+    plane records with large object-space coordinates."""
+    def make():
+        v = [api.vec3(-3 + d, -1, -3 + d), api.vec3(-3 + d, -1, 3 + d), api.vec3(3 + d, -1, 3 + d), api.vec3(3 + d, -1, -3 + d)]
+        quad = api.polygon(v)
+        scene = api.Scene()
+        scene.add(api.Object(quad.translate(api.vec3(-d, 0.0, -d)) if d else quad).material(api.Material.diffuse(api.hex_color(0xAAAAAA))))
+        wall = api.plane(api.vec3(0, 0, 1), -2.0 + d)
+        scene.add(api.Object(wall.translate(api.vec3(0, 0, -d)) if d else wall).material(api.Material.diffuse(api.hex_color(0x88AACC))))
+        scene.add(api.Object(api.sphere().scale(api.vec3(0.7, 0.7, 0.7)).translate(api.vec3(0.3, -0.3, 0.0)))
+                  .material(api.Material.specular(api.hex_color(0xCC3333), 0.2)))
+        scene.add(api.Light.Point(api.vec3(40.0, 40.0, 40.0), api.vec3(-2.0, 4.0, 4.0)))
+        return scene, api.Camera.look_at(api.vec3(0, 1.5, 6), api.vec3(0, -0.3, 0), api.vec3(0, 1, 0), 0.8)
+    return make
+
+
+def _far_instance(shape: str, far: float):
+    """A teapot or a sphere of size ~1e-2 at the origin on a floor, seen from `far` through a field of view narrowed to
+    match: object-space ray origins lie 1e4 - 1e5 extents from the object."""
+    def make():
+        k = 1e-2
+        if shape == "teapot":
+            obj = api.Mesh(scenes.teapot_triangles()).scale(api.vec3(0.5 * k, 0.5 * k, 0.5 * k))
+        else:
+            obj = api.sphere().scale(api.vec3(0.8 * k, 0.8 * k, 0.8 * k))
+        scene = api.Scene()
+        scene.add(api.Object(obj).material(api.Material.specular(api.hex_color(0x3366CC), 0.2)))
+        scene.add(api.Object(api.plane(api.vec3(0, 1, 0), -0.8 * k)).material(api.Material.diffuse(api.hex_color(0xAAAAAA))))
+        scene.add(api.Light.Point(api.vec3(40.0, 40.0, 40.0) * k * k, api.vec3(-2.0, 4.0, 4.0) * k))
+        return scene, api.Camera.look_at(api.vec3(0, 0.3 * far, far), api.vec3(0, 0, 0), api.vec3(0, 1, 0), 3.0 * k / far)
+    return make
+
+
+def _scaled(make, s):
+    return make if s == 1.0 else moved(make, np.diag([s, s, s, 1.0]), s)
+
+
+_TEAPOT = dict(w=32, h=32, spp=16, max_bounces=3)
+_SMALL = dict(w=32, h=32, spp=16)
+_D = (("1e2", 1e2), ("1e3", 1e3), ("1e4", 1e4))
+# off-center teapot: (floor, slack below the base's floor) per shift; 1e4 is the measured limit (test_hostemu_placement.py)
+_OFF = {"1e2": (0.999, 0.0), "1e3": (0.998, 0.0), "1e4": (0.982, 0.014)}
+
+
+def _teapots(prefix, accel, feat, group, shifts, **kw):
+    out = {prefix + "_0": Case(_teapot_at(0.0, group), **_TEAPOT, accel=accel, feat=feat, floor=0.999, gpu_floor=0.998, **kw)}
+    for t, d in shifts:
+        fl, slack = _OFF[t]
+        out["%s_%s" % (prefix, t)] = Case(_teapot_at(d, group), **_TEAPOT, accel=accel, feat=feat, floor=fl, gpu_floor=fl - 0.002,
+                                          base=prefix + "_0", base_slack=slack, **kw)
+    return out
+
+
+def _far(shp, t, far, s, floor, bias):
+    return Case(_scaled(_far_instance(shp, far), s), **_SMALL, max_bounces=3, accel=(B if shp == "teapot" else A),
+                feat=(F_TREE | F_BVH if shp == "teapot" else F_FLAT | F_SMALL), floor=floor, gpu_floor=floor - 0.02, bias=bias,
+                base="" if s != 1.0 else "far_%s_%s_x100" % (shp, t), degrades=True)
+
+
+PLACEMENTS: Dict[str, Case] = {
+    # name: Case(scene, width, height, spp, max_bounces, accel, FEAT, floor, gpu_floor, ..., base=)
+    # off-center meshes: the world geometry of the *_0 case, vertices at 1e2 .. 1e4 in object space
+    **_teapots("teapot_kd", K, F_TREE, False, _D, wavefront=True),
+    **_teapots("teapot_bvh", B, F_TREE | F_BVH, False, _D),
+    **_teapots("teapot_group", K, F_EVERY, True, _D),
+    **_teapots("teapot_group_bvh", B, F_EVERY | F_BVH, True, _D),
+    # the packed table's one-leaf mesh and plane, coordinates at 1e4 in object space
+    "quad_plane_0": Case(_quad_plane_at(0.0), **_SMALL, max_bounces=3, accel=A, feat=F_FLAT | F_SMALL, floor=0.999, gpu_floor=0.998),
+    "quad_plane_1e4": Case(_quad_plane_at(1e4), **_SMALL, max_bounces=3, accel=A, feat=F_FLAT | F_SMALL, floor=0.976, gpu_floor=0.974,
+                           bias=4e-5, base="quad_plane_0", base_slack=0.02),
+    # uniform scale, camera included (point lights x s^2); at s = 1e3 the oracle's own image moves (F64_FLOOR)
+    "cornell_1": Case(_cfg(scenes.cornell_scene), **_SMALL, max_bounces=6, accel=A, feat=F_FLAT, floor=0.982, gpu_floor=0.980),
+    "cornell_s1e-3": Case(_scaled(_cfg(scenes.cornell_scene), 1e-3), **_SMALL, max_bounces=6, accel=A, feat=F_FLAT, floor=0.998,
+                          gpu_floor=0.996, base="cornell_1"),
+    "cornell_s1e3": Case(_scaled(_cfg(scenes.cornell_scene), 1e3), **_SMALL, max_bounces=6, accel=A, feat=F_FLAT, floor=0.775,
+                         gpu_floor=0.765, base="cornell_1", degrades=True),
+    "glass_1": Case(_cfg(lambda: scenes.glass_scene(64, 32)), **_SMALL, max_bounces=12, accel=A, feat=F_TRANSP | F_HDRI | F_SMALL,
+                    floor=0.974, gpu_floor=0.972),
+    "glass_s1e-3": Case(_scaled(_cfg(lambda: scenes.glass_scene(64, 32)), 1e-3), **_SMALL, max_bounces=12, accel=A,
+                        feat=F_TRANSP | F_HDRI | F_SMALL, floor=0.974, gpu_floor=0.972, base="glass_1"),
+    "glass_s1e3": Case(_scaled(_cfg(lambda: scenes.glass_scene(64, 32)), 1e3), **_SMALL, max_bounces=12, accel=A,
+                       feat=F_TRANSP | F_HDRI | F_SMALL, floor=0.889, gpu_floor=0.88, base="glass_1", degrades=True),
+    # a small instance (1e-2) seen from 1e2 and 1e3 world units; its base is the same view scaled by 1e2 (the instance of
+    # size ~1 seen from 1e4 and 1e5), which puts the object-space origins as far out but moves the absolute thresholds
+    "far_teapot_1e2": _far("teapot", "1e2", 1e2, 1.0, 0.821, 1e-4),
+    "far_teapot_1e2_x100": _far("teapot", "1e2", 1e2, 1e2, 0.785, 1e-4),
+    "far_teapot_1e3": _far("teapot", "1e3", 1e3, 1.0, 0.341, 3e-4),
+    "far_teapot_1e3_x100": _far("teapot", "1e3", 1e3, 1e2, 0.370, 3e-4),
+    "far_sphere_1e2": _far("sphere", "1e2", 1e2, 1.0, 0.822, 1e-4),
+    "far_sphere_1e2_x100": _far("sphere", "1e2", 1e2, 1e2, 0.824, 1e-4),
+    "far_sphere_1e3": _far("sphere", "1e3", 1e3, 1.0, 0.294, 3e-4),
+    "far_sphere_1e3_x100": _far("sphere", "1e3", 1e3, 1e2, 0.341, 3e-4),
+    # far from the world origin: the f32 offset is 32 ulp of 1e4 there, 0.03 units, and agreement drops by design
+    "cornell_far": Case(moved(_cfg(scenes.cornell_scene), _translation((1e4, 0.0, 0.0))), **_SMALL, max_bounces=6, accel=A,
+                        feat=F_FLAT, floor=0.921, gpu_floor=0.91, bias=2e-5, base="cornell_1", degrades=True),
 }

@@ -28,6 +28,10 @@ $(OBJDIR)/kernels_vx.o: $(CSRC)/kernels_vx.cu $(HDRS)
 $(OBJDIR)/kernels_f64.o: $(CSRC)/kernels_f64.cu $(HDRS)
 	@mkdir -p $(OBJDIR)
 	$(NVCC) $(NVFLAGS) -fmad=false -c $< -o $@ 2> $(OBJDIR)/kernels_f64.ptxas.log || (cat $(OBJDIR)/kernels_f64.ptxas.log; false)
+# the adaptive criterion (adaptive.h) rounds every operation on its own, like its numpy and host-emulation restatements
+$(OBJDIR)/adaptive.o: $(CSRC)/adaptive.cu $(HDRS)
+	@mkdir -p $(OBJDIR)
+	$(NVCC) $(NVFLAGS) -fmad=false -c $< -o $@ 2> $(OBJDIR)/adaptive.ptxas.log || (cat $(OBJDIR)/adaptive.ptxas.log; false)
 $(OBJDIR)/film.o: $(CSRC)/film.cu $(HDRS)
 	@mkdir -p $(OBJDIR)
 	$(NVCC) $(NVFLAGS) -c $< -o $@ 2> $(OBJDIR)/film.ptxas.log || (cat $(OBJDIR)/film.ptxas.log; false)
@@ -44,7 +48,7 @@ $(OBJDIR)/objparse.o: $(CSRC)/objparse.cpp
 	@mkdir -p $(OBJDIR)
 	$(CXX) -std=c++17 -O3 -fPIC -Wall -c $< -o $@
 
-$(LIB): $(OBJDIR)/kernels_f32.o $(OBJDIR)/kernels_vx.o $(OBJDIR)/kernels_f64.o $(OBJDIR)/film.o $(OBJDIR)/api.o $(OBJDIR)/kdbuild.o $(OBJDIR)/bvhbuild.o $(OBJDIR)/objparse.o
+$(LIB): $(OBJDIR)/kernels_f32.o $(OBJDIR)/kernels_vx.o $(OBJDIR)/kernels_f64.o $(OBJDIR)/film.o $(OBJDIR)/adaptive.o $(OBJDIR)/api.o $(OBJDIR)/kdbuild.o $(OBJDIR)/bvhbuild.o $(OBJDIR)/objparse.o
 	@mkdir -p rpt_b200/lib
 	$(NVCC) -shared $(ARCH) -o $@ $^ -Xcompiler -fopenmp -lgomp -cudart shared
 
@@ -63,10 +67,15 @@ build/%_cpp: examples/%.cpp include/rpt.hpp include/rpt_b200.h $(LIB)
 # library is loaded next to librpt_b200.so (RTLD_GLOBAL), whose copies of the inline flatteners were compiled with other
 # switches (RPTB_BUILD_BVH8) -- hostemu must call its own
 HOSTEMU := tests/hostemu/_build/libhostemu.so
-hostemu: $(HOSTEMU)
+# the same emulation plus adaptive sampling's list-scheduled megakernel and convergence test (tests/hostemu/hostemu_list.cu)
+HOSTEMU_LIST := tests/hostemu/_build/libhostemu_list.so
+hostemu: $(HOSTEMU) $(HOSTEMU_LIST)
 $(HOSTEMU): tests/hostemu/hostemu.cu $(CSRC)/kdbuild.cpp $(CSRC)/bvhbuild.cpp $(HDRS)
 	@mkdir -p $(dir $@)
 	nvcc -std=c++17 -O2 -DRPTB_HOST_EMU -DRPTB_BUILD_BVH8=1 -DRPTB_BUILD_BVH4=1 -gencode arch=compute_90a,code=sm_90a -Xcompiler -fPIC,-fopenmp,-ffp-contract=off -shared -Xlinker -Bsymbolic -o $@ tests/hostemu/hostemu.cu $(CSRC)/kdbuild.cpp $(CSRC)/bvhbuild.cpp -lgomp
+$(HOSTEMU_LIST): tests/hostemu/hostemu_list.cu tests/hostemu/hostemu.cu $(CSRC)/kdbuild.cpp $(CSRC)/bvhbuild.cpp $(HDRS)
+	@mkdir -p $(dir $@)
+	nvcc -std=c++17 -O2 -DRPTB_HOST_EMU -DRPTB_BUILD_BVH8=1 -DRPTB_BUILD_BVH4=1 -gencode arch=compute_90a,code=sm_90a -Xcompiler -fPIC,-fopenmp,-ffp-contract=off -shared -Xlinker -Bsymbolic -o $@ tests/hostemu/hostemu_list.cu $(CSRC)/kdbuild.cpp $(CSRC)/bvhbuild.cpp -lgomp
 
 clean:
 	rm -rf build $(LIB) $(ORACLE) tests/hostemu/_build

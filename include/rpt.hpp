@@ -288,6 +288,22 @@ public:
         check(rptb_buffer_sums(handle_, out.data(), nullptr));
         return out;
     }
+    // Per pixel, row-major: sums (3 per pixel), M2 summed over the channels, entry counts (rptb_buffer_pixel_stats).
+    struct PixelStats {
+        std::vector<double> sums, m2;
+        std::vector<uint32_t> counts;
+    };
+    PixelStats pixel_stats() const {
+        const size_t n = (size_t)width_ * height_;
+        PixelStats s{std::vector<double>(n * 3), std::vector<double>(n), std::vector<uint32_t>(n)};
+        check(rptb_buffer_pixel_stats(handle_, s.sums.data(), s.m2.data(), s.counts.data()));
+        return s;
+    }
+    std::vector<uint32_t> counts() const {  // entries per pixel, row-major
+        std::vector<uint32_t> out((size_t)width_ * height_);
+        check(rptb_buffer_pixel_stats(handle_, nullptr, nullptr, out.data()));
+        return out;
+    }
     rptb_buffer* handle() const { return handle_; }
 
 private:
@@ -357,6 +373,30 @@ public:
             const uint32_t steps = std::min(num_samples_ - iteration, interval);
             sample(steps, buffer);
             iteration += steps;
+            cb(iteration, buffer);
+        }
+    }
+    // Adaptive sampling (rptb_sample_into_adaptive): the entry goes only to the pixels `criterion` leaves active.
+    // Returns how many pixels got it (which waits for the call).
+    uint64_t sample(uint32_t iterations, DeviceBuffer& buffer, const rptb_adaptive& criterion) {
+        ensure_scene();
+        const rptb_render_params p = params(iterations);
+        const rptb_camera c = camera();
+        uint64_t active = 0;
+        if (rptb_sample_into_adaptive(handle_, &c, &p, &criterion, buffer.handle(), &active, nullptr) != RPTB_OK)
+            throw std::runtime_error(rptb_last_error());
+        next_sample_ += iterations;
+        return active;
+    }
+    // The same loop with every batch adaptive; it stops early after a batch that rendered no pixel.
+    void iterative_render(uint32_t interval, DeviceBuffer& buffer, const rptb_adaptive& criterion,
+                          const std::function<void(uint32_t, const DeviceBuffer&)>& cb) {
+        uint32_t iteration = 0;
+        while (iteration < num_samples_) {
+            const uint32_t steps = std::min(num_samples_ - iteration, interval);
+            const uint64_t active = sample(steps, buffer, criterion);
+            iteration += steps;
+            if (active == 0) break;
             cb(iteration, buffer);
         }
     }

@@ -413,8 +413,45 @@ int rptb_buffer_image(rptb_buffer* buffer, uint8_t* out_rgb8);
 /* Replaces: Buffer::variance (src/buffer.rs:59-73): the mean over pixels of M2 / (entries - 1), reduced in a
  * fixed order.  NaN with fewer than two entries, as in the reference.                                        */
 int rptb_buffer_variance(rptb_buffer* buffer, double* out);
-/* The per-pixel sums (width*height*3 doubles, row-major) and the entry count (out_entries nullable).        */
+/* The per-pixel sums (width*height*3 doubles, row-major) and the entry count (out_entries nullable): the largest
+ * per-pixel count, which is every pixel's count in a buffer that never had an adaptive call.               */
 int rptb_buffer_sums(rptb_buffer* buffer, double* out_sums, uint32_t* out_entries);
+
+/* ---- Adaptive sampling on the device Buffer ---------------------------------------------------------------
+ * The reference's Buffer keeps one list of entries per pixel (src/buffer.rs:24-29), so its pixels may hold
+ * different numbers of entries: image() divides each window's sum by the entries in the window and variance()
+ * each pixel's M2 by its own count - 1 (:59-93).  rptb_sample_into_adaptive adds an entry only to the pixels
+ * that have not converged.  A pixel with n entries, sums S_c and M2 is active iff
+ *     n < min_entries   or   NOT( M2 / ((n-1)*n*3) <= (rel_tol * (S_0+S_1+S_2)/(3n) + abs_tol)^2 ),
+ * evaluated in double with every operation rounded on its own, in the order rpt_b200/csrc/adaptive.h documents:
+ * the channel-mean variance of the pixel's mean against a relative-plus-absolute tolerance.  A NaN statistic
+ * compares false and keeps the pixel active.  The decision is a pure function of the pixel's state, taken
+ * before each render: the first call renders every pixel, a skipped pixel stays skipped under the same
+ * criterion, and a changed criterion simply re-decides.  min_entries must be >= 2 and both tolerances finite
+ * and >= 0 (else RPTB_ERR_BAD_ARG).
+ * Known bias of variance-based stopping: a dark pixel whose first min_entries entries happen to agree stops
+ * early.  min_entries and abs_tol are the guards.                                                            */
+typedef struct rptb_adaptive {
+    double rel_tol;
+    double abs_tol;
+    uint32_t min_entries;
+    uint32_t _pad;
+} rptb_adaptive;
+/* Renders one entry of params->iterations samples for every ACTIVE pixel and adds it to `buffer`; inactive
+ * pixels' sums, M2 and counts do not change.  An active pixel draws exactly the samples rptb_sample_into
+ * would give it (Philox key (seed, pixel, first_sample + i)), so its entry is that call's entry for it.
+ * Argument checks as rptb_sample_into; engine == RPTB_ENGINE_WAVEFRONT is RPTB_ERR_UNSUPPORTED: AUTO and
+ * MEGAKERNEL are the slot megakernel (RPTB_VX is ignored), scheduled over the active 8x4 warp blocks only.
+ * collect_stats 0, 1 and 2 are all supported.  out_active (nullable) receives the number of pixels that got
+ * this entry.  With out_active and stats both NULL the call returns once the work is enqueued.  Once a buffer
+ * has had an adaptive call, rptb_sample_into and rptb_buffer_add_samples keep adding one entry to every pixel
+ * (Buffer::add_samples), on top of each pixel's own count.                                                   */
+int rptb_sample_into_adaptive(rptb_scene* scene, const rptb_camera* camera, const rptb_render_params* params,
+                              const rptb_adaptive* criterion, rptb_buffer* buffer,
+                              uint64_t* out_active /* nullable, forces sync */, rptb_stats* stats /* nullable, forces sync */);
+/* Per-pixel state, row-major, each pointer nullable: sums (width*height*3), M2 (width*height, summed over the
+ * channels) and entry counts (width*height).                                                                 */
+int rptb_buffer_pixel_stats(rptb_buffer* buffer, double* sums, double* m2, uint32_t* counts);
 
 #ifdef __cplusplus
 }

@@ -175,6 +175,16 @@ class Stats(C.Structure):
         return {k: getattr(self, k) for k, _ in self._fields_ if not k.startswith("_")}
 
 
+class Adaptive(C.Structure):
+    """rptb_adaptive: the convergence criterion of rptb_sample_into_adaptive."""
+    _fields_ = [
+        ("rel_tol", C.c_double),
+        ("abs_tol", C.c_double),
+        ("min_entries", C.c_uint32),
+        ("_pad", C.c_uint32),
+    ]
+
+
 class KdTreeOut(C.Structure):
     _fields_ = [
         ("nodes", C.POINTER(KdNode)),
@@ -240,6 +250,10 @@ SYMBOLS = [
     ("rptb_buffer_image", C.c_int, [C.c_void_p, c_u8_p]),
     ("rptb_buffer_variance", C.c_int, [C.c_void_p, c_double_p]),
     ("rptb_buffer_sums", C.c_int, [C.c_void_p, c_double_p, c_u32_p]),
+    ("rptb_sample_into_adaptive", C.c_int,
+     [C.c_void_p, C.POINTER(Camera), C.POINTER(RenderParams), C.POINTER(Adaptive), C.c_void_p, C.POINTER(C.c_uint64),
+      C.POINTER(Stats)]),
+    ("rptb_buffer_pixel_stats", C.c_int, [C.c_void_p, c_double_p, c_double_p, c_u32_p]),
 ]
 
 _lib = None

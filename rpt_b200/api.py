@@ -15,6 +15,7 @@ API, so scene scripts and tests read like the reference's examples:
     Renderer                    src/renderer.rs:18-115
     Buffer / Filter             src/buffer.rs:6-108
     DeviceBuffer                src/buffer.rs:6-93, kept on the GPU (rptb_buffer)
+    Adaptive                    not in the reference: which pixels an adaptive Renderer.sample renders
     hex_color / color_bytes     src/color.rs:10-23
 
 Everything below `Renderer.sample` (src/renderer.rs:117-129) is *not* here:
@@ -832,6 +833,32 @@ class Filter:
         return Filter(radius)
 
 
+class Adaptive:
+    """The convergence criterion of adaptive sampling (rptb_adaptive): Renderer.sample(n, device_buffer, adaptive=...)
+    renders only the pixels that are still active.  A pixel with n entries is active while n < min_entries, or while
+    the channel-mean variance of its mean, M2 / ((n - 1) n 3), exceeds (rel_tol * mean + abs_tol)^2.  Defaults: stop
+    at 2 % relative error of the mean or 1/1000 absolute, and never before 4 entries (the guard against a dark pixel
+    whose first entries happen to agree)."""
+
+    def __init__(self, rel_tol: float = 0.02, abs_tol: float = 1e-3, min_entries: int = 4):
+        self.rel_tol, self.abs_tol, self.min_entries = float(rel_tol), float(abs_tol), int(min_entries)
+
+    def to_c(self) -> capi.Adaptive:
+        return capi.Adaptive(self.rel_tol, self.abs_tol, self.min_entries, 0)
+
+    def active(self, counts, sums, m2) -> np.ndarray:
+        """The criterion in numpy on per-pixel (counts, sums (n, 3), M2): the same operations in the same order as the
+        device (rpt_b200/csrc/adaptive.h), so the same decisions."""
+        n = np.asarray(counts, dtype=np.float64)
+        s = np.asarray(sums, dtype=np.float64).reshape(-1, 3)
+        with np.errstate(divide="ignore", invalid="ignore", over="ignore"):
+            err2 = np.asarray(m2, dtype=np.float64) / (((n - 1.0) * n) * 3.0)
+            m = ((s[:, 0] + s[:, 1]) + s[:, 2]) / (3.0 * n)
+            t = self.rel_tol * m + self.abs_tol
+            converged = err2 <= t * t
+        return (np.asarray(counts) < self.min_entries) | ~converged
+
+
 class Buffer:
     """src/buffer.rs:6-93.  Holds one equally weighted entry per pixel per
     `add_samples` call, like the reference's Vec<Vec<Color>>."""
@@ -883,7 +910,8 @@ class DeviceBuffer:
         self.width, self.height = int(width), int(height)
         self.filter = filter or Filter()
         self.devices = list(scene.devices)
-        self.entries = 0  # entries per pixel: add_samples and Renderer.sample calls
+        self.entries = 0  # entries per pixel: add_samples and Renderer.sample calls; with adaptive calls, the most any pixel has
+        self.counted = False  # an adaptive Renderer.sample happened: pixels may hold different numbers of entries
         self.handle = C.c_void_p()
         capi.check(capi.lib().rptb_buffer_create(scene.handle, self.width, self.height, self.filter.radius,
                                                  C.byref(self.handle)), "rptb_buffer_create")
@@ -901,8 +929,27 @@ class DeviceBuffer:
         n = C.c_uint32(0)
         capi.check(capi.lib().rptb_buffer_sums(self.handle, out.ctypes.data_as(capi.c_double_p), C.byref(n)),
                    "rptb_buffer_sums")
+        if self.counted:
+            self.entries = int(n.value)
         assert n.value == self.entries
         return out
+
+    def pixel_stats(self):
+        """Per pixel, row-major: (sums (width * height, 3), M2 (width * height,) summed over the channels, entry counts
+        (width * height,) uint32)."""
+        npix = self.width * self.height
+        sums, m2, counts = np.empty((npix, 3), np.float64), np.empty(npix, np.float64), np.empty(npix, np.uint32)
+        capi.check(capi.lib().rptb_buffer_pixel_stats(self.handle, sums.ctypes.data_as(capi.c_double_p),
+                                                      m2.ctypes.data_as(capi.c_double_p),
+                                                      counts.ctypes.data_as(capi.c_u32_p)), "rptb_buffer_pixel_stats")
+        return sums, m2, counts
+
+    def counts(self) -> np.ndarray:
+        """(height, width) entries per pixel."""
+        out = np.empty(self.width * self.height, np.uint32)
+        capi.check(capi.lib().rptb_buffer_pixel_stats(self.handle, None, None, out.ctypes.data_as(capi.c_u32_p)),
+                   "rptb_buffer_pixel_stats")
+        return out.reshape(self.height, self.width)
 
     def image(self) -> np.ndarray:
         """:43-56 -> (height, width, 3) uint8."""
@@ -1036,13 +1083,29 @@ class Renderer:
         return DeviceBuffer(self.device_scene(), self._width, self._height, self._filter)
 
     # ---- the seam: Renderer::sample (:117-129) ---------------------------------
-    def sample(self, iterations: int, buffer, collect_stats: int = 0, want_stats: bool = True) -> None:
+    def sample(self, iterations: int, buffer, collect_stats: int = 0, want_stats: bool = True,
+               adaptive: Optional[Adaptive] = None) -> Optional[int]:
         """Adds one entry of `iterations` samples per pixel to `buffer`.  A host Buffer gets the image through
         host memory; a DeviceBuffer gets it on the device, and the call returns once the work is enqueued unless
-        `want_stats` (then last_stats is filled, which waits for the render)."""
+        `want_stats` (then last_stats is filled, which waits for the render).
+        `adaptive` (DeviceBuffer only): add the entry only to the pixels the criterion leaves active
+        (rptb_sample_into_adaptive); returns how many pixels got it, which waits for the call."""
         ds = self.device_scene()
         p = self.params(iterations, self._next_sample, collect_stats=collect_stats)
         cam = self.camera.to_c()
+        if adaptive is not None:
+            if not isinstance(buffer, DeviceBuffer):
+                raise TypeError("adaptive sampling needs a DeviceBuffer (Renderer.device_buffer())")
+            stats, active, crit = capi.Stats(), C.c_uint64(0), adaptive.to_c()
+            capi.check(capi.lib().rptb_sample_into_adaptive(ds.handle, C.byref(cam), C.byref(p), C.byref(crit), buffer.handle,
+                                                            C.byref(active), C.byref(stats) if want_stats else None),
+                       "rptb_sample_into_adaptive")
+            self._next_sample += int(iterations)
+            buffer.counted = True
+            if active.value:  # the largest per-pixel count, as rptb_buffer_sums reports it
+                buffer.entries = int(buffer.counts().max())
+            self.last_stats = stats.as_dict() if want_stats else None
+            return int(active.value)
         if isinstance(buffer, DeviceBuffer):
             stats = capi.Stats()
             capi.check(capi.lib().rptb_sample_into(ds.handle, C.byref(cam), C.byref(p), buffer.handle,
@@ -1068,15 +1131,20 @@ class Renderer:
         return buffer.image()
 
     def iterative_render(self, callback_interval: int, callback: Callable[[int, Buffer], None],
-                         buffer: Optional[DeviceBuffer] = None) -> None:  # :103-115
+                         buffer: Optional[DeviceBuffer] = None, adaptive: Optional[Adaptive] = None) -> None:  # :103-115
         """`buffer`: a DeviceBuffer (Renderer.device_buffer()) to accumulate into on the device; None keeps a
-        host Buffer.  The callback receives whichever it is."""
+        host Buffer.  The callback receives whichever it is.  `adaptive` (needs a DeviceBuffer): every batch renders
+        only the pixels the criterion leaves active, and the render stops early after a batch that rendered none."""
         device = buffer is not None
+        if adaptive is not None and not device:
+            raise TypeError("adaptive sampling needs a DeviceBuffer (Renderer.device_buffer())")
         if buffer is None:
             buffer = Buffer(self._width, self._height, self._filter, self._first_device())
         iteration = 0
         while iteration < self._num_samples:
             steps = min(self._num_samples - iteration, callback_interval)
-            self.sample(steps, buffer, want_stats=not device)
+            active = self.sample(steps, buffer, want_stats=not device, adaptive=adaptive)
             iteration += steps
+            if adaptive is not None and active == 0:
+                break
             callback(iteration, buffer)

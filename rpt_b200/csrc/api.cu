@@ -40,6 +40,23 @@ cudaError_t launch_buffer_scatter(const double* sums, const double* m2, uint64_t
 uint32_t buffer_variance_blocks(uint64_t npixels);
 cudaError_t launch_buffer_variance(const double* m2, uint64_t npixels, uint32_t n, double* partial, double* out_sum,
                                    cudaStream_t stream);
+// per-pixel entry counts (adaptive sampling): film.cu
+cudaError_t launch_buffer_accumulate_counted(const float* in32, const double* in64, bool rowmajor, const uint8_t* mask,
+                                             uint64_t nelem, uint32_t width, uint32_t height, uint32_t shard_index,
+                                             uint32_t shard_count, double* sums, double* m2, uint32_t* counts, cudaStream_t stream);
+cudaError_t launch_buffer_counts_fill(uint32_t* counts, uint64_t nelem, uint32_t value, cudaStream_t stream);
+cudaError_t launch_buffer_scatter_counts(const uint32_t* counts, uint64_t nelem, uint32_t width, uint32_t height,
+                                         uint32_t shard_index, uint32_t shard_count, uint32_t* row_counts, cudaStream_t stream);
+cudaError_t launch_buffer_variance_counted(const double* m2, const uint32_t* counts, uint64_t npixels, double* partial,
+                                           double* out_sum, cudaStream_t stream);
+cudaError_t launch_film_resolve_counted(const double* sums, const uint32_t* counts, uint32_t width, uint32_t height,
+                                        uint32_t radius, uint8_t* out, cudaStream_t stream);
+// the active pixels and warp blocks of an adaptive call: adaptive.cu
+size_t adaptive_temp_bytes(uint32_t tiles);
+cudaError_t launch_adaptive_select(const double* sums, const double* m2, const uint32_t* counts, uint32_t tiles, uint32_t width,
+                                   uint32_t height, uint32_t shard_index, uint32_t shard_count, const rptb_adaptive& crit,
+                                   uint8_t* mask, uint8_t* flags, uint32_t* ids, uint32_t* len, unsigned long long* active_pixels,
+                                   void* temp, size_t temp_bytes, cudaStream_t stream);
 int parse_obj_text(const char* text, size_t len, std::vector<double>& tris, std::string& err);
 struct ObjGroup {
     rptb_material material;
@@ -553,11 +570,23 @@ struct BufferPart {
     double* upload = nullptr;    // a host entry, row-major width*height*3 (first add_samples allocates it)
     cudaStream_t stream = nullptr;
     cudaEvent_t done = nullptr;
+    // from the buffer's first adaptive call on: per-pixel entry counts, and that call's scratch -- the pixel mask
+    // (tiles*128), the flag and the id list of the active 8x4 warp blocks (tiles*4), the list's length, the number of
+    // active pixels, and the select's temporary storage
+    uint32_t* counts = nullptr;
+    uint8_t* mask = nullptr;
+    uint8_t* flags = nullptr;
+    uint32_t* ids = nullptr;
+    uint32_t* len = nullptr;
+    unsigned long long* active = nullptr;
+    void* temp = nullptr;
+    size_t temp_bytes = 0;
 };
 
 struct rptb_buffer {
     uint32_t width = 0, height = 0, radius = 0;
-    uint32_t entries = 0;
+    uint32_t entries = 0;  // accumulate calls; with `counted`, the largest per-pixel count is at most this
+    bool counted = false;  // an adaptive call happened: every part keeps per-pixel counts
     std::vector<BufferPart> parts;
     // on parts[0]'s device, allocated by the first image / variance / sums: the image gathered row-major
     double* row_sums = nullptr;  // width*height*3
@@ -565,6 +594,8 @@ struct rptb_buffer {
     double* gather = nullptr;    // one other part's sums + M2, copied over
     double* partial = nullptr;   // variance block partials, then the total
     uint8_t* rgb8 = nullptr;
+    uint32_t* row_counts = nullptr;     // `counted` only: width*height
+    uint32_t* gather_counts = nullptr;  // one other part's counts
     std::mutex lock;
 };
 
@@ -584,12 +615,21 @@ void buffer_free(rptb_buffer* b) {
         cudaFree(q.sums);
         cudaFree(q.m2);
         cudaFree(q.upload);
+        cudaFree(q.counts);
+        cudaFree(q.mask);
+        cudaFree(q.flags);
+        cudaFree(q.ids);
+        cudaFree(q.len);
+        cudaFree(q.active);
+        cudaFree(q.temp);
         if (i == 0) {
             cudaFree(b->row_sums);
             cudaFree(b->row_m2);
             cudaFree(b->gather);
             cudaFree(b->partial);
             cudaFree(b->rgb8);
+            cudaFree(b->row_counts);
+            cudaFree(b->gather_counts);
         }
         if (q.done) cudaEventDestroy(q.done);
         if (q.stream) cudaStreamDestroy(q.stream);
@@ -642,10 +682,80 @@ int buffer_gather(rptb_buffer* b, bool want_sums, bool want_m2) {
     return RPTB_OK;
 }
 
+// The same for the per-pixel counts of a `counted` buffer, into b->row_counts.  Called after buffer_gather, which has
+// ordered parts[0]'s stream behind every part.
+int buffer_gather_counts(rptb_buffer* b) {
+    BufferPart& q0 = b->parts[0];
+    const uint32_t nparts = (uint32_t)b->parts.size();
+    if (!b->row_counts) {
+        uint32_t most = 0;
+        for (uint32_t i = 1; i < nparts; i++) most = std::max(most, b->parts[i].tiles);
+        CU(cudaMalloc((void**)&b->row_counts, (size_t)b->width * b->height * sizeof(uint32_t)));
+        if (most) CU(cudaMalloc((void**)&b->gather_counts, (size_t)most * 128u * sizeof(uint32_t)));
+    }
+    CU(launch_buffer_scatter_counts(q0.counts, (uint64_t)q0.tiles * 128u, b->width, b->height, 0, nparts, b->row_counts, q0.stream));
+    for (uint32_t i = 1; i < nparts; i++) {
+        const BufferPart& q = b->parts[i];
+        if (!q.tiles) continue;
+        const size_t nelem = (size_t)q.tiles * 128u;
+        CU(cudaMemcpyPeerAsync(b->gather_counts, q0.device, q.counts, q.device, nelem * sizeof(uint32_t), q0.stream));
+        CU(launch_buffer_scatter_counts(b->gather_counts, nelem, b->width, b->height, i, nparts, b->row_counts, q0.stream));
+    }
+    return RPTB_OK;
+}
+
+// Gives part q per-pixel counts, all equal to `entries` (its first adaptive call), and the scratch of the select.
+int buffer_part_count(BufferPart& q, uint32_t entries, cudaStream_t stream) {
+    if (q.len) return RPTB_OK;
+    const size_t nelem = (size_t)q.tiles * 128u, nblocks = (size_t)q.tiles * 4u;
+    CU(cudaMalloc((void**)&q.len, sizeof(uint32_t)));
+    CU(cudaMalloc((void**)&q.active, sizeof(unsigned long long)));
+    if (q.tiles) {
+        CU(cudaMalloc((void**)&q.counts, nelem * sizeof(uint32_t)));
+        CU(cudaMalloc((void**)&q.mask, nelem));
+        CU(cudaMalloc((void**)&q.flags, nblocks));
+        CU(cudaMalloc((void**)&q.ids, nblocks * sizeof(uint32_t)));
+        q.temp_bytes = adaptive_temp_bytes(q.tiles);
+        CU(cudaMalloc(&q.temp, q.temp_bytes ? q.temp_bytes : 1));
+        CU(launch_buffer_counts_fill(q.counts, nelem, entries, stream));
+    }
+    return RPTB_OK;
+}
+
+// The slot megakernel over the warp blocks of `list` only, into the compact out32/out64 scratch (adaptive sampling).
+int render_list_launch(rptb_scene* s, const rptb_camera* cam, const rptb_render_params* p, const RenderList& list,
+                       cudaStream_t stream, bool want_counters, uint32_t* launches) {
+    if (want_counters) CU(cudaMemsetAsync(s->counters, 0, sizeof(DeviceCounters), stream));
+    if (p->precision == RPTB_PRECISION_F32) {
+        RenderArgs<float> a;
+        fill_args(cam, p, a);
+        a.out = s->out32;
+        a.compact = 1u;
+        a.counters = want_counters ? s->counters : nullptr;
+        a.ks = s->sampled_lights;
+        const int rc = ensure_partial(s, a);
+        if (rc != RPTB_OK) return rc;
+        CU(launch_render_list_f32(s->view32, a, list, (int)p->collect_stats, s->features, stream, launches));
+    } else {
+        RenderArgs<double> a;
+        fill_args(cam, p, a);
+        a.out = s->out64;
+        a.compact = 1u;
+        a.counters = want_counters ? s->counters : nullptr;
+        const int rc = ensure_partial(s, a);
+        if (rc != RPTB_OK) return rc;
+        CU(launch_render_list_f64(s->view64, a, list, (int)p->collect_stats, s->features, stream, launches));
+    }
+    return RPTB_OK;
+}
+
 // Enqueues replica `index` of `nparts`'s share of one rptb_sample_into on the replica's own stream: render its
 // tiles into the compact out32/out64 scratch, then add them to the buffer part as entry `n`.  No host synchronise.
+// `crit` (rptb_sample_into_adaptive): first decide which pixels and warp blocks are active, render those through the
+// list schedule and add the entry to them alone.  A `counted` buffer adds with each pixel's own count.
 int sample_part(rptb_scene* r, const rptb_camera* cam, const rptb_render_params* p, uint32_t index, uint32_t nparts,
-                uint32_t n, BufferPart& q, bool want_stats, uint32_t* launches) {
+                uint32_t n, BufferPart& q, bool want_stats, uint32_t* launches, bool counted = false,
+                const rptb_adaptive* crit = nullptr) {
     DeviceGuard g(r->device);
     if (!g.ok) return fail(RPTB_ERR_CUDA, "cudaSetDevice(%d) failed", r->device);
     int rc = wait_busy(r, r->stream);
@@ -657,13 +767,31 @@ int sample_part(rptb_scene* r, const rptb_camera* cam, const rptb_render_params*
     rc = ensure_out(r, nelem ? nelem * 3 : 1);
     if (rc != RPTB_OK) return rc;
     CU(cudaStreamWaitEvent(r->stream, q.done, 0));  // an add_samples on the part's own stream
+    if (crit) {
+        rc = buffer_part_count(q, n - 1u, r->stream);
+        if (rc != RPTB_OK) return rc;
+    }
     if (want_stats) CU(cudaEventRecord(r->ev0, r->stream));
-    rc = render_launch(r, cam, &qp, r->out32, r->out64, r->stream, want_stats, true, launches);
+    if (crit) {
+        CU(launch_adaptive_select(q.sums, q.m2, q.counts, q.tiles, p->width, p->height, index, nparts, *crit, q.mask, q.flags, q.ids,
+                                  q.len, q.active, q.temp, q.temp_bytes, r->stream));
+        const RenderList list = {q.ids, q.len, q.mask};
+        rc = render_list_launch(r, cam, &qp, list, r->stream, want_stats, launches);
+        *launches += q.tiles ? 3u : 0u;  // the mark kernel and the select's two
+    } else {
+        rc = render_launch(r, cam, &qp, r->out32, r->out64, r->stream, want_stats, true, launches);
+    }
     if (rc != RPTB_OK) return rc;
-    if (want_stats) CU(cudaEventRecord(r->ev1, r->stream));
+    if (want_stats && !crit) CU(cudaEventRecord(r->ev1, r->stream));
     const bool f32 = p->precision == RPTB_PRECISION_F32;
-    CU(launch_buffer_accumulate(f32 ? r->out32 : nullptr, f32 ? nullptr : r->out64, false, n, nelem, p->width, p->height,
-                                index, nparts, q.sums, q.m2, r->stream));
+    if (counted)
+        CU(launch_buffer_accumulate_counted(f32 ? r->out32 : nullptr, f32 ? nullptr : r->out64, false, crit ? q.mask : nullptr, nelem,
+                                            p->width, p->height, index, nparts, q.sums, q.m2, q.counts, r->stream));
+    else
+        CU(launch_buffer_accumulate(f32 ? r->out32 : nullptr, f32 ? nullptr : r->out64, false, n, nelem, p->width, p->height,
+                                    index, nparts, q.sums, q.m2, r->stream));
+    // (an adaptive call times the whole entry: select, render and accumulate; a plain one its render)
+    if (want_stats && crit) CU(cudaEventRecord(r->ev1, r->stream));
     (*launches)++;
     CU(cudaEventRecord(q.done, r->stream));
     // the scratch is read until the accumulate has run: later calls on any stream order themselves behind it
@@ -1233,12 +1361,15 @@ void rptb_buffer_destroy(rptb_buffer* b) {
     if (b) buffer_free(b);
 }
 
-int rptb_sample_into(rptb_scene* s, const rptb_camera* cam, const rptb_render_params* p, rptb_buffer* b, rptb_stats* stats) {
+static int sample_into_impl(rptb_scene* s, const rptb_camera* cam, const rptb_render_params* p, const rptb_adaptive* crit,
+                            rptb_buffer* b, uint64_t* out_active, rptb_stats* stats) {
     if (!b) return fail(RPTB_ERR_BAD_ARG, "null argument");
     int rc = check_params(s, cam, p);
     if (rc != RPTB_OK) return rc;
     if (p->shard_count > 1)
         return fail(RPTB_ERR_UNSUPPORTED, "shard_count %u: a buffer holds the whole image (shard with rptb_render_samples_device)", p->shard_count);
+    if (crit && p->engine == RPTB_ENGINE_WAVEFRONT)
+        return fail(RPTB_ERR_UNSUPPORTED, "adaptive sampling renders with the slot megakernel, not the wavefront engine");
     if (p->width != b->width || p->height != b->height)
         return fail(RPTB_ERR_BAD_ARG, "render is %ux%u but the buffer is %ux%u", p->width, p->height, b->width, b->height);
     const uint32_t nparts = 1u + (uint32_t)s->peers.size();
@@ -1248,16 +1379,31 @@ int rptb_sample_into(rptb_scene* s, const rptb_camera* cam, const rptb_render_pa
     std::lock_guard<std::mutex> bl(b->lock);
     if (b->entries == UINT32_MAX) return fail(RPTB_ERR_UNSUPPORTED, "too many entries");
     const uint32_t n = b->entries + 1;
+    const bool counted = b->counted || crit != nullptr;
     // every replica's share is enqueued before any is waited for, so the devices run concurrently
     std::vector<std::unique_lock<std::mutex>> locks;
     std::vector<uint32_t> launches(nparts, 0);
     for (uint32_t i = 0; i < nparts; i++) {
         rptb_scene* r = i == 0 ? s : s->peers[i - 1];
         locks.emplace_back(r->lock);
-        rc = sample_part(r, cam, p, i, nparts, n, b->parts[i], stats != nullptr, &launches[i]);
+        rc = sample_part(r, cam, p, i, nparts, n, b->parts[i], stats != nullptr, &launches[i], counted, crit);
         if (rc != RPTB_OK) return nparts > 1 ? fail(rc, "device %d: %s", r->device, g_error.c_str()) : rc;
     }
     b->entries = n;
+    b->counted = counted;
+    if (out_active) {
+        uint64_t total = 0;
+        for (uint32_t i = 0; i < nparts; i++) {
+            rptb_scene* r = i == 0 ? s : s->peers[i - 1];
+            DeviceGuard g(r->device);
+            unsigned long long a = 0;
+            CU(cudaMemcpyAsync(&a, b->parts[i].active, sizeof(a), cudaMemcpyDeviceToHost, r->stream));
+            CU(cudaStreamSynchronize(r->stream));
+            r->busy_pending = false;
+            total += a;
+        }
+        *out_active = total;
+    }
     if (!stats) return RPTB_OK;
     std::memset(stats, 0, sizeof(*stats));
     for (uint32_t i = 0; i < nparts; i++) {
@@ -1280,8 +1426,21 @@ int rptb_sample_into(rptb_scene* s, const rptb_camera* cam, const rptb_render_pa
         stats->gpu_ms = std::max(stats->gpu_ms, (double)ms);  // the devices run concurrently
         stats->launches += launches[i];
     }
-    stats->engine = use_wavefront(s, p) ? RPTB_ENGINE_WAVEFRONT : RPTB_ENGINE_MEGAKERNEL;
+    stats->engine = !crit && use_wavefront(s, p) ? RPTB_ENGINE_WAVEFRONT : RPTB_ENGINE_MEGAKERNEL;
     return RPTB_OK;
+}
+
+int rptb_sample_into(rptb_scene* s, const rptb_camera* cam, const rptb_render_params* p, rptb_buffer* b, rptb_stats* stats) {
+    return sample_into_impl(s, cam, p, nullptr, b, nullptr, stats);
+}
+
+int rptb_sample_into_adaptive(rptb_scene* s, const rptb_camera* cam, const rptb_render_params* p, const rptb_adaptive* crit,
+                              rptb_buffer* b, uint64_t* out_active, rptb_stats* stats) {
+    if (!crit) return fail(RPTB_ERR_BAD_ARG, "null argument");
+    if (crit->min_entries < 2) return fail(RPTB_ERR_BAD_ARG, "min_entries %u < 2 (a pixel's variance needs two entries)", crit->min_entries);
+    if (!(std::isfinite(crit->rel_tol) && crit->rel_tol >= 0.0) || !(std::isfinite(crit->abs_tol) && crit->abs_tol >= 0.0))
+        return fail(RPTB_ERR_BAD_ARG, "tolerances must be finite and >= 0 (rel_tol %g, abs_tol %g)", crit->rel_tol, crit->abs_tol);
+    return sample_into_impl(s, cam, p, crit, b, out_active, stats);
 }
 
 int rptb_buffer_add_samples(rptb_buffer* b, const double* rgb) {
@@ -1298,8 +1457,12 @@ int rptb_buffer_add_samples(rptb_buffer* b, const double* rgb) {
         CU(cudaStreamWaitEvent(q.stream, q.done, 0));
         // pageable source: the call returns once the bytes are staged, `rgb` may be reused afterwards
         CU(cudaMemcpyAsync(q.upload, rgb, nvals * sizeof(double), cudaMemcpyHostToDevice, q.stream));
-        CU(launch_buffer_accumulate(nullptr, q.upload, true, n, (uint64_t)q.tiles * 128u, b->width, b->height, i, nparts,
-                                    q.sums, q.m2, q.stream));
+        if (b->counted)
+            CU(launch_buffer_accumulate_counted(nullptr, q.upload, true, nullptr, (uint64_t)q.tiles * 128u, b->width, b->height, i,
+                                                nparts, q.sums, q.m2, q.counts, q.stream));
+        else
+            CU(launch_buffer_accumulate(nullptr, q.upload, true, n, (uint64_t)q.tiles * 128u, b->width, b->height, i, nparts,
+                                        q.sums, q.m2, q.stream));
         CU(cudaEventRecord(q.done, q.stream));
     }
     b->entries = n;
@@ -1315,7 +1478,13 @@ int rptb_buffer_image(rptb_buffer* b, uint8_t* out_rgb8) {
     int rc = buffer_gather(b, true, false);
     if (rc != RPTB_OK) return rc;
     const size_t nvals = (size_t)b->width * b->height * 3;
-    CU(launch_film_resolve(b->row_sums, b->entries, b->width, b->height, b->radius, b->rgb8, q0.stream));
+    if (b->counted) {
+        rc = buffer_gather_counts(b);
+        if (rc != RPTB_OK) return rc;
+        CU(launch_film_resolve_counted(b->row_sums, b->row_counts, b->width, b->height, b->radius, b->rgb8, q0.stream));
+    } else {
+        CU(launch_film_resolve(b->row_sums, b->entries, b->width, b->height, b->radius, b->rgb8, q0.stream));
+    }
     CU(cudaMemcpyAsync(out_rgb8, b->rgb8, nvals, cudaMemcpyDeviceToHost, q0.stream));
     CU(cudaStreamSynchronize(q0.stream));
     return RPTB_OK;
@@ -1334,7 +1503,13 @@ int rptb_buffer_variance(rptb_buffer* b, double* out) {
     if (rc != RPTB_OK) return rc;
     const uint64_t npix = (uint64_t)b->width * b->height;
     double* total = b->partial + buffer_variance_blocks(npix);
-    CU(launch_buffer_variance(b->row_m2, npix, b->entries, b->partial, total, q0.stream));
+    if (b->counted) {  // (a pixel with one entry gives 0/0: NaN, as the reference's variance does)
+        rc = buffer_gather_counts(b);
+        if (rc != RPTB_OK) return rc;
+        CU(launch_buffer_variance_counted(b->row_m2, b->row_counts, npix, b->partial, total, q0.stream));
+    } else {
+        CU(launch_buffer_variance(b->row_m2, npix, b->entries, b->partial, total, q0.stream));
+    }
     double sum = 0.0;
     CU(cudaMemcpyAsync(&sum, total, sizeof(double), cudaMemcpyDeviceToHost, q0.stream));
     CU(cudaStreamSynchronize(q0.stream));
@@ -1350,8 +1525,39 @@ int rptb_buffer_sums(rptb_buffer* b, double* out_sums, uint32_t* out_entries) {
     int rc = buffer_gather(b, true, false);
     if (rc != RPTB_OK) return rc;
     CU(cudaMemcpyAsync(out_sums, b->row_sums, (size_t)b->width * b->height * 3 * sizeof(double), cudaMemcpyDeviceToHost, q0.stream));
+    std::vector<uint32_t> counts;
+    if (b->counted && out_entries) {
+        rc = buffer_gather_counts(b);
+        if (rc != RPTB_OK) return rc;
+        counts.resize((size_t)b->width * b->height);
+        CU(cudaMemcpyAsync(counts.data(), b->row_counts, counts.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost, q0.stream));
+    }
     CU(cudaStreamSynchronize(q0.stream));
-    if (out_entries) *out_entries = b->entries;
+    if (out_entries) {
+        uint32_t most = 0;
+        for (uint32_t c : counts) most = std::max(most, c);
+        *out_entries = b->counted ? most : b->entries;
+    }
+    return RPTB_OK;
+}
+
+int rptb_buffer_pixel_stats(rptb_buffer* b, double* sums, double* m2, uint32_t* counts) {
+    if (!b) return fail(RPTB_ERR_BAD_ARG, "null argument");
+    std::lock_guard<std::mutex> bl(b->lock);
+    BufferPart& q0 = b->parts[0];
+    DeviceGuard g(q0.device);
+    const size_t npix = (size_t)b->width * b->height;
+    int rc = buffer_gather(b, sums != nullptr, m2 != nullptr);
+    if (rc != RPTB_OK) return rc;
+    if (sums) CU(cudaMemcpyAsync(sums, b->row_sums, npix * 3 * sizeof(double), cudaMemcpyDeviceToHost, q0.stream));
+    if (m2) CU(cudaMemcpyAsync(m2, b->row_m2, npix * sizeof(double), cudaMemcpyDeviceToHost, q0.stream));
+    if (counts && b->counted) {
+        rc = buffer_gather_counts(b);
+        if (rc != RPTB_OK) return rc;
+        CU(cudaMemcpyAsync(counts, b->row_counts, npix * sizeof(uint32_t), cudaMemcpyDeviceToHost, q0.stream));
+    }
+    CU(cudaStreamSynchronize(q0.stream));
+    if (counts && !b->counted) std::fill(counts, counts + npix, b->entries);
     return RPTB_OK;
 }
 

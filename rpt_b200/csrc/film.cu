@@ -14,11 +14,11 @@
 
 namespace rptb {
 
-__global__ void film_resolve_kernel(const double* __restrict__ sums, uint32_t nbatches, uint32_t width,
-                                    uint32_t height, uint32_t radius, uint8_t* __restrict__ out) {
-    const uint32_t x = blockIdx.x * blockDim.x + threadIdx.x;
-    const uint32_t y = blockIdx.y * blockDim.y + threadIdx.y;
-    if (x >= width || y >= height) return;
+// One output pixel.  COUNTED: pixel q holds counts[q] entries (a buffer with adaptive calls), else every pixel nbatches.
+template <bool COUNTED>
+__device__ __forceinline__ void film_resolve_pixel(const double* __restrict__ sums, uint32_t nbatches,
+                                                   const uint32_t* __restrict__ counts, uint32_t width, uint32_t height,
+                                                   uint32_t radius, uint8_t* __restrict__ out, uint32_t x, uint32_t y) {
     double c0 = 0.0, c1 = 0.0, c2 = 0.0;
     unsigned long long count = 0;
     const uint32_t i0 = x >= radius ? x - radius : 0u;  // saturating_sub
@@ -30,7 +30,8 @@ __global__ void film_resolve_kernel(const double* __restrict__ sums, uint32_t nb
             c0 += p[0];
             c1 += p[1];
             c2 += p[2];
-            count += nbatches;
+            if (COUNTED) count += counts[j * width + i];
+            else count += nbatches;
         }
     const double n = (double)count;
     const double c[3] = {c0 / n, c1 / n, c2 / n};
@@ -40,6 +41,23 @@ __global__ void film_resolve_kernel(const double* __restrict__ sums, uint32_t nb
         const double v = fmin(fmax(c[k], 0.0), 1.0);
         o[k] = (uint8_t)(pow(v, 1.0 / 2.2) * 255.0);  // `as u8` truncates
     }
+}
+
+__global__ void film_resolve_kernel(const double* __restrict__ sums, uint32_t nbatches, uint32_t width,
+                                    uint32_t height, uint32_t radius, uint8_t* __restrict__ out) {
+    const uint32_t x = blockIdx.x * blockDim.x + threadIdx.x;
+    const uint32_t y = blockIdx.y * blockDim.y + threadIdx.y;
+    if (x >= width || y >= height) return;
+    film_resolve_pixel<false>(sums, nbatches, nullptr, width, height, radius, out, x, y);
+}
+
+// get_filtered_color over per-pixel entry counts (src/buffer.rs:75-93: it divides by the entries in the window)
+__global__ void film_resolve_counted_kernel(const double* __restrict__ sums, const uint32_t* __restrict__ counts, uint32_t width,
+                                            uint32_t height, uint32_t radius, uint8_t* __restrict__ out) {
+    const uint32_t x = blockIdx.x * blockDim.x + threadIdx.x;
+    const uint32_t y = blockIdx.y * blockDim.y + threadIdx.y;
+    if (x >= width || y >= height) return;
+    film_resolve_pixel<true>(sums, 0u, counts, width, height, radius, out, x, y);
 }
 
 __global__ void convert_f64_f32_kernel(const double* __restrict__ in, float* __restrict__ out, size_t n) {
@@ -97,6 +115,25 @@ __device__ __forceinline__ int64_t tile_pixel(uint32_t width, uint32_t height, u
 // the render's compact out32/out64) or a row-major width*height*3 image (ROWMAJOR = true: a host entry), widened to
 // double.  The sum is added in entry order, so it is the sequential sum np.sum(batches, axis=0) computes; M2 takes
 // the mean from the sums before and after the entry: M2 += sum_c (x_c - S_old,c/(n-1)) * (x_c - S_new,c/n).
+// Entry n of one pixel: its running sums s[0..3) and M2 *m.
+__device__ __forceinline__ void welford_add(double x0, double x1, double x2, uint32_t n, double* __restrict__ s,
+                                            double* __restrict__ m) {
+    if (n == 1) {  // the first entry is the sum; its M2 is zero
+        s[0] = x0;
+        s[1] = x1;
+        s[2] = x2;
+        *m = 0.0;
+        return;
+    }
+    const double o0 = s[0], o1 = s[1], o2 = s[2];
+    const double n0 = o0 + x0, n1 = o1 + x1, n2 = o2 + x2;
+    const double a = (double)(n - 1), b = (double)n;
+    *m += (x0 - o0 / a) * (x0 - n0 / b) + (x1 - o1 / a) * (x1 - n1 / b) + (x2 - o2 / a) * (x2 - n2 / b);
+    s[0] = n0;
+    s[1] = n1;
+    s[2] = n2;
+}
+
 template <class T, bool ROWMAJOR>
 __global__ void buffer_accumulate_kernel(const T* __restrict__ in, uint32_t n, uint64_t nelem, uint32_t width,
                                          uint32_t height, uint32_t shard_index, uint32_t shard_count,
@@ -109,22 +146,40 @@ __global__ void buffer_accumulate_kernel(const T* __restrict__ in, uint32_t n, u
         if (p < 0) return;
         src = in + 3 * p;
     }
-    const double x0 = (double)src[0], x1 = (double)src[1], x2 = (double)src[2];
-    double* s = sums + 3 * e;
-    if (n == 1) {  // the first entry is the sum; its M2 is zero
-        s[0] = x0;
-        s[1] = x1;
-        s[2] = x2;
-        m2[e] = 0.0;
-        return;
+    welford_add((double)src[0], (double)src[1], (double)src[2], n, sums + 3 * e, m2 + e);
+}
+
+// The same for a buffer with per-pixel entry counts (adaptive sampling): element e takes entry counts[e] + 1, and only
+// where mask[e] is set (mask == nullptr: every element, Buffer::add_samples).
+template <class T, bool ROWMAJOR>
+__global__ void buffer_accumulate_counted_kernel(const T* __restrict__ in, const uint8_t* __restrict__ mask, uint64_t nelem,
+                                                 uint32_t width, uint32_t height, uint32_t shard_index, uint32_t shard_count,
+                                                 double* __restrict__ sums, double* __restrict__ m2, uint32_t* __restrict__ counts) {
+    const uint64_t e = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= nelem) return;
+    if (mask && !mask[e]) return;
+    const T* src = in + 3 * e;
+    if (ROWMAJOR) {
+        const int64_t p = tile_pixel(width, height, shard_index + (uint32_t)(e >> 7) * shard_count, (uint32_t)(e & 127u));
+        if (p < 0) return;
+        src = in + 3 * p;
     }
-    const double o0 = s[0], o1 = s[1], o2 = s[2];
-    const double n0 = o0 + x0, n1 = o1 + x1, n2 = o2 + x2;
-    const double a = (double)(n - 1), b = (double)n;
-    m2[e] += (x0 - o0 / a) * (x0 - n0 / b) + (x1 - o1 / a) * (x1 - n1 / b) + (x2 - o2 / a) * (x2 - n2 / b);
-    s[0] = n0;
-    s[1] = n1;
-    s[2] = n2;
+    const uint32_t n = counts[e] + 1u;
+    welford_add((double)src[0], (double)src[1], (double)src[2], n, sums + 3 * e, m2 + e);
+    counts[e] = n;
+}
+
+__global__ void buffer_counts_fill_kernel(uint32_t* __restrict__ counts, uint64_t nelem, uint32_t value) {
+    const uint64_t e = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e < nelem) counts[e] = value;
+}
+
+__global__ void buffer_scatter_counts_kernel(const uint32_t* __restrict__ counts, uint64_t nelem, uint32_t width, uint32_t height,
+                                             uint32_t shard_index, uint32_t shard_count, uint32_t* __restrict__ row_counts) {
+    const uint64_t e = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= nelem) return;
+    const int64_t p = tile_pixel(width, height, shard_index + (uint32_t)(e >> 7) * shard_count, (uint32_t)(e & 127u));
+    if (p >= 0) row_counts[p] = counts[e];
 }
 
 // Compact tiles of replica `shard_index` of `shard_count` -> the row-major sums / M2 of the whole image.
@@ -169,6 +224,18 @@ __global__ void __launch_bounds__(kVarThreads) buffer_variance_partial_kernel(co
     if (threadIdx.x == 0) partial[blockIdx.x] = s;
 }
 
+// The same sum with each pixel's own count: M2 / (counts - 1), in the same order.
+__global__ void __launch_bounds__(kVarThreads) buffer_variance_partial_counted_kernel(const double* __restrict__ m2,
+                                                                                      const uint32_t* __restrict__ counts,
+                                                                                      uint64_t npixels, double* __restrict__ partial) {
+    const uint64_t base = (uint64_t)blockIdx.x * kVarChunk;
+    double v = 0.0;
+    for (uint32_t i = threadIdx.x; i < kVarChunk; i += kVarThreads)
+        if (base + i < npixels) v += m2[base + i] / ((double)counts[base + i] - 1.0);
+    const double s = block_sum_fixed(v);
+    if (threadIdx.x == 0) partial[blockIdx.x] = s;
+}
+
 __global__ void __launch_bounds__(kVarThreads) buffer_variance_final_kernel(const double* __restrict__ partial, uint32_t nblocks,
                                                                             double* __restrict__ out_sum) {
     double v = 0.0;
@@ -188,6 +255,54 @@ cudaError_t launch_buffer_accumulate(const float* in32, const double* in64, bool
         buffer_accumulate_kernel<double, true><<<grid, 256, 0, stream>>>(in64, n, nelem, width, height, shard_index, shard_count, sums, m2);
     else
         buffer_accumulate_kernel<double, false><<<grid, 256, 0, stream>>>(in64, n, nelem, width, height, shard_index, shard_count, sums, m2);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_buffer_accumulate_counted(const float* in32, const double* in64, bool rowmajor, const uint8_t* mask,
+                                             uint64_t nelem, uint32_t width, uint32_t height, uint32_t shard_index,
+                                             uint32_t shard_count, double* sums, double* m2, uint32_t* counts, cudaStream_t stream) {
+    if (nelem == 0) return cudaSuccess;
+    const unsigned grid = (unsigned)((nelem + 255) / 256);
+    if (in32)
+        buffer_accumulate_counted_kernel<float, false><<<grid, 256, 0, stream>>>(in32, mask, nelem, width, height, shard_index,
+                                                                                 shard_count, sums, m2, counts);
+    else if (rowmajor)
+        buffer_accumulate_counted_kernel<double, true><<<grid, 256, 0, stream>>>(in64, mask, nelem, width, height, shard_index,
+                                                                                 shard_count, sums, m2, counts);
+    else
+        buffer_accumulate_counted_kernel<double, false><<<grid, 256, 0, stream>>>(in64, mask, nelem, width, height, shard_index,
+                                                                                  shard_count, sums, m2, counts);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_buffer_counts_fill(uint32_t* counts, uint64_t nelem, uint32_t value, cudaStream_t stream) {
+    if (nelem == 0) return cudaSuccess;
+    buffer_counts_fill_kernel<<<(unsigned)((nelem + 255) / 256), 256, 0, stream>>>(counts, nelem, value);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_buffer_scatter_counts(const uint32_t* counts, uint64_t nelem, uint32_t width, uint32_t height,
+                                         uint32_t shard_index, uint32_t shard_count, uint32_t* row_counts, cudaStream_t stream) {
+    if (nelem == 0) return cudaSuccess;
+    buffer_scatter_counts_kernel<<<(unsigned)((nelem + 255) / 256), 256, 0, stream>>>(counts, nelem, width, height, shard_index,
+                                                                                    shard_count, row_counts);
+    return cudaGetLastError();
+}
+
+uint32_t buffer_variance_blocks(uint64_t npixels);
+// *out_sum = sum over pixels of m2[p] / (counts[p] - 1); `partial` as in launch_buffer_variance.
+cudaError_t launch_buffer_variance_counted(const double* m2, const uint32_t* counts, uint64_t npixels, double* partial,
+                                           double* out_sum, cudaStream_t stream) {
+    const uint32_t nb = buffer_variance_blocks(npixels);
+    buffer_variance_partial_counted_kernel<<<nb, kVarThreads, 0, stream>>>(m2, counts, npixels, partial);
+    buffer_variance_final_kernel<<<1, kVarThreads, 0, stream>>>(partial, nb, out_sum);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_film_resolve_counted(const double* sums, const uint32_t* counts, uint32_t width, uint32_t height,
+                                        uint32_t radius, uint8_t* out, cudaStream_t stream) {
+    const dim3 block(32, 8), grid((width + 31) / 32, (height + 7) / 8);
+    film_resolve_counted_kernel<<<grid, block, 0, stream>>>(sums, counts, width, height, radius, out);
     return cudaGetLastError();
 }
 

@@ -460,6 +460,26 @@ RPTB_D void render_thread(const SceneView<R>& sv, const RenderArgs<R>& a, const 
     }
 }
 
+// The list schedule (FEAT has F_LIST): warp w of CTA b renders list entry 4b + w -- the same pixels, compact slots and
+// sample streams the tile schedule gives that 8x4 block -- and a pixel the list's mask leaves out returns before the
+// body's W::activemask(), like one past a ragged edge.  The body is render_thread itself, run as that block's thread;
+// its generator keeps this thread's own column of the shared ring, which render_list_kernel pads by LIST_RING_PAD words
+// in front so that the shifted base stays inside the array.  (The list is not a parameter of render_thread: an unused
+// extra parameter alone moved spill slots in the tile-scheduled kernels.)
+constexpr int LIST_RING_PAD = RENDER_THREADS - 32;
+template <class R, int MAXD, bool STATS, int FEAT, class W>
+RPTB_D void render_thread_list(const SceneView<R>& sv, const RenderArgs<R>& a, const RenderList& list, const uint32_t block_x,
+                               const uint32_t block_y, const uint32_t thread_x, uint32_t* rng_ring = nullptr, void* coop = nullptr) {
+    static_assert((FEAT & F_LIST) != 0, "render_thread_list is the F_LIST schedule");
+    const uint32_t e = block_x * (RENDER_THREADS / 32u) + (thread_x >> 5);
+    if (e >= *list.len) return;
+    const uint32_t id = list.ids[e];
+    const uint32_t bx = id >> 2, tid = ((id & 3u) << 5) | (thread_x & 31u);  // the owned tile and its CTA's thread
+    if (!list.mask[(size_t)bx * RENDER_THREADS + tid]) return;
+    uint32_t* ring = rng_ring ? rng_ring + (LIST_RING_PAD + (int)thread_x - (int)tid) : nullptr;  // column tid -> thread_x
+    render_thread<R, MAXD, STATS, FEAT & ~F_LIST, W>(sv, a, bx, block_y, tid, ring, coop);
+}
+
 #ifdef __CUDACC__
 template <class R, int MAXD, bool STATS, int FEAT = F_ALL>
 __global__ void __launch_bounds__(RENDER_THREADS, render_min_blocks(FEAT)) render_kernel(const __grid_constant__ SceneView<R> sv, const __grid_constant__ RenderArgs<R> a) {
@@ -475,6 +495,28 @@ __global__ void __launch_bounds__(RENDER_THREADS, render_min_blocks(FEAT)) rende
 #endif
         {
             render_thread<R, MAXD, STATS, FEAT, DeviceWarp>(sv, a, blockIdx.x, blockIdx.y, threadIdx.x, rng_ring);
+        }
+    }
+}
+
+// The list-scheduled form (FEAT has F_LIST): the grid is sized for every owned tile, and warps past the list's length
+// leave at once.
+template <class R, int MAXD, bool STATS, int FEAT>
+__global__ void __launch_bounds__(RENDER_THREADS, render_min_blocks(FEAT))
+    render_list_kernel(const __grid_constant__ SceneView<R> sv, const __grid_constant__ RenderArgs<R> a, const RenderList list) {
+    static_assert((FEAT & F_LIST) != 0, "render_list_kernel is the F_LIST schedule");
+    if constexpr (M<R>::literal) {
+        render_thread_list<R, MAXD, STATS, FEAT, DeviceWarp>(sv, a, list, blockIdx.x, blockIdx.y, threadIdx.x);
+    } else {
+        __shared__ uint32_t rng_ring[LIST_RING_PAD + RNG_RING * RENDER_THREADS];  // padded in front: see render_thread_list
+#ifndef RPTB_HOST_EMU
+        if constexpr ((FEAT & F_BVH) != 0 && RPTB_COOP_MAX > 0) {
+            __shared__ CoopWarp coop[RENDER_THREADS / 32];
+            render_thread_list<R, MAXD, STATS, FEAT, DeviceWarp>(sv, a, list, blockIdx.x, blockIdx.y, threadIdx.x, rng_ring, &coop[threadIdx.x >> 5]);
+        } else
+#endif
+        {
+            render_thread_list<R, MAXD, STATS, FEAT, DeviceWarp>(sv, a, list, blockIdx.x, blockIdx.y, threadIdx.x, rng_ring);
         }
     }
 }
@@ -502,10 +544,24 @@ RPTB_D void resolve_chunks_thread(const RenderArgs<R>& a, const uint32_t block_x
     out[1] = (R)(s1 / it * (double)a.exposure_scale);
     out[2] = (R)(s2 / it * (double)a.exposure_scale);
 }
+// The chunk sums of the pixels a list-scheduled render wrote, and no others: entry 4b + w of the list, as there.
+template <class R>
+RPTB_D void resolve_chunks_list_thread(const RenderArgs<R>& a, const RenderList& list, const uint32_t block_x, const uint32_t thread_x) {
+    const uint32_t e = block_x * (RENDER_THREADS / 32u) + (thread_x >> 5);
+    if (e >= *list.len) return;
+    const uint32_t id = list.ids[e];
+    const uint32_t bx = id >> 2, tid = ((id & 3u) << 5) | (thread_x & 31u);
+    if (!list.mask[(size_t)bx * RENDER_THREADS + tid]) return;
+    resolve_chunks_thread<R>(a, bx, tid);
+}
 #ifdef __CUDACC__
 template <class R>
 __global__ void resolve_chunks_kernel(const RenderArgs<R> a) {
     resolve_chunks_thread<R>(a, blockIdx.x, threadIdx.x);
+}
+template <class R>
+__global__ void resolve_chunks_list_kernel(const RenderArgs<R> a, const RenderList list) {
+    resolve_chunks_list_thread<R>(a, list, blockIdx.x, threadIdx.x);
 }
 #endif
 

@@ -23,6 +23,13 @@ namespace rptb {
 RPTB_DECLARE_LAUNCHERS(f32, float)
 RPTB_DECLARE_LAUNCHERS(f64, double)
 
+// The slot engine scheduled from `list` (F_LIST): only the listed warp blocks' unmasked pixels are rendered, into the
+// compact layout (args.compact = 1); nothing else is written.  The grid covers every owned tile.
+cudaError_t launch_render_list_f32(const SceneView<float>& sv, const RenderArgs<float>& args, const RenderList& list,
+                                   int stats, int features, cudaStream_t stream, uint32_t* launches);
+cudaError_t launch_render_list_f64(const SceneView<double>& sv, const RenderArgs<double>& args, const RenderList& list,
+                                   int stats, int features, cudaStream_t stream, uint32_t* launches);
+
 // ---- wavefront engine (f32 only; wavefront.cuh) -------------------------------------------
 struct WfBuffers;
 // bytes of device memory the engine needs for (npaths, Ks sampled lights, maxd levels)
@@ -87,6 +94,12 @@ constexpr Variant pick_render(int features, int stats, bool f64, uint32_t max_bo
     return {false, F_ALL, 16};
 }
 
+// render_list_kernel<R, MAXD, STATS, FEAT | F_LIST>: the variant pick_render chooses, scheduled from a RenderList
+constexpr Variant pick_render_list(int features, int stats, bool f64, uint32_t max_bounces) {
+    const Variant v = pick_render(features, stats, f64, max_bounces);
+    return {v.stats, v.feat | F_LIST, v.maxd};
+}
+
 // render_kernel_vx<STATS, FEAT> (f32 only): the slot engine's variants without the packed table
 constexpr Variant pick_render_vx(int features, int stats) {
     const int base = features & F_ALL;
@@ -149,6 +162,15 @@ using RenderVariantsF32 = VariantList<
 using RenderVariantsF64 = VariantList<
     V<true, F_EVERY | F_BVH, 16>, V<true, F_EVERY, 16>, V<false, F_EVERY | F_BVH, 16>, V<false, F_EVERY, 16>,
     V<false, F_ALL, 16>, V<true, F_EVERY, (int)MAX_BOUNCES_SUPPORTED>, V<false, F_EVERY, (int)MAX_BOUNCES_SUPPORTED>>;
+// the list-scheduled twin of every entry of a render list (F_LIST set)
+template <class L>
+struct WithList;
+template <class... Vs>
+struct WithList<VariantList<Vs...>> {
+    using type = VariantList<V<Vs::stats, Vs::feat | F_LIST, Vs::maxd>...>;
+};
+using RenderListVariantsF32 = WithList<RenderVariantsF32>::type;
+using RenderListVariantsF64 = WithList<RenderVariantsF64>::type;
 using RenderVariantsVx = VariantList<
     V<true, F_EVERY | F_BVH>, V<true, F_EVERY>, V<false, F_EVERY | F_BVH>, V<false, F_EVERY>, V<false, F_TREE | F_BVH>,
     V<false, F_ALL | F_BVH>, V<false, F_SMALL>, V<false, 0>, V<false, F_TREE>, V<false, F_TRANSP | F_HDRI | F_SMALL>,

@@ -35,6 +35,28 @@ cudaError_t launch_render_impl(const SceneView<R>& sv, const RenderArgs<R>& args
 }
 
 template <class R>
+cudaError_t launch_render_list_impl(const SceneView<R>& sv, const RenderArgs<R>& args, const RenderList& list, int stats,
+                                    int features, cudaStream_t stream, uint32_t* launches) {
+    uint32_t nl = 0;
+    if (args.ntiles_mine > 0) {
+        const dim3 grid(args.ntiles_mine, args.ngroups), block(RENDER_THREADS);
+        using List = std::conditional_t<M<R>::literal, RenderListVariantsF64, RenderListVariantsF32>;
+        const bool found = visit(List{}, pick_render_list(features, stats, M<R>::literal, args.max_bounces), [&](auto v) {
+            using T = decltype(v);
+            render_list_kernel<R, T::maxd, T::stats, T::feat><<<grid, block, 0, stream>>>(sv, args, list);
+        });
+        if (!found) return cudaErrorInvalidValue;
+        nl++;
+        if (args.nchunks > 1) {
+            resolve_chunks_list_kernel<R><<<args.ntiles_mine, RENDER_THREADS, 0, stream>>>(args, list);
+            nl++;
+        }
+    }
+    if (launches) *launches = nl;
+    return cudaGetLastError();
+}
+
+template <class R>
 cudaError_t launch_closest_hit_impl(const SceneView<R>& sv, const double* rays, uint64_t n, double tmin, double* out_t,
                                     int32_t* out_obj, double* out_n, DeviceCounters* counters, int stats, int features,
                                     cudaStream_t stream) {
@@ -80,6 +102,11 @@ cudaError_t launch_illuminate_impl(const SceneView<R>& sv, uint32_t light, const
     cudaError_t launch_render_##SUFFIX(const SceneView<R>& sv, const RenderArgs<R>& args, int stats,                \
                                        int features, cudaStream_t stream, uint32_t* launches) {                     \
         return launch_render_impl<R>(sv, args, stats, features, stream, launches);                                  \
+    }                                                                                                               \
+    cudaError_t launch_render_list_##SUFFIX(const SceneView<R>& sv, const RenderArgs<R>& args,                      \
+                                            const RenderList& list, int stats, int features, cudaStream_t stream,   \
+                                            uint32_t* launches) {                                                   \
+        return launch_render_list_impl<R>(sv, args, list, stats, features, stream, launches);                       \
     }                                                                                                               \
     cudaError_t launch_closest_hit_##SUFFIX(const SceneView<R>& sv, const double* rays, uint64_t n, double tmin,    \
                                             double* out_t, int32_t* out_obj, double* out_n,                         \

@@ -39,7 +39,8 @@ enum : int {
     F_GROUP = 16 /* kd-trees over whole shapes (KdTree<Box<dyn Bounded>>) */, F_MONO = 32 /* MonomialSurface */,
     F_EXT = F_GROUP | F_MONO, F_EVERY = F_ALL | F_EXT /* the one instantiation that knows every shape */,
     F_BVH = 64 /* f32 only: meshes are traversed through their BVH (MeshRec::bvh_*) instead of the reference-shaped kd-tree */,
-    F_FLAT = 128 /* f32 only: get_closest_hit walks the packed primitive table (SceneView::flat) instead of the objects */
+    F_FLAT = 128 /* f32 only: get_closest_hit walks the packed primitive table (SceneView::flat) instead of the objects */,
+    F_LIST = 256 /* scheduling, not a scene feature: warps take their 8x4 pixel blocks from a RenderList (adaptive sampling) */
 };
 
 // Two experiments on the mesh configs (teapot / dragon-proxy / dragon-knot), both measured slower than what they were
@@ -283,6 +284,15 @@ struct RenderArgs {
     // copies exactly its own pixels back this way (api.cu); 0 = the full row-major width * height * 3 image.
     uint32_t compact;
     uint32_t ks;  // sampled (non-ambient) lights of the scene: the vertex-at-once engine's shadow ray slots (integrator_vx.cuh)
+};
+
+// The warp blocks a list-scheduled render (F_LIST) covers: ids[0 .. *len) are k*4 + w in increasing order -- warp w
+// (an 8x4 block) of the k-th owned tile -- and mask[k*128 + j] says whether pixel j of that tile takes part.  `len`
+// lives in device memory: the count is never brought to the host.
+struct RenderList {
+    const uint32_t* ids;
+    const uint32_t* len;
+    const uint8_t* mask;
 };
 
 // chunk = max(64, ceil(iterations / 32)) samples, so at most 32 chunks

@@ -32,6 +32,10 @@ $(OBJDIR)/kernels_f64.o: $(CSRC)/kernels_f64.cu $(HDRS)
 $(OBJDIR)/adaptive.o: $(CSRC)/adaptive.cu $(HDRS)
 	@mkdir -p $(OBJDIR)
 	$(NVCC) $(NVFLAGS) -fmad=false -c $< -o $@ 2> $(OBJDIR)/adaptive.ptxas.log || (cat $(OBJDIR)/adaptive.ptxas.log; false)
+# the denoiser (denoise.h) likewise: its numpy restatement and host emulation round every operation on its own
+$(OBJDIR)/denoise.o: $(CSRC)/denoise.cu $(HDRS)
+	@mkdir -p $(OBJDIR)
+	$(NVCC) $(NVFLAGS) -fmad=false -c $< -o $@ 2> $(OBJDIR)/denoise.ptxas.log || (cat $(OBJDIR)/denoise.ptxas.log; false)
 $(OBJDIR)/film.o: $(CSRC)/film.cu $(HDRS)
 	@mkdir -p $(OBJDIR)
 	$(NVCC) $(NVFLAGS) -c $< -o $@ 2> $(OBJDIR)/film.ptxas.log || (cat $(OBJDIR)/film.ptxas.log; false)
@@ -48,7 +52,7 @@ $(OBJDIR)/objparse.o: $(CSRC)/objparse.cpp
 	@mkdir -p $(OBJDIR)
 	$(CXX) -std=c++17 -O3 -fPIC -Wall -c $< -o $@
 
-$(LIB): $(OBJDIR)/kernels_f32.o $(OBJDIR)/kernels_vx.o $(OBJDIR)/kernels_f64.o $(OBJDIR)/film.o $(OBJDIR)/adaptive.o $(OBJDIR)/api.o $(OBJDIR)/kdbuild.o $(OBJDIR)/bvhbuild.o $(OBJDIR)/objparse.o
+$(LIB): $(OBJDIR)/kernels_f32.o $(OBJDIR)/kernels_vx.o $(OBJDIR)/kernels_f64.o $(OBJDIR)/film.o $(OBJDIR)/adaptive.o $(OBJDIR)/denoise.o $(OBJDIR)/api.o $(OBJDIR)/kdbuild.o $(OBJDIR)/bvhbuild.o $(OBJDIR)/objparse.o
 	@mkdir -p rpt_b200/lib
 	$(NVCC) -shared $(ARCH) -o $@ $^ -Xcompiler -fopenmp -lgomp -cudart shared
 
@@ -69,13 +73,18 @@ build/%_cpp: examples/%.cpp include/rpt.hpp include/rpt_b200.h $(LIB)
 HOSTEMU := tests/hostemu/_build/libhostemu.so
 # the same emulation plus adaptive sampling's list-scheduled megakernel and convergence test (tests/hostemu/hostemu_list.cu)
 HOSTEMU_LIST := tests/hostemu/_build/libhostemu_list.so
-hostemu: $(HOSTEMU) $(HOSTEMU_LIST)
+# the same emulation plus the feature pass (features.cuh) and the denoiser's per-pixel functions (tests/hostemu/hostemu_denoise.cu)
+HOSTEMU_DENOISE := tests/hostemu/_build/libhostemu_denoise.so
+hostemu: $(HOSTEMU) $(HOSTEMU_LIST) $(HOSTEMU_DENOISE)
 $(HOSTEMU): tests/hostemu/hostemu.cu $(CSRC)/kdbuild.cpp $(CSRC)/bvhbuild.cpp $(HDRS)
 	@mkdir -p $(dir $@)
 	nvcc -std=c++17 -O2 -DRPTB_HOST_EMU -DRPTB_BUILD_BVH8=1 -DRPTB_BUILD_BVH4=1 -gencode arch=compute_90a,code=sm_90a -Xcompiler -fPIC,-fopenmp,-ffp-contract=off -shared -Xlinker -Bsymbolic -o $@ tests/hostemu/hostemu.cu $(CSRC)/kdbuild.cpp $(CSRC)/bvhbuild.cpp -lgomp
 $(HOSTEMU_LIST): tests/hostemu/hostemu_list.cu tests/hostemu/hostemu.cu $(CSRC)/kdbuild.cpp $(CSRC)/bvhbuild.cpp $(HDRS)
 	@mkdir -p $(dir $@)
 	nvcc -std=c++17 -O2 -DRPTB_HOST_EMU -DRPTB_BUILD_BVH8=1 -DRPTB_BUILD_BVH4=1 -gencode arch=compute_90a,code=sm_90a -Xcompiler -fPIC,-fopenmp,-ffp-contract=off -shared -Xlinker -Bsymbolic -o $@ tests/hostemu/hostemu_list.cu $(CSRC)/kdbuild.cpp $(CSRC)/bvhbuild.cpp -lgomp
+$(HOSTEMU_DENOISE): tests/hostemu/hostemu_denoise.cu tests/hostemu/hostemu.cu $(CSRC)/kdbuild.cpp $(CSRC)/bvhbuild.cpp $(HDRS)
+	@mkdir -p $(dir $@)
+	nvcc -std=c++17 -O2 -DRPTB_HOST_EMU -DRPTB_BUILD_BVH8=1 -DRPTB_BUILD_BVH4=1 -gencode arch=compute_90a,code=sm_90a -Xcompiler -fPIC,-fopenmp,-ffp-contract=off -shared -Xlinker -Bsymbolic -o $@ tests/hostemu/hostemu_denoise.cu $(CSRC)/kdbuild.cpp $(CSRC)/bvhbuild.cpp -lgomp
 
 clean:
 	rm -rf build $(LIB) $(ORACLE) tests/hostemu/_build

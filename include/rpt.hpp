@@ -267,7 +267,9 @@ public:
     ~DeviceBuffer() { if (handle_) rptb_buffer_destroy(handle_); }
     DeviceBuffer(const DeviceBuffer&) = delete;
     DeviceBuffer& operator=(const DeviceBuffer&) = delete;
-    DeviceBuffer(DeviceBuffer&& o) noexcept : width_(o.width_), height_(o.height_), handle_(o.handle_) { o.handle_ = nullptr; }
+    DeviceBuffer(DeviceBuffer&& o) noexcept : width_(o.width_), height_(o.height_), handle_(o.handle_), feature_rays_(o.feature_rays_) {
+        o.handle_ = nullptr;
+    }
 
     void add_samples(const std::vector<double>& rgb) {  // :32-40
         if (rgb.size() != (size_t)width_ * height_ * 3) throw std::invalid_argument("Invalid sample dimension");
@@ -304,12 +306,38 @@ public:
         check(rptb_buffer_pixel_stats(handle_, nullptr, nullptr, out.data()));
         return out;
     }
+    // Camera rays per pixel in the features (Renderer::sample_features keeps the count).
+    uint64_t feature_rays() const { return feature_rays_; }
+    void add_feature_rays(uint64_t n) { feature_rays_ += n; }
+    // The first-hit features (rptb_buffer_features), row-major: normal (3 per pixel), depth, albedo (3), hit fraction.
+    struct Features {
+        std::vector<double> normal, depth, albedo, hit_fraction;
+    };
+    Features features() const {
+        const size_t n = (size_t)width_ * height_;
+        Features f{std::vector<double>(n * 3), std::vector<double>(n), std::vector<double>(n * 3), std::vector<double>(n)};
+        check(rptb_buffer_features(handle_, f.normal.data(), f.depth.data(), f.albedo.data(), f.hit_fraction.data()));
+        return f;
+    }
+    // The mean image through the edge-avoiding filter (rptb_buffer_denoise): linear doubles, 3 per pixel, row-major.
+    std::vector<double> denoise(const rptb_denoise& d) const {
+        std::vector<double> out((size_t)width_ * height_ * 3);
+        check(rptb_buffer_denoise(handle_, &d, out.data(), nullptr));
+        return out;
+    }
+    // The same through Buffer::image's clamp, gamma and cast (no box filter).
+    std::vector<uint8_t> denoised_image(const rptb_denoise& d) const {
+        std::vector<uint8_t> out((size_t)width_ * height_ * 3);
+        check(rptb_buffer_denoise(handle_, &d, nullptr, out.data()));
+        return out;
+    }
     rptb_buffer* handle() const { return handle_; }
 
 private:
     static void check(int rc) { if (rc != RPTB_OK) throw std::runtime_error(rptb_last_error()); }
     uint32_t width_, height_;
     rptb_buffer* handle_ = nullptr;
+    uint64_t feature_rays_ = 0;
 };
 
 // Renderer (src/renderer.rs:18-115); `sample` is the seam into the CUDA library.
@@ -387,6 +415,16 @@ public:
             throw std::runtime_error(rptb_last_error());
         next_sample_ += iterations;
         return active;
+    }
+    // Adds the first hits of `iterations` more camera rays per pixel to the buffer's features: the samples after those
+    // its features already hold (0 .. iterations-1 on the first call).
+    void sample_features(uint32_t iterations, DeviceBuffer& buffer) {
+        ensure_scene();
+        rptb_render_params p = params(iterations);
+        p.first_sample = buffer.feature_rays();
+        const rptb_camera c = camera();
+        if (rptb_buffer_add_features(handle_, &c, &p, buffer.handle(), nullptr) != RPTB_OK) throw std::runtime_error(rptb_last_error());
+        buffer.add_feature_rays(iterations);
     }
     // The same loop with every batch adaptive; it stops early after a batch that rendered no pixel.
     void iterative_render(uint32_t interval, DeviceBuffer& buffer, const rptb_adaptive& criterion,

@@ -453,6 +453,47 @@ int rptb_sample_into_adaptive(rptb_scene* scene, const rptb_camera* camera, cons
  * channels) and entry counts (width*height).                                                                 */
 int rptb_buffer_pixel_stats(rptb_buffer* buffer, double* sums, double* m2, uint32_t* counts);
 
+/* ---- Denoising the device Buffer ---------------------------------------------------------------------------
+ * Not in the reference, which has one filter, Filter::Box(radius) (src/buffer.rs:75-108): it averages a square
+ * window and blurs silhouettes and shadow edges as much as noise.  These stand beside it: a first-hit feature
+ * pass, and the spatial part of SVGF (Schied et al., HPG 2017), an edge-avoiding a-trous wavelet filter
+ * (Dammertz et al., HPG 2010) guided by the features and by each pixel's variance of the mean -- the statistic
+ * rptb_adaptive tests.  Temporal reprojection is not done: the Buffer is one image.
+ *
+ * Adds, for every pixel and every sample i in [first_sample, first_sample + iterations), the first hit of the
+ * render's camera ray for Philox key (seed, pixel, i) -- the same draws in the same order, tmin 1e-12, in
+ * params->precision -- to per-pixel double sums kept in the buffer: on a hit, the hit count, the shading normal
+ * turned to face the ray, the distance t and the material's colour; on a miss, only the ray count.  The sums are
+ * added in sample order; features may be added before, between or after entries and never touch them.  Argument
+ * checks as rptb_sample_into.  The results are the same bits for any device count.  stats (nullable, forces
+ * sync): rays, gpu_ms, launches.                                                                             */
+int rptb_buffer_add_features(rptb_scene* scene, const rptb_camera* camera, const rptb_render_params* params,
+                             rptb_buffer* buffer, rptb_stats* stats /* nullable, forces sync */);
+/* The resolved features (AOVs), row-major, each pointer nullable: normal (width*height*3) = the normalised sum of
+ * the hit normals, 0 where nothing was hit; depth (width*height) = the mean hit distance, +inf where nothing was
+ * hit; albedo (width*height*3) = the mean material colour over all rays, a miss counting 1 (it sees the
+ * environment); hit_fraction (width*height) = hits / rays.  No features yet: RPTB_ERR_BAD_ARG.              */
+int rptb_buffer_features(rptb_buffer* buffer, double* normal, double* depth, double* albedo, double* hit_fraction);
+/* The filter's parameters (rpt_b200/csrc/denoise.h gives every formula and its order of operations).
+ * iterations: a-trous passes with steps 1, 2, 4, ... (0 = the mean itself, <= 12); sigma_normal: the exponent of
+ * the normal weight; sigma_depth, sigma_luminance: the depth and luminance tolerances; albedo_eps: added to the
+ * albedo before the colour is divided by it.  Defaults 5, 128, 1, 4, 1e-3.                                   */
+typedef struct rptb_denoise {
+    uint32_t iterations;
+    uint32_t sigma_normal;
+    double sigma_depth;
+    double sigma_luminance;
+    double albedo_eps;
+} rptb_denoise;
+/* Denoises the buffer's mean image on its first device, each pixel with its own entry count (adaptive buffers
+ * included): out_rgb (nullable) = width*height*3 linear doubles; out_rgb8 (nullable) = their bytes through the
+ * film resolve of Buffer::image with one entry and radius 0 (clamp, gamma 1/2.2, truncation) -- the buffer's box
+ * radius does not apply to a denoised image.  RPTB_ERR_BAD_ARG: no entries ("Pixel found with no samples"), a
+ * pixel with fewer than 2 entries (no variance), no features, iterations > 12, or a sigma / albedo_eps that is
+ * negative or not finite.                                                                                     */
+int rptb_buffer_denoise(rptb_buffer* buffer, const rptb_denoise* params, double* out_rgb /* nullable */,
+                        uint8_t* out_rgb8 /* nullable */);
+
 #ifdef __cplusplus
 }
 #endif

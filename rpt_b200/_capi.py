@@ -185,6 +185,17 @@ class Adaptive(C.Structure):
     ]
 
 
+class Denoise(C.Structure):
+    """rptb_denoise: the parameters of rptb_buffer_denoise."""
+    _fields_ = [
+        ("iterations", C.c_uint32),
+        ("sigma_normal", C.c_uint32),
+        ("sigma_depth", C.c_double),
+        ("sigma_luminance", C.c_double),
+        ("albedo_eps", C.c_double),
+    ]
+
+
 class KdTreeOut(C.Structure):
     _fields_ = [
         ("nodes", C.POINTER(KdNode)),
@@ -254,6 +265,10 @@ SYMBOLS = [
      [C.c_void_p, C.POINTER(Camera), C.POINTER(RenderParams), C.POINTER(Adaptive), C.c_void_p, C.POINTER(C.c_uint64),
       C.POINTER(Stats)]),
     ("rptb_buffer_pixel_stats", C.c_int, [C.c_void_p, c_double_p, c_double_p, c_u32_p]),
+    ("rptb_buffer_add_features", C.c_int,
+     [C.c_void_p, C.POINTER(Camera), C.POINTER(RenderParams), C.c_void_p, C.POINTER(Stats)]),
+    ("rptb_buffer_features", C.c_int, [C.c_void_p, c_double_p, c_double_p, c_double_p, c_double_p]),
+    ("rptb_buffer_denoise", C.c_int, [C.c_void_p, C.POINTER(Denoise), c_double_p, c_u8_p]),
 ]
 
 _lib = None

@@ -16,6 +16,7 @@ API, so scene scripts and tests read like the reference's examples:
     Buffer / Filter             src/buffer.rs:6-108
     DeviceBuffer                src/buffer.rs:6-93, kept on the GPU (rptb_buffer)
     Adaptive                    not in the reference: which pixels an adaptive Renderer.sample renders
+    Denoise                     not in the reference: the edge-avoiding filter of DeviceBuffer.denoise
     hex_color / color_bytes     src/color.rs:10-23
 
 Everything below `Renderer.sample` (src/renderer.rs:117-129) is *not* here:
@@ -859,6 +860,23 @@ class Adaptive:
         return (np.asarray(counts) < self.min_entries) | ~converged
 
 
+class Denoise:
+    """Parameters of DeviceBuffer.denoise (rptb_denoise), which stands beside the reference's Filter::Box: the spatial
+    part of SVGF, an edge-avoiding a-trous wavelet filter guided by the buffer's first-hit features (normal, depth,
+    albedo) and by each pixel's variance of the mean.  `iterations` passes (0 = the mean itself, at most 12);
+    sigma_normal is the exponent of the normal weight, sigma_depth and sigma_luminance the depth and luminance
+    tolerances, albedo_eps what is added to the albedo before the colour is divided by it (a black surface would
+    otherwise divide by zero).  rpt_b200/csrc/denoise.h gives every formula."""
+
+    def __init__(self, iterations: int = 5, sigma_normal: int = 128, sigma_depth: float = 1.0, sigma_luminance: float = 4.0,
+                 albedo_eps: float = 1e-3):
+        self.iterations, self.sigma_normal = int(iterations), int(sigma_normal)
+        self.sigma_depth, self.sigma_luminance, self.albedo_eps = float(sigma_depth), float(sigma_luminance), float(albedo_eps)
+
+    def to_c(self) -> capi.Denoise:
+        return capi.Denoise(self.iterations, self.sigma_normal, self.sigma_depth, self.sigma_luminance, self.albedo_eps)
+
+
 class Buffer:
     """src/buffer.rs:6-93.  Holds one equally weighted entry per pixel per
     `add_samples` call, like the reference's Vec<Vec<Color>>."""
@@ -912,6 +930,7 @@ class DeviceBuffer:
         self.devices = list(scene.devices)
         self.entries = 0  # entries per pixel: add_samples and Renderer.sample calls; with adaptive calls, the most any pixel has
         self.counted = False  # an adaptive Renderer.sample happened: pixels may hold different numbers of entries
+        self.feature_rays = 0  # camera rays per pixel in the features (Renderer.sample_features)
         self.handle = C.c_void_p()
         capi.check(capi.lib().rptb_buffer_create(scene.handle, self.width, self.height, self.filter.radius,
                                                  C.byref(self.handle)), "rptb_buffer_create")
@@ -962,6 +981,33 @@ class DeviceBuffer:
         out = C.c_double(0.0)
         capi.check(capi.lib().rptb_buffer_variance(self.handle, C.byref(out)), "rptb_buffer_variance")
         return float(out.value)
+
+    def features(self):
+        """The first-hit features added by Renderer.sample_features, row-major: (normal (H, W, 3), 0 where nothing was
+        hit; depth (H, W), +inf where nothing was hit; albedo (H, W, 3), a miss counting 1; hit fraction (H, W))."""
+        h, w = self.height, self.width
+        nrm, depth, alb, frac = np.empty((h, w, 3)), np.empty((h, w)), np.empty((h, w, 3)), np.empty((h, w))
+        capi.check(capi.lib().rptb_buffer_features(self.handle, nrm.ctypes.data_as(capi.c_double_p), depth.ctypes.data_as(capi.c_double_p),
+                                                   alb.ctypes.data_as(capi.c_double_p), frac.ctypes.data_as(capi.c_double_p)),
+                   "rptb_buffer_features")
+        return nrm, depth, alb, frac
+
+    def denoise(self, d: Optional[Denoise] = None) -> np.ndarray:
+        """The mean image through the edge-avoiding filter: (H, W, 3) float64, linear.  Needs features and at least two
+        entries per pixel."""
+        out = np.empty((self.height, self.width, 3))
+        c = (d or Denoise()).to_c()
+        capi.check(capi.lib().rptb_buffer_denoise(self.handle, C.byref(c), out.ctypes.data_as(capi.c_double_p), None),
+                   "rptb_buffer_denoise")
+        return out
+
+    def denoised_image(self, d: Optional[Denoise] = None) -> np.ndarray:
+        """denoise() through Buffer::image's clamp, gamma and cast (no box filter): (H, W, 3) uint8."""
+        out = np.empty((self.height, self.width, 3), np.uint8)
+        c = (d or Denoise()).to_c()
+        capi.check(capi.lib().rptb_buffer_denoise(self.handle, C.byref(c), None, out.ctypes.data_as(capi.c_u8_p)),
+                   "rptb_buffer_denoise")
+        return out
 
     def close(self) -> None:
         if self.handle:
@@ -1125,10 +1171,37 @@ class Renderer:
         self.last_stats = stats.as_dict()
         buffer.add_samples(colors)
 
-    def render(self) -> np.ndarray:  # :96-100
-        buffer = Buffer(self._width, self._height, self._filter, self._first_device())
-        self.sample(self._num_samples, buffer)
-        return buffer.image()
+    def sample_features(self, iterations: int, buffer: "DeviceBuffer", want_stats: bool = False) -> None:
+        """Adds the first hits of `iterations` more camera rays per pixel to the buffer's features
+        (rptb_buffer_add_features): the samples after those the buffer's features already hold (0 .. iterations - 1 on
+        the first call, the camera rays of the first entries' samples) of this renderer's seed, in its precision,
+        through its camera.  The entries of the buffer are not touched."""
+        if not isinstance(buffer, DeviceBuffer):
+            raise TypeError("features live in a DeviceBuffer (Renderer.device_buffer())")
+        ds = self.device_scene()
+        p = self.params(iterations, buffer.feature_rays)
+        cam = self.camera.to_c()
+        stats = capi.Stats()
+        capi.check(capi.lib().rptb_buffer_add_features(ds.handle, C.byref(cam), C.byref(p), buffer.handle,
+                                                       C.byref(stats) if want_stats else None), "rptb_buffer_add_features")
+        buffer.feature_rays += int(iterations)
+        self.last_stats = stats.as_dict() if want_stats else None
+
+    def render(self, denoise: Optional[Denoise] = None, entries: int = 8, feature_samples: int = 16) -> np.ndarray:  # :96-100
+        """Renderer::render.  With `denoise`, num_samples are rendered as `entries` equal entries of a DeviceBuffer,
+        `feature_samples` camera rays per pixel give it features, and the denoised bytes are returned."""
+        if denoise is None:
+            buffer = Buffer(self._width, self._height, self._filter, self._first_device())
+            self.sample(self._num_samples, buffer)
+            return buffer.image()
+        if entries < 2 or self._num_samples % entries:
+            # the entries are weighted equally: unequal ones would bias the mean
+            raise ValueError(f"num_samples {self._num_samples} must be a multiple of entries {entries} (and entries >= 2)")
+        with self.device_buffer() as buf:
+            for _ in range(entries):
+                self.sample(self._num_samples // entries, buf, want_stats=False)
+            self.sample_features(feature_samples, buf)
+            return buf.denoised_image(denoise)
 
     def iterative_render(self, callback_interval: int, callback: Callable[[int, Buffer], None],
                          buffer: Optional[DeviceBuffer] = None, adaptive: Optional[Adaptive] = None) -> None:  # :103-115

@@ -16,10 +16,16 @@
 
 namespace rptb {
 
+// err2 above: the channel-mean variance of the mean of a pixel with n entries and M2 (also the denoiser's, denoise.h)
+RPTB_HD double mean_variance(uint32_t n, double m2) {
+    const double dn = (double)n;
+    return m2 / (((dn - 1.0) * dn) * 3.0);
+}
+
 RPTB_HD bool adaptive_active(uint32_t n, double s0, double s1, double s2, double m2, const rptb_adaptive& c) {
     if (n < c.min_entries) return true;
     const double dn = (double)n;
-    const double err2 = m2 / (((dn - 1.0) * dn) * 3.0);
+    const double err2 = mean_variance(n, m2);
     const double m = ((s0 + s1) + s2) / (3.0 * dn);
     const double t = c.rel_tol * m + c.abs_tol;
     return !(err2 <= t * t);

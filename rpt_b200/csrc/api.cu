@@ -23,6 +23,7 @@
 #include <vector>
 
 #include "../../include/rpt_b200.h"
+#include "denoise.h"
 #include "flatten.h"
 #include "launch.h"
 
@@ -57,6 +58,12 @@ cudaError_t launch_adaptive_select(const double* sums, const double* m2, const u
                                    uint32_t height, uint32_t shard_index, uint32_t shard_count, const rptb_adaptive& crit,
                                    uint8_t* mask, uint8_t* flags, uint32_t* ids, uint32_t* len, unsigned long long* active_pixels,
                                    void* temp, size_t temp_bytes, cudaStream_t stream);
+// the feature planes and the denoiser: denoise.cu
+cudaError_t launch_features_resolve(const double* row_feat, uint64_t npix, double rays, double* nrm, double* depth, double* albedo,
+                                    double* frac, cudaStream_t stream);
+cudaError_t launch_denoise(const double* sums, const double* m2, const uint32_t* counts, uint32_t n, const double* nrm,
+                           const double* depth, const double* albedo, uint32_t width, uint32_t height, const rptb_denoise& d,
+                           double* const col[2], double* const var[2], double* out, cudaStream_t stream, uint32_t* launches);
 int parse_obj_text(const char* text, size_t len, std::vector<double>& tris, std::string& err);
 struct ObjGroup {
     rptb_material material;
@@ -581,6 +588,8 @@ struct BufferPart {
     unsigned long long* active = nullptr;
     void* temp = nullptr;
     size_t temp_bytes = 0;
+    // from the buffer's first rptb_buffer_add_features on: the first-hit feature sums, tiles*128*8 (features.cuh planes)
+    double* feat = nullptr;
 };
 
 struct rptb_buffer {
@@ -596,6 +605,12 @@ struct rptb_buffer {
     uint8_t* rgb8 = nullptr;
     uint32_t* row_counts = nullptr;     // `counted` only: width*height
     uint32_t* gather_counts = nullptr;  // one other part's counts
+    // features and denoiser, on parts[0]'s device, allocated by their first call
+    uint64_t feature_rays = 0;       // camera rays per pixel in the feature sums
+    double* row_feat = nullptr;      // width*height*8: the sums gathered row-major (features.cuh planes)
+    double* gather_feat = nullptr;   // one other part's feature sums
+    double* aov = nullptr;           // width*height*8: normal (3), albedo (3), depth, hit fraction planes
+    double* dn = nullptr;            // width*height*11: colour (3) and variance ping-pong planes, then c' (3)
     std::mutex lock;
 };
 
@@ -622,6 +637,7 @@ void buffer_free(rptb_buffer* b) {
         cudaFree(q.len);
         cudaFree(q.active);
         cudaFree(q.temp);
+        cudaFree(q.feat);
         if (i == 0) {
             cudaFree(b->row_sums);
             cudaFree(b->row_m2);
@@ -630,6 +646,10 @@ void buffer_free(rptb_buffer* b) {
             cudaFree(b->rgb8);
             cudaFree(b->row_counts);
             cudaFree(b->gather_counts);
+            cudaFree(b->row_feat);
+            cudaFree(b->gather_feat);
+            cudaFree(b->aov);
+            cudaFree(b->dn);
         }
         if (q.done) cudaEventDestroy(q.done);
         if (q.stream) cudaStreamDestroy(q.stream);
@@ -701,6 +721,42 @@ int buffer_gather_counts(rptb_buffer* b) {
         CU(cudaMemcpyPeerAsync(b->gather_counts, q0.device, q.counts, q.device, nelem * sizeof(uint32_t), q0.stream));
         CU(launch_buffer_scatter_counts(b->gather_counts, nelem, b->width, b->height, i, nparts, b->row_counts, q0.stream));
     }
+    return RPTB_OK;
+}
+
+// Brings every part's feature sums to parts[0] row-major (b->row_feat) and resolves the feature planes into b->aov, on
+// parts[0]'s stream (its device current).  The normal / albedo planes go through the Buffer's scatter as "sums", the hit
+// and depth planes as "M2".
+int buffer_features(rptb_buffer* b) {
+    BufferPart& q0 = b->parts[0];
+    const uint32_t nparts = (uint32_t)b->parts.size();
+    const size_t npix = (size_t)b->width * b->height;
+    if (!b->row_feat) {
+        uint32_t most = 0;
+        for (uint32_t i = 1; i < nparts; i++) most = std::max(most, b->parts[i].tiles);
+        CU(cudaMalloc((void**)&b->row_feat, npix * 8 * sizeof(double)));
+        CU(cudaMalloc((void**)&b->aov, npix * 8 * sizeof(double)));
+        if (most) CU(cudaMalloc((void**)&b->gather_feat, (size_t)most * 128u * 8u * sizeof(double)));
+    }
+    double* rn = b->row_feat;
+    double* ra = rn + 3 * npix;
+    double* rh = rn + 6 * npix;
+    double* rz = rn + 7 * npix;
+    for (uint32_t i = 0; i < nparts; i++) {
+        const BufferPart& q = b->parts[i];
+        if (!q.tiles) continue;
+        const size_t nelem = (size_t)q.tiles * 128u;
+        CU(cudaStreamWaitEvent(q0.stream, q.done, 0));
+        const double* src = q.feat;
+        if (i > 0) {
+            CU(cudaMemcpyPeerAsync(b->gather_feat, q0.device, q.feat, q.device, nelem * 8 * sizeof(double), q0.stream));
+            src = b->gather_feat;
+        }
+        CU(launch_buffer_scatter(src, src + 6 * nelem, nelem, b->width, b->height, i, nparts, rn, rh, q0.stream));
+        CU(launch_buffer_scatter(src + 3 * nelem, src + 7 * nelem, nelem, b->width, b->height, i, nparts, ra, rz, q0.stream));
+    }
+    double* a = b->aov;
+    CU(launch_features_resolve(b->row_feat, npix, (double)b->feature_rays, a, a + 6 * npix, a + 3 * npix, a + 7 * npix, q0.stream));
     return RPTB_OK;
 }
 
@@ -1558,6 +1614,130 @@ int rptb_buffer_pixel_stats(rptb_buffer* b, double* sums, double* m2, uint32_t* 
     }
     CU(cudaStreamSynchronize(q0.stream));
     if (counts && !b->counted) std::fill(counts, counts + npix, b->entries);
+    return RPTB_OK;
+}
+
+int rptb_buffer_add_features(rptb_scene* s, const rptb_camera* cam, const rptb_render_params* p, rptb_buffer* b, rptb_stats* stats) {
+    if (!b) return fail(RPTB_ERR_BAD_ARG, "null argument");
+    int rc = check_params(s, cam, p);
+    if (rc != RPTB_OK) return rc;
+    if (p->shard_count > 1)
+        return fail(RPTB_ERR_UNSUPPORTED, "shard_count %u: a buffer holds the whole image (shard with rptb_render_samples_device)", p->shard_count);
+    if (p->width != b->width || p->height != b->height)
+        return fail(RPTB_ERR_BAD_ARG, "render is %ux%u but the buffer is %ux%u", p->width, p->height, b->width, b->height);
+    const uint32_t nparts = 1u + (uint32_t)s->peers.size();
+    bool same = nparts == b->parts.size();
+    for (uint32_t i = 0; same && i < nparts; i++) same = (i == 0 ? s->device : s->peers[i - 1]->device) == b->parts[i].device;
+    if (!same) return fail(RPTB_ERR_BAD_ARG, "the buffer was created on a scene with another device list");
+    std::lock_guard<std::mutex> bl(b->lock);
+    if (b->feature_rays > UINT64_MAX / 2) return fail(RPTB_ERR_UNSUPPORTED, "too many feature rays");
+    // every replica's share is enqueued before any is waited for
+    std::vector<std::unique_lock<std::mutex>> locks;
+    for (uint32_t i = 0; i < nparts; i++) {
+        rptb_scene* r = i == 0 ? s : s->peers[i - 1];
+        BufferPart& q = b->parts[i];
+        locks.emplace_back(r->lock);
+        DeviceGuard g(r->device);
+        if (!g.ok) return fail(RPTB_ERR_CUDA, "cudaSetDevice(%d) failed", r->device);
+        const size_t nelem = (size_t)q.tiles * 128u;
+        CU(cudaStreamWaitEvent(r->stream, q.done, 0));
+        if (!q.feat && nelem) {
+            CU(cudaMalloc((void**)&q.feat, nelem * 8 * sizeof(double)));
+            CU(cudaMemsetAsync(q.feat, 0, nelem * 8 * sizeof(double), r->stream));
+        }
+        rptb_render_params qp = *p;
+        qp.shard_index = i;
+        qp.shard_count = nparts;
+        if (stats) CU(cudaEventRecord(r->ev0, r->stream));
+        if (p->precision == RPTB_PRECISION_F32) {
+            RenderArgs<float> a;
+            fill_args(cam, &qp, a);
+            CU(launch_features_f32(r->view32, a, r->features, q.feat, r->stream));
+        } else {
+            RenderArgs<double> a;
+            fill_args(cam, &qp, a);
+            CU(launch_features_f64(r->view64, a, r->features, q.feat, r->stream));
+        }
+        if (stats) CU(cudaEventRecord(r->ev1, r->stream));
+        CU(cudaEventRecord(q.done, r->stream));
+    }
+    b->feature_rays += p->iterations;
+    if (!stats) return RPTB_OK;
+    std::memset(stats, 0, sizeof(*stats));
+    for (uint32_t i = 0; i < nparts; i++) {
+        rptb_scene* r = i == 0 ? s : s->peers[i - 1];
+        DeviceGuard g(r->device);
+        CU(cudaEventSynchronize(r->ev1));
+        float ms = 0;
+        CU(cudaEventElapsedTime(&ms, r->ev0, r->ev1));
+        stats->gpu_ms = std::max(stats->gpu_ms, (double)ms);  // the devices run concurrently
+        stats->launches += b->parts[i].tiles ? 1u : 0u;
+    }
+    stats->rays = (uint64_t)b->width * b->height * p->iterations;
+    stats->engine = RPTB_ENGINE_MEGAKERNEL;
+    return RPTB_OK;
+}
+
+int rptb_buffer_features(rptb_buffer* b, double* normal, double* depth, double* albedo, double* hit_fraction) {
+    if (!b) return fail(RPTB_ERR_BAD_ARG, "null argument");
+    std::lock_guard<std::mutex> bl(b->lock);
+    if (b->feature_rays == 0) return fail(RPTB_ERR_BAD_ARG, "the buffer holds no features (rptb_buffer_add_features)");
+    BufferPart& q0 = b->parts[0];
+    DeviceGuard g(q0.device);
+    const int rc = buffer_features(b);
+    if (rc != RPTB_OK) return rc;
+    const size_t npix = (size_t)b->width * b->height;
+    if (normal) CU(cudaMemcpyAsync(normal, b->aov, npix * 3 * sizeof(double), cudaMemcpyDeviceToHost, q0.stream));
+    if (albedo) CU(cudaMemcpyAsync(albedo, b->aov + 3 * npix, npix * 3 * sizeof(double), cudaMemcpyDeviceToHost, q0.stream));
+    if (depth) CU(cudaMemcpyAsync(depth, b->aov + 6 * npix, npix * sizeof(double), cudaMemcpyDeviceToHost, q0.stream));
+    if (hit_fraction) CU(cudaMemcpyAsync(hit_fraction, b->aov + 7 * npix, npix * sizeof(double), cudaMemcpyDeviceToHost, q0.stream));
+    CU(cudaStreamSynchronize(q0.stream));
+    return RPTB_OK;
+}
+
+int rptb_buffer_denoise(rptb_buffer* b, const rptb_denoise* d, double* out_rgb, uint8_t* out_rgb8) {
+    if (!b || !d) return fail(RPTB_ERR_BAD_ARG, "null argument");
+    if (d->iterations > kDenoiseMaxIterations)
+        return fail(RPTB_ERR_BAD_ARG, "iterations %u > %u", d->iterations, kDenoiseMaxIterations);
+    if (!(std::isfinite(d->sigma_depth) && d->sigma_depth >= 0.0) || !(std::isfinite(d->sigma_luminance) && d->sigma_luminance >= 0.0) ||
+        !(std::isfinite(d->albedo_eps) && d->albedo_eps >= 0.0))
+        return fail(RPTB_ERR_BAD_ARG, "sigma_depth, sigma_luminance and albedo_eps must be finite and >= 0 (%g, %g, %g)", d->sigma_depth,
+                    d->sigma_luminance, d->albedo_eps);
+    std::lock_guard<std::mutex> bl(b->lock);
+    if (b->entries == 0) return fail(RPTB_ERR_BAD_ARG, "Pixel found with no samples");  // buffer.rs:89
+    if (!b->counted && b->entries < 2) return fail(RPTB_ERR_BAD_ARG, "a pixel has fewer than 2 entries (no variance to guide the filter)");
+    if (b->feature_rays == 0) return fail(RPTB_ERR_BAD_ARG, "the buffer holds no features (rptb_buffer_add_features)");
+    BufferPart& q0 = b->parts[0];
+    DeviceGuard g(q0.device);
+    const size_t npix = (size_t)b->width * b->height;
+    int rc = buffer_gather(b, true, true);
+    if (rc != RPTB_OK) return rc;
+    if (b->counted) {
+        rc = buffer_gather_counts(b);
+        if (rc != RPTB_OK) return rc;
+        std::vector<uint32_t> counts(npix);
+        CU(cudaMemcpyAsync(counts.data(), b->row_counts, npix * sizeof(uint32_t), cudaMemcpyDeviceToHost, q0.stream));
+        CU(cudaStreamSynchronize(q0.stream));
+        for (uint32_t c : counts)
+            if (c < 2) return fail(RPTB_ERR_BAD_ARG, "a pixel has fewer than 2 entries (no variance to guide the filter)");
+    }
+    rc = buffer_features(b);
+    if (rc != RPTB_OK) return rc;
+    if (!b->dn) CU(cudaMalloc((void**)&b->dn, npix * 11 * sizeof(double)));
+    double* const col[2] = {b->dn, b->dn + 3 * npix};
+    double* const var[2] = {b->dn + 6 * npix, b->dn + 7 * npix};
+    double* out = b->dn + 8 * npix;
+    const double* a = b->aov;
+    uint32_t launches = 0;
+    CU(launch_denoise(b->row_sums, b->row_m2, b->counted ? b->row_counts : nullptr, b->entries, a, a + 6 * npix, a + 3 * npix, b->width,
+                      b->height, *d, col, var, out, q0.stream, &launches));
+    if (out_rgb) CU(cudaMemcpyAsync(out_rgb, out, npix * 3 * sizeof(double), cudaMemcpyDeviceToHost, q0.stream));
+    if (out_rgb8) {
+        // the film resolve of one entry at radius 0: clamp, gamma and the truncating cast of Buffer::image
+        CU(launch_film_resolve(out, 1u, b->width, b->height, 0u, b->rgb8, q0.stream));
+        CU(cudaMemcpyAsync(out_rgb8, b->rgb8, npix * 3, cudaMemcpyDeviceToHost, q0.stream));
+    }
+    CU(cudaStreamSynchronize(q0.stream));
     return RPTB_OK;
 }
 

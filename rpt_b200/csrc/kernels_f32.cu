@@ -3,11 +3,15 @@
 
 #include <cstring>
 
+#include "features.cuh"
 #include "launch_impl.cuh"
 #include "wavefront.cuh"
 
 namespace rptb {
 RPTB_DEFINE_LAUNCHERS(f32, float)
+cudaError_t launch_features_f32(const SceneView<float>& sv, const RenderArgs<float>& args, int features, double* acc, cudaStream_t stream) {
+    return launch_features_impl<float>(sv, args, features, acc, stream);
+}
 
 static size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
 

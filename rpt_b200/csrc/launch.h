@@ -30,6 +30,11 @@ cudaError_t launch_render_list_f32(const SceneView<float>& sv, const RenderArgs<
 cudaError_t launch_render_list_f64(const SceneView<double>& sv, const RenderArgs<double>& args, const RenderList& list,
                                    int stats, int features, cudaStream_t stream, uint32_t* launches);
 
+// The first-hit feature pass (features.cuh) over args' owned tiles: adds args.iterations camera rays per pixel to the
+// compact per-pixel sums `acc` (ntiles_mine * 128 * 8 doubles).
+cudaError_t launch_features_f32(const SceneView<float>& sv, const RenderArgs<float>& args, int features, double* acc, cudaStream_t stream);
+cudaError_t launch_features_f64(const SceneView<double>& sv, const RenderArgs<double>& args, int features, double* acc, cudaStream_t stream);
+
 // ---- wavefront engine (f32 only; wavefront.cuh) -------------------------------------------
 struct WfBuffers;
 // bytes of device memory the engine needs for (npaths, Ks sampled lights, maxd levels)

@@ -928,8 +928,7 @@ class DeviceBuffer:
         self.width, self.height = int(width), int(height)
         self.filter = filter or Filter()
         self.devices = list(scene.devices)
-        self.entries = 0  # entries per pixel: add_samples and Renderer.sample calls; with adaptive calls, the most any pixel has
-        self.counted = False  # an adaptive Renderer.sample happened: pixels may hold different numbers of entries
+        self.entries = 0  # the most entries any pixel holds (every pixel, without adaptive calls)
         self.feature_rays = 0  # camera rays per pixel in the features (Renderer.sample_features)
         self.handle = C.c_void_p()
         capi.check(capi.lib().rptb_buffer_create(scene.handle, self.width, self.height, self.filter.radius,
@@ -948,9 +947,7 @@ class DeviceBuffer:
         n = C.c_uint32(0)
         capi.check(capi.lib().rptb_buffer_sums(self.handle, out.ctypes.data_as(capi.c_double_p), C.byref(n)),
                    "rptb_buffer_sums")
-        if self.counted:
-            self.entries = int(n.value)
-        assert n.value == self.entries
+        self.entries = int(n.value)
         return out
 
     def pixel_stats(self):
@@ -1147,7 +1144,6 @@ class Renderer:
                                                             C.byref(active), C.byref(stats) if want_stats else None),
                        "rptb_sample_into_adaptive")
             self._next_sample += int(iterations)
-            buffer.counted = True
             if active.value:  # the largest per-pixel count, as rptb_buffer_sums reports it
                 buffer.entries = int(buffer.counts().max())
             self.last_stats = stats.as_dict() if want_stats else None

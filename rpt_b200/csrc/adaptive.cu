@@ -9,6 +9,7 @@
 #include <cub/iterator/counting_input_iterator.cuh>
 
 #include "adaptive.h"
+#include "tile.h"
 
 namespace rptb {
 
@@ -19,17 +20,14 @@ __global__ void __launch_bounds__(128) adaptive_mark_kernel(const double* __rest
                                                             unsigned long long* __restrict__ active_pixels) {
     const uint32_t k = blockIdx.x, j = threadIdx.x;
     const uint64_t e = (uint64_t)k * 128u + j;
-    // pixel j of owned tile k (rptb_tile_pixel); the slots past a ragged edge are never active
-    const uint32_t tile = shard_index + k * shard_count, tiles_x = (width + 15u) / 16u;
-    const uint32_t warp = j >> 5, lane = j & 31u;
-    const uint32_t x = (tile % tiles_x) * 16u + (warp & 1u) * 8u + (lane & 7u);
-    const uint32_t y = (tile / tiles_x) * 8u + (warp >> 1) * 4u + (lane >> 3);
+    // pixel j of owned tile k; the slots past a ragged edge are never active
     bool on = false;
-    if (x < width && y < height) on = adaptive_active(counts[e], sums[3 * e], sums[3 * e + 1], sums[3 * e + 2], m2[e], crit);
+    if (tile_pixel(width, height, shard_index + k * shard_count, j) >= 0)
+        on = adaptive_active(counts[e], sums[3 * e], sums[3 * e + 1], sums[3 * e + 2], m2[e], crit);
     mask[e] = on ? 1u : 0u;
     const unsigned votes = __ballot_sync(0xffffffffu, on);
-    if (lane == 0) {
-        flags[(uint64_t)k * 4u + warp] = votes != 0u ? 1u : 0u;
+    if ((j & 31u) == 0) {
+        flags[(uint64_t)k * 4u + (j >> 5)] = votes != 0u ? 1u : 0u;
         if (votes) atomicAdd(active_pixels, (unsigned long long)__popc(votes));
     }
 }

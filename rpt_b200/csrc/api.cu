@@ -11,6 +11,7 @@
 //   rptb_film_resolve          Buffer::image (src/buffer.rs:43-56,75-93)
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <cmath>
 #include <cstdarg>
 #include <cstdio>
@@ -26,30 +27,23 @@
 #include "denoise.h"
 #include "flatten.h"
 #include "launch.h"
+#include "tile.h"
 
 namespace rptb {
 cudaError_t launch_film_resolve(const double* sums, uint32_t nbatches, uint32_t width, uint32_t height,
                                 uint32_t radius, uint8_t* out, cudaStream_t stream);
 cudaError_t launch_convert_f64_to_f32(const double* in, float* out, size_t n, cudaStream_t stream);
 cudaError_t launch_film_variance(const double* batches, uint32_t nbatches, uint64_t npixels, double* out_sum, cudaStream_t stream);
-cudaError_t launch_buffer_accumulate(const float* in32, const double* in64, bool rowmajor, uint32_t n, uint64_t nelem,
-                                     uint32_t width, uint32_t height, uint32_t shard_index, uint32_t shard_count,
-                                     double* sums, double* m2, cudaStream_t stream);
-cudaError_t launch_buffer_scatter(const double* sums, const double* m2, uint64_t nelem, uint32_t width, uint32_t height,
-                                  uint32_t shard_index, uint32_t shard_count, double* row_sums, double* row_m2,
-                                  cudaStream_t stream);
+// the device Buffer: film.cu
+cudaError_t launch_buffer_accumulate(const float* in32, const double* in64, bool rowmajor, const uint8_t* mask, uint64_t nelem,
+                                     uint32_t width, uint32_t height, uint32_t shard_index, uint32_t shard_count, double* sums,
+                                     double* m2, uint32_t* counts, cudaStream_t stream);
+cudaError_t launch_buffer_scatter(const double* sums, const double* m2, const uint32_t* counts, uint64_t nelem, uint32_t width,
+                                  uint32_t height, uint32_t shard_index, uint32_t shard_count, double* row_sums, double* row_m2,
+                                  uint32_t* row_counts, cudaStream_t stream);
 uint32_t buffer_variance_blocks(uint64_t npixels);
-cudaError_t launch_buffer_variance(const double* m2, uint64_t npixels, uint32_t n, double* partial, double* out_sum,
-                                   cudaStream_t stream);
-// per-pixel entry counts (adaptive sampling): film.cu
-cudaError_t launch_buffer_accumulate_counted(const float* in32, const double* in64, bool rowmajor, const uint8_t* mask,
-                                             uint64_t nelem, uint32_t width, uint32_t height, uint32_t shard_index,
-                                             uint32_t shard_count, double* sums, double* m2, uint32_t* counts, cudaStream_t stream);
-cudaError_t launch_buffer_counts_fill(uint32_t* counts, uint64_t nelem, uint32_t value, cudaStream_t stream);
-cudaError_t launch_buffer_scatter_counts(const uint32_t* counts, uint64_t nelem, uint32_t width, uint32_t height,
-                                         uint32_t shard_index, uint32_t shard_count, uint32_t* row_counts, cudaStream_t stream);
-cudaError_t launch_buffer_variance_counted(const double* m2, const uint32_t* counts, uint64_t npixels, double* partial,
-                                           double* out_sum, cudaStream_t stream);
+cudaError_t launch_buffer_variance_sum(const double* m2, const uint32_t* counts, uint64_t npixels, double* partial,
+                                       double* out_sum, cudaStream_t stream);
 cudaError_t launch_film_resolve_counted(const double* sums, const uint32_t* counts, uint32_t width, uint32_t height,
                                         uint32_t radius, uint8_t* out, cudaStream_t stream);
 // the active pixels and warp blocks of an adaptive call: adaptive.cu
@@ -61,7 +55,7 @@ cudaError_t launch_adaptive_select(const double* sums, const double* m2, const u
 // the feature planes and the denoiser: denoise.cu
 cudaError_t launch_features_resolve(const double* row_feat, uint64_t npix, double rays, double* nrm, double* depth, double* albedo,
                                     double* frac, cudaStream_t stream);
-cudaError_t launch_denoise(const double* sums, const double* m2, const uint32_t* counts, uint32_t n, const double* nrm,
+cudaError_t launch_denoise(const double* sums, const double* m2, const uint32_t* counts, const double* nrm,
                            const double* depth, const double* albedo, uint32_t width, uint32_t height, const rptb_denoise& d,
                            double* const col[2], double* const var[2], double* out, cudaStream_t stream, uint32_t* launches);
 int parse_obj_text(const char* text, size_t len, std::vector<double>& tris, std::string& err);
@@ -565,7 +559,7 @@ void destroy_replica(rptb_scene* s) {
 
 // ---- the device-resident Buffer (src/buffer.rs:6-93) ------------------------------------------------------------
 // One part per replica of the scene it was created on, each holding that replica's own 16x8 tiles in the compact
-// tile-major layout (film.cu): 3 running sums and one Welford M2 per pixel, in double.  The buffer owns its memory
+// tile-major layout (film.cu): 3 running sums and one Welford M2 per pixel, in double, and its entry count.  The buffer owns its memory
 // (cudaMalloc, so destroy hands it back to the driver), its streams and its events, so it and its scene may be
 // destroyed in either order.  `done` is recorded behind every accumulate -- on the scene's stream (rptb_sample_into)
 // or on the part's own (rptb_buffer_add_samples) -- and every later operation on the part waits for it.
@@ -574,13 +568,13 @@ struct BufferPart {
     uint32_t tiles = 0;          // tiles t with t % nparts == this part's index
     double* sums = nullptr;      // tiles * 128 * 3
     double* m2 = nullptr;        // tiles * 128
+    uint32_t* counts = nullptr;  // tiles * 128
     double* upload = nullptr;    // a host entry, row-major width*height*3 (first add_samples allocates it)
     cudaStream_t stream = nullptr;
     cudaEvent_t done = nullptr;
-    // from the buffer's first adaptive call on: per-pixel entry counts, and that call's scratch -- the pixel mask
-    // (tiles*128), the flag and the id list of the active 8x4 warp blocks (tiles*4), the list's length, the number of
-    // active pixels, and the select's temporary storage
-    uint32_t* counts = nullptr;
+    // from the buffer's first adaptive call on, that call's scratch: the pixel mask (tiles*128), the flag and the id
+    // list of the active 8x4 warp blocks (tiles*4), the list's length, the number of active pixels, and the select's
+    // temporary storage
     uint8_t* mask = nullptr;
     uint8_t* flags = nullptr;
     uint32_t* ids = nullptr;
@@ -594,17 +588,17 @@ struct BufferPart {
 
 struct rptb_buffer {
     uint32_t width = 0, height = 0, radius = 0;
-    uint32_t entries = 0;  // accumulate calls; with `counted`, the largest per-pixel count is at most this
-    bool counted = false;  // an adaptive call happened: every part keeps per-pixel counts
+    // accumulate calls.  No pixel holds more entries, and every pixel holds at least min(entries, 2): see
+    // rptb_buffer_denoise
+    uint32_t entries = 0;
     std::vector<BufferPart> parts;
     // on parts[0]'s device, allocated by the first image / variance / sums: the image gathered row-major
     double* row_sums = nullptr;  // width*height*3
-    double* row_m2 = nullptr;    // width*height
-    double* gather = nullptr;    // one other part's sums + M2, copied over
-    double* partial = nullptr;   // variance block partials, then the total
+    double* row_m2 = nullptr;        // width*height
+    uint32_t* row_counts = nullptr;  // width*height
+    double* gather = nullptr;        // one other part's sums + M2 + counts, copied over
+    double* partial = nullptr;       // variance block partials, then the total
     uint8_t* rgb8 = nullptr;
-    uint32_t* row_counts = nullptr;     // `counted` only: width*height
-    uint32_t* gather_counts = nullptr;  // one other part's counts
     // features and denoiser, on parts[0]'s device, allocated by their first call
     uint64_t feature_rays = 0;       // camera rays per pixel in the feature sums
     double* row_feat = nullptr;      // width*height*8: the sums gathered row-major (features.cuh planes)
@@ -645,7 +639,6 @@ void buffer_free(rptb_buffer* b) {
             cudaFree(b->partial);
             cudaFree(b->rgb8);
             cudaFree(b->row_counts);
-            cudaFree(b->gather_counts);
             cudaFree(b->row_feat);
             cudaFree(b->gather_feat);
             cudaFree(b->aov);
@@ -664,16 +657,18 @@ int buffer_part_alloc(BufferPart& q) {
         const size_t nelem = (size_t)q.tiles * 128u;
         CU(cudaMalloc((void**)&q.sums, nelem * 3 * sizeof(double)));
         CU(cudaMalloc((void**)&q.m2, nelem * sizeof(double)));
+        CU(cudaMalloc((void**)&q.counts, nelem * sizeof(uint32_t)));
         CU(cudaMemsetAsync(q.sums, 0, nelem * 3 * sizeof(double), q.stream));  // sums() of an empty buffer reads zero
         CU(cudaMemsetAsync(q.m2, 0, nelem * sizeof(double), q.stream));
+        CU(cudaMemsetAsync(q.counts, 0, nelem * sizeof(uint32_t), q.stream));
     }
     CU(cudaEventRecord(q.done, q.stream));
     return RPTB_OK;
 }
 
-// Brings every part's sums and/or M2 to parts[0]'s device in row-major order, on parts[0]'s stream (the caller has
-// made that device current).  Other parts are copied with cudaMemcpyPeerAsync, which needs no peer access.
-int buffer_gather(rptb_buffer* b, bool want_sums, bool want_m2) {
+// Brings every part's sums, M2 and/or counts to parts[0]'s device in row-major order, on parts[0]'s stream (the caller
+// has made that device current).  Other parts are copied with cudaMemcpyPeerAsync, which needs no peer access.
+int buffer_gather(rptb_buffer* b, bool want_sums, bool want_m2, bool want_counts) {
     BufferPart& q0 = b->parts[0];
     const uint32_t nparts = (uint32_t)b->parts.size();
     const size_t npix = (size_t)b->width * b->height;
@@ -682,44 +677,28 @@ int buffer_gather(rptb_buffer* b, bool want_sums, bool want_m2) {
         for (uint32_t i = 1; i < nparts; i++) most = std::max(most, b->parts[i].tiles);
         CU(cudaMalloc((void**)&b->row_sums, npix * 3 * sizeof(double)));
         CU(cudaMalloc((void**)&b->row_m2, npix * sizeof(double)));
-        if (most) CU(cudaMalloc((void**)&b->gather, (size_t)most * 128u * 4u * sizeof(double)));
+        CU(cudaMalloc((void**)&b->row_counts, npix * sizeof(uint32_t)));
+        if (most) CU(cudaMalloc((void**)&b->gather, (size_t)most * 128u * (4u * sizeof(double) + sizeof(uint32_t))));
         CU(cudaMalloc((void**)&b->partial, (buffer_variance_blocks(npix) + 1) * sizeof(double)));
         CU(cudaMalloc((void**)&b->rgb8, npix * 3));
     }
     double* rs = want_sums ? b->row_sums : nullptr;
     double* rm = want_m2 ? b->row_m2 : nullptr;
+    uint32_t* rc = want_counts ? b->row_counts : nullptr;
     CU(cudaStreamWaitEvent(q0.stream, q0.done, 0));
-    CU(launch_buffer_scatter(q0.sums, q0.m2, (uint64_t)q0.tiles * 128u, b->width, b->height, 0, nparts, rs, rm, q0.stream));
+    CU(launch_buffer_scatter(q0.sums, q0.m2, q0.counts, (uint64_t)q0.tiles * 128u, b->width, b->height, 0, nparts, rs, rm, rc,
+                             q0.stream));
     for (uint32_t i = 1; i < nparts; i++) {
         const BufferPart& q = b->parts[i];
         if (!q.tiles) continue;
         const size_t nelem = (size_t)q.tiles * 128u;
+        uint32_t* counts = (uint32_t*)(b->gather + nelem * 4);
         CU(cudaStreamWaitEvent(q0.stream, q.done, 0));
         if (want_sums) CU(cudaMemcpyPeerAsync(b->gather, q0.device, q.sums, q.device, nelem * 3 * sizeof(double), q0.stream));
         if (want_m2) CU(cudaMemcpyPeerAsync(b->gather + nelem * 3, q0.device, q.m2, q.device, nelem * sizeof(double), q0.stream));
-        CU(launch_buffer_scatter(b->gather, b->gather + nelem * 3, nelem, b->width, b->height, i, nparts, rs, rm, q0.stream));
-    }
-    return RPTB_OK;
-}
-
-// The same for the per-pixel counts of a `counted` buffer, into b->row_counts.  Called after buffer_gather, which has
-// ordered parts[0]'s stream behind every part.
-int buffer_gather_counts(rptb_buffer* b) {
-    BufferPart& q0 = b->parts[0];
-    const uint32_t nparts = (uint32_t)b->parts.size();
-    if (!b->row_counts) {
-        uint32_t most = 0;
-        for (uint32_t i = 1; i < nparts; i++) most = std::max(most, b->parts[i].tiles);
-        CU(cudaMalloc((void**)&b->row_counts, (size_t)b->width * b->height * sizeof(uint32_t)));
-        if (most) CU(cudaMalloc((void**)&b->gather_counts, (size_t)most * 128u * sizeof(uint32_t)));
-    }
-    CU(launch_buffer_scatter_counts(q0.counts, (uint64_t)q0.tiles * 128u, b->width, b->height, 0, nparts, b->row_counts, q0.stream));
-    for (uint32_t i = 1; i < nparts; i++) {
-        const BufferPart& q = b->parts[i];
-        if (!q.tiles) continue;
-        const size_t nelem = (size_t)q.tiles * 128u;
-        CU(cudaMemcpyPeerAsync(b->gather_counts, q0.device, q.counts, q.device, nelem * sizeof(uint32_t), q0.stream));
-        CU(launch_buffer_scatter_counts(b->gather_counts, nelem, b->width, b->height, i, nparts, b->row_counts, q0.stream));
+        if (want_counts) CU(cudaMemcpyPeerAsync(counts, q0.device, q.counts, q.device, nelem * sizeof(uint32_t), q0.stream));
+        CU(launch_buffer_scatter(b->gather, b->gather + nelem * 3, counts, nelem, b->width, b->height, i, nparts, rs, rm, rc,
+                                 q0.stream));
     }
     return RPTB_OK;
 }
@@ -752,28 +731,27 @@ int buffer_features(rptb_buffer* b) {
             CU(cudaMemcpyPeerAsync(b->gather_feat, q0.device, q.feat, q.device, nelem * 8 * sizeof(double), q0.stream));
             src = b->gather_feat;
         }
-        CU(launch_buffer_scatter(src, src + 6 * nelem, nelem, b->width, b->height, i, nparts, rn, rh, q0.stream));
-        CU(launch_buffer_scatter(src + 3 * nelem, src + 7 * nelem, nelem, b->width, b->height, i, nparts, ra, rz, q0.stream));
+        CU(launch_buffer_scatter(src, src + 6 * nelem, nullptr, nelem, b->width, b->height, i, nparts, rn, rh, nullptr, q0.stream));
+        CU(launch_buffer_scatter(src + 3 * nelem, src + 7 * nelem, nullptr, nelem, b->width, b->height, i, nparts, ra, rz, nullptr,
+                                 q0.stream));
     }
     double* a = b->aov;
     CU(launch_features_resolve(b->row_feat, npix, (double)b->feature_rays, a, a + 6 * npix, a + 3 * npix, a + 7 * npix, q0.stream));
     return RPTB_OK;
 }
 
-// Gives part q per-pixel counts, all equal to `entries` (its first adaptive call), and the scratch of the select.
-int buffer_part_count(BufferPart& q, uint32_t entries, cudaStream_t stream) {
+// Gives part q the scratch of the select (its first adaptive call).
+int buffer_part_select_alloc(BufferPart& q) {
     if (q.len) return RPTB_OK;
     const size_t nelem = (size_t)q.tiles * 128u, nblocks = (size_t)q.tiles * 4u;
     CU(cudaMalloc((void**)&q.len, sizeof(uint32_t)));
     CU(cudaMalloc((void**)&q.active, sizeof(unsigned long long)));
     if (q.tiles) {
-        CU(cudaMalloc((void**)&q.counts, nelem * sizeof(uint32_t)));
         CU(cudaMalloc((void**)&q.mask, nelem));
         CU(cudaMalloc((void**)&q.flags, nblocks));
         CU(cudaMalloc((void**)&q.ids, nblocks * sizeof(uint32_t)));
         q.temp_bytes = adaptive_temp_bytes(q.tiles);
         CU(cudaMalloc(&q.temp, q.temp_bytes ? q.temp_bytes : 1));
-        CU(launch_buffer_counts_fill(q.counts, nelem, entries, stream));
     }
     return RPTB_OK;
 }
@@ -806,12 +784,11 @@ int render_list_launch(rptb_scene* s, const rptb_camera* cam, const rptb_render_
 }
 
 // Enqueues replica `index` of `nparts`'s share of one rptb_sample_into on the replica's own stream: render its
-// tiles into the compact out32/out64 scratch, then add them to the buffer part as entry `n`.  No host synchronise.
-// `crit` (rptb_sample_into_adaptive): first decide which pixels and warp blocks are active, render those through the
-// list schedule and add the entry to them alone.  A `counted` buffer adds with each pixel's own count.
+// tiles into the compact out32/out64 scratch, then add them to the buffer part as one more entry of every pixel.  No
+// host synchronise.  `crit` (rptb_sample_into_adaptive): first decide which pixels and warp blocks are active, render
+// those through the list schedule and add the entry to them alone.
 int sample_part(rptb_scene* r, const rptb_camera* cam, const rptb_render_params* p, uint32_t index, uint32_t nparts,
-                uint32_t n, BufferPart& q, bool want_stats, uint32_t* launches, bool counted = false,
-                const rptb_adaptive* crit = nullptr) {
+                BufferPart& q, bool want_stats, uint32_t* launches, const rptb_adaptive* crit = nullptr) {
     DeviceGuard g(r->device);
     if (!g.ok) return fail(RPTB_ERR_CUDA, "cudaSetDevice(%d) failed", r->device);
     int rc = wait_busy(r, r->stream);
@@ -824,7 +801,7 @@ int sample_part(rptb_scene* r, const rptb_camera* cam, const rptb_render_params*
     if (rc != RPTB_OK) return rc;
     CU(cudaStreamWaitEvent(r->stream, q.done, 0));  // an add_samples on the part's own stream
     if (crit) {
-        rc = buffer_part_count(q, n - 1u, r->stream);
+        rc = buffer_part_select_alloc(q);
         if (rc != RPTB_OK) return rc;
     }
     if (want_stats) CU(cudaEventRecord(r->ev0, r->stream));
@@ -840,12 +817,8 @@ int sample_part(rptb_scene* r, const rptb_camera* cam, const rptb_render_params*
     if (rc != RPTB_OK) return rc;
     if (want_stats && !crit) CU(cudaEventRecord(r->ev1, r->stream));
     const bool f32 = p->precision == RPTB_PRECISION_F32;
-    if (counted)
-        CU(launch_buffer_accumulate_counted(f32 ? r->out32 : nullptr, f32 ? nullptr : r->out64, false, crit ? q.mask : nullptr, nelem,
-                                            p->width, p->height, index, nparts, q.sums, q.m2, q.counts, r->stream));
-    else
-        CU(launch_buffer_accumulate(f32 ? r->out32 : nullptr, f32 ? nullptr : r->out64, false, n, nelem, p->width, p->height,
-                                    index, nparts, q.sums, q.m2, r->stream));
+    CU(launch_buffer_accumulate(f32 ? r->out32 : nullptr, f32 ? nullptr : r->out64, false, crit ? q.mask : nullptr, nelem, p->width,
+                                p->height, index, nparts, q.sums, q.m2, q.counts, r->stream));
     // (an adaptive call times the whole entry: select, render and accumulate; a plain one its render)
     if (want_stats && crit) CU(cudaEventRecord(r->ev1, r->stream));
     (*launches)++;
@@ -1115,12 +1088,10 @@ int64_t rptb_tile_pixel(uint32_t width, uint32_t height, uint32_t shard_index, u
     const uint32_t sc = shard_count ? shard_count : 1u;
     const uint32_t tiles_x = (width + 15u) / 16u, tiles_y = (height + 7u) / 8u;
     const uint64_t tile = (uint64_t)shard_index + (uint64_t)k * sc;
-    if (width == 0 || height == 0 || j >= 128u || shard_index >= sc || tile >= (uint64_t)tiles_x * tiles_y) return -1;
-    const uint32_t tx = (uint32_t)(tile % tiles_x), ty = (uint32_t)(tile / tiles_x);
-    const uint32_t warp = j >> 5, lane = j & 31u;
-    const uint32_t x = tx * 16u + (warp & 1u) * 8u + (lane & 7u), y = ty * 8u + (warp >> 1) * 4u + (lane >> 3);
-    if (x >= width || y >= height) return -1;
-    return (int64_t)y * width + x;
+    // (a tile index past 32 bits needs an image of 2^39 pixels or more; a render takes at most 2^29)
+    if (width == 0 || height == 0 || j >= 128u || shard_index >= sc || tile >= (uint64_t)tiles_x * tiles_y || tile > UINT32_MAX)
+        return -1;
+    return tile_pixel(width, height, (uint32_t)tile, j);
 }
 
 int rptb_illuminate(rptb_scene* s, uint32_t light, const double* pos, uint64_t n, uint64_t seed, uint32_t precision,
@@ -1434,19 +1405,16 @@ static int sample_into_impl(rptb_scene* s, const rptb_camera* cam, const rptb_re
     if (!same) return fail(RPTB_ERR_BAD_ARG, "the buffer was created on a scene with another device list");
     std::lock_guard<std::mutex> bl(b->lock);
     if (b->entries == UINT32_MAX) return fail(RPTB_ERR_UNSUPPORTED, "too many entries");
-    const uint32_t n = b->entries + 1;
-    const bool counted = b->counted || crit != nullptr;
     // every replica's share is enqueued before any is waited for, so the devices run concurrently
     std::vector<std::unique_lock<std::mutex>> locks;
     std::vector<uint32_t> launches(nparts, 0);
     for (uint32_t i = 0; i < nparts; i++) {
         rptb_scene* r = i == 0 ? s : s->peers[i - 1];
         locks.emplace_back(r->lock);
-        rc = sample_part(r, cam, p, i, nparts, n, b->parts[i], stats != nullptr, &launches[i], counted, crit);
+        rc = sample_part(r, cam, p, i, nparts, b->parts[i], stats != nullptr, &launches[i], crit);
         if (rc != RPTB_OK) return nparts > 1 ? fail(rc, "device %d: %s", r->device, g_error.c_str()) : rc;
     }
-    b->entries = n;
-    b->counted = counted;
+    b->entries++;
     if (out_active) {
         uint64_t total = 0;
         for (uint32_t i = 0; i < nparts; i++) {
@@ -1503,7 +1471,7 @@ int rptb_buffer_add_samples(rptb_buffer* b, const double* rgb) {
     if (!b || !rgb) return fail(RPTB_ERR_BAD_ARG, "null argument");
     std::lock_guard<std::mutex> bl(b->lock);
     if (b->entries == UINT32_MAX) return fail(RPTB_ERR_UNSUPPORTED, "too many entries");
-    const uint32_t n = b->entries + 1, nparts = (uint32_t)b->parts.size();
+    const uint32_t nparts = (uint32_t)b->parts.size();
     const size_t nvals = (size_t)b->width * b->height * 3;
     for (uint32_t i = 0; i < nparts; i++) {
         BufferPart& q = b->parts[i];
@@ -1513,15 +1481,11 @@ int rptb_buffer_add_samples(rptb_buffer* b, const double* rgb) {
         CU(cudaStreamWaitEvent(q.stream, q.done, 0));
         // pageable source: the call returns once the bytes are staged, `rgb` may be reused afterwards
         CU(cudaMemcpyAsync(q.upload, rgb, nvals * sizeof(double), cudaMemcpyHostToDevice, q.stream));
-        if (b->counted)
-            CU(launch_buffer_accumulate_counted(nullptr, q.upload, true, nullptr, (uint64_t)q.tiles * 128u, b->width, b->height, i,
-                                                nparts, q.sums, q.m2, q.counts, q.stream));
-        else
-            CU(launch_buffer_accumulate(nullptr, q.upload, true, n, (uint64_t)q.tiles * 128u, b->width, b->height, i, nparts,
-                                        q.sums, q.m2, q.stream));
+        CU(launch_buffer_accumulate(nullptr, q.upload, true, nullptr, (uint64_t)q.tiles * 128u, b->width, b->height, i, nparts,
+                                    q.sums, q.m2, q.counts, q.stream));
         CU(cudaEventRecord(q.done, q.stream));
     }
-    b->entries = n;
+    b->entries++;
     return RPTB_OK;
 }
 
@@ -1531,16 +1495,10 @@ int rptb_buffer_image(rptb_buffer* b, uint8_t* out_rgb8) {
     if (b->entries == 0) return fail(RPTB_ERR_BAD_ARG, "Pixel found with no samples");  // buffer.rs:89
     BufferPart& q0 = b->parts[0];
     DeviceGuard g(q0.device);
-    int rc = buffer_gather(b, true, false);
+    const int rc = buffer_gather(b, true, false, true);
     if (rc != RPTB_OK) return rc;
     const size_t nvals = (size_t)b->width * b->height * 3;
-    if (b->counted) {
-        rc = buffer_gather_counts(b);
-        if (rc != RPTB_OK) return rc;
-        CU(launch_film_resolve_counted(b->row_sums, b->row_counts, b->width, b->height, b->radius, b->rgb8, q0.stream));
-    } else {
-        CU(launch_film_resolve(b->row_sums, b->entries, b->width, b->height, b->radius, b->rgb8, q0.stream));
-    }
+    CU(launch_film_resolve_counted(b->row_sums, b->row_counts, b->width, b->height, b->radius, b->rgb8, q0.stream));
     CU(cudaMemcpyAsync(out_rgb8, b->rgb8, nvals, cudaMemcpyDeviceToHost, q0.stream));
     CU(cudaStreamSynchronize(q0.stream));
     return RPTB_OK;
@@ -1555,17 +1513,11 @@ int rptb_buffer_variance(rptb_buffer* b, double* out) {
     }
     BufferPart& q0 = b->parts[0];
     DeviceGuard g(q0.device);
-    int rc = buffer_gather(b, false, true);
+    const int rc = buffer_gather(b, false, true, true);
     if (rc != RPTB_OK) return rc;
     const uint64_t npix = (uint64_t)b->width * b->height;
     double* total = b->partial + buffer_variance_blocks(npix);
-    if (b->counted) {  // (a pixel with one entry gives 0/0: NaN, as the reference's variance does)
-        rc = buffer_gather_counts(b);
-        if (rc != RPTB_OK) return rc;
-        CU(launch_buffer_variance_counted(b->row_m2, b->row_counts, npix, b->partial, total, q0.stream));
-    } else {
-        CU(launch_buffer_variance(b->row_m2, npix, b->entries, b->partial, total, q0.stream));
-    }
+    CU(launch_buffer_variance_sum(b->row_m2, b->row_counts, npix, b->partial, total, q0.stream));
     double sum = 0.0;
     CU(cudaMemcpyAsync(&sum, total, sizeof(double), cudaMemcpyDeviceToHost, q0.stream));
     CU(cudaStreamSynchronize(q0.stream));
@@ -1578,22 +1530,16 @@ int rptb_buffer_sums(rptb_buffer* b, double* out_sums, uint32_t* out_entries) {
     std::lock_guard<std::mutex> bl(b->lock);
     BufferPart& q0 = b->parts[0];
     DeviceGuard g(q0.device);
-    int rc = buffer_gather(b, true, false);
+    const int rc = buffer_gather(b, true, false, out_entries != nullptr);
     if (rc != RPTB_OK) return rc;
     CU(cudaMemcpyAsync(out_sums, b->row_sums, (size_t)b->width * b->height * 3 * sizeof(double), cudaMemcpyDeviceToHost, q0.stream));
     std::vector<uint32_t> counts;
-    if (b->counted && out_entries) {
-        rc = buffer_gather_counts(b);
-        if (rc != RPTB_OK) return rc;
+    if (out_entries) {
         counts.resize((size_t)b->width * b->height);
         CU(cudaMemcpyAsync(counts.data(), b->row_counts, counts.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost, q0.stream));
     }
     CU(cudaStreamSynchronize(q0.stream));
-    if (out_entries) {
-        uint32_t most = 0;
-        for (uint32_t c : counts) most = std::max(most, c);
-        *out_entries = b->counted ? most : b->entries;
-    }
+    if (out_entries) *out_entries = *std::max_element(counts.begin(), counts.end());
     return RPTB_OK;
 }
 
@@ -1603,17 +1549,12 @@ int rptb_buffer_pixel_stats(rptb_buffer* b, double* sums, double* m2, uint32_t* 
     BufferPart& q0 = b->parts[0];
     DeviceGuard g(q0.device);
     const size_t npix = (size_t)b->width * b->height;
-    int rc = buffer_gather(b, sums != nullptr, m2 != nullptr);
+    const int rc = buffer_gather(b, sums != nullptr, m2 != nullptr, counts != nullptr);
     if (rc != RPTB_OK) return rc;
     if (sums) CU(cudaMemcpyAsync(sums, b->row_sums, npix * 3 * sizeof(double), cudaMemcpyDeviceToHost, q0.stream));
     if (m2) CU(cudaMemcpyAsync(m2, b->row_m2, npix * sizeof(double), cudaMemcpyDeviceToHost, q0.stream));
-    if (counts && b->counted) {
-        rc = buffer_gather_counts(b);
-        if (rc != RPTB_OK) return rc;
-        CU(cudaMemcpyAsync(counts, b->row_counts, npix * sizeof(uint32_t), cudaMemcpyDeviceToHost, q0.stream));
-    }
+    if (counts) CU(cudaMemcpyAsync(counts, b->row_counts, npix * sizeof(uint32_t), cudaMemcpyDeviceToHost, q0.stream));
     CU(cudaStreamSynchronize(q0.stream));
-    if (counts && !b->counted) std::fill(counts, counts + npix, b->entries);
     return RPTB_OK;
 }
 
@@ -1705,22 +1646,16 @@ int rptb_buffer_denoise(rptb_buffer* b, const rptb_denoise* d, double* out_rgb, 
                     d->sigma_luminance, d->albedo_eps);
     std::lock_guard<std::mutex> bl(b->lock);
     if (b->entries == 0) return fail(RPTB_ERR_BAD_ARG, "Pixel found with no samples");  // buffer.rs:89
-    if (!b->counted && b->entries < 2) return fail(RPTB_ERR_BAD_ARG, "a pixel has fewer than 2 entries (no variance to guide the filter)");
+    // Every pixel holds at least min(entries, 2) entries, so this is exact for any mix of calls: the first call of any
+    // kind reaches every pixel (an adaptive one because n = 0 < min_entries); plain calls and add_samples reach every
+    // pixel; and rptb_sample_into_adaptive refuses min_entries < 2, so a pixel with one entry is always active.
+    if (b->entries < 2) return fail(RPTB_ERR_BAD_ARG, "a pixel has fewer than 2 entries (no variance to guide the filter)");
     if (b->feature_rays == 0) return fail(RPTB_ERR_BAD_ARG, "the buffer holds no features (rptb_buffer_add_features)");
     BufferPart& q0 = b->parts[0];
     DeviceGuard g(q0.device);
     const size_t npix = (size_t)b->width * b->height;
-    int rc = buffer_gather(b, true, true);
+    int rc = buffer_gather(b, true, true, true);
     if (rc != RPTB_OK) return rc;
-    if (b->counted) {
-        rc = buffer_gather_counts(b);
-        if (rc != RPTB_OK) return rc;
-        std::vector<uint32_t> counts(npix);
-        CU(cudaMemcpyAsync(counts.data(), b->row_counts, npix * sizeof(uint32_t), cudaMemcpyDeviceToHost, q0.stream));
-        CU(cudaStreamSynchronize(q0.stream));
-        for (uint32_t c : counts)
-            if (c < 2) return fail(RPTB_ERR_BAD_ARG, "a pixel has fewer than 2 entries (no variance to guide the filter)");
-    }
     rc = buffer_features(b);
     if (rc != RPTB_OK) return rc;
     if (!b->dn) CU(cudaMalloc((void**)&b->dn, npix * 11 * sizeof(double)));
@@ -1729,8 +1664,8 @@ int rptb_buffer_denoise(rptb_buffer* b, const rptb_denoise* d, double* out_rgb, 
     double* out = b->dn + 8 * npix;
     const double* a = b->aov;
     uint32_t launches = 0;
-    CU(launch_denoise(b->row_sums, b->row_m2, b->counted ? b->row_counts : nullptr, b->entries, a, a + 6 * npix, a + 3 * npix, b->width,
-                      b->height, *d, col, var, out, q0.stream, &launches));
+    CU(launch_denoise(b->row_sums, b->row_m2, b->row_counts, a, a + 6 * npix, a + 3 * npix, b->width, b->height, *d, col, var, out,
+                      q0.stream, &launches));
     if (out_rgb) CU(cudaMemcpyAsync(out_rgb, out, npix * 3 * sizeof(double), cudaMemcpyDeviceToHost, q0.stream));
     if (out_rgb8) {
         // the film resolve of one entry at radius 0: clamp, gamma and the truncating cast of Buffer::image

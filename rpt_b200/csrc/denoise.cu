@@ -21,14 +21,13 @@ __global__ void features_resolve_kernel(const double* __restrict__ sn, const dou
     frac[p] = f;
 }
 
-// counts == nullptr: every pixel holds n entries
 __global__ void denoise_demodulate_kernel(const double* __restrict__ sums, const double* __restrict__ m2,
-                                          const uint32_t* __restrict__ counts, uint32_t n, uint64_t npix,
+                                          const uint32_t* __restrict__ counts, uint64_t npix,
                                           const double* __restrict__ albedo, double eps_a, double* __restrict__ col,
                                           double* __restrict__ var) {
     const uint64_t p = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (p >= npix) return;
-    denoise_demodulate(sums + 3 * p, m2[p], counts ? counts[p] : n, albedo + 3 * p, eps_a, col + 3 * p, var + p);
+    denoise_demodulate(sums + 3 * p, m2[p], counts[p], albedo + 3 * p, eps_a, col + 3 * p, var + p);
 }
 
 __global__ void __launch_bounds__(256) denoise_pass_kernel(const double* __restrict__ col, const double* __restrict__ var,
@@ -45,12 +44,12 @@ __global__ void __launch_bounds__(256) denoise_pass_kernel(const double* __restr
 
 // c' = i * (a + eps_a); iterations == 0 (identity): c = S / n, the value Buffer::image divides out
 __global__ void denoise_finish_kernel(const double* __restrict__ col, const double* __restrict__ albedo, double eps_a,
-                                      const double* __restrict__ sums, const uint32_t* __restrict__ counts, uint32_t n,
-                                      uint64_t npix, double* __restrict__ out) {
+                                      const double* __restrict__ sums, const uint32_t* __restrict__ counts, uint64_t npix,
+                                      double* __restrict__ out) {
     const uint64_t p = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (p >= npix) return;
     for (int k = 0; k < 3; k++)
-        out[3 * p + k] = col ? col[3 * p + k] * (albedo[3 * p + k] + eps_a) : sums[3 * p + k] / (double)(counts ? counts[p] : n);
+        out[3 * p + k] = col ? col[3 * p + k] * (albedo[3 * p + k] + eps_a) : sums[3 * p + k] / (double)counts[p];
 }
 
 cudaError_t launch_features_resolve(const double* row_feat, uint64_t npix, double rays, double* nrm, double* depth, double* albedo,
@@ -63,20 +62,20 @@ cudaError_t launch_features_resolve(const double* row_feat, uint64_t npix, doubl
     return cudaGetLastError();
 }
 
-// The whole filter: sums / m2 / counts (nullable: n entries each) and the resolved features in, c' (width*height*3) out.
+// The whole filter: sums / m2 / counts and the resolved features in, c' (width*height*3) out.
 // col[2] / var[2]: the ping-pong planes.  *launches: kernels enqueued.
-cudaError_t launch_denoise(const double* sums, const double* m2, const uint32_t* counts, uint32_t n, const double* nrm,
+cudaError_t launch_denoise(const double* sums, const double* m2, const uint32_t* counts, const double* nrm,
                            const double* depth, const double* albedo, uint32_t width, uint32_t height, const rptb_denoise& d,
                            double* const col[2], double* const var[2], double* out, cudaStream_t stream, uint32_t* launches) {
     const uint64_t npix = (uint64_t)width * height;
     const unsigned grid = (unsigned)((npix + 255) / 256);
     uint32_t nl = 0;
     if (d.iterations == 0) {
-        denoise_finish_kernel<<<grid, 256, 0, stream>>>(nullptr, albedo, d.albedo_eps, sums, counts, n, npix, out);
+        denoise_finish_kernel<<<grid, 256, 0, stream>>>(nullptr, albedo, d.albedo_eps, sums, counts, npix, out);
         *launches = 1;
         return cudaGetLastError();
     }
-    denoise_demodulate_kernel<<<grid, 256, 0, stream>>>(sums, m2, counts, n, npix, albedo, d.albedo_eps, col[0], var[0]);
+    denoise_demodulate_kernel<<<grid, 256, 0, stream>>>(sums, m2, counts, npix, albedo, d.albedo_eps, col[0], var[0]);
     nl++;
     const dim3 block(32, 8), grid2((width + 31) / 32, (height + 7) / 8);
     uint32_t cur = 0;
@@ -85,7 +84,7 @@ cudaError_t launch_denoise(const double* sums, const double* m2, const uint32_t*
                                                          var[cur ^ 1u]);
         nl++;
     }
-    denoise_finish_kernel<<<grid, 256, 0, stream>>>(col[cur], albedo, d.albedo_eps, sums, counts, n, npix, out);
+    denoise_finish_kernel<<<grid, 256, 0, stream>>>(col[cur], albedo, d.albedo_eps, sums, counts, npix, out);
     nl++;
     *launches = nl;
     return cudaGetLastError();

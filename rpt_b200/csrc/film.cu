@@ -8,13 +8,17 @@
 // restatement exactly.
 //
 // The device-resident Buffer (rptb_buffer, src/buffer.rs:6-93) keeps those sums on the GPU: every entry is added
-// there by buffer_accumulate_kernel, together with a streaming (Welford) variance, and the same resolve reads them.
+// there by buffer_accumulate_kernel, together with a streaming (Welford) variance and the pixel's entry count, and
+// film_resolve_counted_kernel reads them.
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "tile.h"
+
 namespace rptb {
 
-// One output pixel.  COUNTED: pixel q holds counts[q] entries (a buffer with adaptive calls), else every pixel nbatches.
+// One output pixel.  COUNTED: pixel q holds counts[q] entries (the device Buffer), else every pixel nbatches (the host
+// Buffer, and a denoised image).
 template <bool COUNTED>
 __device__ __forceinline__ void film_resolve_pixel(const double* __restrict__ sums, uint32_t nbatches,
                                                    const uint32_t* __restrict__ counts, uint32_t width, uint32_t height,
@@ -99,62 +103,29 @@ __global__ void film_variance_kernel(const double* __restrict__ batches, uint32_
 // ---- the device-resident Buffer (rptb_buffer) ---------------------------------------------------------------------
 // A replica holds its own 16x8 tiles in the compact tile-major layout of rptb_tile_pixel: element e = k*128 + j is
 // pixel j of the k-th owned tile, sums[3e..3e+3) its running per-channel sum, m2[e] its Welford M2 summed over the
-// channels.  `n` is the entry count after this entry.
+// channels and counts[e] its number of entries (pixels may hold different numbers: adaptive sampling).
 
-// Pixel (y*width + x) of element j of tile `tile`, or -1 past a ragged edge (rptb_tile_pixel).
-__device__ __forceinline__ int64_t tile_pixel(uint32_t width, uint32_t height, uint32_t tile, uint32_t j) {
-    const uint32_t tiles_x = (width + 15u) / 16u;
-    const uint32_t tx = tile % tiles_x, ty = tile / tiles_x;
-    const uint32_t warp = j >> 5, lane = j & 31u;
-    const uint32_t x = tx * 16u + (warp & 1u) * 8u + (lane & 7u), y = ty * 8u + (warp >> 1) * 4u + (lane >> 3);
-    if (x >= width || y >= height) return -1;
-    return (int64_t)y * width + x;
-}
-
-// Buffer::add_samples (src/buffer.rs:32-40) of one entry: the entry is `in` in the compact layout (ROWMAJOR = false:
-// the render's compact out32/out64) or a row-major width*height*3 image (ROWMAJOR = true: a host entry), widened to
-// double.  The sum is added in entry order, so it is the sequential sum np.sum(batches, axis=0) computes; M2 takes
-// the mean from the sums before and after the entry: M2 += sum_c (x_c - S_old,c/(n-1)) * (x_c - S_new,c/n).
-// Entry n of one pixel: its running sums s[0..3) and M2 *m.
+// Entry n of one pixel into its running sums s[0..3) and M2 *m.  The sum is added in entry order, so it is the
+// sequential sum np.sum(batches, axis=0) computes; M2 takes the mean from the sums before and after the entry:
+// M2 += sum_c (x_c - S_old,c/(n-1)) * (x_c - S_new,c/n); the first entry is the sum, and its M2 is zero.  Written
+// without a branch on n, so that the loads of the old state do not wait for the load of n.
 __device__ __forceinline__ void welford_add(double x0, double x1, double x2, uint32_t n, double* __restrict__ s,
                                             double* __restrict__ m) {
-    if (n == 1) {  // the first entry is the sum; its M2 is zero
-        s[0] = x0;
-        s[1] = x1;
-        s[2] = x2;
-        *m = 0.0;
-        return;
-    }
-    const double o0 = s[0], o1 = s[1], o2 = s[2];
+    const double o0 = s[0], o1 = s[1], o2 = s[2], om = *m;
     const double n0 = o0 + x0, n1 = o1 + x1, n2 = o2 + x2;
     const double a = (double)(n - 1), b = (double)n;
-    *m += (x0 - o0 / a) * (x0 - n0 / b) + (x1 - o1 / a) * (x1 - n1 / b) + (x2 - o2 / a) * (x2 - n2 / b);
-    s[0] = n0;
-    s[1] = n1;
-    s[2] = n2;
+    const double dm = (x0 - o0 / a) * (x0 - n0 / b) + (x1 - o1 / a) * (x1 - n1 / b) + (x2 - o2 / a) * (x2 - n2 / b);
+    const bool first = n == 1;
+    s[0] = first ? x0 : n0;
+    s[1] = first ? x1 : n1;
+    s[2] = first ? x2 : n2;
+    *m = first ? 0.0 : om + dm;
 }
 
 template <class T, bool ROWMAJOR>
-__global__ void buffer_accumulate_kernel(const T* __restrict__ in, uint32_t n, uint64_t nelem, uint32_t width,
-                                         uint32_t height, uint32_t shard_index, uint32_t shard_count,
-                                         double* __restrict__ sums, double* __restrict__ m2) {
-    const uint64_t e = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (e >= nelem) return;
-    const T* src = in + 3 * e;
-    if (ROWMAJOR) {
-        const int64_t p = tile_pixel(width, height, shard_index + (uint32_t)(e >> 7) * shard_count, (uint32_t)(e & 127u));
-        if (p < 0) return;
-        src = in + 3 * p;
-    }
-    welford_add((double)src[0], (double)src[1], (double)src[2], n, sums + 3 * e, m2 + e);
-}
-
-// The same for a buffer with per-pixel entry counts (adaptive sampling): element e takes entry counts[e] + 1, and only
-// where mask[e] is set (mask == nullptr: every element, Buffer::add_samples).
-template <class T, bool ROWMAJOR>
-__global__ void buffer_accumulate_counted_kernel(const T* __restrict__ in, const uint8_t* __restrict__ mask, uint64_t nelem,
-                                                 uint32_t width, uint32_t height, uint32_t shard_index, uint32_t shard_count,
-                                                 double* __restrict__ sums, double* __restrict__ m2, uint32_t* __restrict__ counts) {
+__global__ void buffer_accumulate_kernel(const T* __restrict__ in, const uint8_t* __restrict__ mask, uint64_t nelem,
+                                         uint32_t width, uint32_t height, uint32_t shard_index, uint32_t shard_count,
+                                         double* __restrict__ sums, double* __restrict__ m2, uint32_t* __restrict__ counts) {
     const uint64_t e = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (e >= nelem) return;
     if (mask && !mask[e]) return;
@@ -169,23 +140,12 @@ __global__ void buffer_accumulate_counted_kernel(const T* __restrict__ in, const
     counts[e] = n;
 }
 
-__global__ void buffer_counts_fill_kernel(uint32_t* __restrict__ counts, uint64_t nelem, uint32_t value) {
-    const uint64_t e = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (e < nelem) counts[e] = value;
-}
-
-__global__ void buffer_scatter_counts_kernel(const uint32_t* __restrict__ counts, uint64_t nelem, uint32_t width, uint32_t height,
-                                             uint32_t shard_index, uint32_t shard_count, uint32_t* __restrict__ row_counts) {
-    const uint64_t e = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (e >= nelem) return;
-    const int64_t p = tile_pixel(width, height, shard_index + (uint32_t)(e >> 7) * shard_count, (uint32_t)(e & 127u));
-    if (p >= 0) row_counts[p] = counts[e];
-}
-
-// Compact tiles of replica `shard_index` of `shard_count` -> the row-major sums / M2 of the whole image.
-__global__ void buffer_scatter_kernel(const double* __restrict__ sums, const double* __restrict__ m2, uint64_t nelem,
-                                      uint32_t width, uint32_t height, uint32_t shard_index, uint32_t shard_count,
-                                      double* __restrict__ row_sums, double* __restrict__ row_m2) {
+// Compact tiles of replica `shard_index` of `shard_count` -> the row-major sums / M2 / counts of the whole image; a
+// null output plane is skipped.
+__global__ void buffer_scatter_kernel(const double* __restrict__ sums, const double* __restrict__ m2,
+                                      const uint32_t* __restrict__ counts, uint64_t nelem, uint32_t width, uint32_t height,
+                                      uint32_t shard_index, uint32_t shard_count, double* __restrict__ row_sums,
+                                      double* __restrict__ row_m2, uint32_t* __restrict__ row_counts) {
     const uint64_t e = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (e >= nelem) return;
     const int64_t p = tile_pixel(width, height, shard_index + (uint32_t)(e >> 7) * shard_count, (uint32_t)(e & 127u));
@@ -196,9 +156,11 @@ __global__ void buffer_scatter_kernel(const double* __restrict__ sums, const dou
         row_sums[3 * p + 2] = sums[3 * e + 2];
     }
     if (row_m2) row_m2[p] = m2[e];
+    if (row_counts) row_counts[p] = counts[e];
 }
 
-// Buffer::variance from the row-major M2: the sum over pixels of M2/(n-1), in a fixed order and without atomics, so
+// Buffer::variance from the row-major M2 and counts: the sum over pixels of M2/(n-1), each pixel with its own n (a
+// pixel with one entry gives 0/0: NaN, as the reference's variance does), in a fixed order and without atomics, so
 // the bits do not depend on the run or on how many devices rendered.  Block b sums pixels [b*CHUNK, (b+1)*CHUNK):
 // thread t its pixels t, t+256, ... in order, then a fixed tree; one block then reduces the block partials the same way.
 constexpr uint32_t kVarThreads = 256, kVarChunk = kVarThreads * 16;
@@ -214,20 +176,9 @@ __device__ __forceinline__ double block_sum_fixed(double v) {
     return sh[0];
 }
 
-__global__ void __launch_bounds__(kVarThreads) buffer_variance_partial_kernel(const double* __restrict__ m2, uint64_t npixels,
-                                                                              double nm1, double* __restrict__ partial) {
-    const uint64_t base = (uint64_t)blockIdx.x * kVarChunk;
-    double v = 0.0;
-    for (uint32_t i = threadIdx.x; i < kVarChunk; i += kVarThreads)
-        if (base + i < npixels) v += m2[base + i] / nm1;
-    const double s = block_sum_fixed(v);
-    if (threadIdx.x == 0) partial[blockIdx.x] = s;
-}
-
-// The same sum with each pixel's own count: M2 / (counts - 1), in the same order.
-__global__ void __launch_bounds__(kVarThreads) buffer_variance_partial_counted_kernel(const double* __restrict__ m2,
-                                                                                      const uint32_t* __restrict__ counts,
-                                                                                      uint64_t npixels, double* __restrict__ partial) {
+__global__ void __launch_bounds__(kVarThreads) buffer_variance_partial_kernel(const double* __restrict__ m2,
+                                                                              const uint32_t* __restrict__ counts,
+                                                                              uint64_t npixels, double* __restrict__ partial) {
     const uint64_t base = (uint64_t)blockIdx.x * kVarChunk;
     double v = 0.0;
     for (uint32_t i = threadIdx.x; i < kVarChunk; i += kVarThreads)
@@ -244,57 +195,30 @@ __global__ void __launch_bounds__(kVarThreads) buffer_variance_final_kernel(cons
     if (threadIdx.x == 0) *out_sum = s;
 }
 
-cudaError_t launch_buffer_accumulate(const float* in32, const double* in64, bool rowmajor, uint32_t n, uint64_t nelem,
-                                     uint32_t width, uint32_t height, uint32_t shard_index, uint32_t shard_count,
-                                     double* sums, double* m2, cudaStream_t stream) {
+cudaError_t launch_buffer_accumulate(const float* in32, const double* in64, bool rowmajor, const uint8_t* mask, uint64_t nelem,
+                                     uint32_t width, uint32_t height, uint32_t shard_index, uint32_t shard_count, double* sums,
+                                     double* m2, uint32_t* counts, cudaStream_t stream) {
     if (nelem == 0) return cudaSuccess;
     const unsigned grid = (unsigned)((nelem + 255) / 256);
     if (in32)
-        buffer_accumulate_kernel<float, false><<<grid, 256, 0, stream>>>(in32, n, nelem, width, height, shard_index, shard_count, sums, m2);
+        buffer_accumulate_kernel<float, false><<<grid, 256, 0, stream>>>(in32, mask, nelem, width, height, shard_index, shard_count,
+                                                                         sums, m2, counts);
     else if (rowmajor)
-        buffer_accumulate_kernel<double, true><<<grid, 256, 0, stream>>>(in64, n, nelem, width, height, shard_index, shard_count, sums, m2);
+        buffer_accumulate_kernel<double, true><<<grid, 256, 0, stream>>>(in64, mask, nelem, width, height, shard_index, shard_count,
+                                                                         sums, m2, counts);
     else
-        buffer_accumulate_kernel<double, false><<<grid, 256, 0, stream>>>(in64, n, nelem, width, height, shard_index, shard_count, sums, m2);
+        buffer_accumulate_kernel<double, false><<<grid, 256, 0, stream>>>(in64, mask, nelem, width, height, shard_index, shard_count,
+                                                                          sums, m2, counts);
     return cudaGetLastError();
 }
 
-cudaError_t launch_buffer_accumulate_counted(const float* in32, const double* in64, bool rowmajor, const uint8_t* mask,
-                                             uint64_t nelem, uint32_t width, uint32_t height, uint32_t shard_index,
-                                             uint32_t shard_count, double* sums, double* m2, uint32_t* counts, cudaStream_t stream) {
-    if (nelem == 0) return cudaSuccess;
-    const unsigned grid = (unsigned)((nelem + 255) / 256);
-    if (in32)
-        buffer_accumulate_counted_kernel<float, false><<<grid, 256, 0, stream>>>(in32, mask, nelem, width, height, shard_index,
-                                                                                 shard_count, sums, m2, counts);
-    else if (rowmajor)
-        buffer_accumulate_counted_kernel<double, true><<<grid, 256, 0, stream>>>(in64, mask, nelem, width, height, shard_index,
-                                                                                 shard_count, sums, m2, counts);
-    else
-        buffer_accumulate_counted_kernel<double, false><<<grid, 256, 0, stream>>>(in64, mask, nelem, width, height, shard_index,
-                                                                                  shard_count, sums, m2, counts);
-    return cudaGetLastError();
-}
+uint32_t buffer_variance_blocks(uint64_t npixels) { return (uint32_t)((npixels + kVarChunk - 1) / kVarChunk); }
 
-cudaError_t launch_buffer_counts_fill(uint32_t* counts, uint64_t nelem, uint32_t value, cudaStream_t stream) {
-    if (nelem == 0) return cudaSuccess;
-    buffer_counts_fill_kernel<<<(unsigned)((nelem + 255) / 256), 256, 0, stream>>>(counts, nelem, value);
-    return cudaGetLastError();
-}
-
-cudaError_t launch_buffer_scatter_counts(const uint32_t* counts, uint64_t nelem, uint32_t width, uint32_t height,
-                                         uint32_t shard_index, uint32_t shard_count, uint32_t* row_counts, cudaStream_t stream) {
-    if (nelem == 0) return cudaSuccess;
-    buffer_scatter_counts_kernel<<<(unsigned)((nelem + 255) / 256), 256, 0, stream>>>(counts, nelem, width, height, shard_index,
-                                                                                    shard_count, row_counts);
-    return cudaGetLastError();
-}
-
-uint32_t buffer_variance_blocks(uint64_t npixels);
-// *out_sum = sum over pixels of m2[p] / (counts[p] - 1); `partial` as in launch_buffer_variance.
-cudaError_t launch_buffer_variance_counted(const double* m2, const uint32_t* counts, uint64_t npixels, double* partial,
-                                           double* out_sum, cudaStream_t stream) {
+// *out_sum = sum over pixels of m2[p] / (counts[p] - 1); `partial` holds buffer_variance_blocks(npixels) doubles.
+cudaError_t launch_buffer_variance_sum(const double* m2, const uint32_t* counts, uint64_t npixels, double* partial,
+                                       double* out_sum, cudaStream_t stream) {
     const uint32_t nb = buffer_variance_blocks(npixels);
-    buffer_variance_partial_counted_kernel<<<nb, kVarThreads, 0, stream>>>(m2, counts, npixels, partial);
+    buffer_variance_partial_kernel<<<nb, kVarThreads, 0, stream>>>(m2, counts, npixels, partial);
     buffer_variance_final_kernel<<<1, kVarThreads, 0, stream>>>(partial, nb, out_sum);
     return cudaGetLastError();
 }
@@ -306,23 +230,12 @@ cudaError_t launch_film_resolve_counted(const double* sums, const uint32_t* coun
     return cudaGetLastError();
 }
 
-cudaError_t launch_buffer_scatter(const double* sums, const double* m2, uint64_t nelem, uint32_t width, uint32_t height,
-                                  uint32_t shard_index, uint32_t shard_count, double* row_sums, double* row_m2,
-                                  cudaStream_t stream) {
+cudaError_t launch_buffer_scatter(const double* sums, const double* m2, const uint32_t* counts, uint64_t nelem, uint32_t width,
+                                  uint32_t height, uint32_t shard_index, uint32_t shard_count, double* row_sums, double* row_m2,
+                                  uint32_t* row_counts, cudaStream_t stream) {
     if (nelem == 0) return cudaSuccess;
-    buffer_scatter_kernel<<<(unsigned)((nelem + 255) / 256), 256, 0, stream>>>(sums, m2, nelem, width, height, shard_index,
-                                                                             shard_count, row_sums, row_m2);
-    return cudaGetLastError();
-}
-
-uint32_t buffer_variance_blocks(uint64_t npixels) { return (uint32_t)((npixels + kVarChunk - 1) / kVarChunk); }
-
-// *out_sum = sum over pixels of m2[p] / (n - 1); `partial` holds buffer_variance_blocks(npixels) doubles.
-cudaError_t launch_buffer_variance(const double* m2, uint64_t npixels, uint32_t n, double* partial, double* out_sum,
-                                   cudaStream_t stream) {
-    const uint32_t nb = buffer_variance_blocks(npixels);
-    buffer_variance_partial_kernel<<<nb, kVarThreads, 0, stream>>>(m2, npixels, (double)n - 1.0, partial);
-    buffer_variance_final_kernel<<<1, kVarThreads, 0, stream>>>(partial, nb, out_sum);
+    buffer_scatter_kernel<<<(unsigned)((nelem + 255) / 256), 256, 0, stream>>>(sums, m2, counts, nelem, width, height, shard_index,
+                                                                             shard_count, row_sums, row_m2, row_counts);
     return cudaGetLastError();
 }
 

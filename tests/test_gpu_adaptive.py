@@ -26,7 +26,6 @@ def _adaptive(r, n, buf, crit, want_stats=True):
     capi.check(capi.lib().rptb_sample_into_adaptive(ds.handle, C.byref(cam), C.byref(p), C.byref(c), buf.handle, C.byref(active),
                                                     C.byref(st) if want_stats else None), "rptb_sample_into_adaptive")
     r._next_sample += n
-    buf.counted = True
     return int(active.value), st.as_dict()
 
 
@@ -149,11 +148,13 @@ def test_mixed_counts_are_the_reference_buffer(gpu_ok, radius):
     buf = r.device_buffer()
     crit = api.Adaptive(0.1, 2e-3, 2)
     entries, takes = [], []
-    for _ in range(6):
+    for calls in range(1, 7):
         s0, m0, c0 = buf.pixel_stats()
         first = r._next_sample
         _adaptive(r, spp, buf, crit, want_stats=False)
-        takes.append(buf.counts().reshape(-1) > c0)
+        c1 = buf.counts().reshape(-1)
+        assert c1.min() >= min(calls, 2)  # what rptb_buffer_denoise's "fewer than 2 entries" check relies on
+        takes.append(c1 > c0)
         entries.append(_plain_entry(r, spp, first))
     counts = buf.counts().reshape(-1)
     assert counts.min() < counts.max()

@@ -97,6 +97,12 @@ def test_errors(gpu_ok):
         buf.features()
     r.sample_features(1, buf)
     assert np.isfinite(buf.denoise()).all()
+    # one adaptive entry is one entry in every pixel, too few
+    ad = r.device_buffer()
+    r.sample(1, ad, want_stats=False, adaptive=api.Adaptive(0.0, 0.0, 2))
+    r.sample_features(1, ad)
+    with pytest.raises(capi.RptbError, match="fewer than 2"):
+        ad.denoise()
 
 
 def test_same_bits_for_every_device_count(gpu_ok):

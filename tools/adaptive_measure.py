@@ -1,7 +1,7 @@
 """Adaptive sampling on the device Buffer, measured on the GPU (prints one JSON line per measurement; --out FILE
 also writes every figure, the per-call rows included, to FILE).
 
-  overhead   an always-active adaptive call (select + list-scheduled render + counted accumulate) against
+  overhead   an always-active adaptive call (select + list-scheduled render + masked accumulate) against
              rptb_sample_into (render + accumulate) at the bench sizes of sphere and Cornell: host clock around each
              call, which ends in a device synchronise (both calls are given a stats struct), median of --reps
   scaling    per adaptive call while the active fraction falls: device time, segments, active pixels, listed warp
@@ -52,7 +52,6 @@ def adaptive_call(r, n, buf, crit):
     capi.check(capi.lib().rptb_sample_into_adaptive(ds.handle, C.byref(cam), C.byref(p), C.byref(c), buf.handle, C.byref(active),
                                                     C.byref(st)), "rptb_sample_into_adaptive")
     r._next_sample += n
-    buf.counted = True
     return int(active.value), st.as_dict()
 
 

@@ -6,7 +6,7 @@ through the DeviceBuffer, on three configs:
 Each (config, buffer) pair runs in its own process so that the peak host RSS is its own.  Printed per pair:
 wall time per callback (mean and last) and in total, and the peak RSS.  Then, per config, the device time of
 buffer_accumulate_kernel (kernel durations as CUPTI records them, through torch.profiler) and its achieved
-bandwidth at 76 B per pixel: 12 B of f32 entry read, 32 B of sums + M2 read and 32 B written.  The card's name
+bandwidth at 84 B per pixel: 12 B of f32 entry read, 36 B of sums + M2 + entry count read and 36 B written.  The card's name
 and power limit are printed in the same run."""
 import json
 import os
@@ -80,7 +80,7 @@ def run_kernel(name):
           if "buffer_accumulate_kernel" in e.name and e.device_type == torch.autograd.DeviceType.CUDA]
     w, h = CONFIGS[name][1], CONFIGS[name][2]
     mean_us = sum(us) / len(us) if us else float("nan")
-    gbs = w * h * 76 / (mean_us * 1e-6) / 1e9 if us else float("nan")
+    gbs = w * h * 84 / (mean_us * 1e-6) / 1e9 if us else float("nan")
     print(json.dumps({"config": name, "accumulate_launches": len(us), "accumulate_us_mean": mean_us,
                       "accumulate_us_min": min(us) if us else None, "accumulate_GBps": gbs,
                       "of_peak": gbs / (HBM_TBS * 1e3)}), flush=True)

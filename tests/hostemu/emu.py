@@ -42,6 +42,39 @@ def lib():
     return _lib
 
 
+LIST_LIB_PATH = os.path.join(_HERE, "_build", "libhostemu_list.so")
+_list_lib = None
+
+
+def list_lib():
+    """tests/hostemu/_build/libhostemu_list.so: this emulation plus adaptive sampling's list schedule and criterion
+    (hostemu_list.cu)."""
+    global _list_lib
+    if _list_lib is None:
+        lib()  # `make hostemu` builds both emulation libraries
+        L = C.CDLL(LIST_LIB_PATH)
+        L.hostemu_scene_create.restype = C.c_void_p
+        L.hostemu_scene_create.argtypes = [C.POINTER(capi.SceneDesc), C.c_char_p, C.c_size_t]
+        L.hostemu_scene_destroy.argtypes = [C.c_void_p]
+        L.hostemu_scene_features.argtypes = [C.c_void_p]
+        L.hostemu_render.argtypes = [C.c_void_p, C.POINTER(capi.Camera), C.POINTER(capi.RenderParams), C.c_int, dp, C.POINTER(capi.Stats)]
+        L.hostemu_render_list.argtypes = [C.c_void_p, C.POINTER(capi.Camera), C.POINTER(capi.RenderParams), C.c_int,
+                                          C.POINTER(C.c_uint8), dp, C.POINTER(capi.Stats)]
+        L.hostemu_adaptive_active.restype = None
+        L.hostemu_adaptive_active.argtypes = [capi.c_u32_p, dp, dp, C.c_uint64, C.POINTER(capi.Adaptive), C.POINTER(C.c_uint8)]
+        L.hostemu_pick_render_list.argtypes = [C.c_int, C.c_int, C.c_uint32, C.c_uint32, capi.c_i32_p]
+        _list_lib = L
+    return _list_lib
+
+
+def pick_render_list(features, stats, precision, max_bounces):
+    """The list-scheduled variant launch_render_list_impl picks (pick_render_list, launch.h): ((STATS, FEAT, MAXD), whether
+    it is in RenderListVariantsF32 / F64)."""
+    out = (C.c_int32 * 3)()
+    compiled = list_lib().hostemu_pick_render_list(features, stats, precision, max_bounces, out)
+    return (bool(out[0]), int(out[1]), int(out[2])), bool(compiled)
+
+
 ENGINE_RENDER, ENGINE_VX, ENGINE_CLOSEST_HIT = 0, 1, 2
 
 

@@ -43,9 +43,10 @@ extern "C" {
 // The list-scheduled megakernel (render_list_kernel) over the pixels pixel_mask (width*height bytes, row-major) sets:
 // the mask and the warp-block list are built the way adaptive.cu builds them (blocks with an active pixel, in tile-major
 // order), and out_rgb gets the render's pixels and NaN wherever nothing was written.  Same contract as hostemu_render
-// otherwise (the slot engine always; no ext_bvh).  Returns the FEAT bits that ran (F_LIST included), or -1.
-int hostemu_render_list(const hostemu_scene* s, const rptb_camera* cam, const rptb_render_params* p, const uint8_t* pixel_mask,
-                        double* out_rgb, rptb_stats* stats) {
+// otherwise: the slot engine always, ext_bvh as there, and the same counters.  Returns the FEAT bits that ran (F_LIST
+// included), or -1.
+int hostemu_render_list(const hostemu_scene* s, const rptb_camera* cam, const rptb_render_params* p, int ext_bvh,
+                        const uint8_t* pixel_mask, double* out_rgb, rptb_stats* stats) {
     if (!s || !cam || !p || !pixel_mask || !out_rgb || p->width == 0 || p->height == 0 || p->iterations == 0 ||
         p->max_bounces > MAX_BOUNCES_SUPPORTED)
         return -1;
@@ -83,13 +84,27 @@ int hostemu_render_list(const hostemu_scene* s, const rptb_camera* cam, const rp
         for (size_t i = 0; i < nvals; i++) out_rgb[i] = (double)out[i];
         if (stats) {
             std::memset(stats, 0, sizeof(*stats));
-            stats->segments = counters.segments; stats->rays = counters.rays;
+            stats->segments = counters.segments; stats->rays = counters.rays; stats->node_visits = counters.node_visits;
+            stats->tri_tests = counters.tri_tests; stats->mesh_hits = counters.mesh_hits; stats->env_lookups = counters.env_lookups;
+            stats->object_tests = counters.object_tests;
+            stats->bvh_node_visits = counters.bvh_node_visits; stats->bvh_tri_tests = counters.bvh_tri_tests;
             stats->engine = RPTB_ENGINE_MEGAKERNEL;
         }
         return feat;
     };
     if (p->precision == RPTB_PRECISION_F64) return run(0.0, s->v64, s->features);
-    return run(0.0f, s->v32, (s->features & F_EXT) ? s->features & ~(int)F_BVH : s->features);
+    return run(0.0f, s->v32, ((s->features & F_EXT) && !ext_bvh) ? s->features & ~(int)F_BVH : s->features);
+}
+
+// The list variant launch_render_list_impl picks (pick_render_list): out = {STATS, FEAT, MAXD}; returns 1 if it is in the
+// compiled list (RenderListVariantsF32 / F64), else 0.
+int hostemu_pick_render_list(int features, int stats, uint32_t precision, uint32_t max_bounces, int32_t* out) {
+    const bool f64 = precision == RPTB_PRECISION_F64;
+    const Variant v = pick_render_list(features, stats, f64, max_bounces);
+    out[0] = v.stats ? 1 : 0;
+    out[1] = v.feat;
+    out[2] = v.maxd;
+    return (f64 ? RenderListVariantsF64::has(v) : RenderListVariantsF32::has(v)) ? 1 : 0;
 }
 
 // The adaptive criterion (adaptive.h) on n pixels: out[i] = 1 iff pixel i (counts[i], sums[3i..3i+3), m2[i]) is active.

@@ -263,6 +263,56 @@ CASES: Dict[str, Case] = {
     "smooth_glass_bvh": Case(_smooth(True), 32, 32, 16, 4, B, F_ALL | F_BVH, 0.995, 0.995),
 }
 
+# ------------------------------------------------------------------------------------------------ list schedule ---
+# Adaptive sampling renders through the list-scheduled twins of the variants above (render_list_kernel, F_LIST).  The
+# matrix of (case, precision, collect_stats) both tiers run it on (test_hostemu_paths.py checks that it reaches every
+# list variant pick_render_list can return, test_gpu_list_matrix.py runs it): every case in f32 without counters, f64
+# on one case per f64 variant, and the counting variants on cases with meshes, kd-trees and a BVH.
+LIST_MATRIX = ([(name, capi.PRECISION_F32, 0) for name in sorted(CASES)] + [
+    ("fractal_teapots_bvh", capi.PRECISION_F32, 1),   # STATS F_EVERY | F_BVH
+    ("fractal_teapots_bvh", capi.PRECISION_F32, 2),   # STATS F_EVERY over the reference-shaped kd-trees
+    ("teapot_kd", capi.PRECISION_F32, 1),             # STATS F_EVERY
+    ("sphere", capi.PRECISION_F64, 0),                # F_ALL / 16
+    ("fractal_spheres", capi.PRECISION_F64, 0),       # F_EVERY / 16
+    ("glass_deep", capi.PRECISION_F64, 0),            # F_EVERY / 64 (40 bounces)
+    ("monomial_glass", capi.PRECISION_F64, 1),        # STATS F_EVERY / 16
+    ("glass_deep", capi.PRECISION_F64, 2),            # STATS F_EVERY / 64
+])
+
+TILE_W, TILE_H = 16, 8   # a CTA's tile; its four warps each take an 8x4 block (tile.h)
+
+
+def list_mask(w: int, h: int, seed: int = 0) -> np.ndarray:
+    """(h, w) bool: about half the pixels at random, with the ragged last row and column on, tile (0, 0) wholly off and
+    a listed tile (the next one) whose first 8x4 warp block is off.  Needs at least two tiles."""
+    rng = np.random.default_rng(seed)
+    m = rng.random((h, w)) < 0.5
+    m[-1, :] = True
+    m[:, -1] = True
+    m[:TILE_H, :TILE_W] = False
+    y0, x0 = (0, TILE_W) if w > TILE_W else (TILE_H, 0)
+    assert y0 < h and x0 < w, "list_mask needs two tiles"
+    m[y0:y0 + 4, x0:x0 + 8] = False
+    m[min(y0 + 4, h - 1), min(x0 + 8, w - 1)] = True
+    return m
+
+
+def edge_masks(w: int, h: int) -> Dict[str, np.ndarray]:
+    """The masks where a list schedule goes wrong first, as (h, w) bool: nothing, everything, the last pixel (in the
+    last, ragged tile), only the pixels of ragged tiles, a checkerboard of 8x4 warp blocks, every other tile."""
+    y, x = np.mgrid[0:h, 0:w]
+    tiles_x = -(-w // TILE_W)
+    last = np.zeros((h, w), bool)
+    last[-1, -1] = True
+    return {
+        "none": np.zeros((h, w), bool),
+        "all": np.ones((h, w), bool),
+        "last_pixel": last,
+        "ragged": (x >= w // TILE_W * TILE_W) | (y >= h // TILE_H * TILE_H),
+        "warp_checker": (x // 8 + y // 4) % 2 == 0,
+        "tile_checker": ((y // TILE_H) * tiles_x + x // TILE_W) % 2 == 0,
+    }
+
 
 # ------------------------------------------------------------------------------------------------ placements ------
 # The same world geometry placed where the f32 path's magnitude-dependent rules are stretched: meshes whose vertices

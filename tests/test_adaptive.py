@@ -9,34 +9,16 @@ import pytest
 
 from rpt_b200 import _capi as capi
 from rpt_b200 import api, scenes
+from tests import pathwise as pw
 from tests.hostemu import emu
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 F_FLAT, F_LIST, F_EVERY = 128, 256, 55
 
 
-_list_lib = None
-
-
 def _emu():
     """tests/hostemu/_build/libhostemu_list.so: the host emulation of hostemu.cu plus the list schedule and the criterion."""
-    global _list_lib
-    if _list_lib is not None:
-        return _list_lib
-    emu.lib()  # `make hostemu` builds both emulation libraries
-    L = C.CDLL(os.path.join(ROOT, "tests", "hostemu", "_build", "libhostemu_list.so"))
-    L.hostemu_scene_create.restype = C.c_void_p
-    L.hostemu_scene_create.argtypes = [C.POINTER(capi.SceneDesc), C.c_char_p, C.c_size_t]
-    L.hostemu_scene_destroy.argtypes = [C.c_void_p]
-    L.hostemu_render.argtypes = [C.c_void_p, C.POINTER(capi.Camera), C.POINTER(capi.RenderParams), C.c_int, capi.c_double_p,
-                                 C.POINTER(capi.Stats)]
-    L.hostemu_render_list.argtypes = [C.c_void_p, C.POINTER(capi.Camera), C.POINTER(capi.RenderParams), C.POINTER(C.c_uint8),
-                                      capi.c_double_p, C.POINTER(capi.Stats)]
-    L.hostemu_adaptive_active.restype = None
-    L.hostemu_adaptive_active.argtypes = [capi.c_u32_p, capi.c_double_p, capi.c_double_p, C.c_uint64, C.POINTER(capi.Adaptive),
-                                          C.POINTER(C.c_uint8)]
-    _list_lib = L
-    return L
+    return emu.list_lib()
 
 
 class ListEmuScene:
@@ -49,13 +31,28 @@ class ListEmuScene:
         if not self.handle:
             raise ValueError(err.value.decode())
 
-    def render(self, camera, params):
+    def render(self, camera, params, ext_bvh=False):
         """The tile-scheduled megakernel body, as emu.EmuScene.render: ((w*h, 3), stats dict, FEAT)."""
         out = np.empty((params.width * params.height, 3))
         st = capi.Stats()
         cam = camera.to_c()
-        feat = _emu().hostemu_render(self.handle, C.byref(cam), C.byref(params), 0, out.ctypes.data_as(capi.c_double_p), C.byref(st))
+        feat = _emu().hostemu_render(self.handle, C.byref(cam), C.byref(params), 1 if ext_bvh else 0, out.ctypes.data_as(capi.c_double_p),
+                                     C.byref(st))
         return out, st.as_dict(), int(feat)
+
+    def render_list(self, camera, params, mask, ext_bvh=False):
+        """The list-scheduled body over the pixels `mask` (w*h bools) sets: ((w*h, 3), NaN off the mask; stats dict; FEAT)."""
+        out = np.empty((params.width * params.height, 3))
+        st = capi.Stats()
+        cam = camera.to_c()
+        m = np.ascontiguousarray(mask, np.uint8).reshape(-1)
+        feat = _emu().hostemu_render_list(self.handle, C.byref(cam), C.byref(params), 1 if ext_bvh else 0,
+                                          m.ctypes.data_as(C.POINTER(C.c_uint8)), out.ctypes.data_as(capi.c_double_p), C.byref(st))
+        return out, st.as_dict(), int(feat)
+
+    @property
+    def features(self) -> int:
+        return int(_emu().hostemu_scene_features(self.handle))
 
     def __del__(self):
         if getattr(self, "handle", None):
@@ -163,7 +160,7 @@ def test_list_schedule_is_the_plain_render_on_the_mask(orc, name):
         out = np.empty((w * h, 3))
         st = capi.Stats()
         p = _params(cfg, w, h, spp, mb, precision)
-        feat = _emu().hostemu_render_list(e.handle, C.byref(cam), C.byref(p), mask.ctypes.data_as(C.POINTER(C.c_uint8)),
+        feat = _emu().hostemu_render_list(e.handle, C.byref(cam), C.byref(p), 0, mask.ctypes.data_as(C.POINTER(C.c_uint8)),
                                           out.ctypes.data_as(capi.c_double_p), C.byref(st))
         return out, st.as_dict(), feat
 
@@ -183,3 +180,60 @@ def test_list_schedule_is_the_plain_render_on_the_mask(orc, name):
     assert f32 == want_feat and fp32 == want_feat & ~F_LIST
     assert np.array_equal(g32[on], plain32[on]) and np.isnan(g32[~on]).all()
     assert 0 < s32["segments"] < sp32["segments"]
+
+
+COUNTERS = ("segments", "rays", "node_visits", "tri_tests", "object_tests", "bvh_node_visits", "bvh_tri_tests", "mesh_hits",
+            "env_lookups")
+
+
+@pytest.mark.parametrize("name", sorted(pw.CASES))
+def test_list_matrix_is_the_plain_render_on_the_mask(name):
+    """Every case of the pathwise matrix, 2 spp, f32 and f64: through the list schedule, each mask of
+    pathwise.edge_masks and a random one (pathwise.list_mask) gets exactly the plain render's pixels and nothing else,
+    and the counters of a mask and its complement add up to the plain render's, without counters and with both kinds."""
+    c = pw.CASES[name]
+    scene, cam = c.make()
+    with pw.scene_env(c.env):
+        e = ListEmuScene(api.FlatScene(scene, accel=c.accel))
+    ext_bvh = (e.features & pw.F_BVH) != 0  # as test_hostemu_paths: the library sends F_BVH with F_EXT
+    masks = {"random": pw.list_mask(c.w, c.h, 5), **pw.edge_masks(c.w, c.h)}
+    for precision in (capi.PRECISION_F32, capi.PRECISION_F64):
+        for stats in (0, 1, 2):
+            r = pw.renderer(c, scene, cam, 1, precision)
+            p = r.params(2, 0, collect_stats=stats)
+            plain, pst, pfeat = e.render(cam, p, ext_bvh)
+            assert pfeat >= 0 and not pfeat & F_LIST
+            if precision == capi.PRECISION_F32 and stats == 0:
+                assert pfeat == c.feat
+            for mname, m in masks.items():
+                if stats and mname != "random":
+                    continue
+                on = m.reshape(-1)
+                (g, st, feat), (gc, stc, featc) = (e.render_list(cam, p, on, ext_bvh), e.render_list(cam, p, ~on, ext_bvh))
+                where = (name, precision, stats, mname)
+                assert feat == featc == pfeat | F_LIST, where
+                assert np.array_equal(g[on], plain[on]) and np.isnan(g[~on]).all(), where
+                assert np.array_equal(gc[~on], plain[~on]) and np.isnan(gc[on]).all(), where
+                for k in COUNTERS:
+                    assert st[k] + stc[k] == pst[k], where + (k, st[k], stc[k], pst[k])
+                if mname == "none":
+                    assert st["segments"] == 0 and st["rays"] == 0, where
+            if stats:
+                assert pst["node_visits"] > 0 or pst["object_tests"] > 0 or pst["bvh_node_visits"] > 0, (name, precision, stats)
+
+
+def test_programmed_state_is_the_mask():
+    """The state test_gpu_list_matrix.py programs through rptb_buffer_add_samples: entries (1, 1, 1) then (-1, -1, -1)
+    leave S = 0, M2 = 6, n = 2 (err^2 = 6 / (1 * 2 * 3) = 1), entries 0 then 0 leave everything 0; under
+    Adaptive(0, 0.5, 2) the first is active (1 > 0.25) and the second not, on the device criterion and in numpy."""
+    crit = api.Adaptive(0.0, 0.5, 2)
+    counts = np.array([2, 2], np.uint32)
+    sums = np.zeros((2, 3))
+    m2 = np.array([6.0, 0.0])
+    assert list(emu_active(counts, sums, m2, crit)) == [True, False]
+    assert list(crit.active(counts, sums, m2)) == [True, False]
+    # Welford over the two entries, as the buffer adds them
+    for x1, x2, want in (((1.0,) * 3, (-1.0,) * 3, 6.0), ((0.0,) * 3, (0.0,) * 3, 0.0)):
+        a, b = np.array(x1), np.array(x2)
+        mean1 = a / 1.0
+        assert float((((b - mean1) * (b - (a + b) / 2.0))).sum()) == want

@@ -177,6 +177,10 @@ def test_buffer_outlives_its_scene(gpu_ok):
 
 
 def test_buffers_give_their_device_memory_back(gpu_ok):
+    """50 buffers of 1920x1080 (~150 MB each) keep less than 32 MB of device memory between them.  The free memory
+    cudaMemGetInfo reports is the whole device's, which other processes share: one that starts on the GPU while this
+    runs takes ~0.5 GB for its CUDA context in a single step.  A buffer that keeps memory does so at every step, so the
+    free memory is read after each buffer, and the check is on the 50 smallest of 51 steps."""
     torch = pytest.importorskip("torch")
     cfg = scenes.sphere_scene()
     r = _renderer(cfg, 1920, 1080, 0)
@@ -185,14 +189,16 @@ def test_buffers_give_their_device_memory_back(gpu_ok):
     warm.image()
     warm.close()  # the scene's own scratch for this size now exists
     torch.cuda.synchronize()
-    free0 = torch.cuda.mem_get_info(0)[0]
-    for _ in range(50):
+    free = [torch.cuda.mem_get_info(0)[0]]
+    for _ in range(51):
         b = r.device_buffer()
         r.sample(1, b, want_stats=False)
         b.image()
         b.close()
-    free1 = torch.cuda.mem_get_info(0)[0]
-    assert free1 >= free0 - (32 << 20), (free0 - free1) / 2**20  # one buffer at this size holds ~140 MB
+        free.append(torch.cuda.mem_get_info(0)[0])
+    steps = -np.diff(np.array(free, dtype=np.int64))  # device memory taken over each buffer's life
+    kept = int(np.sort(steps)[:-1].sum())
+    assert kept <= (32 << 20), (kept / 2**20, (steps / 2**20).tolist())  # one buffer at this size holds ~150 MB
     r.close()
 
 

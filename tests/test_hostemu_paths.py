@@ -61,6 +61,7 @@ from rpt_b200 import api
 from tests import pathwise as pw
 from tests.hostemu import emu
 
+F_LIST = 256
 _CACHE = {}
 
 
@@ -122,3 +123,33 @@ def test_the_matrix_reaches_every_f32_variant():
         assert feat == c.feat, name
         served.setdefault(feat, []).append(name)
     assert set(served) == pw.F32_RENDER_VARIANTS, sorted(pw.F32_RENDER_VARIANTS - set(served))
+
+
+def test_the_list_matrix_reaches_every_list_variant():
+    """Adaptive sampling's list-scheduled variants (pick_render_list): every one returned for any feature set, counting
+    pass, precision and depth is compiled, and pathwise.LIST_MATRIX, the matrix test_gpu_list_matrix.py runs, reaches
+    exactly that set."""
+    reachable = set()
+    for features in range(256):
+        for stats in (0, 1, 2):
+            for precision in (capi.PRECISION_F32, capi.PRECISION_F64):
+                for max_bounces in (6, 40):
+                    v, compiled = emu.pick_render_list(features, stats, precision, max_bounces)
+                    assert compiled, (features, stats, precision, max_bounces, v)
+                    assert v[1] & F_LIST and v[0] == (stats != 0)
+                    reachable.add((precision,) + v)
+    served = {}
+    for name, precision, stats in pw.LIST_MATRIX:
+        c = pw.CASES[name]
+        scene, _ = c.make()
+        with pw.scene_env(c.env):
+            e = emu.EmuScene(api.FlatScene(scene, accel=c.accel))
+        v, _ = emu.pick_render_list(e.features, stats, precision, c.max_bounces)
+        e.close()
+        served.setdefault((precision,) + v, []).append((name, stats))
+    for k in sorted(reachable):
+        print("%s STATS %d FEAT %3d MAXD %2d  %s" % ("f64" if k[0] == capi.PRECISION_F64 else "f32", k[1], k[2], k[3], served.get(k)))
+    assert set(served) == reachable, sorted(reachable ^ set(served))
+    # the f32 ones are the twins of every compiled f32 render variant; f64 never picks F_BVH
+    assert len([k for k in reachable if k[0] == capi.PRECISION_F32]) == 14
+    assert len([k for k in reachable if k[0] == capi.PRECISION_F64]) == 5

@@ -43,19 +43,20 @@ void wavefront_carve(void* mem, uint32_t npix, uint32_t G, uint32_t Ks, uint32_t
     out->rays = (WfRay*)p; p += align256(slots * sizeof(WfRay));
     out->hits = (WfHit*)p; p += align256(slots * sizeof(WfHit));
     out->list = (uint32_t*)p; p += align256(slots * sizeof(uint32_t));
-    out->count = (uint32_t*)p;  // [0] rays emitted this step, [1] fetch cursor of the trace kernel, [2] steps left
+    out->count = (uint32_t*)p;  // [0] rays emitted this step, [1] fetch cursor of the trace kernel, [2] a path is pending, [3] steps left
     out->npaths = npaths;
     out->Ks = Ks;
     out->maxd = maxd;
 }
 
-// Closes one step of the loop ON THE DEVICE: the body of the graph's WHILE node runs again iff this step emitted a ray
-// and the step budget is not spent.
+// Closes one step of the loop ON THE DEVICE: the body of the graph's WHILE node runs again iff a path is still not done
+// after this step (wf_shade_kernel sets count[2]; a path that emitted a ray is one of them) and the step budget is not
+// spent.
 __global__ void wf_continue_kernel(const WfBuffers b, cudaGraphConditionalHandle handle) {
-    uint32_t left = b.count[2];
+    uint32_t left = b.count[3];
     if (left) left--;
-    b.count[2] = left;
-    cudaGraphSetConditional(handle, (b.count[0] != 0u && left != 0u) ? 1u : 0u);
+    b.count[3] = left;
+    cudaGraphSetConditional(handle, (b.count[2] != 0u && left != 0u) ? 1u : 0u);
 }
 __global__ void wf_set_kernel(uint32_t* p, uint32_t v) { *p = v; }
 
@@ -102,13 +103,16 @@ cudaError_t run_wavefront_f32(const SceneView<float>& sv, const RenderArgs<float
     else if (bvh) WF_CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, wf_trace_kernel<false, true>, WF_THREADS, 0));
     else WF_CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, wf_trace_kernel<false, false>, WF_THREADS, 0));
     const unsigned tgrid = (unsigned)(sms * (per_sm > 0 ? per_sm : 1));
-    // a sample with n <= max_bounces + 1 segments takes n + 1 steps (camera ray, one per vertex,
-    // and the step that consumes the last vertex's shadow rays and emits the next camera ray); a path
-    // runs ceil(nchunks / G) chunks of `chunk` samples
+    // The step budget.  A sample with n <= max_bounces + 1 segments takes at most n + 1 steps after the step that emitted
+    // its camera ray: one per segment, and the step that finishes it (it consumes the last vertex's shadow rays, or the
+    // miss of its last segment) emits the next sample's camera ray or marks the path done.  The first step emits the
+    // first camera ray, so a path of S samples needs at most S (max_bounces + 2) + 1 steps, within the budget of
+    // S (max_bounces + 2) + 2.  A path runs ceil(nchunks / G) chunks of `chunk` samples.  The loop ends earlier, after
+    // the first step that leaves every path done.
     const unsigned long long per_path = (unsigned long long)((args.nchunks + b.G - 1) / b.G) * args.chunk;
     unsigned long long max_steps = (per_path < args.iterations ? per_path : args.iterations) * (args.max_bounces + 2ull) + 2ull;
     if (max_steps > 0xFFFFFFFFull) max_steps = 0xFFFFFFFFull;
-    wf_set_kernel<<<1, 1, 0, stream>>>(b.count + 2, (uint32_t)max_steps);
+    wf_set_kernel<<<1, 1, 0, stream>>>(b.count + 3, (uint32_t)max_steps);
 
     // graph = one WHILE node; its body = one step (reset the ray list, shade, trace, decide whether to go on)
     WF_CU(cudaGraphCreate(&graph, 0));
@@ -124,7 +128,7 @@ cudaError_t run_wavefront_f32(const SceneView<float>& sv, const RenderArgs<float
     cudaGraph_t body = np.conditional.phGraph_out[0];
     WF_CU(cudaStreamCreateWithFlags(&cap, cudaStreamNonBlocking));
     WF_CU(cudaStreamBeginCaptureToGraph(cap, body, nullptr, nullptr, 0, cudaStreamCaptureModeRelaxed));
-    cudaMemsetAsync(b.count, 0, 2 * sizeof(uint32_t), cap);
+    cudaMemsetAsync(b.count, 0, 3 * sizeof(uint32_t), cap);
     if (stats) wf_shade_kernel<true><<<pgrid, WF_THREADS, 0, cap>>>(sv, args, b);
     else wf_shade_kernel<false><<<pgrid, WF_THREADS, 0, cap>>>(sv, args, b);
     if (stats) wf_trace_kernel<true, false><<<tgrid, WF_THREADS, 0, cap>>>(sv, b, b.list, args.counters);

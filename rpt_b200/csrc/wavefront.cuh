@@ -85,7 +85,8 @@ struct WfBuffers {
     WfRay* rays;      // npaths * (Ks + 1)
     WfHit* hits;      // npaths * (Ks + 1)
     uint32_t* list;   // compact list of live ray slots
-    uint32_t* count;  // [0] rays emitted this step, [1] fetch cursor of the trace kernel
+    uint32_t* count;  // [0] rays emitted this step, [1] fetch cursor of the trace kernel, [2] != 0: a path is not done
+                      // after this step, [3] steps left (run_wavefront_f32 clears [0..2] before every step)
     // npaths = npix * G: every owned pixel slot has G paths in flight, path (slot, g) sums the sample
     // chunks g, g + G, g + 2G, ... one after the other (the chunk sums are resolved in chunk order, so
     // the image does not depend on G -- which is chosen per launch to keep ~2M paths in flight)
@@ -374,6 +375,13 @@ __global__ void __launch_bounds__(WF_THREADS) wf_shade_kernel(const SceneView<fl
     for (uint32_t k = 0; k < Ks; k++) wf_emit(b, (shadow_mask >> k) & 1u, p * nslot + k);
     wf_emit(b, emit_seg, p * nslot + Ks);
     n_rays = __popc(shadow_mask) + (emit_seg ? 1u : 0u);
+    // A path can be pending without a ray in flight: a vertex that is dead, or at max_bounces with no sampled light in
+    // front of it, still needs the next step to finish its sample.  So the loop goes on while any path is not done,
+    // not while rays are emitted.
+    {
+        const unsigned m = __activemask();
+        if (__ballot_sync(m, st.status != WF_DONE) != 0u && (threadIdx.x & 31u) == (uint32_t)(__ffs(m) - 1)) b.count[2] = 1u;
+    }
 
     if (live) {
         st.color[0] = color.x; st.color[1] = color.y; st.color[2] = color.z;

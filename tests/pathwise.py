@@ -60,7 +60,7 @@ class Case:
     bias: float = 1e-5
     ev: float = 0.0
     env: Dict[str, str] = field(default_factory=dict)
-    wavefront: bool = False        # also rendered through ENGINE_WAVEFRONT on the GPU (kd-tree scenes)
+    wavefront: bool = False        # also rendered through ENGINE_WAVEFRONT on the GPU (every case it serves: not F_GROUP / F_MONO)
     base: str = ""                 # PLACEMENTS: the case whose world geometry this one shares ("" = none)
     degrades: bool = False         # PLACEMENTS: f32 agreement below the base's by design, or the oracle's own image moves
     base_slack: float = 0.0        # PLACEMENTS: measured shortfall of the f32 agreement below the base's floor
@@ -243,24 +243,24 @@ NO_FLAT, NO_SMALL = {"RPTB_NO_FLAT": "1"}, {"RPTB_NO_SMALL": "1"}
 CASES: Dict[str, Case] = {
     # name: Case(scene, width, height, spp, max_bounces, accel, FEAT, floor, gpu_floor, ...)
     # the product's scenes
-    "cornell": Case(_cfg(scenes.cornell_scene), 32, 32, 16, 6, A, F_FLAT, 0.982, 0.982),
+    "cornell": Case(_cfg(scenes.cornell_scene), 32, 32, 16, 6, A, F_FLAT, 0.982, 0.982, wavefront=True),
     "cornell_scan": Case(_cfg(scenes.cornell_scene), 32, 32, 16, 6, A, 0, 0.982, 0.982, env=NO_FLAT),
-    "sphere": Case(_cfg(scenes.sphere_scene), 32, 32, 16, 2, A, F_FLAT | F_SMALL, 0.999, 0.999),
+    "sphere": Case(_cfg(scenes.sphere_scene), 32, 32, 16, 2, A, F_FLAT | F_SMALL, 0.999, 0.999, wavefront=True),
     "sphere_scan": Case(_cfg(scenes.sphere_scene), 32, 32, 16, 2, A, F_SMALL, 0.999, 0.999, env=NO_FLAT),
     "teapot_kd": Case(_cfg(scenes.teapot_scene), 32, 32, 16, 2, K, F_TREE, 0.999, 0.999, wavefront=True),
-    "teapot_bvh": Case(_cfg(scenes.teapot_scene), 32, 32, 16, 2, B, F_TREE | F_BVH, 0.999, 0.999),
-    "glass": Case(_cfg(lambda: scenes.glass_scene(64, 32)), 32, 32, 16, 12, A, F_TRANSP | F_HDRI | F_SMALL, 0.974, 0.974),
-    "glass_deep": Case(_glass_lit, 32, 32, 16, 40, A, F_TRANSP | F_HDRI, 0.968, 0.968, env=NO_SMALL),
+    "teapot_bvh": Case(_cfg(scenes.teapot_scene), 32, 32, 16, 2, B, F_TREE | F_BVH, 0.999, 0.999, wavefront=True),
+    "glass": Case(_cfg(lambda: scenes.glass_scene(64, 32)), 32, 32, 16, 12, A, F_TRANSP | F_HDRI | F_SMALL, 0.974, 0.974, wavefront=True),
+    "glass_deep": Case(_glass_lit, 32, 32, 16, 40, A, F_TRANSP | F_HDRI, 0.968, 0.968, env=NO_SMALL, wavefront=True),
     "fractal_spheres": Case(_cfg(lambda: scenes.fractal_spheres_scene(3)), 32, 32, 16, 2, A, F_EVERY, 0.997, 0.997),
     "fractal_teapots_kd": Case(_cfg(lambda: scenes.fractal_teapots_scene(3)), 32, 32, 16, 2, K, F_EVERY, 0.997, 0.997),
     "fractal_teapots_bvh": Case(_cfg(lambda: scenes.fractal_teapots_scene(3)), 32, 32, 16, 2, B, F_EVERY | F_BVH, 0.997, 0.997),
     "monomial_glass": Case(_cfg(lambda: scenes.monomial_glass_scene(64, 32)), 32, 32, 16, 3, A, F_EVERY, 0.990, 0.990),
     # the f32-only rules
-    "clamp": Case(_clamp, 32, 32, 16, 6, A, F_FLAT | F_SMALL, 0.998, 0.998, ev=-1.0),
-    "clamp_glass": Case(_clamp_glass, 48, 32, 24, 8, A, F_ALL, 0.9965, 0.9965),
-    "lights_lens": Case(_lights, 37, 23, 20, 3, A, F_FLAT, 0.999, 0.999),
+    "clamp": Case(_clamp, 32, 32, 16, 6, A, F_FLAT | F_SMALL, 0.998, 0.998, ev=-1.0, wavefront=True),
+    "clamp_glass": Case(_clamp_glass, 48, 32, 24, 8, A, F_ALL, 0.9965, 0.9965, wavefront=True),
+    "lights_lens": Case(_lights, 37, 23, 20, 3, A, F_FLAT, 0.999, 0.999, wavefront=True),
     "smooth_kd": Case(_smooth(False), 32, 32, 16, 3, K, F_TREE, 0.999, 0.999, wavefront=True),
-    "smooth_glass_bvh": Case(_smooth(True), 32, 32, 16, 4, B, F_ALL | F_BVH, 0.995, 0.995),
+    "smooth_glass_bvh": Case(_smooth(True), 32, 32, 16, 4, B, F_ALL | F_BVH, 0.995, 0.995, wavefront=True),
 }
 
 # ------------------------------------------------------------------------------------------------ list schedule ---

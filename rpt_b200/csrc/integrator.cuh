@@ -33,11 +33,20 @@ constexpr int RENDER_THREADS = 128;  // 4 warps: a 16x8 pixel tile
 // LITE (the feature-free kernels: Cornell, sphere), Cornell through the packed primitive table at the bench size on one
 // H100 80GB HBM3 at a 400 W power limit: 246.0 ms at 6 (80 registers, 232 B spill stores), 237.3 ms at 7 (72 registers,
 // 320 B spill stores), 238.6 ms at 8 (64 registers, 404 B spill stores).
+// FLAT: the same kernels without counters (F_NOCOUNT: what a render given no counters runs), Cornell at the bench size
+// on one H100 80GB HBM3 at a 700 W power limit, SM clock 1980 MHz, against 220.6-221.5 ms for the counting kernel at 7:
+// 211.0-213.8 ms at 7 (72 registers, 296 B spill stores), 204.4-206.3 ms at 8 (64 registers, 384 B spill stores).
+// (Measured and dropped: keeping the per-sample state -- f64 sums in shared memory, pixel constants and chunk recomputed
+// where a sample starts or ends -- out of the loop's registers cut the spills to 228 B at 7 and 332 B at 8, but ran
+// 226.5 ms at 7, 228 ms at 8 and 236.8 ms at 9 CTAs; the counting kernel went from 219 to 236 ms with it.)
 #ifndef RPTB_MIN_BLOCKS
 #define RPTB_MIN_BLOCKS 5
 #endif
 #ifndef RPTB_MIN_BLOCKS_LITE
 #define RPTB_MIN_BLOCKS_LITE 7
+#endif
+#ifndef RPTB_MIN_BLOCKS_FLAT
+#define RPTB_MIN_BLOCKS_FLAT 8   // F_FLAT | F_NOCOUNT, no trees: the packed-table LITE kernels that keep no counters
 #endif
 #ifndef RPTB_MIN_BLOCKS_TREE
 #define RPTB_MIN_BLOCKS_TREE 8   // F_TREE only (teapot: fastest of 5 / 6 / 8)
@@ -56,6 +65,7 @@ constexpr int render_min_blocks(int feat) {
     if (feat & F_EXT) return RPTB_MIN_BLOCKS_EXT;
     if (feat & F_BVH) return RPTB_MIN_BLOCKS_BVH;
     const int base = feat & F_ALL;  // F_SMALL does not change the register budget
+    if (base == 0 && (feat & F_FLAT) != 0 && (feat & F_NOCOUNT) != 0) return RPTB_MIN_BLOCKS_FLAT;
     return base == 0 ? RPTB_MIN_BLOCKS_LITE : base == F_TREE ? RPTB_MIN_BLOCKS_TREE : base == (F_TRANSP | F_HDRI) ? RPTB_MIN_BLOCKS_GLASS : RPTB_MIN_BLOCKS;
 }
 constexpr int TILE_W = 16, TILE_H = 8;
@@ -86,6 +96,9 @@ struct PathCounters {
     uint32_t segments, rays, mesh_hits, env_lookups;
     TravStats ts;
 };
+// whether a render kernel variant keeps counters (FEAT without F_NOCOUNT)
+template <int FEAT>
+constexpr bool counts = (FEAT & F_NOCOUNT) == 0;
 
 // scene.lights[i]: from parameter space when the scene's tables ride in the kernel parameters
 template <int FEAT, class R>
@@ -144,6 +157,7 @@ struct MegaRng<float, FEAT> { typedef RngRing type; };
 
 // `rng_ring`: RNG_RING * RENDER_THREADS words of shared memory (f32 on the device; null otherwise).
 // `coop`: this warp's CoopWarp block (geometry.cuh) when meshes are traversed by lane groups (F_BVH on the device), else null.
+// FEAT with F_NOCOUNT: the render is given no counters (a.counters is null), and the counting is compiled out.
 template <class R, int MAXD, bool STATS, int FEAT, class W>
 RPTB_D void render_thread(const SceneView<R>& sv, const RenderArgs<R>& a, const uint32_t block_x, const uint32_t block_y,
                           const uint32_t thread_x, uint32_t* rng_ring = nullptr, void* coop = nullptr) {
@@ -376,14 +390,16 @@ RPTB_D void render_thread(const SceneView<R>& sv, const RenderArgs<R>& a, const 
             // meshes through the eight-wide BVH, eight lanes per ray (every lane of the warp takes part, with or without a ray
             // of its own); a warp at the image's edge, with fewer than 32 lanes, keeps the per-lane binary traversal
             if (coop != nullptr && wmask == 0xffffffffu) {
-                if (active) pc.rays++;
+                if constexpr (counts<FEAT>) {
+                    if (active) pc.rays++;
+                }
                 closest_hit_coop<STATS, FEAT>(sv, active, ro, rd, tmin, light_slot, h, pc.ts, lane, *static_cast<CoopWarp*>(coop));
                 traced = true;
             }
         }
 #endif
         if (!traced && active) {
-            pc.rays++;
+            if constexpr (counts<FEAT>) pc.rays++;
             closest_hit<R, STATS, FEAT>(sv, ro, rd, tmin, light_slot, h, pc.ts);
         }
 
@@ -392,15 +408,19 @@ RPTB_D void render_thread(const SceneView<R>& sv, const RenderArgs<R>& a, const 
             if (light_slot) {
                 if (h.obj < 0) color = color + contrib;
             } else {
-                pc.segments++;  // one trace_ray invocation
+                if constexpr (counts<FEAT>) pc.segments++;  // one trace_ray invocation
                 if (h.obj < 0) {
-                    if ((FEAT & F_HDRI) && sv.env.kind != 0) pc.env_lookups++;
+                    if constexpr (counts<FEAT>) {
+                        if ((FEAT & F_HDRI) && sv.env.kind != 0) pc.env_lookups++;
+                    }
                     Lterm = env_color<R, FEAT>(sv.env, rd);
                     status = ST_FINISH;
                 } else {
                     const ObjectRec<R>& ob = sv.objects[h.obj];
                     const Surface<R> sf = finalize_hit<R, FEAT>(sv, ob, ro, rd, h);
-                    if (sf.on_mesh) pc.mesh_hits++;
+                    if constexpr (counts<FEAT>) {
+                        if (sf.on_mesh) pc.mesh_hits++;
+                    }
                     pos = ro + h.t * rd;
                     n = sf.n;
                     ng = sf.ng;
@@ -432,28 +452,30 @@ RPTB_D void render_thread(const SceneView<R>& sv, const RenderArgs<R>& a, const 
         out[2] = (R)(acc2 / it * (double)a.exposure_scale);
     }
 
-    if (a.counters) {
-        const unsigned m = W::activemask();
-        const uint32_t v0 = W::reduce_add(m, pc.segments), v1 = W::reduce_add(m, pc.rays);
-        const uint32_t v2 = W::reduce_add(m, pc.mesh_hits), v3 = W::reduce_add(m, pc.env_lookups);
-        // node/tri counters can exceed 2^32 per warp on long renders: reduce in two halves
-        const uint32_t n_lo = W::reduce_add(m, pc.ts.node_visits & 0xFFFFu), n_hi = W::reduce_add(m, pc.ts.node_visits >> 16);
-        const uint32_t t_lo = W::reduce_add(m, pc.ts.tri_tests & 0xFFFFu), t_hi = W::reduce_add(m, pc.ts.tri_tests >> 16);
-        const uint32_t o_lo = W::reduce_add(m, pc.ts.object_tests & 0xFFFFu), o_hi = W::reduce_add(m, pc.ts.object_tests >> 16);
-        const uint32_t bn_lo = W::reduce_add(m, pc.ts.bvh_nodes & 0xFFFFu), bn_hi = W::reduce_add(m, pc.ts.bvh_nodes >> 16);
-        const uint32_t bt_lo = W::reduce_add(m, pc.ts.bvh_tris & 0xFFFFu), bt_hi = W::reduce_add(m, pc.ts.bvh_tris >> 16);
-        if (W::is_leader(m, lane)) {
-            W::add(&a.counters->segments, (unsigned long long)v0);
-            W::add(&a.counters->rays, (unsigned long long)v1);
-            W::add(&a.counters->mesh_hits, (unsigned long long)v2);
-            W::add(&a.counters->env_lookups, (unsigned long long)v3);
-            if (STATS) {
-                W::add(&a.counters->node_visits, (unsigned long long)n_lo + ((unsigned long long)n_hi << 16));
-                W::add(&a.counters->tri_tests, (unsigned long long)t_lo + ((unsigned long long)t_hi << 16));
-                W::add(&a.counters->object_tests, (unsigned long long)o_lo + ((unsigned long long)o_hi << 16));
-                if ((FEAT & F_BVH) != 0) {
-                    W::add(&a.counters->bvh_node_visits, (unsigned long long)bn_lo + ((unsigned long long)bn_hi << 16));
-                    W::add(&a.counters->bvh_tri_tests, (unsigned long long)bt_lo + ((unsigned long long)bt_hi << 16));
+    if constexpr (counts<FEAT>) {
+        if (a.counters) {
+            const unsigned m = W::activemask();
+            const uint32_t v0 = W::reduce_add(m, pc.segments), v1 = W::reduce_add(m, pc.rays);
+            const uint32_t v2 = W::reduce_add(m, pc.mesh_hits), v3 = W::reduce_add(m, pc.env_lookups);
+            // node/tri counters can exceed 2^32 per warp on long renders: reduce in two halves
+            const uint32_t n_lo = W::reduce_add(m, pc.ts.node_visits & 0xFFFFu), n_hi = W::reduce_add(m, pc.ts.node_visits >> 16);
+            const uint32_t t_lo = W::reduce_add(m, pc.ts.tri_tests & 0xFFFFu), t_hi = W::reduce_add(m, pc.ts.tri_tests >> 16);
+            const uint32_t o_lo = W::reduce_add(m, pc.ts.object_tests & 0xFFFFu), o_hi = W::reduce_add(m, pc.ts.object_tests >> 16);
+            const uint32_t bn_lo = W::reduce_add(m, pc.ts.bvh_nodes & 0xFFFFu), bn_hi = W::reduce_add(m, pc.ts.bvh_nodes >> 16);
+            const uint32_t bt_lo = W::reduce_add(m, pc.ts.bvh_tris & 0xFFFFu), bt_hi = W::reduce_add(m, pc.ts.bvh_tris >> 16);
+            if (W::is_leader(m, lane)) {
+                W::add(&a.counters->segments, (unsigned long long)v0);
+                W::add(&a.counters->rays, (unsigned long long)v1);
+                W::add(&a.counters->mesh_hits, (unsigned long long)v2);
+                W::add(&a.counters->env_lookups, (unsigned long long)v3);
+                if (STATS) {
+                    W::add(&a.counters->node_visits, (unsigned long long)n_lo + ((unsigned long long)n_hi << 16));
+                    W::add(&a.counters->tri_tests, (unsigned long long)t_lo + ((unsigned long long)t_hi << 16));
+                    W::add(&a.counters->object_tests, (unsigned long long)o_lo + ((unsigned long long)o_hi << 16));
+                    if ((FEAT & F_BVH) != 0) {
+                        W::add(&a.counters->bvh_node_visits, (unsigned long long)bn_lo + ((unsigned long long)bn_hi << 16));
+                        W::add(&a.counters->bvh_tri_tests, (unsigned long long)bt_lo + ((unsigned long long)bt_hi << 16));
+                    }
                 }
             }
         }

@@ -69,8 +69,11 @@ struct Variant {
 };
 
 // render_kernel<R, MAXD, STATS, FEAT> (the slot engine).  stats: rptb_render_params::collect_stats -- 1 counts what the
-// product path traverses (the BVH when the scene has one), 2 walks the reference-shaped kd-trees.
-constexpr Variant pick_render(int features, int stats, bool f64, uint32_t max_bounces) {
+// product path traverses (the BVH when the scene has one), 2 walks the reference-shaped kd-trees.  counters: the render
+// is given counters (RenderArgs::counters), which every variant fills with segments and rays; the packed-table variants
+// also come without any counting (F_NOCOUNT) for the renders that are given none.  The launchers pass `counters`; a
+// caller that always hands counters in (the host emulation does) may leave it at its default.
+constexpr Variant pick_render(int features, int stats, bool f64, uint32_t max_bounces, bool counters = true) {
     const int base = features & F_ALL;
     const bool small = (features & F_SMALL) != 0, ext = (features & F_EXT) != 0;
     const bool bvh = !f64 && (features & F_BVH) != 0;  // F_BVH and F_FLAT are f32 only
@@ -89,8 +92,9 @@ constexpr Variant pick_render(int features, int stats, bool f64, uint32_t max_bo
     if (bvh) return {false, F_ALL | F_BVH, 16};
     // (the glass variant keeps the scan: its two transformed spheres are cheaper from parameter space than the table
     // is through L1 -- 43.7 against 44.0 ms at 256 spp on one H100 80GB HBM3 at a 400 W power limit)
-    if (base == 0 && flat && small) return {false, F_FLAT | F_SMALL, 16};
-    if (base == 0 && flat) return {false, F_FLAT, 16};
+    const int nocount = counters ? 0 : F_NOCOUNT;
+    if (base == 0 && flat && small) return {false, F_FLAT | F_SMALL | nocount, 16};
+    if (base == 0 && flat) return {false, F_FLAT | nocount, 16};
     if (base == 0 && small) return {false, F_SMALL, 16};
     if (base == 0) return {false, 0, 16};
     if (base == F_TREE) return {false, F_TREE, 16};
@@ -100,8 +104,8 @@ constexpr Variant pick_render(int features, int stats, bool f64, uint32_t max_bo
 }
 
 // render_list_kernel<R, MAXD, STATS, FEAT | F_LIST>: the variant pick_render chooses, scheduled from a RenderList
-constexpr Variant pick_render_list(int features, int stats, bool f64, uint32_t max_bounces) {
-    const Variant v = pick_render(features, stats, f64, max_bounces);
+constexpr Variant pick_render_list(int features, int stats, bool f64, uint32_t max_bounces, bool counters = true) {
+    const Variant v = pick_render(features, stats, f64, max_bounces, counters);
     return {v.stats, v.feat | F_LIST, v.maxd};
 }
 
@@ -161,8 +165,8 @@ bool visit(VariantList<First, Rest...>, Variant v, Fn&& fn) {
 using RenderVariantsF32 = VariantList<
     V<true, F_EVERY | F_BVH, 16>, V<true, F_EVERY, 16>, V<false, F_EVERY | F_BVH, 16>, V<false, F_EVERY, 16>,
     V<false, F_TREE | F_BVH, 16>, V<false, F_ALL | F_BVH, 16>, V<false, F_FLAT | F_SMALL, 16>, V<false, F_FLAT, 16>,
-    V<false, F_SMALL, 16>, V<false, 0, 16>, V<false, F_TREE, 16>, V<false, F_TRANSP | F_HDRI | F_SMALL, 16>,
-    V<false, F_TRANSP | F_HDRI, 16>, V<false, F_ALL, 16>>;
+    V<false, F_FLAT | F_SMALL | F_NOCOUNT, 16>, V<false, F_FLAT | F_NOCOUNT, 16>, V<false, F_SMALL, 16>, V<false, 0, 16>,
+    V<false, F_TREE, 16>, V<false, F_TRANSP | F_HDRI | F_SMALL, 16>, V<false, F_TRANSP | F_HDRI, 16>, V<false, F_ALL, 16>>;
 // (the F_BVH entries of the f64 lists are compiled but never picked: F_BVH is f32 only)
 using RenderVariantsF64 = VariantList<
     V<true, F_EVERY | F_BVH, 16>, V<true, F_EVERY, 16>, V<false, F_EVERY | F_BVH, 16>, V<false, F_EVERY, 16>,
@@ -176,6 +180,24 @@ struct WithList<VariantList<Vs...>> {
 };
 using RenderListVariantsF32 = WithList<RenderVariantsF32>::type;
 using RenderListVariantsF64 = WithList<RenderVariantsF64>::type;
+
+// Every slot-engine variant a launcher can pick -- any feature set, counting pass, precision and depth, with counters or
+// without, tile or list schedule -- is compiled; F_NOCOUNT is picked only without counters, and only for the packed table.
+constexpr bool every_render_pick_is_compiled() {
+    for (int features = 0; features < 2 * F_FLAT; features++)
+        for (int stats = 0; stats <= 2; stats++)
+            for (int f64 = 0; f64 <= 1; f64++)
+                for (uint32_t max_bounces : {6u, 40u})
+                    for (int counters = 0; counters <= 1; counters++) {
+                        const Variant v = pick_render(features, stats, f64 != 0, max_bounces, counters != 0);
+                        const Variant l = pick_render_list(features, stats, f64 != 0, max_bounces, counters != 0);
+                        if (!(f64 ? RenderVariantsF64::has(v) : RenderVariantsF32::has(v))) return false;
+                        if (!(f64 ? RenderListVariantsF64::has(l) : RenderListVariantsF32::has(l))) return false;
+                        if ((v.feat & F_NOCOUNT) != 0 && (counters || (v.feat & (F_FLAT | F_ALL)) != F_FLAT)) return false;
+                    }
+    return true;
+}
+static_assert(every_render_pick_is_compiled(), "pick_render / pick_render_list return a variant that is not compiled");
 using RenderVariantsVx = VariantList<
     V<true, F_EVERY | F_BVH>, V<true, F_EVERY>, V<false, F_EVERY | F_BVH>, V<false, F_EVERY>, V<false, F_TREE | F_BVH>,
     V<false, F_ALL | F_BVH>, V<false, F_SMALL>, V<false, 0>, V<false, F_TREE>, V<false, F_TRANSP | F_HDRI | F_SMALL>,

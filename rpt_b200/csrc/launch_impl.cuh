@@ -19,7 +19,7 @@ cudaError_t launch_render_impl(const SceneView<R>& sv, const RenderArgs<R>& args
     if (args.ntiles_mine > 0) {
         const dim3 grid(args.ntiles_mine, args.ngroups), block(RENDER_THREADS);
         using List = std::conditional_t<M<R>::literal, RenderVariantsF64, RenderVariantsF32>;
-        const bool found = visit(List{}, pick_render(features, stats, M<R>::literal, args.max_bounces), [&](auto v) {
+        const bool found = visit(List{}, pick_render(features, stats, M<R>::literal, args.max_bounces, args.counters != nullptr), [&](auto v) {
             using T = decltype(v);
             render_kernel<R, T::maxd, T::stats, T::feat><<<grid, block, 0, stream>>>(sv, args);
         });
@@ -41,7 +41,7 @@ cudaError_t launch_render_list_impl(const SceneView<R>& sv, const RenderArgs<R>&
     if (args.ntiles_mine > 0) {
         const dim3 grid(args.ntiles_mine, args.ngroups), block(RENDER_THREADS);
         using List = std::conditional_t<M<R>::literal, RenderListVariantsF64, RenderListVariantsF32>;
-        const bool found = visit(List{}, pick_render_list(features, stats, M<R>::literal, args.max_bounces), [&](auto v) {
+        const bool found = visit(List{}, pick_render_list(features, stats, M<R>::literal, args.max_bounces, args.counters != nullptr), [&](auto v) {
             using T = decltype(v);
             render_list_kernel<R, T::maxd, T::stats, T::feat><<<grid, block, 0, stream>>>(sv, args, list);
         });

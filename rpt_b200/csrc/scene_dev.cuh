@@ -40,7 +40,8 @@ enum : int {
     F_EXT = F_GROUP | F_MONO, F_EVERY = F_ALL | F_EXT /* the one instantiation that knows every shape */,
     F_BVH = 64 /* f32 only: meshes are traversed through their BVH (MeshRec::bvh_*) instead of the reference-shaped kd-tree */,
     F_FLAT = 128 /* f32 only: get_closest_hit walks the packed primitive table (SceneView::flat) instead of the objects */,
-    F_LIST = 256 /* scheduling, not a scene feature: warps take their 8x4 pixel blocks from a RenderList (adaptive sampling) */
+    F_LIST = 256 /* scheduling, not a scene feature: warps take their 8x4 pixel blocks from a RenderList (adaptive sampling) */,
+    F_NOCOUNT = 512 /* not a scene feature: the render is given no counters (RenderArgs::counters is null), so it keeps none */
 };
 
 // Two experiments on the mesh configs (teapot / dragon-proxy / dragon-knot), both measured slower than what they were

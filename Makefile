@@ -75,7 +75,9 @@ HOSTEMU := tests/hostemu/_build/libhostemu.so
 HOSTEMU_LIST := tests/hostemu/_build/libhostemu_list.so
 # the same emulation plus the feature pass (features.cuh) and the denoiser's per-pixel functions (tests/hostemu/hostemu_denoise.cu)
 HOSTEMU_DENOISE := tests/hostemu/_build/libhostemu_denoise.so
-hostemu: $(HOSTEMU) $(HOSTEMU_LIST) $(HOSTEMU_DENOISE)
+# the same emulation plus the renders given no counters (the packed-table F_NOCOUNT twins; tests/hostemu/hostemu_slim.cu)
+HOSTEMU_SLIM := tests/hostemu/_build/libhostemu_slim.so
+hostemu: $(HOSTEMU) $(HOSTEMU_LIST) $(HOSTEMU_DENOISE) $(HOSTEMU_SLIM)
 $(HOSTEMU): tests/hostemu/hostemu.cu $(CSRC)/kdbuild.cpp $(CSRC)/bvhbuild.cpp $(HDRS)
 	@mkdir -p $(dir $@)
 	nvcc -std=c++17 -O2 -DRPTB_HOST_EMU -DRPTB_BUILD_BVH8=1 -DRPTB_BUILD_BVH4=1 -gencode arch=compute_90a,code=sm_90a -Xcompiler -fPIC,-fopenmp,-ffp-contract=off -shared -Xlinker -Bsymbolic -o $@ tests/hostemu/hostemu.cu $(CSRC)/kdbuild.cpp $(CSRC)/bvhbuild.cpp -lgomp
@@ -85,6 +87,9 @@ $(HOSTEMU_LIST): tests/hostemu/hostemu_list.cu tests/hostemu/hostemu.cu $(CSRC)/
 $(HOSTEMU_DENOISE): tests/hostemu/hostemu_denoise.cu tests/hostemu/hostemu.cu $(CSRC)/kdbuild.cpp $(CSRC)/bvhbuild.cpp $(HDRS)
 	@mkdir -p $(dir $@)
 	nvcc -std=c++17 -O2 -DRPTB_HOST_EMU -DRPTB_BUILD_BVH8=1 -DRPTB_BUILD_BVH4=1 -gencode arch=compute_90a,code=sm_90a -Xcompiler -fPIC,-fopenmp,-ffp-contract=off -shared -Xlinker -Bsymbolic -o $@ tests/hostemu/hostemu_denoise.cu $(CSRC)/kdbuild.cpp $(CSRC)/bvhbuild.cpp -lgomp
+$(HOSTEMU_SLIM): tests/hostemu/hostemu_slim.cu tests/hostemu/hostemu.cu $(CSRC)/kdbuild.cpp $(CSRC)/bvhbuild.cpp $(HDRS)
+	@mkdir -p $(dir $@)
+	nvcc -std=c++17 -O2 -DRPTB_HOST_EMU -DRPTB_BUILD_BVH8=1 -DRPTB_BUILD_BVH4=1 -gencode arch=compute_90a,code=sm_90a -Xcompiler -fPIC,-fopenmp,-ffp-contract=off -shared -Xlinker -Bsymbolic -o $@ tests/hostemu/hostemu_slim.cu $(CSRC)/kdbuild.cpp $(CSRC)/bvhbuild.cpp -lgomp
 
 clean:
 	rm -rf build $(LIB) $(ORACLE) tests/hostemu/_build

@@ -46,6 +46,8 @@ constexpr int RENDER_THREADS = 128;  // 4 warps: a 16x8 pixel tile
 #define RPTB_MIN_BLOCKS_LITE 7
 #endif
 #ifndef RPTB_MIN_BLOCKS_FLAT
+// With the slim lane (slim_lane below; 64 registers, 332 B spill stores), same card and clock, bench.py alternated with the
+// build before it: 199.1-199.5 ms against 203.1-205.0 ms at 8 (9 CTAs with it: not timed).
 #define RPTB_MIN_BLOCKS_FLAT 8   // F_FLAT | F_NOCOUNT, no trees: the packed-table LITE kernels that keep no counters
 #endif
 #ifndef RPTB_MIN_BLOCKS_TREE
@@ -143,6 +145,12 @@ struct DeviceWarp {
 };
 #endif
 
+// The packed-table kernels without counters (F_FLAT | F_NOCOUNT and no other scene feature: Cornell and the sphere, at
+// RPTB_MIN_BLOCKS_FLAT CTAs per SM) keep a slimmer lane: status, dead and depth share one word, and the run of samples
+// is two words, s and the end of its chunk.  Same draws, same sums, same bits.
+template <class R, int FEAT>
+constexpr bool slim_lane = !M<R>::literal && (FEAT & (F_ALL | F_EXT | F_BVH)) == 0 && (FEAT & F_FLAT) != 0 && (FEAT & F_NOCOUNT) != 0;
+
 // The generator the megakernel draws from: f64 the oracle's; f32 the same stream buffered in registers the way that
 // suits the instantiation (rng.cuh: the 64-register F_BVH kernels take the smallest buffer), or the shared-memory ring
 template <class R, int FEAT>
@@ -207,11 +215,13 @@ RPTB_D void render_thread(const SceneView<R>& sv, const RenderArgs<R>& a, const 
     // this thread's run of samples: [s, s_end) of [0, iterations) = chunks_per_group whole chunks
     uint32_t s = block_y * a.chunks_per_group * a.chunk;
     const uint32_t s_end = min(s + a.chunks_per_group * a.chunk, a.iterations);
-    uint32_t chunk_id = block_y * a.chunks_per_group, chunk_left = a.chunk;
+    // slim: chunk_id is not kept, and chunk_left holds the end of the chunk that s is in, or s_end if that is sooner
+    constexpr bool slim = slim_lane<R, FEAT>;
+    uint32_t chunk_id = block_y * a.chunks_per_group, chunk_left = slim ? min(s + a.chunk, s_end) : a.chunk;
     const size_t pslot = (size_t)block_x * RENDER_THREADS + thread_x;
     const size_t pstride = (size_t)a.ntiles_mine * RENDER_THREADS;
     int depth = 0;
-    int status = ST_FRESH;
+    int status = ST_FRESH;  // slim: status in bits 0-1, dead (valid in ST_VERTEX) in bit 2, depth from bit 3; `depth` and `dead` unused
     // f32 only: trace_ray's value as a function of the radiance x that comes back from below the deepest level
     // reached so far, per channel:  L(x) = fwdA + min(fwdT x, fwdC).  A level contributes x -> a + min(w x, 100)
     // (renderer.rs:153-167: a = Le + direct light, w = f |cos| / pdf >= 0), and for W >= 0
@@ -230,9 +240,9 @@ RPTB_D void render_thread(const SceneView<R>& sv, const RenderArgs<R>& a, const 
         // than the refills it merges.)
         {   // converged here: the lanes that are short of draws for this slot compute their Philox blocks together
             uint32_t need = 0;
-            if (status == ST_VERTEX && !dead) {
+            if (slim ? (status & 7) == ST_VERTEX : status == ST_VERTEX && !dead) {
                 if (light_slot) need = slot < 8u ? (draw_hint >> (4u * slot)) & 15u : 4u;
-                else if ((uint32_t)depth < a.max_bounces) need = 4u;  // gen_bool + Beckmann (1 + UnitCircle) or UnitDisc
+                else if ((uint32_t)(slim ? status >> 3 : depth) < a.max_bounces) need = 4u;  // gen_bool + Beckmann (1 + UnitCircle) or UnitDisc
             }
             rng.template ensure<W>(wmask, need);
         }
@@ -240,7 +250,7 @@ RPTB_D void render_thread(const SceneView<R>& sv, const RenderArgs<R>& a, const 
 
         if (light_slot) {
             // ================= sample_lights, one sampled light per slot ==================
-            if (status == ST_VERTEX && !dead) {
+            if (slim ? (status & 7) == ST_VERTEX : status == ST_VERTEX && !dead) {
                 const MaterialRec<R> mat = sv.materials[mat_id];
                 while (scene_light<FEAT>(sv, li).kind == LIGHT_AMBIENT) {  // ambient lights listed before it
                     const LightRec<R>& l = scene_light<FEAT>(sv, li);
@@ -269,7 +279,7 @@ RPTB_D void render_thread(const SceneView<R>& sv, const RenderArgs<R>& a, const 
             }
         } else {
             // ================= segment slot: bounce, finish, regenerate ====================
-            if (status == ST_VERTEX) {
+            if ((slim ? status & 3 : status) == ST_VERTEX) {
                 const MaterialRec<R> mat = sv.materials[mat_id];
                 while (li < sv.nlights) {  // trailing ambient lights (and, for a dead vertex, all of them)
                     const LightRec<R>& l = scene_light<FEAT>(sv, li);
@@ -279,7 +289,7 @@ RPTB_D void render_thread(const SceneView<R>& sv, const RenderArgs<R>& a, const 
                 Vec3<R> wi = rd;
                 R pdf = (R)1;
                 bool bounce = false;
-                if ((uint32_t)depth < a.max_bounces && !dead) bounce = sample_f<R, FEAT>(mat, n, wo, rng, wi, pdf);
+                if ((uint32_t)(slim ? status >> 3 : depth) < a.max_bounces && !(slim ? (status & 4) != 0 : dead)) bounce = sample_f<R, FEAT>(mat, n, wo, rng, wi, pdf);
                 if (bounce) {  // renderer.rs:157-164
                     const Vec3<R> f = bsdf<R, FEAT>(mat, n, wo, wi);
                     const R abscos = M<R>::abs(dot(wi, n));
@@ -307,7 +317,8 @@ RPTB_D void render_thread(const SceneView<R>& sv, const RenderArgs<R>& a, const 
                         bounce = !(w.x == (R)0 && w.y == (R)0 && w.z == (R)0);
                     }
                     if (bounce) {
-                        depth++;
+                        if constexpr (slim) status += 8;
+                        else depth++;
                         tmax = M<R>::inf();
                         ro = offset_origin(pos, ng, wi, err_scale);
                         rd = wi;
@@ -319,10 +330,10 @@ RPTB_D void render_thread(const SceneView<R>& sv, const RenderArgs<R>& a, const 
                     // this vertex's colour, so the composite evaluates to it whatever Lterm is; f64: the level at
                     // stack[depth] is not unwound, Lterm = color is the value of this vertex)
                     Lterm = color;
-                    status = ST_FINISH;
+                    status = slim ? (status & ~3) | ST_FINISH : ST_FINISH;
                 }
             }
-            if (status == ST_FINISH) {
+            if ((slim ? status & 3 : status) == ST_FINISH) {
                 Vec3<R> L = Lterm;
                 if constexpr (!M<R>::literal) {
                     // the composite of every level's clamp, applied to what came back from the last ray
@@ -339,18 +350,29 @@ RPTB_D void render_thread(const SceneView<R>& sv, const RenderArgs<R>& a, const 
                 acc1 += (double)L.y;
                 acc2 += (double)L.z;
                 s++;
-                if (a.nchunks > 1 && (--chunk_left == 0 || s == s_end)) {  // chunk complete: publish its sum
+                if constexpr (slim) {
+                    if (s == chunk_left) {  // chunk complete: publish its sum (chunk c holds samples [c chunk, (c + 1) chunk))
+                        if (a.nchunks > 1) {
+                            double* o = a.partial + ((size_t)((s - 1u) / a.chunk) * pstride + pslot) * 3;
+                            o[0] = acc0; o[1] = acc1; o[2] = acc2;
+                            acc0 = acc1 = acc2 = 0.0;
+                        }
+                        // s is s_end iff it is the image's last sample or starts a group (groups start at multiples of
+                        // chunks_per_group chunks); otherwise the next chunk ends inside this group
+                        chunk_left = s == a.iterations || s % (a.chunks_per_group * a.chunk) == 0u ? s : min(s + a.chunk, a.iterations);
+                    }
+                } else if (a.nchunks > 1 && (--chunk_left == 0 || s == s_end)) {  // chunk complete: publish its sum
                     double* o = a.partial + ((size_t)chunk_id * pstride + pslot) * 3;
                     o[0] = acc0; o[1] = acc1; o[2] = acc2;
                     acc0 = acc1 = acc2 = 0.0;
                     chunk_id++;
                     chunk_left = a.chunk;
                 }
-                status = ST_FRESH;
+                status = slim ? status & ~3 : ST_FRESH;
             }
-            if (status == ST_FRESH) {
-                if (s >= s_end) {
-                    status = ST_IDLE;
+            if ((slim ? status & 3 : status) == ST_FRESH) {
+                if (s >= (slim ? chunk_left : s_end)) {
+                    status = slim ? status | ST_IDLE : ST_IDLE;
                 } else {
                     rng.init(a.seed, pix, a.first_sample + s);
                     const R dx = gen_range(rng, (R)-1 / dim, (R)1 / dim);
@@ -373,14 +395,15 @@ RPTB_D void render_thread(const SceneView<R>& sv, const RenderArgs<R>& a, const 
                     ro = origin;
                     rd = M<R>::normalize(new_dir);
                     tmax = M<R>::inf();
-                    depth = 0;
+                    if constexpr (slim) status &= 7;
+                    else depth = 0;
                     active = true;
                 }
             }
         }
 
         // ================= the single get_closest_hit site ==============================
-        if (W::all(wmask, status == ST_IDLE)) break;  // also re-converges the warp
+        if (W::all(wmask, (slim ? status & 3 : status) == ST_IDLE)) break;  // also re-converges the warp
         Hit<R> h;
         h.t = tmax;
         h.obj = -1;
@@ -414,7 +437,7 @@ RPTB_D void render_thread(const SceneView<R>& sv, const RenderArgs<R>& a, const 
                         if ((FEAT & F_HDRI) && sv.env.kind != 0) pc.env_lookups++;
                     }
                     Lterm = env_color<R, FEAT>(sv.env, rd);
-                    status = ST_FINISH;
+                    status = slim ? (status & ~3) | ST_FINISH : ST_FINISH;
                 } else {
                     const ObjectRec<R>& ob = sv.objects[h.obj];
                     const Surface<R> sf = finalize_hit<R, FEAT>(sv, ob, ro, rd, h);
@@ -432,9 +455,14 @@ RPTB_D void render_thread(const SceneView<R>& sv, const RenderArgs<R>& a, const 
                     color = mat.emittance * mat_color(mat);
                     // opaque surface seen from its back: bsdf == 0 for every wi (material.rs:130-133),
                     // so neither the lights nor the bounce can contribute (f32 only; f64 stays literal)
-                    dead = !M<R>::literal && !mat.transparent && M<R>::signbit(dot(n, wo));
-                    li = 0;
-                    status = ST_VERTEX;
+                    if constexpr (slim) {
+                        status = (status & ~7) | (!mat.transparent && M<R>::signbit(dot(n, wo)) ? 4 : 0) | ST_VERTEX;
+                        li = 0;
+                    } else {
+                        dead = !M<R>::literal && !mat.transparent && M<R>::signbit(dot(n, wo));
+                        li = 0;
+                        status = ST_VERTEX;
+                    }
                 }
             }
         }

@@ -36,6 +36,10 @@ $(OBJDIR)/adaptive.o: $(CSRC)/adaptive.cu $(HDRS)
 $(OBJDIR)/denoise.o: $(CSRC)/denoise.cu $(HDRS)
 	@mkdir -p $(OBJDIR)
 	$(NVCC) $(NVFLAGS) -fmad=false -c $< -o $@ 2> $(OBJDIR)/denoise.ptxas.log || (cat $(OBJDIR)/denoise.ptxas.log; false)
+# the reprojection (reproject.h) likewise: its numpy restatement and host emulation round every operation on its own
+$(OBJDIR)/reproject.o: $(CSRC)/reproject.cu $(HDRS)
+	@mkdir -p $(OBJDIR)
+	$(NVCC) $(NVFLAGS) -fmad=false -c $< -o $@ 2> $(OBJDIR)/reproject.ptxas.log || (cat $(OBJDIR)/reproject.ptxas.log; false)
 $(OBJDIR)/film.o: $(CSRC)/film.cu $(HDRS)
 	@mkdir -p $(OBJDIR)
 	$(NVCC) $(NVFLAGS) -c $< -o $@ 2> $(OBJDIR)/film.ptxas.log || (cat $(OBJDIR)/film.ptxas.log; false)
@@ -52,7 +56,7 @@ $(OBJDIR)/objparse.o: $(CSRC)/objparse.cpp
 	@mkdir -p $(OBJDIR)
 	$(CXX) -std=c++17 -O3 -fPIC -Wall -c $< -o $@
 
-$(LIB): $(OBJDIR)/kernels_f32.o $(OBJDIR)/kernels_vx.o $(OBJDIR)/kernels_f64.o $(OBJDIR)/film.o $(OBJDIR)/adaptive.o $(OBJDIR)/denoise.o $(OBJDIR)/api.o $(OBJDIR)/kdbuild.o $(OBJDIR)/bvhbuild.o $(OBJDIR)/objparse.o
+$(LIB): $(OBJDIR)/kernels_f32.o $(OBJDIR)/kernels_vx.o $(OBJDIR)/kernels_f64.o $(OBJDIR)/film.o $(OBJDIR)/adaptive.o $(OBJDIR)/denoise.o $(OBJDIR)/reproject.o $(OBJDIR)/api.o $(OBJDIR)/kdbuild.o $(OBJDIR)/bvhbuild.o $(OBJDIR)/objparse.o
 	@mkdir -p rpt_b200/lib
 	$(NVCC) -shared $(ARCH) -o $@ $^ -Xcompiler -fopenmp -lgomp -cudart shared
 
@@ -77,7 +81,9 @@ HOSTEMU_LIST := tests/hostemu/_build/libhostemu_list.so
 HOSTEMU_DENOISE := tests/hostemu/_build/libhostemu_denoise.so
 # the same emulation plus the renders given no counters (the packed-table F_NOCOUNT twins; tests/hostemu/hostemu_slim.cu)
 HOSTEMU_SLIM := tests/hostemu/_build/libhostemu_slim.so
-hostemu: $(HOSTEMU) $(HOSTEMU_LIST) $(HOSTEMU_DENOISE) $(HOSTEMU_SLIM)
+# the denoiser's emulation plus the reprojection's per-pixel function (reproject.h; tests/hostemu/hostemu_reproject.cu)
+HOSTEMU_REPROJECT := tests/hostemu/_build/libhostemu_reproject.so
+hostemu: $(HOSTEMU) $(HOSTEMU_LIST) $(HOSTEMU_DENOISE) $(HOSTEMU_SLIM) $(HOSTEMU_REPROJECT)
 $(HOSTEMU): tests/hostemu/hostemu.cu $(CSRC)/kdbuild.cpp $(CSRC)/bvhbuild.cpp $(HDRS)
 	@mkdir -p $(dir $@)
 	nvcc -std=c++17 -O2 -DRPTB_HOST_EMU -DRPTB_BUILD_BVH8=1 -DRPTB_BUILD_BVH4=1 -gencode arch=compute_90a,code=sm_90a -Xcompiler -fPIC,-fopenmp,-ffp-contract=off -shared -Xlinker -Bsymbolic -o $@ tests/hostemu/hostemu.cu $(CSRC)/kdbuild.cpp $(CSRC)/bvhbuild.cpp -lgomp
@@ -90,6 +96,9 @@ $(HOSTEMU_DENOISE): tests/hostemu/hostemu_denoise.cu tests/hostemu/hostemu.cu $(
 $(HOSTEMU_SLIM): tests/hostemu/hostemu_slim.cu tests/hostemu/hostemu.cu $(CSRC)/kdbuild.cpp $(CSRC)/bvhbuild.cpp $(HDRS)
 	@mkdir -p $(dir $@)
 	nvcc -std=c++17 -O2 -DRPTB_HOST_EMU -DRPTB_BUILD_BVH8=1 -DRPTB_BUILD_BVH4=1 -gencode arch=compute_90a,code=sm_90a -Xcompiler -fPIC,-fopenmp,-ffp-contract=off -shared -Xlinker -Bsymbolic -o $@ tests/hostemu/hostemu_slim.cu $(CSRC)/kdbuild.cpp $(CSRC)/bvhbuild.cpp -lgomp
+$(HOSTEMU_REPROJECT): tests/hostemu/hostemu_reproject.cu tests/hostemu/hostemu_denoise.cu tests/hostemu/hostemu.cu $(CSRC)/kdbuild.cpp $(CSRC)/bvhbuild.cpp $(HDRS)
+	@mkdir -p $(dir $@)
+	nvcc -std=c++17 -O2 -DRPTB_HOST_EMU -DRPTB_BUILD_BVH8=1 -DRPTB_BUILD_BVH4=1 -gencode arch=compute_90a,code=sm_90a -Xcompiler -fPIC,-fopenmp,-ffp-contract=off -shared -Xlinker -Bsymbolic -o $@ tests/hostemu/hostemu_reproject.cu $(CSRC)/kdbuild.cpp $(CSRC)/bvhbuild.cpp -lgomp
 
 clean:
 	rm -rf build $(LIB) $(ORACLE) tests/hostemu/_build

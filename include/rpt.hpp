@@ -331,6 +331,13 @@ public:
         check(rptb_buffer_denoise(handle_, &d, nullptr, out.data()));
         return out;
     }
+    // Carries src's entries over a camera move into this buffer, which holds features and no entries
+    // (rptb_buffer_reproject).  Returns the number of pixels that got history.
+    uint64_t reproject_from(const DeviceBuffer& src, const rptb_reproject& params) {
+        uint64_t n = 0;
+        check(rptb_buffer_reproject(handle_, src.handle_, &params, &n));
+        return n;
+    }
     rptb_buffer* handle() const { return handle_; }
 
 private:

@@ -458,7 +458,7 @@ int rptb_buffer_pixel_stats(rptb_buffer* buffer, double* sums, double* m2, uint3
  * window and blurs silhouettes and shadow edges as much as noise.  These stand beside it: a first-hit feature
  * pass, and the spatial part of SVGF (Schied et al., HPG 2017), an edge-avoiding a-trous wavelet filter
  * (Dammertz et al., HPG 2010) guided by the features and by each pixel's variance of the mean -- the statistic
- * rptb_adaptive tests.  Temporal reprojection is not done: the Buffer is one image.
+ * rptb_adaptive tests.  Temporal reprojection across camera moves: rptb_buffer_reproject.
  *
  * Adds, for every pixel and every sample i in [first_sample, first_sample + iterations), the first hit of the
  * render's camera ray for Philox key (seed, pixel, i) -- the same draws in the same order, tmin 1e-12, in
@@ -493,6 +493,35 @@ typedef struct rptb_denoise {
  * negative or not finite.                                                                                     */
 int rptb_buffer_denoise(rptb_buffer* buffer, const rptb_denoise* params, double* out_rgb /* nullable */,
                         uint8_t* out_rgb8 /* nullable */);
+
+/* ---- Reprojecting the device Buffer across a camera move ---------------------------------------------------
+ * The temporal half of SVGF for a static scene: each pixel of `dst`'s view finds, through its own first-hit depth,
+ * the world point it sees, projects it into `src`'s view and takes the history of the (up to four, bilinear) src
+ * pixels there whose depth, normal and hit fraction agree with it -- their mean, their per-entry variance and at
+ * most max_history entries.  A pixel with no consistent history (a disocclusion, the edge of the old view) gets
+ * count 0, and an adaptive call renders it first.  rpt_b200/csrc/reproject.h gives every formula and its order of
+ * operations.
+ *
+ * A buffer records the camera its entries were rendered through (rptb_sample_into, rptb_sample_into_adaptive) and
+ * the camera of its features (rptb_buffer_add_features), compared bitwise; a second, different camera makes that
+ * side "mixed", and rptb_buffer_add_samples makes the entries "unknown".  The recording changes no other call.
+ *
+ * RPTB_ERR_BAD_ARG: a null pointer or src == dst; params out of range; dst holding entries or no features; src
+ * holding no entries or no features; entries or features of either buffer mixed or unknown, or src's entry camera
+ * not its feature camera; buffers created on scenes with different device lists.  RPTB_ERR_UNSUPPORTED: an open
+ * aperture on either camera (depth of field blurs the first hits: there is no one point to reproject).  The two
+ * buffers may differ in size.  The results are the same bits for any device count.  Afterwards dst's entries count
+ * as rendered through its feature camera.  A reprojected buffer may hold pixels with 0 or 1 entries: its image()
+ * fails ("Pixel found with no samples") while a pixel has none, denoise() while a pixel has fewer than 2, and its
+ * variance() is NaN while a pixel has fewer than 2.                                                            */
+typedef struct rptb_reproject {
+    double depth_tol;      /* relative depth tolerance, finite, >= 0                        */
+    double normal_cos;     /* least N_p . N_q, in [-1, 1]                                  */
+    uint32_t max_history;  /* entries a reprojected pixel keeps, >= 2                       */
+    uint32_t _pad;
+} rptb_reproject;
+int rptb_buffer_reproject(rptb_buffer* dst, rptb_buffer* src, const rptb_reproject* params,
+                          uint64_t* out_reused /* nullable, forces sync: pixels that got history */);
 
 #ifdef __cplusplus
 }

@@ -196,6 +196,16 @@ class Denoise(C.Structure):
     ]
 
 
+class Reproject(C.Structure):
+    """rptb_reproject: the parameters of rptb_buffer_reproject."""
+    _fields_ = [
+        ("depth_tol", C.c_double),
+        ("normal_cos", C.c_double),
+        ("max_history", C.c_uint32),
+        ("_pad", C.c_uint32),
+    ]
+
+
 class KdTreeOut(C.Structure):
     _fields_ = [
         ("nodes", C.POINTER(KdNode)),
@@ -269,6 +279,7 @@ SYMBOLS = [
      [C.c_void_p, C.POINTER(Camera), C.POINTER(RenderParams), C.c_void_p, C.POINTER(Stats)]),
     ("rptb_buffer_features", C.c_int, [C.c_void_p, c_double_p, c_double_p, c_double_p, c_double_p]),
     ("rptb_buffer_denoise", C.c_int, [C.c_void_p, C.POINTER(Denoise), c_double_p, c_u8_p]),
+    ("rptb_buffer_reproject", C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(Reproject), C.POINTER(C.c_uint64)]),
 ]
 
 _lib = None

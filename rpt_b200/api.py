@@ -877,6 +877,22 @@ class Denoise:
         return capi.Denoise(self.iterations, self.sigma_normal, self.sigma_depth, self.sigma_luminance, self.albedo_eps)
 
 
+class Reproject:
+    """Parameters of DeviceBuffer.reproject_from (rptb_reproject): how a pixel of the new view decides which pixels of the
+    old view saw the same surface.  depth_tol: the largest |z_q - l| / l between an old pixel's first-hit depth z_q and
+    the distance l from the old eye to the new pixel's first hit; normal_cos: the least dot product of the two
+    first-hit normals; max_history: the most entries a reprojected pixel keeps, which bounds how long a view-dependent
+    highlight lags behind the camera.  Defaults 0.02, 0.9, 8: over 16-frame orbits of the sphere, Cornell, the teapot
+    and glass they are the setting of tools/reproject_measure.py's sweep under which no scene's raw MSE loses to fresh
+    frames, and the best for the denoised ones (DESIGN.md section 6c).  rpt_b200/csrc/reproject.h gives every formula."""
+
+    def __init__(self, depth_tol: float = 0.02, normal_cos: float = 0.9, max_history: int = 8):
+        self.depth_tol, self.normal_cos, self.max_history = float(depth_tol), float(normal_cos), int(max_history)
+
+    def to_c(self) -> capi.Reproject:
+        return capi.Reproject(self.depth_tol, self.normal_cos, self.max_history, 0)
+
+
 class Buffer:
     """src/buffer.rs:6-93.  Holds one equally weighted entry per pixel per
     `add_samples` call, like the reference's Vec<Vec<Color>>."""
@@ -1005,6 +1021,17 @@ class DeviceBuffer:
         capi.check(capi.lib().rptb_buffer_denoise(self.handle, C.byref(c), None, out.ctypes.data_as(capi.c_u8_p)),
                    "rptb_buffer_denoise")
         return out
+
+    def reproject_from(self, src: "DeviceBuffer", params: Optional[Reproject] = None) -> int:
+        """Carries `src`'s entries over a camera move into this buffer, which must hold features (Renderer.sample_features
+        through its camera) and no entries; `src` must hold entries and features made through one camera.  Each pixel
+        takes the history of the old pixels that saw its first-hit point, or none (count 0: a disocclusion or the edge of
+        the old view, which an adaptive sample() renders first).  Returns the number of pixels that got history."""
+        c = (params or Reproject()).to_c()
+        n = C.c_uint64(0)
+        capi.check(capi.lib().rptb_buffer_reproject(self.handle, src.handle, C.byref(c), C.byref(n)), "rptb_buffer_reproject")
+        self.entries = int(self.counts().max())
+        return int(n.value)
 
     def close(self) -> None:
         if self.handle:
@@ -1198,6 +1225,37 @@ class Renderer:
                 self.sample(self._num_samples // entries, buf, want_stats=False)
             self.sample_features(feature_samples, buf)
             return buf.denoised_image(denoise)
+
+    def render_frames(self, cameras, entries: int = 8, feature_samples: int = 16, reproject: Optional[Reproject] = Reproject(),
+                      adaptive: Optional[Adaptive] = None, denoise: Optional[Denoise] = None):
+        """Renders one frame per camera of a static scene and yields each as (height, width, 3) uint8.  Per frame: a new
+        DeviceBuffer gets `feature_samples` feature rays through the frame's camera, the previous frame's buffer is
+        reprojected into it (unless `reproject` is None), and `entries` entries of num_samples / entries samples each are
+        added -- adaptive ones with `adaptive` -- continuing the renderer's sample streams; the frame is image(), or
+        denoised_image(denoise).  The device scene is uploaded once for all frames."""
+        if entries < 1 or self._num_samples % entries:
+            raise ValueError(f"num_samples {self._num_samples} must be a multiple of entries {entries} (and entries >= 1)")
+        if denoise is not None and entries < 2 and adaptive is None:
+            raise ValueError("a denoised frame needs entries >= 2 (or adaptive entries)")
+        own, prev = self.camera, None
+        try:
+            for cam in cameras:
+                self.camera = cam
+                buf = self.device_buffer()
+                self.sample_features(feature_samples, buf)
+                if prev is not None and reproject is not None:
+                    buf.reproject_from(prev, reproject)
+                for _ in range(entries):
+                    self.sample(self._num_samples // entries, buf, want_stats=False, adaptive=adaptive)
+                img = buf.image() if denoise is None else buf.denoised_image(denoise)
+                if prev is not None:
+                    prev.close()
+                prev = buf
+                yield img
+        finally:
+            self.camera = own
+            if prev is not None:
+                prev.close()
 
     def iterative_render(self, callback_interval: int, callback: Callable[[int, Buffer], None],
                          buffer: Optional[DeviceBuffer] = None, adaptive: Optional[Adaptive] = None) -> None:  # :103-115

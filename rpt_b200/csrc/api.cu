@@ -27,6 +27,7 @@
 #include "denoise.h"
 #include "flatten.h"
 #include "launch.h"
+#include "reproject.h"
 #include "tile.h"
 
 namespace rptb {
@@ -58,6 +59,14 @@ cudaError_t launch_features_resolve(const double* row_feat, uint64_t npix, doubl
 cudaError_t launch_denoise(const double* sums, const double* m2, const uint32_t* counts, const double* nrm,
                            const double* depth, const double* albedo, uint32_t width, uint32_t height, const rptb_denoise& d,
                            double* const col[2], double* const var[2], double* out, cudaStream_t stream, uint32_t* launches);
+// the reprojection, the row-major -> compact copy back and the least count: reproject.cu
+cudaError_t launch_reproject(const ReprojectView& dv, const ReprojectView& sv, const ReprojectSource& s, const double* dnrm,
+                             const double* ddepth, const double* dfrac, const rptb_reproject& prm, double* sums, double* m2,
+                             uint32_t* counts, unsigned long long* reused, cudaStream_t stream);
+cudaError_t launch_buffer_compact(const double* row_sums, const double* row_m2, const uint32_t* row_counts, uint64_t nelem,
+                                  uint32_t width, uint32_t height, uint32_t shard_index, uint32_t shard_count, double* sums,
+                                  double* m2, uint32_t* counts, cudaStream_t stream);
+cudaError_t launch_buffer_min_count(const uint32_t* counts, uint64_t npix, uint32_t* out, cudaStream_t stream);
 int parse_obj_text(const char* text, size_t len, std::vector<double>& tris, std::string& err);
 struct ObjGroup {
     rptb_material material;
@@ -586,11 +595,30 @@ struct BufferPart {
     double* feat = nullptr;
 };
 
+// The camera one side of a buffer (its entries or its features) was made with, for rptb_buffer_reproject: none yet, one
+// camera (bitwise), several, or unknown (a host entry).
+struct CameraRecord {
+    enum State { NONE, ONE, MIXED, UNKNOWN } state = NONE;
+    rptb_camera cam;
+    void note(const rptb_camera& c) {
+        if (state == NONE) {
+            state = ONE;
+            cam = c;
+        } else if (state == ONE && std::memcmp(&cam, &c, sizeof(c)) != 0) {
+            state = MIXED;
+        }
+    }
+};
+
 struct rptb_buffer {
     uint32_t width = 0, height = 0, radius = 0;
-    // accumulate calls.  No pixel holds more entries, and every pixel holds at least min(entries, 2): see
-    // rptb_buffer_denoise
+    // accumulate calls.  No pixel holds more entries, and -- unless the buffer was reprojected -- every pixel holds at
+    // least min(entries, 2): see rptb_buffer_denoise
     uint32_t entries = 0;
+    // rptb_buffer_reproject wrote its entries: pixels may hold 0 or 1 entries, and image / variance / denoise look at the
+    // least count on the device.  `entries` is then max_history plus the calls since, a bound.
+    bool reprojected = false;
+    CameraRecord entry_cam, feat_cam;
     std::vector<BufferPart> parts;
     // on parts[0]'s device, allocated by the first image / variance / sums: the image gathered row-major
     double* row_sums = nullptr;  // width*height*3
@@ -605,6 +633,9 @@ struct rptb_buffer {
     double* gather_feat = nullptr;   // one other part's feature sums
     double* aov = nullptr;           // width*height*8: normal (3), albedo (3), depth, hit fraction planes
     double* dn = nullptr;            // width*height*11: colour (3) and variance ping-pong planes, then c' (3)
+    // on parts[0]'s device, allocated by the first reprojection into the buffer: the reused-pixel counter and the least count
+    unsigned long long* reused = nullptr;
+    uint32_t* min_count = nullptr;
     std::mutex lock;
 };
 
@@ -643,6 +674,8 @@ void buffer_free(rptb_buffer* b) {
             cudaFree(b->gather_feat);
             cudaFree(b->aov);
             cudaFree(b->dn);
+            cudaFree(b->reused);
+            cudaFree(b->min_count);
         }
         if (q.done) cudaEventDestroy(q.done);
         if (q.stream) cudaStreamDestroy(q.stream);
@@ -666,21 +699,30 @@ int buffer_part_alloc(BufferPart& q) {
     return RPTB_OK;
 }
 
+// The row-major planes on parts[0]'s device (its device current), allocated on first use.
+int buffer_rows_alloc(rptb_buffer* b) {
+    if (b->row_sums) return RPTB_OK;
+    const uint32_t nparts = (uint32_t)b->parts.size();
+    const size_t npix = (size_t)b->width * b->height;
+    uint32_t most = 0;
+    for (uint32_t i = 1; i < nparts; i++) most = std::max(most, b->parts[i].tiles);
+    CU(cudaMalloc((void**)&b->row_sums, npix * 3 * sizeof(double)));
+    CU(cudaMalloc((void**)&b->row_m2, npix * sizeof(double)));
+    CU(cudaMalloc((void**)&b->row_counts, npix * sizeof(uint32_t)));
+    if (most) CU(cudaMalloc((void**)&b->gather, (size_t)most * 128u * (4u * sizeof(double) + sizeof(uint32_t))));
+    CU(cudaMalloc((void**)&b->partial, (buffer_variance_blocks(npix) + 1) * sizeof(double)));
+    CU(cudaMalloc((void**)&b->rgb8, npix * 3));
+    return RPTB_OK;
+}
+
 // Brings every part's sums, M2 and/or counts to parts[0]'s device in row-major order, on parts[0]'s stream (the caller
 // has made that device current).  Other parts are copied with cudaMemcpyPeerAsync, which needs no peer access.
 int buffer_gather(rptb_buffer* b, bool want_sums, bool want_m2, bool want_counts) {
     BufferPart& q0 = b->parts[0];
     const uint32_t nparts = (uint32_t)b->parts.size();
-    const size_t npix = (size_t)b->width * b->height;
-    if (!b->row_sums) {
-        uint32_t most = 0;
-        for (uint32_t i = 1; i < nparts; i++) most = std::max(most, b->parts[i].tiles);
-        CU(cudaMalloc((void**)&b->row_sums, npix * 3 * sizeof(double)));
-        CU(cudaMalloc((void**)&b->row_m2, npix * sizeof(double)));
-        CU(cudaMalloc((void**)&b->row_counts, npix * sizeof(uint32_t)));
-        if (most) CU(cudaMalloc((void**)&b->gather, (size_t)most * 128u * (4u * sizeof(double) + sizeof(uint32_t))));
-        CU(cudaMalloc((void**)&b->partial, (buffer_variance_blocks(npix) + 1) * sizeof(double)));
-        CU(cudaMalloc((void**)&b->rgb8, npix * 3));
+    {
+        const int rc = buffer_rows_alloc(b);
+        if (rc != RPTB_OK) return rc;
     }
     double* rs = want_sums ? b->row_sums : nullptr;
     double* rm = want_m2 ? b->row_m2 : nullptr;
@@ -737,6 +779,16 @@ int buffer_features(rptb_buffer* b) {
     }
     double* a = b->aov;
     CU(launch_features_resolve(b->row_feat, npix, (double)b->feature_rays, a, a + 6 * npix, a + 3 * npix, a + 7 * npix, q0.stream));
+    return RPTB_OK;
+}
+
+// The least per-pixel count of a reprojected buffer, from the row-major counts buffer_gather left (parts[0]'s device
+// current).  Waits for it.
+int buffer_min_count(rptb_buffer* b, uint32_t* out) {
+    BufferPart& q0 = b->parts[0];
+    CU(launch_buffer_min_count(b->row_counts, (uint64_t)b->width * b->height, b->min_count, q0.stream));
+    CU(cudaMemcpyAsync(out, b->min_count, sizeof(uint32_t), cudaMemcpyDeviceToHost, q0.stream));
+    CU(cudaStreamSynchronize(q0.stream));
     return RPTB_OK;
 }
 
@@ -1415,6 +1467,7 @@ static int sample_into_impl(rptb_scene* s, const rptb_camera* cam, const rptb_re
         if (rc != RPTB_OK) return nparts > 1 ? fail(rc, "device %d: %s", r->device, g_error.c_str()) : rc;
     }
     b->entries++;
+    b->entry_cam.note(*cam);
     if (out_active) {
         uint64_t total = 0;
         for (uint32_t i = 0; i < nparts; i++) {
@@ -1486,6 +1539,7 @@ int rptb_buffer_add_samples(rptb_buffer* b, const double* rgb) {
         CU(cudaEventRecord(q.done, q.stream));
     }
     b->entries++;
+    b->entry_cam.state = CameraRecord::UNKNOWN;
     return RPTB_OK;
 }
 
@@ -1495,8 +1549,14 @@ int rptb_buffer_image(rptb_buffer* b, uint8_t* out_rgb8) {
     if (b->entries == 0) return fail(RPTB_ERR_BAD_ARG, "Pixel found with no samples");  // buffer.rs:89
     BufferPart& q0 = b->parts[0];
     DeviceGuard g(q0.device);
-    const int rc = buffer_gather(b, true, false, true);
+    int rc = buffer_gather(b, true, false, true);
     if (rc != RPTB_OK) return rc;
+    if (b->reprojected) {
+        uint32_t least = 0;
+        rc = buffer_min_count(b, &least);
+        if (rc != RPTB_OK) return rc;
+        if (least == 0) return fail(RPTB_ERR_BAD_ARG, "Pixel found with no samples");  // buffer.rs:89
+    }
     const size_t nvals = (size_t)b->width * b->height * 3;
     CU(launch_film_resolve_counted(b->row_sums, b->row_counts, b->width, b->height, b->radius, b->rgb8, q0.stream));
     CU(cudaMemcpyAsync(out_rgb8, b->rgb8, nvals, cudaMemcpyDeviceToHost, q0.stream));
@@ -1513,8 +1573,17 @@ int rptb_buffer_variance(rptb_buffer* b, double* out) {
     }
     BufferPart& q0 = b->parts[0];
     DeviceGuard g(q0.device);
-    const int rc = buffer_gather(b, false, true, true);
+    int rc = buffer_gather(b, false, true, true);
     if (rc != RPTB_OK) return rc;
+    if (b->reprojected) {
+        uint32_t least = 0;
+        rc = buffer_min_count(b, &least);
+        if (rc != RPTB_OK) return rc;
+        if (least < 2) {
+            *out = NAN;
+            return RPTB_OK;
+        }
+    }
     const uint64_t npix = (uint64_t)b->width * b->height;
     double* total = b->partial + buffer_variance_blocks(npix);
     CU(launch_buffer_variance_sum(b->row_m2, b->row_counts, npix, b->partial, total, q0.stream));
@@ -1603,6 +1672,7 @@ int rptb_buffer_add_features(rptb_scene* s, const rptb_camera* cam, const rptb_r
         CU(cudaEventRecord(q.done, r->stream));
     }
     b->feature_rays += p->iterations;
+    b->feat_cam.note(*cam);
     if (!stats) return RPTB_OK;
     std::memset(stats, 0, sizeof(*stats));
     for (uint32_t i = 0; i < nparts; i++) {
@@ -1656,6 +1726,13 @@ int rptb_buffer_denoise(rptb_buffer* b, const rptb_denoise* d, double* out_rgb, 
     const size_t npix = (size_t)b->width * b->height;
     int rc = buffer_gather(b, true, true, true);
     if (rc != RPTB_OK) return rc;
+    if (b->reprojected) {  // the invariant above does not hold: look at the counts
+        uint32_t least = 0;
+        rc = buffer_min_count(b, &least);
+        if (rc != RPTB_OK) return rc;
+        if (least == 0) return fail(RPTB_ERR_BAD_ARG, "Pixel found with no samples");  // buffer.rs:89
+        if (least < 2) return fail(RPTB_ERR_BAD_ARG, "a pixel has fewer than 2 entries (no variance to guide the filter)");
+    }
     rc = buffer_features(b);
     if (rc != RPTB_OK) return rc;
     if (!b->dn) CU(cudaMalloc((void**)&b->dn, npix * 11 * sizeof(double)));
@@ -1673,6 +1750,98 @@ int rptb_buffer_denoise(rptb_buffer* b, const rptb_denoise* d, double* out_rgb, 
         CU(cudaMemcpyAsync(out_rgb8, b->rgb8, npix * 3, cudaMemcpyDeviceToHost, q0.stream));
     }
     CU(cudaStreamSynchronize(q0.stream));
+    return RPTB_OK;
+}
+
+int rptb_buffer_reproject(rptb_buffer* dst, rptb_buffer* src, const rptb_reproject* prm, uint64_t* out_reused) {
+    if (!dst || !src || !prm) return fail(RPTB_ERR_BAD_ARG, "null argument");
+    if (dst == src) return fail(RPTB_ERR_BAD_ARG, "src and dst are the same buffer");
+    if (!(std::isfinite(prm->depth_tol) && prm->depth_tol >= 0.0))
+        return fail(RPTB_ERR_BAD_ARG, "depth_tol must be finite and >= 0 (%g)", prm->depth_tol);
+    if (!(prm->normal_cos >= -1.0 && prm->normal_cos <= 1.0)) return fail(RPTB_ERR_BAD_ARG, "normal_cos must lie in [-1, 1] (%g)", prm->normal_cos);
+    if (prm->max_history < 2) return fail(RPTB_ERR_BAD_ARG, "max_history %u < 2 (a pixel's variance needs two entries)", prm->max_history);
+    std::scoped_lock both(dst->lock, src->lock);
+    bool same = dst->parts.size() == src->parts.size();
+    for (size_t i = 0; same && i < dst->parts.size(); i++) same = dst->parts[i].device == src->parts[i].device;
+    if (!same) return fail(RPTB_ERR_BAD_ARG, "the buffers were created on scenes with different device lists");
+    if (dst->entries) return fail(RPTB_ERR_BAD_ARG, "dst already holds entries");
+    if (dst->feature_rays == 0) return fail(RPTB_ERR_BAD_ARG, "dst holds no features (rptb_buffer_add_features)");
+    if (src->entries == 0) return fail(RPTB_ERR_BAD_ARG, "src holds no entries");
+    if (src->feature_rays == 0) return fail(RPTB_ERR_BAD_ARG, "src holds no features (rptb_buffer_add_features)");
+    const char* why[] = {"none", "one", "mixed (several cameras)", "unknown (a host entry)"};
+    if (src->entry_cam.state != CameraRecord::ONE)
+        return fail(RPTB_ERR_BAD_ARG, "src's entries have no single camera: %s", why[src->entry_cam.state]);
+    if (src->feat_cam.state != CameraRecord::ONE)
+        return fail(RPTB_ERR_BAD_ARG, "src's features have no single camera: %s", why[src->feat_cam.state]);
+    if (dst->feat_cam.state != CameraRecord::ONE)
+        return fail(RPTB_ERR_BAD_ARG, "dst's features have no single camera: %s", why[dst->feat_cam.state]);
+    if (std::memcmp(&src->entry_cam.cam, &src->feat_cam.cam, sizeof(rptb_camera)) != 0)
+        return fail(RPTB_ERR_BAD_ARG, "src's entries and features were made through different cameras");
+    if (src->feat_cam.cam.aperture > 0.0 || dst->feat_cam.cam.aperture > 0.0)
+        return fail(RPTB_ERR_UNSUPPORTED, "an open aperture: depth of field blurs the first hits, no one point to reproject");
+    BufferPart& d0 = dst->parts[0];
+    BufferPart& s0 = src->parts[0];
+    DeviceGuard g(d0.device);
+    if (!g.ok) return fail(RPTB_ERR_CUDA, "cudaSetDevice(%d) failed", d0.device);
+    // src's state and both buffers' features, row-major on parts[0]'s device
+    int rc = buffer_gather(src, true, true, true);
+    if (rc != RPTB_OK) return rc;
+    rc = buffer_features(src);
+    if (rc != RPTB_OK) return rc;
+    CU(cudaEventRecord(s0.done, s0.stream));
+    rc = buffer_rows_alloc(dst);
+    if (rc != RPTB_OK) return rc;
+    rc = buffer_features(dst);
+    if (rc != RPTB_OK) return rc;
+    if (!dst->reused) {
+        CU(cudaMalloc((void**)&dst->reused, sizeof(unsigned long long)));
+        CU(cudaMalloc((void**)&dst->min_count, sizeof(uint32_t)));
+    }
+    CU(cudaStreamWaitEvent(d0.stream, s0.done, 0));
+    if (out_reused) CU(cudaMemsetAsync(dst->reused, 0, sizeof(unsigned long long), d0.stream));
+    const size_t snpix = (size_t)src->width * src->height, dnpix = (size_t)dst->width * dst->height;
+    const ReprojectView dv = reproject_view(dst->feat_cam.cam, dst->width, dst->height);
+    const ReprojectView sv = reproject_view(src->feat_cam.cam, src->width, src->height);
+    const double* sa = src->aov;
+    const ReprojectSource sp = {src->row_sums, src->row_m2, src->row_counts, sa, sa + 6 * snpix, sa + 7 * snpix};
+    const double* da = dst->aov;
+    CU(launch_reproject(dv, sv, sp, da, da + 6 * dnpix, da + 7 * dnpix, *prm, dst->row_sums, dst->row_m2, dst->row_counts,
+                        out_reused ? dst->reused : nullptr, d0.stream));
+    // back to every dst part's compact tiles: part 0 in place, the others through the gather scratch and a peer copy
+    const uint32_t nparts = (uint32_t)dst->parts.size();
+    for (uint32_t i = 0; i < nparts; i++) {
+        BufferPart& q = dst->parts[i];
+        if (!q.tiles) continue;
+        const size_t nelem = (size_t)q.tiles * 128u;
+        double* sums = i == 0 ? q.sums : dst->gather;
+        double* m2 = i == 0 ? q.m2 : dst->gather + nelem * 3;
+        uint32_t* counts = i == 0 ? q.counts : (uint32_t*)(dst->gather + nelem * 4);
+        CU(launch_buffer_compact(dst->row_sums, dst->row_m2, dst->row_counts, nelem, dst->width, dst->height, i, nparts, sums, m2, counts,
+                                 d0.stream));
+        if (i == 0) continue;
+        CU(cudaMemcpyPeerAsync(q.sums, q.device, sums, d0.device, nelem * 3 * sizeof(double), d0.stream));
+        CU(cudaMemcpyPeerAsync(q.m2, q.device, m2, d0.device, nelem * sizeof(double), d0.stream));
+        CU(cudaMemcpyPeerAsync(q.counts, q.device, counts, d0.device, nelem * sizeof(uint32_t), d0.stream));
+    }
+    // every later call on either buffer is ordered behind this one
+    CU(cudaEventRecord(d0.done, d0.stream));
+    CU(cudaEventRecord(s0.done, d0.stream));
+    for (rptb_buffer* b : {dst, src})
+        for (size_t i = 1; i < b->parts.size(); i++) {
+            BufferPart& q = b->parts[i];
+            DeviceGuard gi(q.device);
+            CU(cudaStreamWaitEvent(q.stream, d0.done, 0));
+            CU(cudaEventRecord(q.done, q.stream));
+        }
+    dst->entries = prm->max_history;
+    dst->reprojected = true;
+    dst->entry_cam = dst->feat_cam;
+    if (out_reused) {
+        unsigned long long n = 0;
+        CU(cudaMemcpyAsync(&n, dst->reused, sizeof(n), cudaMemcpyDeviceToHost, d0.stream));
+        CU(cudaStreamSynchronize(d0.stream));
+        *out_reused = n;
+    }
     return RPTB_OK;
 }
 

@@ -1,0 +1,178 @@
+// reproject.h -- the per-pixel arithmetic of rptb_buffer_reproject, one set of functions for the device (reproject.cu,
+// compiled with -fmad=false) and the host emulation (tests/hostemu, -ffp-contract=off).  Every operation is a double
+// rounded on its own, in the order written here, so tests/reproject_ref.py (numpy float64) restates it bit for bit.
+//
+// The temporal half of SVGF (Schied et al., HPG 2017) for a camera move over an immutable scene: a pixel of the new
+// view finds the world point its first hits saw, projects it into the old view and takes the history of the old
+// pixels around it that saw the same surface.
+//
+// Cameras.  D = direction, U = up, R = normalize(D x U), dc = 1 / tan(fov / 2), as fill_args (flatten.h) derives them.
+// In a W x H view, dim = max(W, H), the centre ray of pixel (x, y) is r = (dc D + xn R) + yn U (per component), with
+//     xn = ((2x + 1) - W) / dim,   yn = ((2(H - y) - 1) - H) / dim.
+// dot(a, b) = (a0 b0 + a1 b1) + a2 b2;  cross(a, b) = (a1 b2 - a2 b1, a2 b0 - a0 b2, a0 b1 - a1 b0);  |a| = sqrt(dot(a, a)).
+//
+// Per destination pixel p with resolved features N_p, z_p and hit fraction f_p:
+//     f_p > 0:  X = eye_dst + z_p (r / |r|),  v = X - eye_src,  l = |v|     (a surface: reprojected by position)
+//     f_p = 0:  v = r / |r|,  l = +inf                                      (the environment: reprojected by direction)
+// Projection into the source view, by Cramer's rule (up need not be orthogonal to direction):
+//     a = dc_s D_s,  b = R_s,  c = U_s,  det = dot(a, cross(b, c))
+//     alpha = dot(v, cross(b, c)) / det,  beta = dot(a, cross(v, c)) / det,  gamma = dot(a, cross(b, v)) / det
+//     only alpha > 0 has history;  xs = beta / alpha,  ys = gamma / alpha
+//     px = (xs dim_s + (W_s - 1)) / 2,  py = ((H_s - 1) - ys dim_s) / 2     (continuous source pixel; integers are centres)
+// Taps: x0 = floor(px), y0 = floor(py), fx = px - x0, fy = py - y0; the four taps (x0, y0), (x0 + 1, y0), (x0, y0 + 1),
+// (x0 + 1, y0 + 1) in that order, with weights wx * wy from wx = (1 - fx, fx), wy = (1 - fy, fy).  A tap q is valid iff
+// its weight is > 0, it lies in the source image, n_q >= 2, its three sums and its M2 are finite, and
+//     surface (f_p > 0):      f_q > 0,  |z_q - l| <= depth_tol * l,  dot(N_p, N_q) >= normal_cos
+//     environment (f_p = 0):  f_q = 0.
+// History: W = sum of the valid taps' weights (in tap order).  W < kReprojectMinWeight: no history (sums 0, M2 0, count
+// 0).  Otherwise, with w^_q = w_q / W, in tap order:
+//     mu_c = sum w^_q * (S_qc / n_q),   s2 = sum w^_q * (M2_q / (n_q - 1)),   n_h = min(max_history, min over valid q of n_q)
+// and the pixel gets sums mu_c * n_h, M2 s2 * (n_h - 1) and count n_h: the mean and the per-entry variance of its
+// neighbourhood, carried as if n_h entries had made them.
+#pragma once
+#include <cmath>
+
+#include "../../include/rpt_b200.h"
+#include "vec.cuh"
+
+namespace rptb {
+
+constexpr double kReprojectMinWeight = 1e-2;  // SVGF's threshold on the summed weight of the consistent taps
+
+// One view: a camera and the image size it renders.
+struct ReprojectView {
+    double eye[3], D[3], U[3], R[3];
+    double dc, dim;
+    uint32_t width, height;
+};
+
+// The source planes, row-major: sums (3 per pixel), M2, counts, and the resolved features normal (3), depth, hit fraction.
+struct ReprojectSource {
+    const double* sums;
+    const double* m2;
+    const uint32_t* counts;
+    const double* nrm;
+    const double* depth;
+    const double* frac;
+};
+
+inline ReprojectView reproject_view(const rptb_camera& c, uint32_t width, uint32_t height) {
+    ReprojectView v;
+    const double* di = c.direction;
+    const double* up = c.up;
+    const double right[3] = {di[1] * up[2] - di[2] * up[1], di[2] * up[0] - di[0] * up[2], di[0] * up[1] - di[1] * up[0]};
+    const double len = std::sqrt((right[0] * right[0] + right[1] * right[1]) + right[2] * right[2]);
+    for (int k = 0; k < 3; k++) {
+        v.eye[k] = c.eye[k];
+        v.D[k] = di[k];
+        v.U[k] = up[k];
+        v.R[k] = right[k] / len;
+    }
+    v.dc = 1.0 / std::tan(c.fov / 2.0);
+    v.width = width;
+    v.height = height;
+    v.dim = (double)(width > height ? width : height);
+    return v;
+}
+
+RPTB_HD double reproject_dot(const double* a, const double* b) { return (a[0] * b[0] + a[1] * b[1]) + a[2] * b[2]; }
+
+RPTB_HD void reproject_cross(const double* a, const double* b, double* o) {
+    o[0] = a[1] * b[2] - a[2] * b[1];
+    o[1] = a[2] * b[0] - a[0] * b[2];
+    o[2] = a[0] * b[1] - a[1] * b[0];
+}
+
+RPTB_HD bool reproject_finite(double x) { return x - x == 0.0; }
+
+// The history of destination pixel (x, y) of view dv from the source state s seen through view sv.  Np (3), zp, fp: the
+// pixel's resolved features.  Writes out_sums[3] and *out_m2, returns the count.
+RPTB_HD uint32_t reproject_pixel(const ReprojectView& dv, const ReprojectView& sv, const ReprojectSource& s, uint32_t x, uint32_t y,
+                                 const double* Np, double zp, double fp, const rptb_reproject& prm, double* out_sums, double* out_m2) {
+    out_sums[0] = 0.0;
+    out_sums[1] = 0.0;
+    out_sums[2] = 0.0;
+    *out_m2 = 0.0;
+    const double xn = ((double)(2u * x + 1u) - (double)dv.width) / dv.dim;
+    const double yn = ((double)(2u * (dv.height - y) - 1u) - (double)dv.height) / dv.dim;
+    double r[3];
+    for (int k = 0; k < 3; k++) r[k] = (dv.dc * dv.D[k] + xn * dv.R[k]) + yn * dv.U[k];
+    const double rl = ::sqrt(reproject_dot(r, r));
+    const bool surface = fp > 0.0;
+    double v[3], ell;
+    if (surface) {
+        for (int k = 0; k < 3; k++) v[k] = (dv.eye[k] + zp * (r[k] / rl)) - sv.eye[k];
+        ell = ::sqrt(reproject_dot(v, v));
+    } else {
+        for (int k = 0; k < 3; k++) v[k] = r[k] / rl;
+        ell = (double)INFINITY;
+    }
+    const double a[3] = {sv.dc * sv.D[0], sv.dc * sv.D[1], sv.dc * sv.D[2]};
+    double bc[3], vc[3], bv[3];
+    reproject_cross(sv.R, sv.U, bc);
+    reproject_cross(v, sv.U, vc);
+    reproject_cross(sv.R, v, bv);
+    const double det = reproject_dot(a, bc);
+    const double alpha = reproject_dot(v, bc) / det;
+    const double beta = reproject_dot(a, vc) / det;
+    const double gamma = reproject_dot(a, bv) / det;
+    if (!(alpha > 0.0)) return 0u;
+    const double xs = beta / alpha, ys = gamma / alpha;
+    const double px = (xs * sv.dim + (double)(sv.width - 1u)) / 2.0;
+    const double py = ((double)(sv.height - 1u) - ys * sv.dim) / 2.0;
+    // every tap lies outside (or has weight 0) past these bounds; they also keep a huge or NaN position off the casts
+    if (!(px > -1.0 && px < (double)sv.width && py > -1.0 && py < (double)sv.height)) return 0u;
+    const double x0 = ::floor(px), y0 = ::floor(py);
+    const double fx = px - x0, fy = py - y0;
+    const double wx[2] = {1.0 - fx, fx}, wy[2] = {1.0 - fy, fy};
+    double w[4];
+    int64_t q[4];
+    double W = 0.0;
+    uint32_t nmin = 0xFFFFFFFFu;
+    for (int t = 0; t < 4; t++) {
+        w[t] = 0.0;
+        q[t] = -1;
+        const double wt = wx[t & 1] * wy[t >> 1];
+        const int64_t qx = (int64_t)x0 + (t & 1), qy = (int64_t)y0 + (t >> 1);
+        if (!(wt > 0.0) || qx < 0 || qy < 0 || qx >= (int64_t)sv.width || qy >= (int64_t)sv.height) continue;
+        const int64_t i = qy * (int64_t)sv.width + qx;
+        const uint32_t n = s.counts[i];
+        if (n < 2u) continue;
+        if (!(reproject_finite(s.sums[3 * i]) && reproject_finite(s.sums[3 * i + 1]) && reproject_finite(s.sums[3 * i + 2]) &&
+              reproject_finite(s.m2[i])))
+            continue;
+        const double fq = s.frac[i];
+        if (surface) {
+            if (!(fq > 0.0)) continue;
+            if (!(::fabs(s.depth[i] - ell) <= prm.depth_tol * ell)) continue;
+            if (!(reproject_dot(Np, s.nrm + 3 * i) >= prm.normal_cos)) continue;
+        } else if (fq != 0.0) {
+            continue;
+        }
+        w[t] = wt;
+        q[t] = i;
+        W = W + wt;
+        nmin = n < nmin ? n : nmin;
+    }
+    if (!(W >= kReprojectMinWeight)) return 0u;
+    double mu0 = 0.0, mu1 = 0.0, mu2 = 0.0, s2 = 0.0;
+    for (int t = 0; t < 4; t++) {
+        if (q[t] < 0) continue;
+        const int64_t i = q[t];
+        const double wh = w[t] / W;
+        const double dn = (double)s.counts[i];
+        mu0 = mu0 + wh * (s.sums[3 * i] / dn);
+        mu1 = mu1 + wh * (s.sums[3 * i + 1] / dn);
+        mu2 = mu2 + wh * (s.sums[3 * i + 2] / dn);
+        s2 = s2 + wh * (s.m2[i] / (double)(s.counts[i] - 1u));
+    }
+    const uint32_t nh = prm.max_history < nmin ? prm.max_history : nmin;
+    const double dh = (double)nh;
+    out_sums[0] = mu0 * dh;
+    out_sums[1] = mu1 * dh;
+    out_sums[2] = mu2 * dh;
+    *out_m2 = s2 * (double)(nh - 1u);
+    return nh;
+}
+
+}  // namespace rptb

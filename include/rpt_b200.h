@@ -402,7 +402,8 @@ void rptb_buffer_destroy(rptb_buffer* buffer);
  * f32 path's float widened to double) -- to `buffer`, on the device.  The render is not copied to the host; with
  * stats == NULL the call returns once the work is enqueued.  width/height must be the buffer's and `scene` must have
  * the device list of the scene the buffer was created on (else RPTB_ERR_BAD_ARG); shard_count > 1 is
- * RPTB_ERR_UNSUPPORTED (a buffer holds the whole image); compact_out is ignored.                              */
+ * RPTB_ERR_UNSUPPORTED on a whole buffer, and a shard buffer (rptb_buffer_create_shard) takes exactly its own
+ * shard_index / shard_count (else RPTB_ERR_BAD_ARG); compact_out is ignored.                                  */
 int rptb_sample_into(rptb_scene* scene, const rptb_camera* camera, const rptb_render_params* params,
                      rptb_buffer* buffer, rptb_stats* stats /* nullable, forces sync */);
 /* Replaces: Buffer::add_samples (src/buffer.rs:32-40) of a host entry: width*height*3 doubles, row-major.      */
@@ -522,6 +523,41 @@ typedef struct rptb_reproject {
 } rptb_reproject;
 int rptb_buffer_reproject(rptb_buffer* dst, rptb_buffer* src, const rptb_reproject* params,
                           uint64_t* out_reused /* nullable, forces sync: pixels that got history */);
+
+/* ---- Sharding the device Buffer across processes ---------------------------------------------------------
+ * Stands beside rptb_render_samples_device's shards for hosts that run one process per GPU (torchrun): each process
+ * keeps a buffer of its own tiles, samples, adapts and adds features into it with no exchange, and one all-gather of
+ * the shards' blocks gives every process an ordinary whole buffer whose image, variance, pixel_stats, features and
+ * denoise are the same bits as those of one whole buffer given the same calls -- same bits for any shard count.
+ *
+ * A buffer holding only the 16x8 tiles t with t % shard_count == shard_index (a shard may own none: its calls are then
+ * no-ops), in one part on scene's device.  rptb_sample_into, rptb_sample_into_adaptive and rptb_buffer_add_features
+ * take it when params->shard_index / shard_count are its own (else RPTB_ERR_BAD_ARG); out_active counts this shard's
+ * pixels.  Its whole-image calls -- image, variance, sums, pixel_stats, features, denoise, reproject (as dst or src)
+ * and add_samples -- are RPTB_ERR_UNSUPPORTED: gather the shards first.  RPTB_ERR_BAD_ARG: shard_index >=
+ * shard_count, and the checks of rptb_buffer_create; RPTB_ERR_UNSUPPORTED: a scene with more than one replica.   */
+int rptb_buffer_create_shard(rptb_scene* scene, uint32_t width, uint32_t height, uint32_t box_radius, uint32_t shard_index,
+                             uint32_t shard_count, rptb_buffer** out);
+/* The size in bytes of the shard buffer's exchange block, the same for every shard of one image and shard count: a
+ * 256-byte header, then the shard's planes, each padded to shard 0's pixel slots P = (its tiles) * 128 -- sums (3P
+ * doubles), M2 (P doubles), with_features the feature sums (8P doubles: normal 3P, albedo 3P, hits P, depth P), then
+ * counts (P uint32).  256 + 36 P bytes, 256 + 100 P with features.  0 for NULL or a whole buffer.           */
+uint64_t rptb_buffer_shard_bytes(const rptb_buffer* buffer, uint32_t with_features);
+/* Writes the shard buffer's block (rptb_buffer_shard_bytes) to dst_device, on `stream` (a cudaStream_t, behind the
+ * buffer's earlier calls; NULL = the buffer's own stream, and the call then synchronises).  The header holds the
+ * image size, shard_index, shard_count, with_features, the entry count, the feature rays and the recorded entry and
+ * feature cameras; the planes are device-to-device copies of the shard's own.  Slots past the shard's own are not
+ * written.  RPTB_ERR_BAD_ARG: a null pointer, a whole buffer, or with_features on a buffer holding no features.  */
+int rptb_buffer_export_shard(rptb_buffer* buffer, void* dst_device, uint32_t with_features, void* stream);
+/* Replaces the state of `dst`, a whole buffer, with the shards gathered in `gathered_device` on dst's first device:
+ * shard_count blocks of rptb_buffer_shard_bytes each, shard 0 first -- what an all-gather of every shard's export
+ * gives.  The bytes must be complete when the call is made; it returns once it has read them.  Afterwards dst holds
+ * the shards' entries, counts and recorded cameras -- and their features with with_features, none without -- and is
+ * indistinguishable from a whole buffer that received the same calls (it may be reprojected from or into).
+ * RPTB_ERR_BAD_ARG: a null pointer or shard_count 0; dst a shard buffer; a block that is not an export, or was made
+ * for another image size, shard count or with_features; shards out of order (block i must hold shard i); shards that
+ * received different calls (entry counts, feature rays or cameras differ).                                        */
+int rptb_buffer_import_shards(rptb_buffer* dst, const void* gathered_device, uint32_t shard_count, uint32_t with_features);
 
 #ifdef __cplusplus
 }

@@ -280,6 +280,11 @@ SYMBOLS = [
     ("rptb_buffer_features", C.c_int, [C.c_void_p, c_double_p, c_double_p, c_double_p, c_double_p]),
     ("rptb_buffer_denoise", C.c_int, [C.c_void_p, C.POINTER(Denoise), c_double_p, c_u8_p]),
     ("rptb_buffer_reproject", C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(Reproject), C.POINTER(C.c_uint64)]),
+    ("rptb_buffer_create_shard", C.c_int,
+     [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(C.c_void_p)]),
+    ("rptb_buffer_shard_bytes", C.c_uint64, [C.c_void_p, C.c_uint32]),
+    ("rptb_buffer_export_shard", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p]),
+    ("rptb_buffer_import_shards", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32]),
 ]
 
 _lib = None

@@ -940,6 +940,8 @@ class DeviceBuffer:
     holds.  The numbers are those of the host Buffer over the same entries: sums() is np.sum(batches, axis=0)
     bit for bit, image() gives the same bytes, variance() agrees to rounding (Welford instead of two passes)."""
 
+    shard: Optional[tuple] = None  # (shard_index, shard_count) of a distributed.ShardBuffer; None = the whole image
+
     def __init__(self, scene: DeviceScene, width: int, height: int, filter: Optional[Filter] = None):
         self.width, self.height = int(width), int(height)
         self.filter = filter or Filter()
@@ -1159,9 +1161,11 @@ class Renderer:
         host memory; a DeviceBuffer gets it on the device, and the call returns once the work is enqueued unless
         `want_stats` (then last_stats is filled, which waits for the render).
         `adaptive` (DeviceBuffer only): add the entry only to the pixels the criterion leaves active
-        (rptb_sample_into_adaptive); returns how many pixels got it, which waits for the call."""
+        (rptb_sample_into_adaptive); returns how many pixels got it, which waits for the call.
+        A distributed.ShardBuffer renders and adds its own shard's tiles only; `adaptive` then counts its pixels."""
         ds = self.device_scene()
-        p = self.params(iterations, self._next_sample, collect_stats=collect_stats)
+        shard = getattr(buffer, "shard", None) or (0, 1)
+        p = self.params(iterations, self._next_sample, *shard, collect_stats=collect_stats)
         cam = self.camera.to_c()
         if adaptive is not None:
             if not isinstance(buffer, DeviceBuffer):
@@ -1171,7 +1175,9 @@ class Renderer:
                                                             C.byref(active), C.byref(stats) if want_stats else None),
                        "rptb_sample_into_adaptive")
             self._next_sample += int(iterations)
-            if active.value:  # the largest per-pixel count, as rptb_buffer_sums reports it
+            if buffer.shard is not None:  # a shard's counts are read after the gather; the calls bound them
+                buffer.entries += 1
+            elif active.value:  # the largest per-pixel count, as rptb_buffer_sums reports it
                 buffer.entries = int(buffer.counts().max())
             self.last_stats = stats.as_dict() if want_stats else None
             return int(active.value)
@@ -1202,7 +1208,7 @@ class Renderer:
         if not isinstance(buffer, DeviceBuffer):
             raise TypeError("features live in a DeviceBuffer (Renderer.device_buffer())")
         ds = self.device_scene()
-        p = self.params(iterations, buffer.feature_rays)
+        p = self.params(iterations, buffer.feature_rays, *(buffer.shard or (0, 1)))
         cam = self.camera.to_c()
         stats = capi.Stats()
         capi.check(capi.lib().rptb_buffer_add_features(ds.handle, C.byref(cam), C.byref(p), buffer.handle,

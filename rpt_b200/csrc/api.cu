@@ -574,7 +574,10 @@ void destroy_replica(rptb_scene* s) {
 // or on the part's own (rptb_buffer_add_samples) -- and every later operation on the part waits for it.
 struct BufferPart {
     int device = 0;
-    uint32_t tiles = 0;          // tiles t with t % nparts == this part's index
+    // this part's place in the tile deal: it holds the tiles t with t % count == index.  Part i of a whole buffer of n
+    // parts is (i, n); the one part of a shard buffer (rptb_buffer_create_shard) is the shard's own pair.
+    uint32_t index = 0, count = 1;
+    uint32_t tiles = 0;          // tiles t with t % count == index
     double* sums = nullptr;      // tiles * 128 * 3
     double* m2 = nullptr;        // tiles * 128
     uint32_t* counts = nullptr;  // tiles * 128
@@ -618,6 +621,9 @@ struct rptb_buffer {
     // rptb_buffer_reproject wrote its entries: pixels may hold 0 or 1 entries, and image / variance / denoise look at the
     // least count on the device.  `entries` is then max_history plus the calls since, a bound.
     bool reprojected = false;
+    // rptb_buffer_create_shard: the buffer holds one shard of the image (parts[0]'s index and count), and its whole-image
+    // reads are refused until the shards are gathered into a whole buffer (rptb_buffer_import_shards)
+    bool shard = false;
     CameraRecord entry_cam, feat_cam;
     std::vector<BufferPart> parts;
     // on parts[0]'s device, allocated by the first image / variance / sums: the image gathered row-major
@@ -745,6 +751,19 @@ int buffer_gather(rptb_buffer* b, bool want_sums, bool want_m2, bool want_counts
     return RPTB_OK;
 }
 
+// The row-major feature planes on parts[0]'s device (its device current), allocated on first use.
+int buffer_feat_rows_alloc(rptb_buffer* b) {
+    if (b->row_feat) return RPTB_OK;
+    const uint32_t nparts = (uint32_t)b->parts.size();
+    const size_t npix = (size_t)b->width * b->height;
+    uint32_t most = 0;
+    for (uint32_t i = 1; i < nparts; i++) most = std::max(most, b->parts[i].tiles);
+    CU(cudaMalloc((void**)&b->row_feat, npix * 8 * sizeof(double)));
+    CU(cudaMalloc((void**)&b->aov, npix * 8 * sizeof(double)));
+    if (most) CU(cudaMalloc((void**)&b->gather_feat, (size_t)most * 128u * 8u * sizeof(double)));
+    return RPTB_OK;
+}
+
 // Brings every part's feature sums to parts[0] row-major (b->row_feat) and resolves the feature planes into b->aov, on
 // parts[0]'s stream (its device current).  The normal / albedo planes go through the Buffer's scatter as "sums", the hit
 // and depth planes as "M2".
@@ -752,12 +771,9 @@ int buffer_features(rptb_buffer* b) {
     BufferPart& q0 = b->parts[0];
     const uint32_t nparts = (uint32_t)b->parts.size();
     const size_t npix = (size_t)b->width * b->height;
-    if (!b->row_feat) {
-        uint32_t most = 0;
-        for (uint32_t i = 1; i < nparts; i++) most = std::max(most, b->parts[i].tiles);
-        CU(cudaMalloc((void**)&b->row_feat, npix * 8 * sizeof(double)));
-        CU(cudaMalloc((void**)&b->aov, npix * 8 * sizeof(double)));
-        if (most) CU(cudaMalloc((void**)&b->gather_feat, (size_t)most * 128u * 8u * sizeof(double)));
+    {
+        const int rc = buffer_feat_rows_alloc(b);
+        if (rc != RPTB_OK) return rc;
     }
     double* rn = b->row_feat;
     double* ra = rn + 3 * npix;
@@ -835,16 +851,17 @@ int render_list_launch(rptb_scene* s, const rptb_camera* cam, const rptb_render_
     return RPTB_OK;
 }
 
-// Enqueues replica `index` of `nparts`'s share of one rptb_sample_into on the replica's own stream: render its
-// tiles into the compact out32/out64 scratch, then add them to the buffer part as one more entry of every pixel.  No
-// host synchronise.  `crit` (rptb_sample_into_adaptive): first decide which pixels and warp blocks are active, render
-// those through the list schedule and add the entry to them alone.
-int sample_part(rptb_scene* r, const rptb_camera* cam, const rptb_render_params* p, uint32_t index, uint32_t nparts,
-                BufferPart& q, bool want_stats, uint32_t* launches, const rptb_adaptive* crit = nullptr) {
+// Enqueues one buffer part's share of one rptb_sample_into on replica r's own stream: render the part's tiles (its
+// index of its count) into the compact out32/out64 scratch, then add them to the part as one more entry of every
+// pixel.  No host synchronise.  `crit` (rptb_sample_into_adaptive): first decide which pixels and warp blocks are
+// active, render those through the list schedule and add the entry to them alone.
+int sample_part(rptb_scene* r, const rptb_camera* cam, const rptb_render_params* p, BufferPart& q, bool want_stats,
+                uint32_t* launches, const rptb_adaptive* crit = nullptr) {
     DeviceGuard g(r->device);
     if (!g.ok) return fail(RPTB_ERR_CUDA, "cudaSetDevice(%d) failed", r->device);
     int rc = wait_busy(r, r->stream);
     if (rc != RPTB_OK) return rc;
+    const uint32_t index = q.index, nparts = q.count;
     rptb_render_params qp = *p;
     qp.shard_index = index;
     qp.shard_count = nparts;
@@ -878,6 +895,122 @@ int sample_part(rptb_scene* r, const rptb_camera* cam, const rptb_render_params*
     // the scratch is read until the accumulate has run: later calls on any stream order themselves behind it
     CU(cudaEventRecord(r->busy, r->stream));
     r->busy_pending = true;
+    return RPTB_OK;
+}
+
+// Writes the row-major sums / M2 / counts on parts[0]'s device (its device current) back into every part's compact tiles,
+// on parts[0]'s stream: part 0 in place, the others through the gather scratch and a peer copy.
+int buffer_rows_to_parts(rptb_buffer* b) {
+    const BufferPart& q0 = b->parts[0];
+    for (size_t i = 0; i < b->parts.size(); i++) {
+        BufferPart& q = b->parts[i];
+        if (!q.tiles) continue;
+        const size_t nelem = (size_t)q.tiles * 128u;
+        double* sums = i == 0 ? q.sums : b->gather;
+        double* m2 = i == 0 ? q.m2 : b->gather + nelem * 3;
+        uint32_t* counts = i == 0 ? q.counts : (uint32_t*)(b->gather + nelem * 4);
+        CU(launch_buffer_compact(b->row_sums, b->row_m2, b->row_counts, nelem, b->width, b->height, q.index, q.count, sums, m2, counts,
+                                 q0.stream));
+        if (i == 0) continue;
+        CU(cudaMemcpyPeerAsync(q.sums, q.device, sums, q0.device, nelem * 3 * sizeof(double), q0.stream));
+        CU(cudaMemcpyPeerAsync(q.m2, q.device, m2, q0.device, nelem * sizeof(double), q0.stream));
+        CU(cudaMemcpyPeerAsync(q.counts, q.device, counts, q0.device, nelem * sizeof(uint32_t), q0.stream));
+    }
+    return RPTB_OK;
+}
+
+// The same for the row-major feature sums (b->row_feat): the normal / albedo planes go through the compact kernel as
+// "sums", the hit and depth planes as "M2", with no counts -- the routes buffer_features takes them the other way.  Every
+// part must hold feature memory.
+int buffer_feat_rows_to_parts(rptb_buffer* b) {
+    const BufferPart& q0 = b->parts[0];
+    const size_t npix = (size_t)b->width * b->height;
+    const double* rn = b->row_feat;
+    const double* ra = rn + 3 * npix;
+    const double* rh = rn + 6 * npix;
+    const double* rz = rn + 7 * npix;
+    for (size_t i = 0; i < b->parts.size(); i++) {
+        BufferPart& q = b->parts[i];
+        if (!q.tiles) continue;
+        const size_t nelem = (size_t)q.tiles * 128u;
+        double* f = i == 0 ? q.feat : b->gather_feat;
+        CU(launch_buffer_compact(rn, rh, nullptr, nelem, b->width, b->height, q.index, q.count, f, f + 6 * nelem, nullptr, q0.stream));
+        CU(launch_buffer_compact(ra, rz, nullptr, nelem, b->width, b->height, q.index, q.count, f + 3 * nelem, f + 7 * nelem, nullptr,
+                                 q0.stream));
+        if (i > 0) CU(cudaMemcpyPeerAsync(q.feat, q.device, f, q0.device, nelem * 8 * sizeof(double), q0.stream));
+    }
+    return RPTB_OK;
+}
+
+// ---- the exchange block of a shard buffer (rptb_buffer_export_shard / rptb_buffer_import_shards) ----
+// A header of kShardHeaderBytes, then the shard's compact planes, each padded to shard 0's slots (the most any shard
+// holds, as distributed.gather_tiles pads): sums (3 doubles a slot), M2 (1 double), with features their 8 planes
+// (normal 3, albedo 3, hits 1, depth 1: 8 doubles a slot), then counts (1 uint32).  Slots past the shard's own are not
+// written.
+constexpr uint32_t kShardMagic = 0x44524853u;  // "SHRD"
+constexpr size_t kShardHeaderBytes = 256;
+struct ShardCamera {
+    uint32_t state, _pad;  // CameraRecord::State
+    rptb_camera cam;       // zero unless state is ONE
+};
+struct ShardHeader {
+    uint32_t magic, with_features, width, height, shard_index, shard_count, entries, _pad;
+    uint64_t feature_rays;
+    ShardCamera entry_cam, feat_cam;
+};
+static_assert(sizeof(ShardHeader) <= kShardHeaderBytes, "the shard header outgrew its slot");
+
+struct ShardLayout {
+    size_t slots;                          // pixel slots of every plane: shard 0's tiles * 128
+    size_t sums, m2, feat, counts, bytes;  // byte offsets in the block, and its size
+};
+ShardLayout shard_layout(uint32_t width, uint32_t height, uint32_t count, bool with_features) {
+    ShardLayout l;
+    l.slots = (size_t)buffer_tiles(width, height, 0, count) * 128u;
+    l.sums = kShardHeaderBytes;
+    l.m2 = l.sums + l.slots * 3 * sizeof(double);
+    l.feat = l.m2 + l.slots * sizeof(double);
+    l.counts = l.feat + (with_features ? l.slots * 8 * sizeof(double) : 0);
+    l.bytes = l.counts + l.slots * sizeof(uint32_t);
+    return l;
+}
+
+ShardCamera shard_camera(const CameraRecord& r) {
+    ShardCamera c;
+    std::memset(&c, 0, sizeof(c));
+    c.state = (uint32_t)r.state;
+    if (r.state == CameraRecord::ONE) c.cam = r.cam;
+    return c;
+}
+
+CameraRecord camera_record(const ShardCamera& c) {
+    CameraRecord r;
+    r.state = (CameraRecord::State)c.state;
+    r.cam = c.cam;
+    return r;
+}
+
+// Whole-image reads need every tile: a shard buffer holds only its own.
+int refuse_shard(const char* what) {
+    return fail(RPTB_ERR_UNSUPPORTED,
+                "%s of a shard buffer: it holds only its own tiles; gather the shards into a whole buffer first "
+                "(rptb_buffer_export_shard, rptb_buffer_import_shards)",
+                what);
+}
+
+// The shard a render into buffer b may name: a whole buffer takes shard_count 0 or 1 only, a shard buffer exactly its own
+// (shard_index, shard_count).
+int check_buffer_shard(const rptb_render_params* p, const rptb_buffer* b) {
+    const uint32_t sc = p->shard_count ? p->shard_count : 1u;
+    if (!b->shard) {
+        if (sc > 1)
+            return fail(RPTB_ERR_UNSUPPORTED, "shard_count %u: a buffer holds the whole image (shard with rptb_buffer_create_shard)", sc);
+        return RPTB_OK;
+    }
+    const BufferPart& q = b->parts[0];
+    if (p->shard_index != q.index || sc != q.count)
+        return fail(RPTB_ERR_BAD_ARG, "the render is shard %u of %u but the buffer holds shard %u of %u", p->shard_index, sc, q.index,
+                    q.count);
     return RPTB_OK;
 }
 
@@ -1406,23 +1539,25 @@ int rptb_film_resolve(const double* sums, uint32_t nbatches, uint32_t width, uin
     return RPTB_OK;
 }
 
-int rptb_buffer_create(rptb_scene* s, uint32_t width, uint32_t height, uint32_t box_radius, rptb_buffer** out) {
-    if (!s || !out) return fail(RPTB_ERR_BAD_ARG, "null argument");
-    *out = nullptr;
-    if (width == 0 || height == 0) return fail(RPTB_ERR_BAD_ARG, "empty image %ux%u", width, height);
-    if ((uint64_t)width * height > 0x7FFFFFFFull / 4) return fail(RPTB_ERR_UNSUPPORTED, "image too large");
+// A whole buffer (shard_count == 0: one part per replica of s, part i dealt (i, nparts)) or the one-part shard buffer of
+// (shard_index, shard_count) on s's device.  The arguments are checked by the callers.
+static int buffer_create_impl(rptb_scene* s, uint32_t width, uint32_t height, uint32_t box_radius, uint32_t shard_index,
+                              uint32_t shard_count, rptb_buffer** out) {
     rptb_buffer* b = new (std::nothrow) rptb_buffer();
     if (!b) return fail(RPTB_ERR_OOM, "host allocation failed");
     b->width = width;
     b->height = height;
     b->radius = box_radius;
-    const uint32_t nparts = 1u + (uint32_t)s->peers.size();
+    b->shard = shard_count > 0;
+    const uint32_t nparts = b->shard ? 1u : 1u + (uint32_t)s->peers.size();
     b->parts.resize(nparts);
     int rc = RPTB_OK;
     for (uint32_t i = 0; rc == RPTB_OK && i < nparts; i++) {
         BufferPart& q = b->parts[i];
         q.device = i == 0 ? s->device : s->peers[i - 1]->device;
-        q.tiles = buffer_tiles(width, height, i, nparts);
+        q.index = b->shard ? shard_index : i;
+        q.count = b->shard ? shard_count : nparts;
+        q.tiles = buffer_tiles(width, height, q.index, q.count);
         DeviceGuard g(q.device);
         rc = g.ok ? buffer_part_alloc(q) : fail(RPTB_ERR_CUDA, "cudaSetDevice(%d) failed", q.device);
     }
@@ -1436,6 +1571,26 @@ int rptb_buffer_create(rptb_scene* s, uint32_t width, uint32_t height, uint32_t 
     return RPTB_OK;
 }
 
+int rptb_buffer_create(rptb_scene* s, uint32_t width, uint32_t height, uint32_t box_radius, rptb_buffer** out) {
+    if (!s || !out) return fail(RPTB_ERR_BAD_ARG, "null argument");
+    *out = nullptr;
+    if (width == 0 || height == 0) return fail(RPTB_ERR_BAD_ARG, "empty image %ux%u", width, height);
+    if ((uint64_t)width * height > 0x7FFFFFFFull / 4) return fail(RPTB_ERR_UNSUPPORTED, "image too large");
+    return buffer_create_impl(s, width, height, box_radius, 0, 0, out);
+}
+
+int rptb_buffer_create_shard(rptb_scene* s, uint32_t width, uint32_t height, uint32_t box_radius, uint32_t shard_index,
+                             uint32_t shard_count, rptb_buffer** out) {
+    if (!s || !out) return fail(RPTB_ERR_BAD_ARG, "null argument");
+    *out = nullptr;
+    if (width == 0 || height == 0) return fail(RPTB_ERR_BAD_ARG, "empty image %ux%u", width, height);
+    if ((uint64_t)width * height > 0x7FFFFFFFull / 4) return fail(RPTB_ERR_UNSUPPORTED, "image too large");
+    if (shard_index >= shard_count) return fail(RPTB_ERR_BAD_ARG, "shard_index %u >= shard_count %u", shard_index, shard_count);
+    if (!s->peers.empty())
+        return fail(RPTB_ERR_UNSUPPORTED, "a shard buffer lives on one device, but the scene has %u replicas", 1u + (uint32_t)s->peers.size());
+    return buffer_create_impl(s, width, height, box_radius, shard_index, shard_count, out);
+}
+
 void rptb_buffer_destroy(rptb_buffer* b) {
     if (b) buffer_free(b);
 }
@@ -1445,8 +1600,8 @@ static int sample_into_impl(rptb_scene* s, const rptb_camera* cam, const rptb_re
     if (!b) return fail(RPTB_ERR_BAD_ARG, "null argument");
     int rc = check_params(s, cam, p);
     if (rc != RPTB_OK) return rc;
-    if (p->shard_count > 1)
-        return fail(RPTB_ERR_UNSUPPORTED, "shard_count %u: a buffer holds the whole image (shard with rptb_render_samples_device)", p->shard_count);
+    rc = check_buffer_shard(p, b);
+    if (rc != RPTB_OK) return rc;
     if (crit && p->engine == RPTB_ENGINE_WAVEFRONT)
         return fail(RPTB_ERR_UNSUPPORTED, "adaptive sampling renders with the slot megakernel, not the wavefront engine");
     if (p->width != b->width || p->height != b->height)
@@ -1463,7 +1618,7 @@ static int sample_into_impl(rptb_scene* s, const rptb_camera* cam, const rptb_re
     for (uint32_t i = 0; i < nparts; i++) {
         rptb_scene* r = i == 0 ? s : s->peers[i - 1];
         locks.emplace_back(r->lock);
-        rc = sample_part(r, cam, p, i, nparts, b->parts[i], stats != nullptr, &launches[i], crit);
+        rc = sample_part(r, cam, p, b->parts[i], stats != nullptr, &launches[i], crit);
         if (rc != RPTB_OK) return nparts > 1 ? fail(rc, "device %d: %s", r->device, g_error.c_str()) : rc;
     }
     b->entries++;
@@ -1522,6 +1677,7 @@ int rptb_sample_into_adaptive(rptb_scene* s, const rptb_camera* cam, const rptb_
 
 int rptb_buffer_add_samples(rptb_buffer* b, const double* rgb) {
     if (!b || !rgb) return fail(RPTB_ERR_BAD_ARG, "null argument");
+    if (b->shard) return refuse_shard("add_samples");
     std::lock_guard<std::mutex> bl(b->lock);
     if (b->entries == UINT32_MAX) return fail(RPTB_ERR_UNSUPPORTED, "too many entries");
     const uint32_t nparts = (uint32_t)b->parts.size();
@@ -1534,7 +1690,7 @@ int rptb_buffer_add_samples(rptb_buffer* b, const double* rgb) {
         CU(cudaStreamWaitEvent(q.stream, q.done, 0));
         // pageable source: the call returns once the bytes are staged, `rgb` may be reused afterwards
         CU(cudaMemcpyAsync(q.upload, rgb, nvals * sizeof(double), cudaMemcpyHostToDevice, q.stream));
-        CU(launch_buffer_accumulate(nullptr, q.upload, true, nullptr, (uint64_t)q.tiles * 128u, b->width, b->height, i, nparts,
+        CU(launch_buffer_accumulate(nullptr, q.upload, true, nullptr, (uint64_t)q.tiles * 128u, b->width, b->height, q.index, q.count,
                                     q.sums, q.m2, q.counts, q.stream));
         CU(cudaEventRecord(q.done, q.stream));
     }
@@ -1545,6 +1701,7 @@ int rptb_buffer_add_samples(rptb_buffer* b, const double* rgb) {
 
 int rptb_buffer_image(rptb_buffer* b, uint8_t* out_rgb8) {
     if (!b || !out_rgb8) return fail(RPTB_ERR_BAD_ARG, "null argument");
+    if (b->shard) return refuse_shard("image");
     std::lock_guard<std::mutex> bl(b->lock);
     if (b->entries == 0) return fail(RPTB_ERR_BAD_ARG, "Pixel found with no samples");  // buffer.rs:89
     BufferPart& q0 = b->parts[0];
@@ -1566,6 +1723,7 @@ int rptb_buffer_image(rptb_buffer* b, uint8_t* out_rgb8) {
 
 int rptb_buffer_variance(rptb_buffer* b, double* out) {
     if (!b || !out) return fail(RPTB_ERR_BAD_ARG, "null argument");
+    if (b->shard) return refuse_shard("variance");
     std::lock_guard<std::mutex> bl(b->lock);
     if (b->entries < 2) {  // n - 1 = 0: the reference divides by it
         *out = NAN;
@@ -1596,6 +1754,7 @@ int rptb_buffer_variance(rptb_buffer* b, double* out) {
 
 int rptb_buffer_sums(rptb_buffer* b, double* out_sums, uint32_t* out_entries) {
     if (!b || !out_sums) return fail(RPTB_ERR_BAD_ARG, "null argument");
+    if (b->shard) return refuse_shard("sums");
     std::lock_guard<std::mutex> bl(b->lock);
     BufferPart& q0 = b->parts[0];
     DeviceGuard g(q0.device);
@@ -1614,6 +1773,7 @@ int rptb_buffer_sums(rptb_buffer* b, double* out_sums, uint32_t* out_entries) {
 
 int rptb_buffer_pixel_stats(rptb_buffer* b, double* sums, double* m2, uint32_t* counts) {
     if (!b) return fail(RPTB_ERR_BAD_ARG, "null argument");
+    if (b->shard) return refuse_shard("pixel_stats");
     std::lock_guard<std::mutex> bl(b->lock);
     BufferPart& q0 = b->parts[0];
     DeviceGuard g(q0.device);
@@ -1631,8 +1791,8 @@ int rptb_buffer_add_features(rptb_scene* s, const rptb_camera* cam, const rptb_r
     if (!b) return fail(RPTB_ERR_BAD_ARG, "null argument");
     int rc = check_params(s, cam, p);
     if (rc != RPTB_OK) return rc;
-    if (p->shard_count > 1)
-        return fail(RPTB_ERR_UNSUPPORTED, "shard_count %u: a buffer holds the whole image (shard with rptb_render_samples_device)", p->shard_count);
+    rc = check_buffer_shard(p, b);
+    if (rc != RPTB_OK) return rc;
     if (p->width != b->width || p->height != b->height)
         return fail(RPTB_ERR_BAD_ARG, "render is %ux%u but the buffer is %ux%u", p->width, p->height, b->width, b->height);
     const uint32_t nparts = 1u + (uint32_t)s->peers.size();
@@ -1656,8 +1816,8 @@ int rptb_buffer_add_features(rptb_scene* s, const rptb_camera* cam, const rptb_r
             CU(cudaMemsetAsync(q.feat, 0, nelem * 8 * sizeof(double), r->stream));
         }
         rptb_render_params qp = *p;
-        qp.shard_index = i;
-        qp.shard_count = nparts;
+        qp.shard_index = q.index;
+        qp.shard_count = q.count;
         if (stats) CU(cudaEventRecord(r->ev0, r->stream));
         if (p->precision == RPTB_PRECISION_F32) {
             RenderArgs<float> a;
@@ -1684,13 +1844,24 @@ int rptb_buffer_add_features(rptb_scene* s, const rptb_camera* cam, const rptb_r
         stats->gpu_ms = std::max(stats->gpu_ms, (double)ms);  // the devices run concurrently
         stats->launches += b->parts[i].tiles ? 1u : 0u;
     }
-    stats->rays = (uint64_t)b->width * b->height * p->iterations;
+    uint64_t npix = (uint64_t)b->width * b->height;
+    if (b->shard) {  // the pixels of the shard's own tiles
+        const BufferPart& q = b->parts[0];
+        const uint32_t tiles_x = (b->width + 15u) / 16u;
+        npix = 0;
+        for (uint32_t k = 0; k < q.tiles; k++) {
+            const uint32_t t = q.index + k * q.count, x0 = t % tiles_x * 16u, y0 = t / tiles_x * 8u;
+            npix += (uint64_t)std::min(16u, b->width - x0) * std::min(8u, b->height - y0);
+        }
+    }
+    stats->rays = npix * p->iterations;
     stats->engine = RPTB_ENGINE_MEGAKERNEL;
     return RPTB_OK;
 }
 
 int rptb_buffer_features(rptb_buffer* b, double* normal, double* depth, double* albedo, double* hit_fraction) {
     if (!b) return fail(RPTB_ERR_BAD_ARG, "null argument");
+    if (b->shard) return refuse_shard("features");
     std::lock_guard<std::mutex> bl(b->lock);
     if (b->feature_rays == 0) return fail(RPTB_ERR_BAD_ARG, "the buffer holds no features (rptb_buffer_add_features)");
     BufferPart& q0 = b->parts[0];
@@ -1714,6 +1885,7 @@ int rptb_buffer_denoise(rptb_buffer* b, const rptb_denoise* d, double* out_rgb, 
         !(std::isfinite(d->albedo_eps) && d->albedo_eps >= 0.0))
         return fail(RPTB_ERR_BAD_ARG, "sigma_depth, sigma_luminance and albedo_eps must be finite and >= 0 (%g, %g, %g)", d->sigma_depth,
                     d->sigma_luminance, d->albedo_eps);
+    if (b->shard) return refuse_shard("denoise");
     std::lock_guard<std::mutex> bl(b->lock);
     if (b->entries == 0) return fail(RPTB_ERR_BAD_ARG, "Pixel found with no samples");  // buffer.rs:89
     // Every pixel holds at least min(entries, 2) entries, so this is exact for any mix of calls: the first call of any
@@ -1760,6 +1932,7 @@ int rptb_buffer_reproject(rptb_buffer* dst, rptb_buffer* src, const rptb_reproje
         return fail(RPTB_ERR_BAD_ARG, "depth_tol must be finite and >= 0 (%g)", prm->depth_tol);
     if (!(prm->normal_cos >= -1.0 && prm->normal_cos <= 1.0)) return fail(RPTB_ERR_BAD_ARG, "normal_cos must lie in [-1, 1] (%g)", prm->normal_cos);
     if (prm->max_history < 2) return fail(RPTB_ERR_BAD_ARG, "max_history %u < 2 (a pixel's variance needs two entries)", prm->max_history);
+    if (dst->shard || src->shard) return refuse_shard("reproject");
     std::scoped_lock both(dst->lock, src->lock);
     bool same = dst->parts.size() == src->parts.size();
     for (size_t i = 0; same && i < dst->parts.size(); i++) same = dst->parts[i].device == src->parts[i].device;
@@ -1807,22 +1980,9 @@ int rptb_buffer_reproject(rptb_buffer* dst, rptb_buffer* src, const rptb_reproje
     const double* da = dst->aov;
     CU(launch_reproject(dv, sv, sp, da, da + 6 * dnpix, da + 7 * dnpix, *prm, dst->row_sums, dst->row_m2, dst->row_counts,
                         out_reused ? dst->reused : nullptr, d0.stream));
-    // back to every dst part's compact tiles: part 0 in place, the others through the gather scratch and a peer copy
-    const uint32_t nparts = (uint32_t)dst->parts.size();
-    for (uint32_t i = 0; i < nparts; i++) {
-        BufferPart& q = dst->parts[i];
-        if (!q.tiles) continue;
-        const size_t nelem = (size_t)q.tiles * 128u;
-        double* sums = i == 0 ? q.sums : dst->gather;
-        double* m2 = i == 0 ? q.m2 : dst->gather + nelem * 3;
-        uint32_t* counts = i == 0 ? q.counts : (uint32_t*)(dst->gather + nelem * 4);
-        CU(launch_buffer_compact(dst->row_sums, dst->row_m2, dst->row_counts, nelem, dst->width, dst->height, i, nparts, sums, m2, counts,
-                                 d0.stream));
-        if (i == 0) continue;
-        CU(cudaMemcpyPeerAsync(q.sums, q.device, sums, d0.device, nelem * 3 * sizeof(double), d0.stream));
-        CU(cudaMemcpyPeerAsync(q.m2, q.device, m2, d0.device, nelem * sizeof(double), d0.stream));
-        CU(cudaMemcpyPeerAsync(q.counts, q.device, counts, d0.device, nelem * sizeof(uint32_t), d0.stream));
-    }
+    // back to every dst part's compact tiles
+    rc = buffer_rows_to_parts(dst);
+    if (rc != RPTB_OK) return rc;
     // every later call on either buffer is ordered behind this one
     CU(cudaEventRecord(d0.done, d0.stream));
     CU(cudaEventRecord(s0.done, d0.stream));
@@ -1842,6 +2002,156 @@ int rptb_buffer_reproject(rptb_buffer* dst, rptb_buffer* src, const rptb_reproje
         CU(cudaStreamSynchronize(d0.stream));
         *out_reused = n;
     }
+    return RPTB_OK;
+}
+
+uint64_t rptb_buffer_shard_bytes(const rptb_buffer* b, uint32_t with_features) {
+    if (!b || !b->shard) return 0;
+    return shard_layout(b->width, b->height, b->parts[0].count, with_features != 0).bytes;
+}
+
+int rptb_buffer_export_shard(rptb_buffer* b, void* dst_device, uint32_t with_features, void* stream) {
+    if (!b || !dst_device) return fail(RPTB_ERR_BAD_ARG, "null argument");
+    if (!b->shard) return fail(RPTB_ERR_BAD_ARG, "not a shard buffer (rptb_buffer_create_shard)");
+    std::lock_guard<std::mutex> bl(b->lock);
+    if (with_features && b->feature_rays == 0) return fail(RPTB_ERR_BAD_ARG, "the buffer holds no features (rptb_buffer_add_features)");
+    BufferPart& q = b->parts[0];
+    DeviceGuard g(q.device);
+    if (!g.ok) return fail(RPTB_ERR_CUDA, "cudaSetDevice(%d) failed", q.device);
+    const ShardLayout l = shard_layout(b->width, b->height, q.count, with_features != 0);
+    ShardHeader h;
+    std::memset(&h, 0, sizeof(h));
+    h.magic = kShardMagic;
+    h.with_features = with_features ? 1u : 0u;
+    h.width = b->width;
+    h.height = b->height;
+    h.shard_index = q.index;
+    h.shard_count = q.count;
+    h.entries = b->entries;
+    h.feature_rays = b->feature_rays;
+    h.entry_cam = shard_camera(b->entry_cam);
+    h.feat_cam = shard_camera(b->feat_cam);
+    cudaStream_t st = stream ? (cudaStream_t)stream : q.stream;
+    char* out = (char*)dst_device;
+    const size_t nelem = (size_t)q.tiles * 128u, slot = l.slots * sizeof(double);
+    CU(cudaStreamWaitEvent(st, q.done, 0));
+    // pageable source: the call returns once the header is staged
+    CU(cudaMemcpyAsync(out, &h, sizeof(h), cudaMemcpyHostToDevice, st));
+    if (nelem) {
+        CU(cudaMemcpyAsync(out + l.sums, q.sums, nelem * 3 * sizeof(double), cudaMemcpyDeviceToDevice, st));
+        CU(cudaMemcpyAsync(out + l.m2, q.m2, nelem * sizeof(double), cudaMemcpyDeviceToDevice, st));
+        if (with_features) {  // the part's planes are nelem long, the block's l.slots
+            CU(cudaMemcpyAsync(out + l.feat, q.feat, nelem * 3 * sizeof(double), cudaMemcpyDeviceToDevice, st));
+            CU(cudaMemcpyAsync(out + l.feat + 3 * slot, q.feat + 3 * nelem, nelem * 3 * sizeof(double), cudaMemcpyDeviceToDevice, st));
+            CU(cudaMemcpyAsync(out + l.feat + 6 * slot, q.feat + 6 * nelem, nelem * sizeof(double), cudaMemcpyDeviceToDevice, st));
+            CU(cudaMemcpyAsync(out + l.feat + 7 * slot, q.feat + 7 * nelem, nelem * sizeof(double), cudaMemcpyDeviceToDevice, st));
+        }
+        CU(cudaMemcpyAsync(out + l.counts, q.counts, nelem * sizeof(uint32_t), cudaMemcpyDeviceToDevice, st));
+    }
+    // a later accumulate into the part waits until the block is read
+    CU(cudaEventRecord(q.done, st));
+    if (!stream) CU(cudaStreamSynchronize(st));
+    return RPTB_OK;
+}
+
+int rptb_buffer_import_shards(rptb_buffer* dst, const void* gathered_device, uint32_t shard_count, uint32_t with_features) {
+    if (!dst || !gathered_device) return fail(RPTB_ERR_BAD_ARG, "null argument");
+    if (shard_count == 0) return fail(RPTB_ERR_BAD_ARG, "shard_count 0");
+    if (dst->shard) return fail(RPTB_ERR_BAD_ARG, "dst is a shard buffer: the shards gather into a whole buffer (rptb_buffer_create)");
+    std::lock_guard<std::mutex> bl(dst->lock);
+    BufferPart& d0 = dst->parts[0];
+    DeviceGuard g(d0.device);
+    if (!g.ok) return fail(RPTB_ERR_CUDA, "cudaSetDevice(%d) failed", d0.device);
+    const uint32_t W = dst->width, H = dst->height;
+    const ShardLayout l = shard_layout(W, H, shard_count, with_features != 0);
+    const char* in = (const char*)gathered_device;
+    // header 0 first: only once it names dst's size, shard_count and with_features is the block stride known to be right
+    std::vector<ShardHeader> hs(shard_count);
+    CU(cudaMemcpyAsync(hs.data(), in, sizeof(ShardHeader), cudaMemcpyDeviceToHost, d0.stream));
+    CU(cudaStreamSynchronize(d0.stream));
+    const ShardHeader& h0 = hs[0];
+    if (h0.magic != kShardMagic) return fail(RPTB_ERR_BAD_ARG, "block 0 is not a shard block (rptb_buffer_export_shard)");
+    if (h0.width != W || h0.height != H)
+        return fail(RPTB_ERR_BAD_ARG, "the shards are %ux%u but dst is %ux%u", h0.width, h0.height, W, H);
+    if (h0.shard_count != shard_count) return fail(RPTB_ERR_BAD_ARG, "the shards are %u but shard_count is %u", h0.shard_count, shard_count);
+    if (h0.with_features != (with_features ? 1u : 0u))
+        return fail(RPTB_ERR_BAD_ARG, "the shards were exported %s features", h0.with_features ? "with" : "without");
+    if (shard_count > 1)
+        CU(cudaMemcpy2DAsync(hs.data() + 1, sizeof(ShardHeader), in + l.bytes, l.bytes, sizeof(ShardHeader), shard_count - 1,
+                             cudaMemcpyDeviceToHost, d0.stream));
+    CU(cudaStreamSynchronize(d0.stream));
+    for (uint32_t i = 0; i < shard_count; i++) {
+        const ShardHeader& h = hs[i];
+        if (h.magic != kShardMagic) return fail(RPTB_ERR_BAD_ARG, "block %u is not a shard block (rptb_buffer_export_shard)", i);
+        if (h.shard_index != i) return fail(RPTB_ERR_BAD_ARG, "block %u holds shard %u: the shards must be in order 0..%u", i, h.shard_index, shard_count - 1);
+        if (h.width != W || h.height != H || h.shard_count != shard_count || h.with_features != h0.with_features)
+            return fail(RPTB_ERR_BAD_ARG, "block %u was exported from another image, shard count or feature choice", i);
+        if (h.entries != h0.entries || h.feature_rays != h0.feature_rays ||
+            std::memcmp(&h.entry_cam, &h0.entry_cam, sizeof(ShardCamera)) != 0 ||
+            std::memcmp(&h.feat_cam, &h0.feat_cam, sizeof(ShardCamera)) != 0)
+            return fail(RPTB_ERR_BAD_ARG, "shard %u received other calls than shard 0 (entries %u / %u, feature rays %llu / %llu, or cameras)",
+                        i, h.entries, h0.entries, (unsigned long long)h.feature_rays, (unsigned long long)h0.feature_rays);
+    }
+    // everything dst holds is overwritten: its earlier work finishes first
+    for (BufferPart& q : dst->parts) CU(cudaStreamWaitEvent(d0.stream, q.done, 0));
+    if (with_features) {
+        for (BufferPart& q : dst->parts) {
+            const size_t nelem = (size_t)q.tiles * 128u;
+            if (q.feat || !nelem) continue;
+            DeviceGuard gq(q.device);
+            CU(cudaMalloc((void**)&q.feat, nelem * 8 * sizeof(double)));
+        }
+    } else {
+        for (BufferPart& q : dst->parts) {  // dst holds no features afterwards; the next feature pass starts from zero
+            if (!q.feat) continue;
+            DeviceGuard gq(q.device);
+            CU(cudaEventSynchronize(q.done));
+            CU(cudaFree(q.feat));
+            q.feat = nullptr;
+        }
+    }
+    int rc = buffer_rows_alloc(dst);
+    if (rc != RPTB_OK) return rc;
+    if (with_features) {
+        rc = buffer_feat_rows_alloc(dst);
+        if (rc != RPTB_OK) return rc;
+    }
+    // every block row-major on dst's first device, then back into dst's own parts
+    const size_t npix = (size_t)W * H, slot = l.slots * sizeof(double);
+    double* rn = dst->row_feat;
+    for (uint32_t i = 0; i < shard_count; i++) {
+        const char* blk = in + (size_t)i * l.bytes;
+        const uint64_t nelem = (uint64_t)buffer_tiles(W, H, i, shard_count) * 128u;
+        CU(launch_buffer_scatter((const double*)(blk + l.sums), (const double*)(blk + l.m2), (const uint32_t*)(blk + l.counts), nelem, W, H,
+                                 i, shard_count, dst->row_sums, dst->row_m2, dst->row_counts, d0.stream));
+        if (!with_features) continue;
+        const char* f = blk + l.feat;
+        CU(launch_buffer_scatter((const double*)f, (const double*)(f + 6 * slot), nullptr, nelem, W, H, i, shard_count, rn, rn + 6 * npix,
+                                 nullptr, d0.stream));
+        CU(launch_buffer_scatter((const double*)(f + 3 * slot), (const double*)(f + 7 * slot), nullptr, nelem, W, H, i, shard_count,
+                                 rn + 3 * npix, rn + 7 * npix, nullptr, d0.stream));
+    }
+    rc = buffer_rows_to_parts(dst);
+    if (rc != RPTB_OK) return rc;
+    if (with_features) {
+        rc = buffer_feat_rows_to_parts(dst);
+        if (rc != RPTB_OK) return rc;
+    }
+    // every later call on dst is ordered behind this one
+    CU(cudaEventRecord(d0.done, d0.stream));
+    for (size_t i = 1; i < dst->parts.size(); i++) {
+        BufferPart& q = dst->parts[i];
+        DeviceGuard gi(q.device);
+        CU(cudaStreamWaitEvent(q.stream, d0.done, 0));
+        CU(cudaEventRecord(q.done, q.stream));
+    }
+    // the caller may reuse the gathered bytes when the call returns
+    CU(cudaStreamSynchronize(d0.stream));
+    dst->entries = h0.entries;
+    dst->reprojected = false;
+    dst->entry_cam = camera_record(h0.entry_cam);
+    dst->feature_rays = with_features ? h0.feature_rays : 0;
+    dst->feat_cam = with_features ? camera_record(h0.feat_cam) : CameraRecord();
     return RPTB_OK;
 }
 

@@ -31,7 +31,8 @@ __global__ void __launch_bounds__(256) reproject_kernel(const ReprojectView dv, 
 }
 
 // The row-major planes of the whole image -> the compact tiles of replica `shard_index` of `shard_count` (the inverse of
-// film.cu's buffer_scatter_kernel).  Elements past a ragged edge are zeroed, as a fresh buffer holds them.
+// film.cu's buffer_scatter_kernel).  Elements past a ragged edge are zeroed, as a fresh buffer holds them.  Null counts
+// planes (the feature sums, which have none) are skipped.
 __global__ void buffer_compact_kernel(const double* __restrict__ row_sums, const double* __restrict__ row_m2,
                                       const uint32_t* __restrict__ row_counts, uint64_t nelem, uint32_t width, uint32_t height,
                                       uint32_t shard_index, uint32_t shard_count, double* __restrict__ sums, double* __restrict__ m2,
@@ -43,7 +44,7 @@ __global__ void buffer_compact_kernel(const double* __restrict__ row_sums, const
     sums[3 * e + 1] = p < 0 ? 0.0 : row_sums[3 * p + 1];
     sums[3 * e + 2] = p < 0 ? 0.0 : row_sums[3 * p + 2];
     m2[e] = p < 0 ? 0.0 : row_m2[p];
-    counts[e] = p < 0 ? 0u : row_counts[p];
+    if (counts) counts[e] = p < 0 ? 0u : row_counts[p];
 }
 
 // *out = min(*out, counts[0..npix)); the caller sets *out to UINT32_MAX first.

@@ -16,7 +16,11 @@ Two ways to assemble, same bits:
     buffer (rptb_render_params.compact_out, 1/N of the image), one all-gather, then a fixed permutation puts the
     pixels in row-major order.  1 x the image in flight, and nothing is summed at all -- what bench.py times.
 
-There is no other exchange step on this path, so no other collective.
+The device Buffer shards the same way (`ShardBuffer`, rptb_buffer_create_shard): every rank samples, adapts and adds
+features into its own tiles with no exchange, and `ShardBuffer.gather` -- one all-gather of the ranks' exchange blocks
+-- gives every rank an ordinary whole DeviceBuffer, the same bits for any world size.  `render_iterative_distributed`
+is Renderer.iterative_render over a ShardBuffer; with adaptive sampling it adds one collective per batch, an
+all-reduce of the ranks' active pixel counts that ends the loop.  Nothing else is exchanged.
 """
 from __future__ import annotations
 
@@ -26,6 +30,7 @@ from typing import Callable, Optional
 import numpy as np
 
 from . import _capi as capi
+from . import api
 
 TILE_W, TILE_H = 16, 8  # must match rpt_b200/csrc/integrator.cuh
 
@@ -150,3 +155,135 @@ def render_distributed_gather(renderer, iterations: int, first_sample: int = 0, 
         return buf
 
     return gather_tiles(shard, w, h, perm, group)
+
+
+# ---- the device Buffer, one shard per rank ---------------------------------------------------------------------------
+SHARD_HEADER_BYTES = 256  # must match rpt_b200/csrc/api.cu (kShardHeaderBytes)
+
+
+def shard_block_layout(width: int, height: int, shard_count: int, with_features: bool = False) -> dict:
+    """Byte offsets of the planes in one shard's exchange block (rptb_buffer_export_shard), the same for every shard:
+    a header, then sums (3 doubles a slot), M2 (1 double), with features the feature sums (8 doubles: normal 3, albedo
+    3, hits 1, depth 1), then counts (1 uint32).  Every plane has `slots` = shard 0's tiles * 128 slots, the padding
+    gather_tiles uses, so slot k * 128 + j of shard s's planes is pixel rptb_tile_pixel(width, height, s, shard_count,
+    k, j) and gather_permutation(width, height, shard_count) // slots / % slots finds a pixel's shard and slot."""
+    slots = shard_tiles(width, height, 0, shard_count) * TILE_W * TILE_H
+    sums = SHARD_HEADER_BYTES
+    m2 = sums + slots * 3 * 8
+    features = m2 + slots * 8
+    counts = features + (slots * 8 * 8 if with_features else 0)
+    return {"slots": slots, "sums": sums, "m2": m2, "features": features, "counts": counts, "bytes": counts + slots * 4}
+
+
+def _rank_world(group=None):
+    import torch.distributed as dist
+
+    if dist.is_available() and dist.is_initialized():
+        return dist.get_rank(group), dist.get_world_size(group)
+    return 0, 1
+
+
+class ShardBuffer(api.DeviceBuffer):
+    """A DeviceBuffer holding one rank's shard of the image (rptb_buffer_create_shard): the 16x8 tiles t with
+    t % world == rank, on the scene's one device.  Renderer.sample and Renderer.sample_features render and add only
+    those tiles, with no exchange; an adaptive sample() returns this rank's active pixel count.  Whole-image reads
+    (image, variance, sums, pixel_stats, counts, features, denoise, reproject_from, add_samples) are refused: gather()
+    first.  `entries` counts the calls (a bound on any pixel's count) until the gather reads the counts."""
+
+    def __init__(self, scene: "api.DeviceScene", width: int, height: int, filter: Optional["api.Filter"] = None, group=None,
+                 rank: Optional[int] = None, world: Optional[int] = None):
+        if rank is None or world is None:
+            rank, world = _rank_world(group)
+        self.width, self.height = int(width), int(height)
+        self.filter = filter or api.Filter()
+        self.devices = list(scene.devices)
+        self.entries = 0
+        self.feature_rays = 0
+        self.shard = (int(rank), int(world))
+        self.group = group
+        self._scene = scene  # the whole buffer of gather() is created on it
+        self.handle = C.c_void_p()
+        capi.check(capi.lib().rptb_buffer_create_shard(scene.handle, self.width, self.height, self.filter.radius, self.shard[0],
+                                                       self.shard[1], C.byref(self.handle)), "rptb_buffer_create_shard")
+
+    def block_bytes(self, with_features: bool = False) -> int:
+        """The size of this shard's exchange block (rptb_buffer_shard_bytes): the same on every rank."""
+        return int(capi.lib().rptb_buffer_shard_bytes(self.handle, 1 if with_features else 0))
+
+    def export(self, out, with_features: bool = False, stream: Optional[int] = None) -> None:
+        """Writes this shard's exchange block into `out`, a CUDA uint8 tensor of block_bytes() on the buffer's device, on
+        `stream` (a raw cudaStream_t; the current torch stream when None)."""
+        import torch
+
+        if stream is None:
+            stream = torch.cuda.current_stream(out.device).cuda_stream
+        capi.check(capi.lib().rptb_buffer_export_shard(self.handle, C.c_void_p(out.data_ptr()), 1 if with_features else 0,
+                                                       C.c_void_p(stream or 1)), "rptb_buffer_export_shard")
+
+    def gather(self, group=None, with_features: bool = False) -> "api.DeviceBuffer":
+        """All ranks call this: export every shard's block, one all_gather_into_tensor, and import the blocks into a new
+        whole DeviceBuffer on this rank's device -- the same bits on every rank, and those of one whole buffer given the
+        same calls.  NCCL gathers GPU to GPU; any other backend (gloo) through a host tensor.  `with_features` carries
+        the feature sums too (denoise and reproject need them), 100 instead of 36 bytes per pixel."""
+        import torch
+        import torch.distributed as dist
+
+        group = self.group if group is None else group
+        rank, world = self.shard
+        if world > 1 and _rank_world(group) != (rank, world):
+            raise ValueError(f"the shard is {rank} of {world} but the process group has rank/world {_rank_world(group)}")
+        nbytes = self.block_bytes(with_features)
+        dev = torch.device("cuda", self.devices[0])
+        with torch.cuda.device(dev):
+            stream = torch.cuda.current_stream(dev)
+            mine = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+            self.export(mine, with_features, stream.cuda_stream)
+            if world == 1:
+                gathered = mine
+            elif dist.get_backend(group) == "nccl":
+                gathered = torch.empty(nbytes * world, dtype=torch.uint8, device=dev)
+                dist.all_gather_into_tensor(gathered, mine, group=group)
+            else:
+                staged = torch.empty(nbytes * world, dtype=torch.uint8)
+                dist.all_gather_into_tensor(staged, mine.cpu(), group=group)
+                gathered = staged.to(dev)
+            stream.synchronize()  # the import reads the gathered bytes on the library's stream
+            whole = api.DeviceBuffer(self._scene, self.width, self.height, self.filter)
+            capi.check(capi.lib().rptb_buffer_import_shards(whole.handle, C.c_void_p(gathered.data_ptr()), world,
+                                                            1 if with_features else 0), "rptb_buffer_import_shards")
+        whole.entries = int(whole.counts().max())
+        whole.feature_rays = self.feature_rays if with_features else 0
+        return whole
+
+
+def render_iterative_distributed(renderer, callback_interval: int, callback: Callable[[int, ShardBuffer], None],
+                                 adaptive: Optional["api.Adaptive"] = None, group=None,
+                                 buffer: Optional[ShardBuffer] = None) -> ShardBuffer:
+    """All ranks call this: Renderer.iterative_render over this rank's ShardBuffer (`buffer`, e.g. one given features
+    first; None creates one for the renderer's size and filter).  Every batch renders and adds this rank's tiles only;
+    the callback receives the ShardBuffer and calls its gather() when it wants an image, so a batch exchanges nothing
+    unless asked.  With `adaptive`, the loop ends after a batch in which no rank rendered a pixel: one all-reduce(sum)
+    of the ranks' active counts per batch.  Returns the ShardBuffer."""
+    import torch
+    import torch.distributed as dist
+
+    if buffer is None:
+        buffer = ShardBuffer(renderer.device_scene(), renderer._width, renderer._height, renderer._filter, group=group)
+    on = dist.is_available() and dist.is_initialized() and buffer.shard[1] > 1
+    count_dev = "cpu"
+    if on and dist.get_backend(group) == "nccl":
+        count_dev = torch.device("cuda", buffer.devices[0])
+    iteration = 0
+    while iteration < renderer._num_samples:
+        steps = min(renderer._num_samples - iteration, callback_interval)
+        active = renderer.sample(steps, buffer, want_stats=False, adaptive=adaptive)
+        iteration += steps
+        if adaptive is not None:
+            if on:
+                total = torch.tensor([active], dtype=torch.int64, device=count_dev)
+                dist.all_reduce(total, op=dist.ReduceOp.SUM, group=group)
+                active = int(total.item())
+            if active == 0:
+                break
+        callback(iteration, buffer)
+    return buffer

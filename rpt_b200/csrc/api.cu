@@ -27,6 +27,7 @@
 #include "denoise.h"
 #include "flatten.h"
 #include "launch.h"
+#include "planes.h"
 #include "reproject.h"
 #include "tile.h"
 
@@ -39,9 +40,8 @@ cudaError_t launch_film_variance(const double* batches, uint32_t nbatches, uint6
 cudaError_t launch_buffer_accumulate(const float* in32, const double* in64, bool rowmajor, const uint8_t* mask, uint64_t nelem,
                                      uint32_t width, uint32_t height, uint32_t shard_index, uint32_t shard_count, double* sums,
                                      double* m2, uint32_t* counts, cudaStream_t stream);
-cudaError_t launch_buffer_scatter(const double* sums, const double* m2, const uint32_t* counts, uint64_t nelem, uint32_t width,
-                                  uint32_t height, uint32_t shard_index, uint32_t shard_count, double* row_sums, double* row_m2,
-                                  uint32_t* row_counts, cudaStream_t stream);
+cudaError_t launch_buffer_move(bool compact, const PlaneSet& src, const PlaneSet& dst, uint64_t nelem, uint32_t width, uint32_t height,
+                               uint32_t shard_index, uint32_t shard_count, cudaStream_t stream);
 uint32_t buffer_variance_blocks(uint64_t npixels);
 cudaError_t launch_buffer_variance_sum(const double* m2, const uint32_t* counts, uint64_t npixels, double* partial,
                                        double* out_sum, cudaStream_t stream);
@@ -54,18 +54,14 @@ cudaError_t launch_adaptive_select(const double* sums, const double* m2, const u
                                    uint8_t* mask, uint8_t* flags, uint32_t* ids, uint32_t* len, unsigned long long* active_pixels,
                                    void* temp, size_t temp_bytes, cudaStream_t stream);
 // the feature planes and the denoiser: denoise.cu
-cudaError_t launch_features_resolve(const double* row_feat, uint64_t npix, double rays, double* nrm, double* depth, double* albedo,
-                                    double* frac, cudaStream_t stream);
+cudaError_t launch_features_resolve(const FeaturePlanes& f, uint64_t npix, double rays, const Aov& out, cudaStream_t stream);
 cudaError_t launch_denoise(const double* sums, const double* m2, const uint32_t* counts, const double* nrm,
                            const double* depth, const double* albedo, uint32_t width, uint32_t height, const rptb_denoise& d,
                            double* const col[2], double* const var[2], double* out, cudaStream_t stream, uint32_t* launches);
-// the reprojection, the row-major -> compact copy back and the least count: reproject.cu
+// the reprojection and the least count: reproject.cu
 cudaError_t launch_reproject(const ReprojectView& dv, const ReprojectView& sv, const ReprojectSource& s, const double* dnrm,
                              const double* ddepth, const double* dfrac, const rptb_reproject& prm, double* sums, double* m2,
                              uint32_t* counts, unsigned long long* reused, cudaStream_t stream);
-cudaError_t launch_buffer_compact(const double* row_sums, const double* row_m2, const uint32_t* row_counts, uint64_t nelem,
-                                  uint32_t width, uint32_t height, uint32_t shard_index, uint32_t shard_count, double* sums,
-                                  double* m2, uint32_t* counts, cudaStream_t stream);
 cudaError_t launch_buffer_min_count(const uint32_t* counts, uint64_t npix, uint32_t* out, cudaStream_t stream);
 int parse_obj_text(const char* text, size_t len, std::vector<double>& tris, std::string& err);
 struct ObjGroup {
@@ -278,6 +274,9 @@ struct rptb_scene {
 };
 
 namespace {
+
+// Replica i of a scene: the handle itself, then its peers.
+rptb_scene* replica(rptb_scene* s, uint32_t i) { return i == 0 ? s : s->peers[i - 1]; }
 
 // rptb_scene_desc::accel: AUTO -> RPTB_ACCEL env (kdtree | bvh) -> the library default
 uint32_t resolve_accel(uint32_t accel) {
@@ -572,15 +571,34 @@ void destroy_replica(rptb_scene* s) {
 // (cudaMalloc, so destroy hands it back to the driver), its streams and its events, so it and its scene may be
 // destroyed in either order.  `done` is recorded behind every accumulate -- on the scene's stream (rptb_sample_into)
 // or on the part's own (rptb_buffer_add_samples) -- and every later operation on the part waits for it.
+
+// One copy of a buffer's per-pixel planes (planes.h), n elements a plane.  Each group is null until allocated: the
+// colour planes, one allocation each, and the feature sums, one allocation of FEATURE_SUMS doubles an element.
+struct Planes {
+    size_t n = 0;
+    double* sums = nullptr;
+    double* m2 = nullptr;
+    uint32_t* counts = nullptr;
+    double* feat = nullptr;
+    // the allocated planes of `mask`
+    PlaneSet set(uint32_t mask) const {
+        const FeaturePlanes f = feat ? feature_planes(feat, n) : FeaturePlanes{};
+        PlaneSet s = {{sums, m2, f.n, f.a, f.h, f.z, counts}};
+        for (int k = 0; k < NPLANES; k++)
+            if (!(mask >> k & 1u)) s.p[k] = nullptr;
+        return s;
+    }
+};
+
 struct BufferPart {
     int device = 0;
     // this part's place in the tile deal: it holds the tiles t with t % count == index.  Part i of a whole buffer of n
     // parts is (i, n); the one part of a shard buffer (rptb_buffer_create_shard) is the shard's own pair.
     uint32_t index = 0, count = 1;
     uint32_t tiles = 0;          // tiles t with t % count == index
-    double* sums = nullptr;      // tiles * 128 * 3
-    double* m2 = nullptr;        // tiles * 128
-    uint32_t* counts = nullptr;  // tiles * 128
+    // tiles * 128 elements: the colour planes from creation on, the feature sums from the buffer's first
+    // rptb_buffer_add_features on
+    Planes planes;
     double* upload = nullptr;    // a host entry, row-major width*height*3 (first add_samples allocates it)
     cudaStream_t stream = nullptr;
     cudaEvent_t done = nullptr;
@@ -594,8 +612,7 @@ struct BufferPart {
     unsigned long long* active = nullptr;
     void* temp = nullptr;
     size_t temp_bytes = 0;
-    // from the buffer's first rptb_buffer_add_features on: the first-hit feature sums, tiles*128*8 (features.cuh planes)
-    double* feat = nullptr;
+    std::vector<void*> mem;      // everything above that cudaMalloc gave, on the part's device
 };
 
 // The camera one side of a buffer (its entries or its features) was made with, for rptb_buffer_reproject: none yet, one
@@ -626,22 +643,19 @@ struct rptb_buffer {
     bool shard = false;
     CameraRecord entry_cam, feat_cam;
     std::vector<BufferPart> parts;
-    // on parts[0]'s device, allocated by the first image / variance / sums: the image gathered row-major
-    double* row_sums = nullptr;  // width*height*3
-    double* row_m2 = nullptr;        // width*height
-    uint32_t* row_counts = nullptr;  // width*height
-    double* gather = nullptr;        // one other part's sums + M2 + counts, copied over
-    double* partial = nullptr;       // variance block partials, then the total
+    // on parts[0]'s device, each group allocated by its first gather: the image's planes row-major (width*height
+    // elements), and the staging another part's planes are copied into (as many elements as the largest such part)
+    Planes rows, staging;
+    // with the colour rows: the variance block partials, then the total; the image
+    double* partial = nullptr;
     uint8_t* rgb8 = nullptr;
-    // features and denoiser, on parts[0]'s device, allocated by their first call
     uint64_t feature_rays = 0;       // camera rays per pixel in the feature sums
-    double* row_feat = nullptr;      // width*height*8: the sums gathered row-major (features.cuh planes)
-    double* gather_feat = nullptr;   // one other part's feature sums
-    double* aov = nullptr;           // width*height*8: normal (3), albedo (3), depth, hit fraction planes
-    double* dn = nullptr;            // width*height*11: colour (3) and variance ping-pong planes, then c' (3)
-    // on parts[0]'s device, allocated by the first reprojection into the buffer: the reused-pixel counter and the least count
+    double* aov = nullptr;           // with the feature rows, width*height*8: the resolved features (buffer_aov)
+    double* dn = nullptr;            // the denoiser's, width*height*11: colour (3) and variance ping-pong planes, then c' (3)
+    // allocated by the first reprojection into the buffer: the reused-pixel counter and the least count
     unsigned long long* reused = nullptr;
     uint32_t* min_count = nullptr;
+    std::vector<void*> mem;          // everything above that cudaMalloc gave, on parts[0]'s device
     std::mutex lock;
 };
 
@@ -652,159 +666,151 @@ uint32_t buffer_tiles(uint32_t width, uint32_t height, uint32_t index, uint32_t 
     return ntiles > index ? (ntiles - index + nparts - 1u) / nparts : 0u;
 }
 
+size_t plane_bytes(int k, size_t n) { return n * plane_shape(k).values * plane_shape(k).bytes; }
+
+// cudaMalloc on the current device, recorded in `mem` for buffer_free.
+template <class T>
+cudaError_t own(std::vector<void*>& mem, T** p, size_t bytes) {
+    const cudaError_t e = cudaMalloc((void**)p, bytes);
+    if (e == cudaSuccess) mem.push_back(*p);
+    return e;
+}
+
 void buffer_free(rptb_buffer* b) {
     for (size_t i = 0; i < b->parts.size(); i++) {
         BufferPart& q = b->parts[i];
         DeviceGuard g(q.device);
         if (q.done) cudaEventSynchronize(q.done);  // an accumulate may still run on the scene's stream
         if (q.stream) cudaStreamSynchronize(q.stream);
-        cudaFree(q.sums);
-        cudaFree(q.m2);
-        cudaFree(q.upload);
-        cudaFree(q.counts);
-        cudaFree(q.mask);
-        cudaFree(q.flags);
-        cudaFree(q.ids);
-        cudaFree(q.len);
-        cudaFree(q.active);
-        cudaFree(q.temp);
-        cudaFree(q.feat);
-        if (i == 0) {
-            cudaFree(b->row_sums);
-            cudaFree(b->row_m2);
-            cudaFree(b->gather);
-            cudaFree(b->partial);
-            cudaFree(b->rgb8);
-            cudaFree(b->row_counts);
-            cudaFree(b->row_feat);
-            cudaFree(b->gather_feat);
-            cudaFree(b->aov);
-            cudaFree(b->dn);
-            cudaFree(b->reused);
-            cudaFree(b->min_count);
-        }
+        for (void* p : q.mem) cudaFree(p);
+        if (i == 0)
+            for (void* p : b->mem) cudaFree(p);
         if (q.done) cudaEventDestroy(q.done);
         if (q.stream) cudaStreamDestroy(q.stream);
     }
     delete b;
 }
 
+// Allocates the groups of `mask` that `s` does not hold yet, n elements a plane, on the current device.
+int planes_alloc(std::vector<void*>& mem, Planes& s, size_t n, uint32_t mask) {
+    s.n = n;
+    if ((mask & COLOUR) && !s.sums) {
+        CU(own(mem, &s.sums, plane_bytes(SUMS, n)));
+        CU(own(mem, &s.m2, plane_bytes(M2, n)));
+        CU(own(mem, &s.counts, plane_bytes(COUNTS, n)));
+    }
+    if ((mask & FEATURES) && !s.feat) CU(own(mem, &s.feat, n * FEATURE_SUMS * sizeof(double)));
+    return RPTB_OK;
+}
+
 int buffer_part_alloc(BufferPart& q) {
     CU(cudaStreamCreateWithFlags(&q.stream, cudaStreamNonBlocking));
     CU(cudaEventCreateWithFlags(&q.done, cudaEventDisableTiming));
     if (q.tiles) {
-        const size_t nelem = (size_t)q.tiles * 128u;
-        CU(cudaMalloc((void**)&q.sums, nelem * 3 * sizeof(double)));
-        CU(cudaMalloc((void**)&q.m2, nelem * sizeof(double)));
-        CU(cudaMalloc((void**)&q.counts, nelem * sizeof(uint32_t)));
-        CU(cudaMemsetAsync(q.sums, 0, nelem * 3 * sizeof(double), q.stream));  // sums() of an empty buffer reads zero
-        CU(cudaMemsetAsync(q.m2, 0, nelem * sizeof(double), q.stream));
-        CU(cudaMemsetAsync(q.counts, 0, nelem * sizeof(uint32_t), q.stream));
+        const int rc = planes_alloc(q.mem, q.planes, (size_t)q.tiles * 128u, COLOUR);
+        if (rc != RPTB_OK) return rc;
+        const PlaneSet s = q.planes.set(COLOUR);  // sums() of an empty buffer reads zero
+        for (int k = 0; k < NPLANES; k++)
+            if (s.p[k]) CU(cudaMemsetAsync(s.p[k], 0, plane_bytes(k, q.planes.n), q.stream));
     }
     CU(cudaEventRecord(q.done, q.stream));
     return RPTB_OK;
 }
 
-// The row-major planes on parts[0]'s device (its device current), allocated on first use.
-int buffer_rows_alloc(rptb_buffer* b) {
-    if (b->row_sums) return RPTB_OK;
-    const uint32_t nparts = (uint32_t)b->parts.size();
+// The row-major planes of `mask` on parts[0]'s device (its device current), each group allocated on first use together
+// with its staging (when the buffer has other parts) and its other scratch.
+int buffer_rows_alloc(rptb_buffer* b, uint32_t mask) {
     const size_t npix = (size_t)b->width * b->height;
-    uint32_t most = 0;
-    for (uint32_t i = 1; i < nparts; i++) most = std::max(most, b->parts[i].tiles);
-    CU(cudaMalloc((void**)&b->row_sums, npix * 3 * sizeof(double)));
-    CU(cudaMalloc((void**)&b->row_m2, npix * sizeof(double)));
-    CU(cudaMalloc((void**)&b->row_counts, npix * sizeof(uint32_t)));
-    if (most) CU(cudaMalloc((void**)&b->gather, (size_t)most * 128u * (4u * sizeof(double) + sizeof(uint32_t))));
-    CU(cudaMalloc((void**)&b->partial, (buffer_variance_blocks(npix) + 1) * sizeof(double)));
-    CU(cudaMalloc((void**)&b->rgb8, npix * 3));
+    size_t most = 0;
+    for (size_t i = 1; i < b->parts.size(); i++) most = std::max(most, (size_t)b->parts[i].tiles * 128u);
+    if ((mask & COLOUR) && !b->rows.sums) {
+        CU(own(b->mem, &b->partial, (buffer_variance_blocks(npix) + 1) * sizeof(double)));
+        CU(own(b->mem, &b->rgb8, npix * 3));
+    }
+    if ((mask & FEATURES) && !b->rows.feat) CU(own(b->mem, &b->aov, npix * FEATURE_SUMS * sizeof(double)));
+    const int rc = planes_alloc(b->mem, b->rows, npix, mask);
+    if (rc != RPTB_OK || !most) return rc;
+    return planes_alloc(b->mem, b->staging, most, mask);
+}
+
+// b->aov's planes
+Aov buffer_aov(const rptb_buffer* b) {
+    const size_t npix = (size_t)b->width * b->height;
+    return {b->aov, b->aov + 3 * npix, b->aov + 6 * npix, b->aov + 7 * npix};
+}
+
+// Copies n elements of every plane present in both sets from device `from` to device `to`, on `stream`: between a part
+// on another device and the staging on parts[0]'s.  cudaMemcpyPeerAsync needs no peer access.
+int copy_planes(const PlaneSet& dst, int to, const PlaneSet& src, int from, size_t n, cudaStream_t stream) {
+    for (int k = 0; k < NPLANES; k++)
+        if (dst.p[k] && src.p[k]) CU(cudaMemcpyPeerAsync(dst.p[k], to, src.p[k], from, plane_bytes(k, n), stream));
     return RPTB_OK;
 }
 
-// Brings every part's sums, M2 and/or counts to parts[0]'s device in row-major order, on parts[0]'s stream (the caller
-// has made that device current).  Other parts are copied with cudaMemcpyPeerAsync, which needs no peer access.
-int buffer_gather(rptb_buffer* b, bool want_sums, bool want_m2, bool want_counts) {
-    BufferPart& q0 = b->parts[0];
-    const uint32_t nparts = (uint32_t)b->parts.size();
-    {
-        const int rc = buffer_rows_alloc(b);
-        if (rc != RPTB_OK) return rc;
-    }
-    double* rs = want_sums ? b->row_sums : nullptr;
-    double* rm = want_m2 ? b->row_m2 : nullptr;
-    uint32_t* rc = want_counts ? b->row_counts : nullptr;
-    CU(cudaStreamWaitEvent(q0.stream, q0.done, 0));
-    CU(launch_buffer_scatter(q0.sums, q0.m2, q0.counts, (uint64_t)q0.tiles * 128u, b->width, b->height, 0, nparts, rs, rm, rc,
-                             q0.stream));
-    for (uint32_t i = 1; i < nparts; i++) {
+// Scatters the compact planes `src` of shard `index` of `count` (one part of b, or one block of
+// rptb_buffer_import_shards) into b's row-major planes of `mask`, on parts[0]'s stream.
+int buffer_scatter(rptb_buffer* b, const PlaneSet& src, uint32_t mask, uint32_t index, uint32_t count) {
+    const uint64_t nelem = (uint64_t)buffer_tiles(b->width, b->height, index, count) * 128u;
+    CU(launch_buffer_move(false, src, b->rows.set(mask), nelem, b->width, b->height, index, count, b->parts[0].stream));
+    return RPTB_OK;
+}
+
+// Brings the planes of `mask` from every part to parts[0]'s device in row-major order, on parts[0]'s stream (the caller
+// has made that device current): part 0 straight from its own planes, the others through the staging.
+int buffer_gather(rptb_buffer* b, uint32_t mask) {
+    const BufferPart& q0 = b->parts[0];
+    int rc = buffer_rows_alloc(b, mask);
+    for (size_t i = 0; rc == RPTB_OK && i < b->parts.size(); i++) {
         const BufferPart& q = b->parts[i];
         if (!q.tiles) continue;
-        const size_t nelem = (size_t)q.tiles * 128u;
-        uint32_t* counts = (uint32_t*)(b->gather + nelem * 4);
         CU(cudaStreamWaitEvent(q0.stream, q.done, 0));
-        if (want_sums) CU(cudaMemcpyPeerAsync(b->gather, q0.device, q.sums, q.device, nelem * 3 * sizeof(double), q0.stream));
-        if (want_m2) CU(cudaMemcpyPeerAsync(b->gather + nelem * 3, q0.device, q.m2, q.device, nelem * sizeof(double), q0.stream));
-        if (want_counts) CU(cudaMemcpyPeerAsync(counts, q0.device, q.counts, q.device, nelem * sizeof(uint32_t), q0.stream));
-        CU(launch_buffer_scatter(b->gather, b->gather + nelem * 3, counts, nelem, b->width, b->height, i, nparts, rs, rm, rc,
-                                 q0.stream));
+        const PlaneSet src = i == 0 ? q.planes.set(mask) : b->staging.set(mask);
+        if (i > 0) rc = copy_planes(src, q0.device, q.planes.set(mask), q.device, q.planes.n, q0.stream);
+        if (rc == RPTB_OK) rc = buffer_scatter(b, src, mask, q.index, q.count);
     }
-    return RPTB_OK;
+    return rc;
 }
 
-// The row-major feature planes on parts[0]'s device (its device current), allocated on first use.
-int buffer_feat_rows_alloc(rptb_buffer* b) {
-    if (b->row_feat) return RPTB_OK;
-    const uint32_t nparts = (uint32_t)b->parts.size();
-    const size_t npix = (size_t)b->width * b->height;
-    uint32_t most = 0;
-    for (uint32_t i = 1; i < nparts; i++) most = std::max(most, b->parts[i].tiles);
-    CU(cudaMalloc((void**)&b->row_feat, npix * 8 * sizeof(double)));
-    CU(cudaMalloc((void**)&b->aov, npix * 8 * sizeof(double)));
-    if (most) CU(cudaMalloc((void**)&b->gather_feat, (size_t)most * 128u * 8u * sizeof(double)));
-    return RPTB_OK;
-}
-
-// Brings every part's feature sums to parts[0] row-major (b->row_feat) and resolves the feature planes into b->aov, on
-// parts[0]'s stream (its device current).  The normal / albedo planes go through the Buffer's scatter as "sums", the hit
-// and depth planes as "M2".
-int buffer_features(rptb_buffer* b) {
-    BufferPart& q0 = b->parts[0];
-    const uint32_t nparts = (uint32_t)b->parts.size();
-    const size_t npix = (size_t)b->width * b->height;
-    {
-        const int rc = buffer_feat_rows_alloc(b);
-        if (rc != RPTB_OK) return rc;
-    }
-    double* rn = b->row_feat;
-    double* ra = rn + 3 * npix;
-    double* rh = rn + 6 * npix;
-    double* rz = rn + 7 * npix;
-    for (uint32_t i = 0; i < nparts; i++) {
+// The mirror of buffer_gather: writes the row-major planes of `mask` back into every part's compact tiles, on parts[0]'s
+// stream (its device current).  Every part must hold those planes.
+int buffer_write_back(rptb_buffer* b, uint32_t mask) {
+    const BufferPart& q0 = b->parts[0];
+    int rc = RPTB_OK;
+    for (size_t i = 0; rc == RPTB_OK && i < b->parts.size(); i++) {
         const BufferPart& q = b->parts[i];
         if (!q.tiles) continue;
-        const size_t nelem = (size_t)q.tiles * 128u;
-        CU(cudaStreamWaitEvent(q0.stream, q.done, 0));
-        const double* src = q.feat;
-        if (i > 0) {
-            CU(cudaMemcpyPeerAsync(b->gather_feat, q0.device, q.feat, q.device, nelem * 8 * sizeof(double), q0.stream));
-            src = b->gather_feat;
-        }
-        CU(launch_buffer_scatter(src, src + 6 * nelem, nullptr, nelem, b->width, b->height, i, nparts, rn, rh, nullptr, q0.stream));
-        CU(launch_buffer_scatter(src + 3 * nelem, src + 7 * nelem, nullptr, nelem, b->width, b->height, i, nparts, ra, rz, nullptr,
-                                 q0.stream));
+        const PlaneSet dst = i == 0 ? q.planes.set(mask) : b->staging.set(mask);
+        CU(launch_buffer_move(true, b->rows.set(mask), dst, q.planes.n, b->width, b->height, q.index, q.count, q0.stream));
+        if (i > 0) rc = copy_planes(q.planes.set(mask), q.device, dst, q0.device, q.planes.n, q0.stream);
     }
-    double* a = b->aov;
-    CU(launch_features_resolve(b->row_feat, npix, (double)b->feature_rays, a, a + 6 * npix, a + 3 * npix, a + 7 * npix, q0.stream));
-    return RPTB_OK;
+    return rc;
 }
 
-// The least per-pixel count of a reprojected buffer, from the row-major counts buffer_gather left (parts[0]'s device
-// current).  Waits for it.
-int buffer_min_count(rptb_buffer* b, uint32_t* out) {
+// The least entry count of any pixel, once buffer_gather has brought the counts (parts[0]'s device current).  A buffer
+// that was never reprojected holds at least min(entries, 2) in every pixel (see rptb_buffer_denoise): that, without
+// device work.  A reprojected one: the minimum of its counts, waited for.
+int buffer_least_count(rptb_buffer* b, uint32_t* least) {
+    if (!b->reprojected) {
+        *least = std::min(b->entries, 2u);
+        return RPTB_OK;
+    }
     BufferPart& q0 = b->parts[0];
-    CU(launch_buffer_min_count(b->row_counts, (uint64_t)b->width * b->height, b->min_count, q0.stream));
-    CU(cudaMemcpyAsync(out, b->min_count, sizeof(uint32_t), cudaMemcpyDeviceToHost, q0.stream));
+    CU(launch_buffer_min_count(b->rows.counts, (uint64_t)b->width * b->height, b->min_count, q0.stream));
+    CU(cudaMemcpyAsync(least, b->min_count, sizeof(uint32_t), cudaMemcpyDeviceToHost, q0.stream));
     CU(cudaStreamSynchronize(q0.stream));
+    return RPTB_OK;
+}
+
+// Orders every later call on b behind the work enqueued so far on `stream`, which is on parts[0]'s device (current).
+int buffer_order_behind(rptb_buffer* b, cudaStream_t stream) {
+    BufferPart& q0 = b->parts[0];
+    CU(cudaEventRecord(q0.done, stream));
+    for (size_t i = 1; i < b->parts.size(); i++) {
+        BufferPart& q = b->parts[i];
+        DeviceGuard g(q.device);
+        CU(cudaStreamWaitEvent(q.stream, q0.done, 0));
+        CU(cudaEventRecord(q.done, q.stream));
+    }
     return RPTB_OK;
 }
 
@@ -812,14 +818,14 @@ int buffer_min_count(rptb_buffer* b, uint32_t* out) {
 int buffer_part_select_alloc(BufferPart& q) {
     if (q.len) return RPTB_OK;
     const size_t nelem = (size_t)q.tiles * 128u, nblocks = (size_t)q.tiles * 4u;
-    CU(cudaMalloc((void**)&q.len, sizeof(uint32_t)));
-    CU(cudaMalloc((void**)&q.active, sizeof(unsigned long long)));
+    CU(own(q.mem, &q.len, sizeof(uint32_t)));
+    CU(own(q.mem, &q.active, sizeof(unsigned long long)));
     if (q.tiles) {
-        CU(cudaMalloc((void**)&q.mask, nelem));
-        CU(cudaMalloc((void**)&q.flags, nblocks));
-        CU(cudaMalloc((void**)&q.ids, nblocks * sizeof(uint32_t)));
+        CU(own(q.mem, &q.mask, nelem));
+        CU(own(q.mem, &q.flags, nblocks));
+        CU(own(q.mem, &q.ids, nblocks * sizeof(uint32_t)));
         q.temp_bytes = adaptive_temp_bytes(q.tiles);
-        CU(cudaMalloc(&q.temp, q.temp_bytes ? q.temp_bytes : 1));
+        CU(own(q.mem, &q.temp, q.temp_bytes ? q.temp_bytes : 1));
     }
     return RPTB_OK;
 }
@@ -875,7 +881,7 @@ int sample_part(rptb_scene* r, const rptb_camera* cam, const rptb_render_params*
     }
     if (want_stats) CU(cudaEventRecord(r->ev0, r->stream));
     if (crit) {
-        CU(launch_adaptive_select(q.sums, q.m2, q.counts, q.tiles, p->width, p->height, index, nparts, *crit, q.mask, q.flags, q.ids,
+        CU(launch_adaptive_select(q.planes.sums, q.planes.m2, q.planes.counts, q.tiles, p->width, p->height, index, nparts, *crit, q.mask, q.flags, q.ids,
                                   q.len, q.active, q.temp, q.temp_bytes, r->stream));
         const RenderList list = {q.ids, q.len, q.mask};
         rc = render_list_launch(r, cam, &qp, list, r->stream, want_stats, launches);
@@ -887,7 +893,7 @@ int sample_part(rptb_scene* r, const rptb_camera* cam, const rptb_render_params*
     if (want_stats && !crit) CU(cudaEventRecord(r->ev1, r->stream));
     const bool f32 = p->precision == RPTB_PRECISION_F32;
     CU(launch_buffer_accumulate(f32 ? r->out32 : nullptr, f32 ? nullptr : r->out64, false, crit ? q.mask : nullptr, nelem, p->width,
-                                p->height, index, nparts, q.sums, q.m2, q.counts, r->stream));
+                                p->height, index, nparts, q.planes.sums, q.planes.m2, q.planes.counts, r->stream));
     // (an adaptive call times the whole entry: select, render and accumulate; a plain one its render)
     if (want_stats && crit) CU(cudaEventRecord(r->ev1, r->stream));
     (*launches)++;
@@ -898,55 +904,10 @@ int sample_part(rptb_scene* r, const rptb_camera* cam, const rptb_render_params*
     return RPTB_OK;
 }
 
-// Writes the row-major sums / M2 / counts on parts[0]'s device (its device current) back into every part's compact tiles,
-// on parts[0]'s stream: part 0 in place, the others through the gather scratch and a peer copy.
-int buffer_rows_to_parts(rptb_buffer* b) {
-    const BufferPart& q0 = b->parts[0];
-    for (size_t i = 0; i < b->parts.size(); i++) {
-        BufferPart& q = b->parts[i];
-        if (!q.tiles) continue;
-        const size_t nelem = (size_t)q.tiles * 128u;
-        double* sums = i == 0 ? q.sums : b->gather;
-        double* m2 = i == 0 ? q.m2 : b->gather + nelem * 3;
-        uint32_t* counts = i == 0 ? q.counts : (uint32_t*)(b->gather + nelem * 4);
-        CU(launch_buffer_compact(b->row_sums, b->row_m2, b->row_counts, nelem, b->width, b->height, q.index, q.count, sums, m2, counts,
-                                 q0.stream));
-        if (i == 0) continue;
-        CU(cudaMemcpyPeerAsync(q.sums, q.device, sums, q0.device, nelem * 3 * sizeof(double), q0.stream));
-        CU(cudaMemcpyPeerAsync(q.m2, q.device, m2, q0.device, nelem * sizeof(double), q0.stream));
-        CU(cudaMemcpyPeerAsync(q.counts, q.device, counts, q0.device, nelem * sizeof(uint32_t), q0.stream));
-    }
-    return RPTB_OK;
-}
-
-// The same for the row-major feature sums (b->row_feat): the normal / albedo planes go through the compact kernel as
-// "sums", the hit and depth planes as "M2", with no counts -- the routes buffer_features takes them the other way.  Every
-// part must hold feature memory.
-int buffer_feat_rows_to_parts(rptb_buffer* b) {
-    const BufferPart& q0 = b->parts[0];
-    const size_t npix = (size_t)b->width * b->height;
-    const double* rn = b->row_feat;
-    const double* ra = rn + 3 * npix;
-    const double* rh = rn + 6 * npix;
-    const double* rz = rn + 7 * npix;
-    for (size_t i = 0; i < b->parts.size(); i++) {
-        BufferPart& q = b->parts[i];
-        if (!q.tiles) continue;
-        const size_t nelem = (size_t)q.tiles * 128u;
-        double* f = i == 0 ? q.feat : b->gather_feat;
-        CU(launch_buffer_compact(rn, rh, nullptr, nelem, b->width, b->height, q.index, q.count, f, f + 6 * nelem, nullptr, q0.stream));
-        CU(launch_buffer_compact(ra, rz, nullptr, nelem, b->width, b->height, q.index, q.count, f + 3 * nelem, f + 7 * nelem, nullptr,
-                                 q0.stream));
-        if (i > 0) CU(cudaMemcpyPeerAsync(q.feat, q.device, f, q0.device, nelem * 8 * sizeof(double), q0.stream));
-    }
-    return RPTB_OK;
-}
-
 // ---- the exchange block of a shard buffer (rptb_buffer_export_shard / rptb_buffer_import_shards) ----
-// A header of kShardHeaderBytes, then the shard's compact planes, each padded to shard 0's slots (the most any shard
-// holds, as distributed.gather_tiles pads): sums (3 doubles a slot), M2 (1 double), with features their 8 planes
-// (normal 3, albedo 3, hits 1, depth 1: 8 doubles a slot), then counts (1 uint32).  Slots past the shard's own are not
-// written.
+// A header of kShardHeaderBytes, then the shard's compact planes in Plane order (planes.h), the feature planes only
+// with features, each padded to shard 0's slots (the most any shard holds, as distributed.gather_tiles pads).  Slots past
+// the shard's own are not written.
 constexpr uint32_t kShardMagic = 0x44524853u;  // "SHRD"
 constexpr size_t kShardHeaderBytes = 256;
 struct ShardCamera {
@@ -961,18 +922,30 @@ struct ShardHeader {
 static_assert(sizeof(ShardHeader) <= kShardHeaderBytes, "the shard header outgrew its slot");
 
 struct ShardLayout {
-    size_t slots;                          // pixel slots of every plane: shard 0's tiles * 128
-    size_t sums, m2, feat, counts, bytes;  // byte offsets in the block, and its size
+    size_t slots;         // pixel slots of every plane: shard 0's tiles * 128
+    uint32_t mask;        // the planes in the block
+    size_t at[NPLANES];   // their byte offsets in the block
+    size_t bytes;         // the block's size
 };
 ShardLayout shard_layout(uint32_t width, uint32_t height, uint32_t count, bool with_features) {
-    ShardLayout l;
+    ShardLayout l = {};
     l.slots = (size_t)buffer_tiles(width, height, 0, count) * 128u;
-    l.sums = kShardHeaderBytes;
-    l.m2 = l.sums + l.slots * 3 * sizeof(double);
-    l.feat = l.m2 + l.slots * sizeof(double);
-    l.counts = l.feat + (with_features ? l.slots * 8 * sizeof(double) : 0);
-    l.bytes = l.counts + l.slots * sizeof(uint32_t);
+    l.mask = COLOUR | (with_features ? FEATURES : 0u);
+    l.bytes = kShardHeaderBytes;
+    for (int k = 0; k < NPLANES; k++)
+        if (l.mask >> k & 1u) {
+            l.at[k] = l.bytes;
+            l.bytes += plane_bytes(k, l.slots);
+        }
     return l;
+}
+
+// The planes of the block at `block`.
+PlaneSet shard_planes(const ShardLayout& l, const void* block) {
+    PlaneSet s = {};
+    for (int k = 0; k < NPLANES; k++)
+        if (l.mask >> k & 1u) s.p[k] = (char*)block + l.at[k];
+    return s;
 }
 
 ShardCamera shard_camera(const CameraRecord& r) {
@@ -998,19 +971,25 @@ int refuse_shard(const char* what) {
                 what);
 }
 
-// The shard a render into buffer b may name: a whole buffer takes shard_count 0 or 1 only, a shard buffer exactly its own
-// (shard_index, shard_count).
-int check_buffer_shard(const rptb_render_params* p, const rptb_buffer* b) {
+// What a render into b checks: its parameters; the shard it names, which for a whole buffer is shard_count 0 or 1 only
+// and for a shard buffer exactly its own (shard_index, shard_count); its size; and the scene's device list.
+int check_render_into(rptb_scene* s, const rptb_camera* cam, const rptb_render_params* p, const rptb_buffer* b) {
+    if (!b) return fail(RPTB_ERR_BAD_ARG, "null argument");
+    const int rc = check_params(s, cam, p);
+    if (rc != RPTB_OK) return rc;
     const uint32_t sc = p->shard_count ? p->shard_count : 1u;
-    if (!b->shard) {
-        if (sc > 1)
-            return fail(RPTB_ERR_UNSUPPORTED, "shard_count %u: a buffer holds the whole image (shard with rptb_buffer_create_shard)", sc);
-        return RPTB_OK;
-    }
     const BufferPart& q = b->parts[0];
-    if (p->shard_index != q.index || sc != q.count)
+    if (!b->shard && sc > 1)
+        return fail(RPTB_ERR_UNSUPPORTED, "shard_count %u: a buffer holds the whole image (shard with rptb_buffer_create_shard)", sc);
+    if (b->shard && (p->shard_index != q.index || sc != q.count))
         return fail(RPTB_ERR_BAD_ARG, "the render is shard %u of %u but the buffer holds shard %u of %u", p->shard_index, sc, q.index,
                     q.count);
+    if (p->width != b->width || p->height != b->height)
+        return fail(RPTB_ERR_BAD_ARG, "render is %ux%u but the buffer is %ux%u", p->width, p->height, b->width, b->height);
+    const uint32_t nparts = 1u + (uint32_t)s->peers.size();
+    bool same = nparts == b->parts.size();
+    for (uint32_t i = 0; same && i < nparts; i++) same = replica(s, i)->device == b->parts[i].device;
+    if (!same) return fail(RPTB_ERR_BAD_ARG, "the buffer was created on a scene with another device list");
     return RPTB_OK;
 }
 
@@ -1192,14 +1171,13 @@ int rptb_render_samples(rptb_scene* s, const rptb_camera* cam, const rptb_render
             rptb_render_params q = *p;
             q.shard_count = outer * nrep;
             q.shard_index = p->shard_index * nrep + i;
-            rptb_scene* rep = i == 0 ? s : s->peers[i - 1];
-            rcs[i] = render_shard_to_host(rep, cam, &q, out_rgb, &sts[i]);
+            rcs[i] = render_shard_to_host(replica(s, i), cam, &q, out_rgb, &sts[i]);
             if (rcs[i] != RPTB_OK) errs[i] = g_error;  // g_error is thread-local
         });
     }
     for (std::thread& t : workers) t.join();
     for (uint32_t i = 0; i < nrep; i++)
-        if (rcs[i] != RPTB_OK) return fail(rcs[i], "device %d: %s", i == 0 ? s->device : s->peers[i - 1]->device, errs[i].c_str());
+        if (rcs[i] != RPTB_OK) return fail(rcs[i], "device %d: %s", replica(s, i)->device, errs[i].c_str());
     if (stats) {
         std::memset(stats, 0, sizeof(*stats));
         for (uint32_t i = 0; i < nrep; i++) {
@@ -1554,7 +1532,7 @@ static int buffer_create_impl(rptb_scene* s, uint32_t width, uint32_t height, ui
     int rc = RPTB_OK;
     for (uint32_t i = 0; rc == RPTB_OK && i < nparts; i++) {
         BufferPart& q = b->parts[i];
-        q.device = i == 0 ? s->device : s->peers[i - 1]->device;
+        q.device = replica(s, i)->device;
         q.index = b->shard ? shard_index : i;
         q.count = b->shard ? shard_count : nparts;
         q.tiles = buffer_tiles(width, height, q.index, q.count);
@@ -1597,26 +1575,18 @@ void rptb_buffer_destroy(rptb_buffer* b) {
 
 static int sample_into_impl(rptb_scene* s, const rptb_camera* cam, const rptb_render_params* p, const rptb_adaptive* crit,
                             rptb_buffer* b, uint64_t* out_active, rptb_stats* stats) {
-    if (!b) return fail(RPTB_ERR_BAD_ARG, "null argument");
-    int rc = check_params(s, cam, p);
-    if (rc != RPTB_OK) return rc;
-    rc = check_buffer_shard(p, b);
+    int rc = check_render_into(s, cam, p, b);
     if (rc != RPTB_OK) return rc;
     if (crit && p->engine == RPTB_ENGINE_WAVEFRONT)
         return fail(RPTB_ERR_UNSUPPORTED, "adaptive sampling renders with the slot megakernel, not the wavefront engine");
-    if (p->width != b->width || p->height != b->height)
-        return fail(RPTB_ERR_BAD_ARG, "render is %ux%u but the buffer is %ux%u", p->width, p->height, b->width, b->height);
-    const uint32_t nparts = 1u + (uint32_t)s->peers.size();
-    bool same = nparts == b->parts.size();
-    for (uint32_t i = 0; same && i < nparts; i++) same = (i == 0 ? s->device : s->peers[i - 1]->device) == b->parts[i].device;
-    if (!same) return fail(RPTB_ERR_BAD_ARG, "the buffer was created on a scene with another device list");
+    const uint32_t nparts = (uint32_t)b->parts.size();
     std::lock_guard<std::mutex> bl(b->lock);
     if (b->entries == UINT32_MAX) return fail(RPTB_ERR_UNSUPPORTED, "too many entries");
     // every replica's share is enqueued before any is waited for, so the devices run concurrently
     std::vector<std::unique_lock<std::mutex>> locks;
     std::vector<uint32_t> launches(nparts, 0);
     for (uint32_t i = 0; i < nparts; i++) {
-        rptb_scene* r = i == 0 ? s : s->peers[i - 1];
+        rptb_scene* r = replica(s, i);
         locks.emplace_back(r->lock);
         rc = sample_part(r, cam, p, b->parts[i], stats != nullptr, &launches[i], crit);
         if (rc != RPTB_OK) return nparts > 1 ? fail(rc, "device %d: %s", r->device, g_error.c_str()) : rc;
@@ -1626,7 +1596,7 @@ static int sample_into_impl(rptb_scene* s, const rptb_camera* cam, const rptb_re
     if (out_active) {
         uint64_t total = 0;
         for (uint32_t i = 0; i < nparts; i++) {
-            rptb_scene* r = i == 0 ? s : s->peers[i - 1];
+            rptb_scene* r = replica(s, i);
             DeviceGuard g(r->device);
             unsigned long long a = 0;
             CU(cudaMemcpyAsync(&a, b->parts[i].active, sizeof(a), cudaMemcpyDeviceToHost, r->stream));
@@ -1639,7 +1609,7 @@ static int sample_into_impl(rptb_scene* s, const rptb_camera* cam, const rptb_re
     if (!stats) return RPTB_OK;
     std::memset(stats, 0, sizeof(*stats));
     for (uint32_t i = 0; i < nparts; i++) {
-        rptb_scene* r = i == 0 ? s : s->peers[i - 1];
+        rptb_scene* r = replica(s, i);
         DeviceGuard g(r->device);
         DeviceCounters c;
         CU(cudaMemcpyAsync(&c, r->counters, sizeof(c), cudaMemcpyDeviceToHost, r->stream));
@@ -1686,12 +1656,12 @@ int rptb_buffer_add_samples(rptb_buffer* b, const double* rgb) {
         BufferPart& q = b->parts[i];
         DeviceGuard g(q.device);
         if (!g.ok) return fail(RPTB_ERR_CUDA, "cudaSetDevice(%d) failed", q.device);
-        if (!q.upload) CU(cudaMalloc((void**)&q.upload, nvals * sizeof(double)));
+        if (!q.upload) CU(own(q.mem, &q.upload, nvals * sizeof(double)));
         CU(cudaStreamWaitEvent(q.stream, q.done, 0));
         // pageable source: the call returns once the bytes are staged, `rgb` may be reused afterwards
         CU(cudaMemcpyAsync(q.upload, rgb, nvals * sizeof(double), cudaMemcpyHostToDevice, q.stream));
         CU(launch_buffer_accumulate(nullptr, q.upload, true, nullptr, (uint64_t)q.tiles * 128u, b->width, b->height, q.index, q.count,
-                                    q.sums, q.m2, q.counts, q.stream));
+                                    q.planes.sums, q.planes.m2, q.planes.counts, q.stream));
         CU(cudaEventRecord(q.done, q.stream));
     }
     b->entries++;
@@ -1706,16 +1676,13 @@ int rptb_buffer_image(rptb_buffer* b, uint8_t* out_rgb8) {
     if (b->entries == 0) return fail(RPTB_ERR_BAD_ARG, "Pixel found with no samples");  // buffer.rs:89
     BufferPart& q0 = b->parts[0];
     DeviceGuard g(q0.device);
-    int rc = buffer_gather(b, true, false, true);
+    uint32_t least = 0;
+    int rc = buffer_gather(b, 1u << SUMS | 1u << COUNTS);
+    if (rc == RPTB_OK) rc = buffer_least_count(b, &least);
     if (rc != RPTB_OK) return rc;
-    if (b->reprojected) {
-        uint32_t least = 0;
-        rc = buffer_min_count(b, &least);
-        if (rc != RPTB_OK) return rc;
-        if (least == 0) return fail(RPTB_ERR_BAD_ARG, "Pixel found with no samples");  // buffer.rs:89
-    }
+    if (least == 0) return fail(RPTB_ERR_BAD_ARG, "Pixel found with no samples");  // buffer.rs:89
     const size_t nvals = (size_t)b->width * b->height * 3;
-    CU(launch_film_resolve_counted(b->row_sums, b->row_counts, b->width, b->height, b->radius, b->rgb8, q0.stream));
+    CU(launch_film_resolve_counted(b->rows.sums, b->rows.counts, b->width, b->height, b->radius, b->rgb8, q0.stream));
     CU(cudaMemcpyAsync(out_rgb8, b->rgb8, nvals, cudaMemcpyDeviceToHost, q0.stream));
     CU(cudaStreamSynchronize(q0.stream));
     return RPTB_OK;
@@ -1731,20 +1698,17 @@ int rptb_buffer_variance(rptb_buffer* b, double* out) {
     }
     BufferPart& q0 = b->parts[0];
     DeviceGuard g(q0.device);
-    int rc = buffer_gather(b, false, true, true);
+    uint32_t least = 0;
+    int rc = buffer_gather(b, 1u << M2 | 1u << COUNTS);
+    if (rc == RPTB_OK) rc = buffer_least_count(b, &least);
     if (rc != RPTB_OK) return rc;
-    if (b->reprojected) {
-        uint32_t least = 0;
-        rc = buffer_min_count(b, &least);
-        if (rc != RPTB_OK) return rc;
-        if (least < 2) {
-            *out = NAN;
-            return RPTB_OK;
-        }
+    if (least < 2) {
+        *out = NAN;
+        return RPTB_OK;
     }
     const uint64_t npix = (uint64_t)b->width * b->height;
     double* total = b->partial + buffer_variance_blocks(npix);
-    CU(launch_buffer_variance_sum(b->row_m2, b->row_counts, npix, b->partial, total, q0.stream));
+    CU(launch_buffer_variance_sum(b->rows.m2, b->rows.counts, npix, b->partial, total, q0.stream));
     double sum = 0.0;
     CU(cudaMemcpyAsync(&sum, total, sizeof(double), cudaMemcpyDeviceToHost, q0.stream));
     CU(cudaStreamSynchronize(q0.stream));
@@ -1758,13 +1722,13 @@ int rptb_buffer_sums(rptb_buffer* b, double* out_sums, uint32_t* out_entries) {
     std::lock_guard<std::mutex> bl(b->lock);
     BufferPart& q0 = b->parts[0];
     DeviceGuard g(q0.device);
-    const int rc = buffer_gather(b, true, false, out_entries != nullptr);
+    const int rc = buffer_gather(b, 1u << SUMS | (out_entries ? 1u << COUNTS : 0u));
     if (rc != RPTB_OK) return rc;
-    CU(cudaMemcpyAsync(out_sums, b->row_sums, (size_t)b->width * b->height * 3 * sizeof(double), cudaMemcpyDeviceToHost, q0.stream));
+    CU(cudaMemcpyAsync(out_sums, b->rows.sums, (size_t)b->width * b->height * 3 * sizeof(double), cudaMemcpyDeviceToHost, q0.stream));
     std::vector<uint32_t> counts;
     if (out_entries) {
         counts.resize((size_t)b->width * b->height);
-        CU(cudaMemcpyAsync(counts.data(), b->row_counts, counts.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost, q0.stream));
+        CU(cudaMemcpyAsync(counts.data(), b->rows.counts, counts.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost, q0.stream));
     }
     CU(cudaStreamSynchronize(q0.stream));
     if (out_entries) *out_entries = *std::max_element(counts.begin(), counts.end());
@@ -1778,42 +1742,35 @@ int rptb_buffer_pixel_stats(rptb_buffer* b, double* sums, double* m2, uint32_t* 
     BufferPart& q0 = b->parts[0];
     DeviceGuard g(q0.device);
     const size_t npix = (size_t)b->width * b->height;
-    const int rc = buffer_gather(b, sums != nullptr, m2 != nullptr, counts != nullptr);
+    const int rc = buffer_gather(b, (sums ? 1u << SUMS : 0u) | (m2 ? 1u << M2 : 0u) | (counts ? 1u << COUNTS : 0u));
     if (rc != RPTB_OK) return rc;
-    if (sums) CU(cudaMemcpyAsync(sums, b->row_sums, npix * 3 * sizeof(double), cudaMemcpyDeviceToHost, q0.stream));
-    if (m2) CU(cudaMemcpyAsync(m2, b->row_m2, npix * sizeof(double), cudaMemcpyDeviceToHost, q0.stream));
-    if (counts) CU(cudaMemcpyAsync(counts, b->row_counts, npix * sizeof(uint32_t), cudaMemcpyDeviceToHost, q0.stream));
+    if (sums) CU(cudaMemcpyAsync(sums, b->rows.sums, npix * 3 * sizeof(double), cudaMemcpyDeviceToHost, q0.stream));
+    if (m2) CU(cudaMemcpyAsync(m2, b->rows.m2, npix * sizeof(double), cudaMemcpyDeviceToHost, q0.stream));
+    if (counts) CU(cudaMemcpyAsync(counts, b->rows.counts, npix * sizeof(uint32_t), cudaMemcpyDeviceToHost, q0.stream));
     CU(cudaStreamSynchronize(q0.stream));
     return RPTB_OK;
 }
 
 int rptb_buffer_add_features(rptb_scene* s, const rptb_camera* cam, const rptb_render_params* p, rptb_buffer* b, rptb_stats* stats) {
-    if (!b) return fail(RPTB_ERR_BAD_ARG, "null argument");
-    int rc = check_params(s, cam, p);
+    const int rc = check_render_into(s, cam, p, b);
     if (rc != RPTB_OK) return rc;
-    rc = check_buffer_shard(p, b);
-    if (rc != RPTB_OK) return rc;
-    if (p->width != b->width || p->height != b->height)
-        return fail(RPTB_ERR_BAD_ARG, "render is %ux%u but the buffer is %ux%u", p->width, p->height, b->width, b->height);
-    const uint32_t nparts = 1u + (uint32_t)s->peers.size();
-    bool same = nparts == b->parts.size();
-    for (uint32_t i = 0; same && i < nparts; i++) same = (i == 0 ? s->device : s->peers[i - 1]->device) == b->parts[i].device;
-    if (!same) return fail(RPTB_ERR_BAD_ARG, "the buffer was created on a scene with another device list");
+    const uint32_t nparts = (uint32_t)b->parts.size();
     std::lock_guard<std::mutex> bl(b->lock);
     if (b->feature_rays > UINT64_MAX / 2) return fail(RPTB_ERR_UNSUPPORTED, "too many feature rays");
     // every replica's share is enqueued before any is waited for
     std::vector<std::unique_lock<std::mutex>> locks;
     for (uint32_t i = 0; i < nparts; i++) {
-        rptb_scene* r = i == 0 ? s : s->peers[i - 1];
+        rptb_scene* r = replica(s, i);
         BufferPart& q = b->parts[i];
         locks.emplace_back(r->lock);
         DeviceGuard g(r->device);
         if (!g.ok) return fail(RPTB_ERR_CUDA, "cudaSetDevice(%d) failed", r->device);
         const size_t nelem = (size_t)q.tiles * 128u;
         CU(cudaStreamWaitEvent(r->stream, q.done, 0));
-        if (!q.feat && nelem) {
-            CU(cudaMalloc((void**)&q.feat, nelem * 8 * sizeof(double)));
-            CU(cudaMemsetAsync(q.feat, 0, nelem * 8 * sizeof(double), r->stream));
+        if (!q.planes.feat && nelem) {
+            const int prc = planes_alloc(q.mem, q.planes, nelem, FEATURES);
+            if (prc != RPTB_OK) return prc;
+            CU(cudaMemsetAsync(q.planes.feat, 0, nelem * FEATURE_SUMS * sizeof(double), r->stream));
         }
         rptb_render_params qp = *p;
         qp.shard_index = q.index;
@@ -1822,11 +1779,11 @@ int rptb_buffer_add_features(rptb_scene* s, const rptb_camera* cam, const rptb_r
         if (p->precision == RPTB_PRECISION_F32) {
             RenderArgs<float> a;
             fill_args(cam, &qp, a);
-            CU(launch_features_f32(r->view32, a, r->features, q.feat, r->stream));
+            CU(launch_features_f32(r->view32, a, r->features, q.planes.feat, r->stream));
         } else {
             RenderArgs<double> a;
             fill_args(cam, &qp, a);
-            CU(launch_features_f64(r->view64, a, r->features, q.feat, r->stream));
+            CU(launch_features_f64(r->view64, a, r->features, q.planes.feat, r->stream));
         }
         if (stats) CU(cudaEventRecord(r->ev1, r->stream));
         CU(cudaEventRecord(q.done, r->stream));
@@ -1836,7 +1793,7 @@ int rptb_buffer_add_features(rptb_scene* s, const rptb_camera* cam, const rptb_r
     if (!stats) return RPTB_OK;
     std::memset(stats, 0, sizeof(*stats));
     for (uint32_t i = 0; i < nparts; i++) {
-        rptb_scene* r = i == 0 ? s : s->peers[i - 1];
+        rptb_scene* r = replica(s, i);
         DeviceGuard g(r->device);
         CU(cudaEventSynchronize(r->ev1));
         float ms = 0;
@@ -1866,13 +1823,15 @@ int rptb_buffer_features(rptb_buffer* b, double* normal, double* depth, double* 
     if (b->feature_rays == 0) return fail(RPTB_ERR_BAD_ARG, "the buffer holds no features (rptb_buffer_add_features)");
     BufferPart& q0 = b->parts[0];
     DeviceGuard g(q0.device);
-    const int rc = buffer_features(b);
-    if (rc != RPTB_OK) return rc;
     const size_t npix = (size_t)b->width * b->height;
-    if (normal) CU(cudaMemcpyAsync(normal, b->aov, npix * 3 * sizeof(double), cudaMemcpyDeviceToHost, q0.stream));
-    if (albedo) CU(cudaMemcpyAsync(albedo, b->aov + 3 * npix, npix * 3 * sizeof(double), cudaMemcpyDeviceToHost, q0.stream));
-    if (depth) CU(cudaMemcpyAsync(depth, b->aov + 6 * npix, npix * sizeof(double), cudaMemcpyDeviceToHost, q0.stream));
-    if (hit_fraction) CU(cudaMemcpyAsync(hit_fraction, b->aov + 7 * npix, npix * sizeof(double), cudaMemcpyDeviceToHost, q0.stream));
+    const int rc = buffer_gather(b, FEATURES);
+    if (rc != RPTB_OK) return rc;
+    const Aov a = buffer_aov(b);
+    CU(launch_features_resolve(feature_planes(b->rows.feat, npix), npix, (double)b->feature_rays, a, q0.stream));
+    if (normal) CU(cudaMemcpyAsync(normal, a.normal, npix * 3 * sizeof(double), cudaMemcpyDeviceToHost, q0.stream));
+    if (albedo) CU(cudaMemcpyAsync(albedo, a.albedo, npix * 3 * sizeof(double), cudaMemcpyDeviceToHost, q0.stream));
+    if (depth) CU(cudaMemcpyAsync(depth, a.depth, npix * sizeof(double), cudaMemcpyDeviceToHost, q0.stream));
+    if (hit_fraction) CU(cudaMemcpyAsync(hit_fraction, a.frac, npix * sizeof(double), cudaMemcpyDeviceToHost, q0.stream));
     CU(cudaStreamSynchronize(q0.stream));
     return RPTB_OK;
 }
@@ -1896,24 +1855,20 @@ int rptb_buffer_denoise(rptb_buffer* b, const rptb_denoise* d, double* out_rgb, 
     BufferPart& q0 = b->parts[0];
     DeviceGuard g(q0.device);
     const size_t npix = (size_t)b->width * b->height;
-    int rc = buffer_gather(b, true, true, true);
+    uint32_t least = 0;  // a reprojected buffer does not keep the invariant above: look at the counts
+    int rc = buffer_gather(b, COLOUR | FEATURES);
+    if (rc == RPTB_OK) rc = buffer_least_count(b, &least);
     if (rc != RPTB_OK) return rc;
-    if (b->reprojected) {  // the invariant above does not hold: look at the counts
-        uint32_t least = 0;
-        rc = buffer_min_count(b, &least);
-        if (rc != RPTB_OK) return rc;
-        if (least == 0) return fail(RPTB_ERR_BAD_ARG, "Pixel found with no samples");  // buffer.rs:89
-        if (least < 2) return fail(RPTB_ERR_BAD_ARG, "a pixel has fewer than 2 entries (no variance to guide the filter)");
-    }
-    rc = buffer_features(b);
-    if (rc != RPTB_OK) return rc;
-    if (!b->dn) CU(cudaMalloc((void**)&b->dn, npix * 11 * sizeof(double)));
+    if (least == 0) return fail(RPTB_ERR_BAD_ARG, "Pixel found with no samples");  // buffer.rs:89
+    if (least < 2) return fail(RPTB_ERR_BAD_ARG, "a pixel has fewer than 2 entries (no variance to guide the filter)");
+    const Aov a = buffer_aov(b);
+    CU(launch_features_resolve(feature_planes(b->rows.feat, npix), npix, (double)b->feature_rays, a, q0.stream));
+    if (!b->dn) CU(own(b->mem, &b->dn, npix * 11 * sizeof(double)));
     double* const col[2] = {b->dn, b->dn + 3 * npix};
     double* const var[2] = {b->dn + 6 * npix, b->dn + 7 * npix};
     double* out = b->dn + 8 * npix;
-    const double* a = b->aov;
     uint32_t launches = 0;
-    CU(launch_denoise(b->row_sums, b->row_m2, b->row_counts, a, a + 6 * npix, a + 3 * npix, b->width, b->height, *d, col, var, out,
+    CU(launch_denoise(b->rows.sums, b->rows.m2, b->rows.counts, a.normal, a.depth, a.albedo, b->width, b->height, *d, col, var, out,
                       q0.stream, &launches));
     if (out_rgb) CU(cudaMemcpyAsync(out_rgb, out, npix * 3 * sizeof(double), cudaMemcpyDeviceToHost, q0.stream));
     if (out_rgb8) {
@@ -1957,42 +1912,33 @@ int rptb_buffer_reproject(rptb_buffer* dst, rptb_buffer* src, const rptb_reproje
     DeviceGuard g(d0.device);
     if (!g.ok) return fail(RPTB_ERR_CUDA, "cudaSetDevice(%d) failed", d0.device);
     // src's state and both buffers' features, row-major on parts[0]'s device
-    int rc = buffer_gather(src, true, true, true);
+    const size_t snpix = (size_t)src->width * src->height, dnpix = (size_t)dst->width * dst->height;
+    int rc = buffer_gather(src, COLOUR | FEATURES);
     if (rc != RPTB_OK) return rc;
-    rc = buffer_features(src);
-    if (rc != RPTB_OK) return rc;
+    const Aov sa = buffer_aov(src);
+    CU(launch_features_resolve(feature_planes(src->rows.feat, snpix), snpix, (double)src->feature_rays, sa, s0.stream));
     CU(cudaEventRecord(s0.done, s0.stream));
-    rc = buffer_rows_alloc(dst);
+    rc = buffer_rows_alloc(dst, COLOUR);
+    if (rc == RPTB_OK) rc = buffer_gather(dst, FEATURES);
     if (rc != RPTB_OK) return rc;
-    rc = buffer_features(dst);
-    if (rc != RPTB_OK) return rc;
+    const Aov da = buffer_aov(dst);
+    CU(launch_features_resolve(feature_planes(dst->rows.feat, dnpix), dnpix, (double)dst->feature_rays, da, d0.stream));
     if (!dst->reused) {
-        CU(cudaMalloc((void**)&dst->reused, sizeof(unsigned long long)));
-        CU(cudaMalloc((void**)&dst->min_count, sizeof(uint32_t)));
+        CU(own(dst->mem, &dst->reused, sizeof(unsigned long long)));
+        CU(own(dst->mem, &dst->min_count, sizeof(uint32_t)));
     }
     CU(cudaStreamWaitEvent(d0.stream, s0.done, 0));
     if (out_reused) CU(cudaMemsetAsync(dst->reused, 0, sizeof(unsigned long long), d0.stream));
-    const size_t snpix = (size_t)src->width * src->height, dnpix = (size_t)dst->width * dst->height;
     const ReprojectView dv = reproject_view(dst->feat_cam.cam, dst->width, dst->height);
     const ReprojectView sv = reproject_view(src->feat_cam.cam, src->width, src->height);
-    const double* sa = src->aov;
-    const ReprojectSource sp = {src->row_sums, src->row_m2, src->row_counts, sa, sa + 6 * snpix, sa + 7 * snpix};
-    const double* da = dst->aov;
-    CU(launch_reproject(dv, sv, sp, da, da + 6 * dnpix, da + 7 * dnpix, *prm, dst->row_sums, dst->row_m2, dst->row_counts,
+    const ReprojectSource sp = {src->rows.sums, src->rows.m2, src->rows.counts, sa.normal, sa.depth, sa.frac};
+    CU(launch_reproject(dv, sv, sp, da.normal, da.depth, da.frac, *prm, dst->rows.sums, dst->rows.m2, dst->rows.counts,
                         out_reused ? dst->reused : nullptr, d0.stream));
-    // back to every dst part's compact tiles
-    rc = buffer_rows_to_parts(dst);
+    // back to every dst part's compact tiles; every later call on either buffer is ordered behind this one
+    rc = buffer_write_back(dst, COLOUR);
+    if (rc == RPTB_OK) rc = buffer_order_behind(dst, d0.stream);
+    if (rc == RPTB_OK) rc = buffer_order_behind(src, d0.stream);
     if (rc != RPTB_OK) return rc;
-    // every later call on either buffer is ordered behind this one
-    CU(cudaEventRecord(d0.done, d0.stream));
-    CU(cudaEventRecord(s0.done, d0.stream));
-    for (rptb_buffer* b : {dst, src})
-        for (size_t i = 1; i < b->parts.size(); i++) {
-            BufferPart& q = b->parts[i];
-            DeviceGuard gi(q.device);
-            CU(cudaStreamWaitEvent(q.stream, d0.done, 0));
-            CU(cudaEventRecord(q.done, q.stream));
-        }
     dst->entries = prm->max_history;
     dst->reprojected = true;
     dst->entry_cam = dst->feat_cam;
@@ -2032,22 +1978,13 @@ int rptb_buffer_export_shard(rptb_buffer* b, void* dst_device, uint32_t with_fea
     h.entry_cam = shard_camera(b->entry_cam);
     h.feat_cam = shard_camera(b->feat_cam);
     cudaStream_t st = stream ? (cudaStream_t)stream : q.stream;
-    char* out = (char*)dst_device;
-    const size_t nelem = (size_t)q.tiles * 128u, slot = l.slots * sizeof(double);
     CU(cudaStreamWaitEvent(st, q.done, 0));
     // pageable source: the call returns once the header is staged
-    CU(cudaMemcpyAsync(out, &h, sizeof(h), cudaMemcpyHostToDevice, st));
-    if (nelem) {
-        CU(cudaMemcpyAsync(out + l.sums, q.sums, nelem * 3 * sizeof(double), cudaMemcpyDeviceToDevice, st));
-        CU(cudaMemcpyAsync(out + l.m2, q.m2, nelem * sizeof(double), cudaMemcpyDeviceToDevice, st));
-        if (with_features) {  // the part's planes are nelem long, the block's l.slots
-            CU(cudaMemcpyAsync(out + l.feat, q.feat, nelem * 3 * sizeof(double), cudaMemcpyDeviceToDevice, st));
-            CU(cudaMemcpyAsync(out + l.feat + 3 * slot, q.feat + 3 * nelem, nelem * 3 * sizeof(double), cudaMemcpyDeviceToDevice, st));
-            CU(cudaMemcpyAsync(out + l.feat + 6 * slot, q.feat + 6 * nelem, nelem * sizeof(double), cudaMemcpyDeviceToDevice, st));
-            CU(cudaMemcpyAsync(out + l.feat + 7 * slot, q.feat + 7 * nelem, nelem * sizeof(double), cudaMemcpyDeviceToDevice, st));
-        }
-        CU(cudaMemcpyAsync(out + l.counts, q.counts, nelem * sizeof(uint32_t), cudaMemcpyDeviceToDevice, st));
-    }
+    CU(cudaMemcpyAsync(dst_device, &h, sizeof(h), cudaMemcpyHostToDevice, st));
+    // the part's planes are q.planes.n long, the block's l.slots
+    const PlaneSet to = shard_planes(l, dst_device), from = q.planes.set(l.mask);
+    for (int k = 0; k < NPLANES; k++)
+        if (to.p[k] && q.tiles) CU(cudaMemcpyAsync(to.p[k], from.p[k], plane_bytes(k, q.planes.n), cudaMemcpyDeviceToDevice, st));
     // a later accumulate into the part waits until the block is read
     CU(cudaEventRecord(q.done, st));
     if (!stream) CU(cudaStreamSynchronize(st));
@@ -2094,57 +2031,26 @@ int rptb_buffer_import_shards(rptb_buffer* dst, const void* gathered_device, uin
     }
     // everything dst holds is overwritten: its earlier work finishes first
     for (BufferPart& q : dst->parts) CU(cudaStreamWaitEvent(d0.stream, q.done, 0));
-    if (with_features) {
-        for (BufferPart& q : dst->parts) {
-            const size_t nelem = (size_t)q.tiles * 128u;
-            if (q.feat || !nelem) continue;
-            DeviceGuard gq(q.device);
-            CU(cudaMalloc((void**)&q.feat, nelem * 8 * sizeof(double)));
-        }
-    } else {
-        for (BufferPart& q : dst->parts) {  // dst holds no features afterwards; the next feature pass starts from zero
-            if (!q.feat) continue;
-            DeviceGuard gq(q.device);
+    for (BufferPart& q : dst->parts) {
+        DeviceGuard gq(q.device);
+        if (with_features && q.tiles) {
+            const int rc = planes_alloc(q.mem, q.planes, (size_t)q.tiles * 128u, FEATURES);
+            if (rc != RPTB_OK) return rc;
+        } else if (!with_features && q.planes.feat) {  // dst holds no features afterwards; the next feature pass starts from zero
             CU(cudaEventSynchronize(q.done));
-            CU(cudaFree(q.feat));
-            q.feat = nullptr;
+            CU(cudaFree(q.planes.feat));
+            q.mem.erase(std::find(q.mem.begin(), q.mem.end(), (void*)q.planes.feat));
+            q.planes.feat = nullptr;
         }
     }
-    int rc = buffer_rows_alloc(dst);
+    // every block row-major on dst's first device, then back into dst's own parts; every later call on dst is ordered
+    // behind this one
+    int rc = buffer_rows_alloc(dst, l.mask);
+    for (uint32_t i = 0; rc == RPTB_OK && i < shard_count; i++)
+        rc = buffer_scatter(dst, shard_planes(l, in + (size_t)i * l.bytes), l.mask, i, shard_count);
+    if (rc == RPTB_OK) rc = buffer_write_back(dst, l.mask);
+    if (rc == RPTB_OK) rc = buffer_order_behind(dst, d0.stream);
     if (rc != RPTB_OK) return rc;
-    if (with_features) {
-        rc = buffer_feat_rows_alloc(dst);
-        if (rc != RPTB_OK) return rc;
-    }
-    // every block row-major on dst's first device, then back into dst's own parts
-    const size_t npix = (size_t)W * H, slot = l.slots * sizeof(double);
-    double* rn = dst->row_feat;
-    for (uint32_t i = 0; i < shard_count; i++) {
-        const char* blk = in + (size_t)i * l.bytes;
-        const uint64_t nelem = (uint64_t)buffer_tiles(W, H, i, shard_count) * 128u;
-        CU(launch_buffer_scatter((const double*)(blk + l.sums), (const double*)(blk + l.m2), (const uint32_t*)(blk + l.counts), nelem, W, H,
-                                 i, shard_count, dst->row_sums, dst->row_m2, dst->row_counts, d0.stream));
-        if (!with_features) continue;
-        const char* f = blk + l.feat;
-        CU(launch_buffer_scatter((const double*)f, (const double*)(f + 6 * slot), nullptr, nelem, W, H, i, shard_count, rn, rn + 6 * npix,
-                                 nullptr, d0.stream));
-        CU(launch_buffer_scatter((const double*)(f + 3 * slot), (const double*)(f + 7 * slot), nullptr, nelem, W, H, i, shard_count,
-                                 rn + 3 * npix, rn + 7 * npix, nullptr, d0.stream));
-    }
-    rc = buffer_rows_to_parts(dst);
-    if (rc != RPTB_OK) return rc;
-    if (with_features) {
-        rc = buffer_feat_rows_to_parts(dst);
-        if (rc != RPTB_OK) return rc;
-    }
-    // every later call on dst is ordered behind this one
-    CU(cudaEventRecord(d0.done, d0.stream));
-    for (size_t i = 1; i < dst->parts.size(); i++) {
-        BufferPart& q = dst->parts[i];
-        DeviceGuard gi(q.device);
-        CU(cudaStreamWaitEvent(q.stream, d0.done, 0));
-        CU(cudaEventRecord(q.done, q.stream));
-    }
     // the caller may reuse the gathered bytes when the call returns
     CU(cudaStreamSynchronize(d0.stream));
     dst->entries = h0.entries;

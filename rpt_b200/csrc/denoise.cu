@@ -8,6 +8,7 @@
 #include <cuda_runtime.h>
 
 #include "denoise.h"
+#include "planes.h"
 
 namespace rptb {
 
@@ -52,13 +53,9 @@ __global__ void denoise_finish_kernel(const double* __restrict__ col, const doub
         out[3 * p + k] = col ? col[3 * p + k] * (albedo[3 * p + k] + eps_a) : sums[3 * p + k] / (double)counts[p];
 }
 
-cudaError_t launch_features_resolve(const double* row_feat, uint64_t npix, double rays, double* nrm, double* depth, double* albedo,
-                                    double* frac, cudaStream_t stream) {
-    const double* sn = row_feat;
-    const double* sa = row_feat + 3 * npix;
-    const double* hits = row_feat + 6 * npix;
-    const double* sz = row_feat + 7 * npix;
-    features_resolve_kernel<<<(unsigned)((npix + 255) / 256), 256, 0, stream>>>(sn, sa, hits, sz, npix, rays, nrm, depth, albedo, frac);
+cudaError_t launch_features_resolve(const FeaturePlanes& f, uint64_t npix, double rays, const Aov& out, cudaStream_t stream) {
+    features_resolve_kernel<<<(unsigned)((npix + 255) / 256), 256, 0, stream>>>(f.n, f.a, f.h, f.z, npix, rays, out.normal, out.depth,
+                                                                               out.albedo, out.frac);
     return cudaGetLastError();
 }
 

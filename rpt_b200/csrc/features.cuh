@@ -8,20 +8,13 @@
 #include "camera.cuh"
 #include "integrator.cuh"
 #include "launch.h"
+#include "planes.h"
 
 namespace rptb {
 
-// The sums of nelem pixels, one plane after the other: normal (3 per pixel), albedo (3), hits, depth -- the first two
-// laid out like a Buffer's colour sums and the last two like its M2, so the Buffer's own scatter gathers them.
-constexpr uint32_t FEATURE_SUMS = 8;
-struct FeaturePlanes {
-    double *n, *a, *h, *z;
-};
-RPTB_HD FeaturePlanes feature_planes(double* base, size_t nelem) { return {base, base + 3 * nelem, base + 6 * nelem, base + 7 * nelem}; }
-
 // Element e = block_x * 128 + thread_x of the replica's compact tile-major layout (RenderArgs::compact): pixel thread_x
-// of owned tile block_x.  Adds samples [first_sample, first_sample + iterations) to element e of the planes at `acc`
-// (ntiles_mine * 128 elements), in sample order.
+// of owned tile block_x.  Adds samples [first_sample, first_sample + iterations) to element e of the feature planes at
+// `acc` (planes.h, ntiles_mine * 128 elements), in sample order.
 template <class R, int FEAT>
 RPTB_D void feature_thread(const SceneView<R>& sv, const RenderArgs<R>& a, const uint32_t block_x, const uint32_t thread_x,
                            double* __restrict__ acc) {

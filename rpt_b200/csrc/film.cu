@@ -13,6 +13,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "planes.h"
 #include "tile.h"
 
 namespace rptb {
@@ -140,23 +141,45 @@ __global__ void buffer_accumulate_kernel(const T* __restrict__ in, const uint8_t
     counts[e] = n;
 }
 
-// Compact tiles of replica `shard_index` of `shard_count` -> the row-major sums / M2 / counts of the whole image; a
-// null output plane is skipped.
-__global__ void buffer_scatter_kernel(const double* __restrict__ sums, const double* __restrict__ m2,
-                                      const uint32_t* __restrict__ counts, uint64_t nelem, uint32_t width, uint32_t height,
-                                      uint32_t shard_index, uint32_t shard_count, double* __restrict__ row_sums,
-                                      double* __restrict__ row_m2, uint32_t* __restrict__ row_counts) {
+// Element `from` of every plane present in both sets (planes.h) -> element `to` of dst; from < 0 writes zeros.  Every
+// value is loaded before any is stored, so the loads of all planes are in flight together.
+__device__ __forceinline__ void move_planes(const PlaneSet& src, const PlaneSet& dst, int64_t from, uint64_t to) {
+    unsigned long long v[NPLANES][3];
+#pragma unroll
+    for (int k = 0; k < NPLANES; k++) {
+        const PlaneShape s = plane_shape(k);
+        if (!src.p[k] || !dst.p[k] || from < 0) continue;
+        for (uint32_t j = 0; j < s.values; j++)
+            v[k][j] = s.bytes == 8 ? ((const unsigned long long*)src.p[k])[s.values * from + j] : ((const uint32_t*)src.p[k])[s.values * from + j];
+    }
+#pragma unroll
+    for (int k = 0; k < NPLANES; k++) {
+        const PlaneShape s = plane_shape(k);
+        if (!src.p[k] || !dst.p[k]) continue;
+        for (uint32_t j = 0; j < s.values; j++) {
+            const unsigned long long x = from < 0 ? 0ull : v[k][j];
+            if (s.bytes == 8) ((unsigned long long*)dst.p[k])[s.values * to + j] = x;
+            else ((uint32_t*)dst.p[k])[s.values * to + j] = (uint32_t)x;
+        }
+    }
+}
+
+// The compact tiles of replica `shard_index` of `shard_count` -> the row-major planes of the whole image.
+__global__ void buffer_scatter_kernel(const PlaneSet src, const PlaneSet dst, uint64_t nelem, uint32_t width, uint32_t height,
+                                      uint32_t shard_index, uint32_t shard_count) {
     const uint64_t e = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (e >= nelem) return;
     const int64_t p = tile_pixel(width, height, shard_index + (uint32_t)(e >> 7) * shard_count, (uint32_t)(e & 127u));
-    if (p < 0) return;
-    if (row_sums) {
-        row_sums[3 * p] = sums[3 * e];
-        row_sums[3 * p + 1] = sums[3 * e + 1];
-        row_sums[3 * p + 2] = sums[3 * e + 2];
-    }
-    if (row_m2) row_m2[p] = m2[e];
-    if (row_counts) row_counts[p] = counts[e];
+    if (p >= 0) move_planes(src, dst, e, p);
+}
+
+// The inverse: the row-major planes -> the compact tiles.  Elements past a ragged edge are zeroed, as a fresh buffer
+// holds them.
+__global__ void buffer_compact_kernel(const PlaneSet src, const PlaneSet dst, uint64_t nelem, uint32_t width, uint32_t height,
+                                      uint32_t shard_index, uint32_t shard_count) {
+    const uint64_t e = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= nelem) return;
+    move_planes(src, dst, tile_pixel(width, height, shard_index + (uint32_t)(e >> 7) * shard_count, (uint32_t)(e & 127u)), e);
 }
 
 // Buffer::variance from the row-major M2 and counts: the sum over pixels of M2/(n-1), each pixel with its own n (a
@@ -230,12 +253,13 @@ cudaError_t launch_film_resolve_counted(const double* sums, const uint32_t* coun
     return cudaGetLastError();
 }
 
-cudaError_t launch_buffer_scatter(const double* sums, const double* m2, const uint32_t* counts, uint64_t nelem, uint32_t width,
-                                  uint32_t height, uint32_t shard_index, uint32_t shard_count, double* row_sums, double* row_m2,
-                                  uint32_t* row_counts, cudaStream_t stream) {
+// `compact`: row-major src -> compact dst (buffer_compact_kernel), else compact src -> row-major dst.
+cudaError_t launch_buffer_move(bool compact, const PlaneSet& src, const PlaneSet& dst, uint64_t nelem, uint32_t width, uint32_t height,
+                               uint32_t shard_index, uint32_t shard_count, cudaStream_t stream) {
     if (nelem == 0) return cudaSuccess;
-    buffer_scatter_kernel<<<(unsigned)((nelem + 255) / 256), 256, 0, stream>>>(sums, m2, counts, nelem, width, height, shard_index,
-                                                                             shard_count, row_sums, row_m2, row_counts);
+    const unsigned grid = (unsigned)((nelem + 255) / 256);
+    if (compact) buffer_compact_kernel<<<grid, 256, 0, stream>>>(src, dst, nelem, width, height, shard_index, shard_count);
+    else buffer_scatter_kernel<<<grid, 256, 0, stream>>>(src, dst, nelem, width, height, shard_index, shard_count);
     return cudaGetLastError();
 }
 

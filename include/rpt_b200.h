@@ -271,7 +271,9 @@ int rptb_scene_create(const rptb_scene_desc* desc, int device, rptb_scene** out)
  * over rows) -- rptb_render_samples on such a handle runs one host thread per GPU, GPU i renders the 16x8-pixel
  * tiles t with t % ndevices == i and copies exactly its own pixels into the caller's image, so there is nothing to
  * reduce and the image is bit-identical for any ndevices.  rptb_render_samples_device, rptb_closest_hit and
- * rptb_illuminate on it address replica 0 (the first is RPTB_ERR_UNSUPPORTED when ndevices > 1).          */
+ * rptb_illuminate on it address replica 0 (the first is RPTB_ERR_UNSUPPORTED when ndevices > 1).  A device listed
+ * twice is RPTB_ERR_BAD_ARG unless the environment has RPTB_ALLOW_REPEATED_DEVICES=1 (a testing switch, read on
+ * every call): then each listing is a replica of its own, as a distinct GPU would be, which is no faster.    */
 int rptb_scene_create_multi(const rptb_scene_desc* desc, const int* devices, int ndevices, rptb_scene** out);
 int rptb_scene_device_count(const rptb_scene* scene);
 void rptb_scene_destroy(rptb_scene* scene);

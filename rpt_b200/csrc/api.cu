@@ -1025,11 +1025,16 @@ int rptb_scene_create_multi(const rptb_scene_desc* desc, const int* devices, int
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return fail(RPTB_ERR_NO_DEVICE, "no CUDA device");
     if (ndevices <= 0 || ndevices > 64) return fail(RPTB_ERR_BAD_ARG, "ndevices %d", ndevices);
+    // RPTB_ALLOW_REPEATED_DEVICES=1 (a testing switch, read on every call): a device may be listed more than once, and
+    // each listing is a replica of its own -- its own stream, scratch and tiles, as on a distinct GPU -- so the
+    // multi-replica paths run on a single GPU.  It is not faster: the replicas share that GPU.
+    const char* rep = getenv("RPTB_ALLOW_REPEATED_DEVICES");
+    const bool repeats = rep && std::strcmp(rep, "1") == 0;
     std::vector<int> devs(ndevices);
     for (int i = 0; i < ndevices; i++) {
         devs[i] = devices ? devices[i] : i;
         if (devs[i] < 0 || devs[i] >= ndev) return fail(RPTB_ERR_BAD_ARG, "device %d of %d", devs[i], ndev);
-        for (int j = 0; j < i; j++)
+        for (int j = 0; j < i && !repeats; j++)
             if (devs[j] == devs[i]) return fail(RPTB_ERR_BAD_ARG, "device %d listed twice", devs[i]);
     }
     std::vector<rptb_scene*> reps;

@@ -8,6 +8,7 @@ import pytest
 
 from rpt_b200 import _capi as capi
 from rpt_b200 import api, scenes
+from tests import util
 
 pytestmark = pytest.mark.gpu
 
@@ -213,13 +214,14 @@ def test_convergence_ends(gpu_ok):
     r2.close()
 
 
-def test_any_device_count_gives_the_same_bits(gpu_ok):
+def test_any_device_count_gives_the_same_bits(gpu_ok, monkeypatch):
+    monkeypatch.setenv(util.REPEATED_DEVICES, "1")
     cfg = scenes.cornell_scene()
     w, h = 203, 117
     crit = api.Adaptive(0.1, 2e-3, 2)
     ref = None
-    for n in range(1, min(gpu_ok, 8) + 1):
-        r = _renderer(cfg, w, h, 3, device=list(range(n)))
+    for devices in util.replica_lists(gpu_ok):
+        r = _renderer(cfg, w, h, 3, device=devices)
         buf = r.device_buffer()
         actives = [_adaptive(r, 2, buf, crit, want_stats=False)[0] for _ in range(5)]
         got = buf.pixel_stats() + (buf.image(), buf.variance(), actives)
@@ -228,7 +230,7 @@ def test_any_device_count_gives_the_same_bits(gpu_ok):
             assert 0 < actives[-1] < w * h
         else:
             for a, b in zip(got[:4], ref[:4]):
-                assert np.array_equal(a, b), n
-            assert got[4] == ref[4] and got[5] == ref[5], n
+                assert np.array_equal(a, b), devices
+            assert got[4] == ref[4] and got[5] == ref[5], devices
         buf.close()
         r.close()

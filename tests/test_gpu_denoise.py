@@ -8,6 +8,7 @@ import pytest
 from rpt_b200 import _capi as capi
 from rpt_b200 import api, scenes
 from tests import denoise_ref as ref
+from tests import util
 
 pytestmark = pytest.mark.gpu
 
@@ -105,14 +106,18 @@ def test_errors(gpu_ok):
         ad.denoise()
 
 
-def test_same_bits_for_every_device_count(gpu_ok):
+def test_same_bits_for_every_device_count(gpu_ok, monkeypatch):
+    monkeypatch.setenv(util.REPEATED_DEVICES, "1")
     cfg = scenes.cornell_scene()
+    lists = util.replica_lists(gpu_ok)
     outs = []
-    for n in range(1, gpu_ok + 1):
-        _, buf = _buffer(cfg, 53, 37, 3, 3, 2, 3, device=list(range(n)))
+    for devices in lists:
+        r, buf = _buffer(cfg, 53, 37, 3, 3, 2, 3, device=devices)
         outs.append((buf.features(), buf.denoise()))
-    for f, d in outs[1:]:
-        assert all(np.array_equal(x, y) for x, y in zip(f, outs[0][0])) and np.array_equal(d, outs[0][1])
+        buf.close()
+        r.close()
+    for devices, (f, d) in zip(lists[1:], outs[1:]):
+        assert all(np.array_equal(x, y) for x, y in zip(f, outs[0][0])) and np.array_equal(d, outs[0][1]), devices
 
 
 def _edge_band(N, z):

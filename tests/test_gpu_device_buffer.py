@@ -8,6 +8,7 @@ import pytest
 
 from rpt_b200 import _capi as capi
 from rpt_b200 import api, scenes
+from tests import util
 
 pytestmark = pytest.mark.gpu
 
@@ -139,12 +140,13 @@ def test_iterative_render_with_a_device_buffer(gpu_ok):
     r.close()
 
 
-def test_any_device_count_gives_the_same_bits(gpu_ok):
+def test_any_device_count_gives_the_same_bits(gpu_ok, monkeypatch):
+    monkeypatch.setenv(util.REPEATED_DEVICES, "1")
     cfg = scenes.cornell_scene()
     w, h = 203, 117
     ref = None
-    for n in range(1, min(gpu_ok, 8) + 1):
-        r = _renderer(cfg, w, h, 3, device=list(range(n)))
+    for devices in util.replica_lists(gpu_ok):
+        r = _renderer(cfg, w, h, 3, device=devices)
         dev = r.device_buffer()
         for k in (4, 4, 2):
             r.sample(k, dev, want_stats=False)
@@ -153,9 +155,9 @@ def test_any_device_count_gives_the_same_bits(gpu_ok):
         if ref is None:
             ref = got
         else:
-            assert np.array_equal(got[0], ref[0])
+            assert np.array_equal(got[0], ref[0]), devices
             np.testing.assert_array_equal(got[1], ref[1])
-            assert got[2] == ref[2], n
+            assert got[2] == ref[2], devices
         dev.close()
         r.close()
 
@@ -234,18 +236,29 @@ def test_error_statuses(gpu_ok):
     r.close()
 
 
-def test_buffer_refuses_a_scene_on_other_devices(gpu_ok):
-    if gpu_ok < 2:
-        pytest.skip("needs two GPUs for two different device lists")
+def test_buffer_refuses_a_scene_on_other_devices(gpu_ok, monkeypatch):
+    """A buffer takes renders only from scenes on its own device list: [0] against [0, 0] and back (a repeated device is a
+    replica of its own), and with two GPUs [0] against [1] and [0, 1].  Nothing a refused call did reaches the buffer."""
+    monkeypatch.setenv(util.REPEATED_DEVICES, "1")
     lib = capi.lib()
     cfg = scenes.sphere_scene()
-    r0 = _renderer(cfg, 32, 16, 1, device=0)
-    r1 = _renderer(cfg, 32, 16, 1, device=1)
-    r01 = _renderer(cfg, 32, 16, 1, device=[0, 1])
-    dev = r0.device_buffer()
-    cam, p = cfg.camera.to_c(), r0.params(1)
-    for other in (r1, r01):
-        assert lib.rptb_sample_into(other.device_scene().handle, C.byref(cam), C.byref(p), dev.handle, None) == capi.ERR_BAD_ARG
-    dev.close()
-    for r in (r0, r1, r01):
+    lists = [[0], [0, 0]] + ([[1], [0, 1]] if gpu_ok >= 2 else [])
+    rs = [_renderer(cfg, 32, 16, 1, device=d) for d in lists]
+    cam, p = cfg.camera.to_c(), rs[0].params(1)
+    for i, mine in enumerate(rs[:2]):
+        dev = mine.device_buffer()
+        for j, other in enumerate(rs):
+            if j != i:
+                rc = lib.rptb_sample_into(other.device_scene().handle, C.byref(cam), C.byref(p), dev.handle, None)
+                assert rc == capi.ERR_BAD_ARG and "another device list" in lib.rptb_last_error().decode(), (lists[i], lists[j])
+                rc = lib.rptb_buffer_add_features(other.device_scene().handle, C.byref(cam), C.byref(p), dev.handle, None)
+                assert rc == capi.ERR_BAD_ARG, (lists[i], lists[j])
+        assert not dev.sums().any()
+        # a scene of its own device list (another handle) is accepted
+        twin = _renderer(cfg, 32, 16, 1, device=lists[i])
+        assert lib.rptb_sample_into(twin.device_scene().handle, C.byref(cam), C.byref(p), dev.handle, None) == capi.OK
+        assert dev.sums().any()
+        twin.close()
+        dev.close()
+    for r in rs:
         r.close()

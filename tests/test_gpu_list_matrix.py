@@ -16,7 +16,7 @@ over any mask through the public C ABI alone:
   * mask edges: no pixel, every pixel, the last pixel, the ragged tiles only, a checkerboard of 8x4 warp blocks and
     every other tile, at 1x1, 7x3, 16x8, 17x9 and 203x117;
   * sample chunks: 130 and 2100 samples in one call (3 and 32 chunks, one group per chunk), f32 and f64;
-  * with two or more GPUs, the same bits on every device list.
+  * the same bits on every device list, replicas repeated on one device included (tests/util.py replica_lists).
 
 On one H100 80GB HBM3 at a 700 W power limit every f32 list entry came out bit-identical to the plain render's entry
 (both schedules inline the same render_thread), so f32 is held to equality like f64, and the counters to exact sums.
@@ -32,6 +32,7 @@ import pytest
 from rpt_b200 import _capi as capi
 from rpt_b200 import api
 from tests import pathwise as pw
+from tests import util
 from tests.hostemu import emu
 
 pytestmark = pytest.mark.gpu
@@ -220,15 +221,14 @@ def test_sample_chunks(gpu_ok, name, precision, n):
     _counters_add_up(st, st_c, sp, True, (name, n))
 
 
-def test_every_device_list_gives_the_same_bits(gpu_ok):
-    if gpu_ok < 2:
-        pytest.skip("one GPU visible")
+def test_every_device_list_gives_the_same_bits(gpu_ok, monkeypatch):
+    monkeypatch.setenv(util.REPEATED_DEVICES, "1")
     c = pw.CASES["fractal_teapots_bvh"]
     scene, cam = c.make()
     w, h = 203, 117
     m = pw.list_mask(w, h, 13)
     ref = None
-    for devices in ([0], [1], [0, 1], list(range(min(gpu_ok, 8)))):
+    for devices in util.replica_lists(gpu_ok) + ([[1]] if gpu_ok >= 2 else []):
         t = Target(c, scene, cam, F32, w, h, device=devices)
         try:
             entry, st = t.masked(m, 2, 1, 1)

@@ -30,9 +30,10 @@ def _render(ds, cfg, w, h, spp, mb, seed, precision=F32, shard=(0, 1), first_sam
 
 
 @pytest.mark.parametrize("name,w,h,spp,mb", [("cornell", 200, 136, 70, 4), ("teapot", 203, 117, 8, 0), ("glass", 160, 90, 130, 12)])
-def test_multi_device_handle_is_bit_identical(gpu_ok, name, w, h, spp, mb):
-    """N in {1, 2, 4, 8} (as many as the box has): same bits through the same call; ragged image sizes, more than one
-    sample chunk, both precisions; counters add up."""
+def test_multi_device_handle_is_bit_identical(gpu_ok, monkeypatch, name, w, h, spp, mb):
+    """Every list of util.replica_lists (1 to 8 replicas, a repeated device being a replica of its own): same bits
+    through the same call; ragged image sizes, more than one sample chunk, both precisions; counters add up."""
+    monkeypatch.setenv(util.REPEATED_DEVICES, "1")
     cfg = scenes.glass_scene(256, 128) if name == "glass" else scenes.CONFIGS[name]()
     flat = api.FlatScene(cfg.scene)
     with api.DeviceScene(flat, 0) as one:
@@ -45,10 +46,9 @@ def test_multi_device_handle_is_bit_identical(gpu_ok, name, w, h, spp, mb):
         np.testing.assert_array_equal(parts[0] + parts[1] + parts[2], ref32)
         assert all((p == 0).any() for p in parts)
     tested = []
-    for n in (1, 2, 3, 4, 8):
-        if n > gpu_ok:
-            continue
-        with api.DeviceScene(flat, list(range(n))) as multi:
+    for devices in util.replica_lists(gpu_ok):
+        n = len(devices)
+        with api.DeviceScene(flat, devices) as multi:
             assert multi.device_count() == n
             a, sa = _render(multi, cfg, w, h, spp, mb, 7)
             np.testing.assert_array_equal(a, ref32)
@@ -70,7 +70,7 @@ def test_multi_device_handle_is_bit_identical(gpu_ok, name, w, h, spp, mb):
                 rc = capi.lib().rptb_render_samples_device(multi.handle, C.byref(cam), C.byref(p), C.c_void_p(t.data_ptr()), None, None)
                 assert rc == -5  # RPTB_ERR_UNSUPPORTED
         tested.append(n)
-    assert 1 in tested
+    assert tested[0] == 1 and max(tested) == 8
 
 
 def test_multi_device_create_rejects_bad_device_lists(gpu_ok):

@@ -10,6 +10,7 @@ import pytest
 from rpt_b200 import _capi as capi
 from rpt_b200 import api, scenes
 from tests import reproject_ref as ref
+from tests import util
 from tests.test_reproject import orbit
 
 pytestmark = pytest.mark.gpu
@@ -105,19 +106,23 @@ def test_identity_keeps_the_mean(gpu_ok):
         assert np.max(np.abs(m2 / (counts - 1.0) - m0 / (n - 1.0))) <= 1e-12 * (m0 / (n - 1.0)).max()
 
 
-def test_same_bits_for_every_device_count(gpu_ok):
+def test_same_bits_for_every_device_count(gpu_ok, monkeypatch):
+    monkeypatch.setenv(util.REPEATED_DEVICES, "1")
     cfg, scam = _setup("cornell")
     dcam = orbit(scam, CENTER["cornell"], -0.05)
+    lists = util.replica_lists(gpu_ok)
     outs = []
-    for k in range(1, gpu_ok + 1):
-        r = _renderer(cfg, scam, 53, 37, device=list(range(k)))
+    for devices in lists:
+        r = _renderer(cfg, scam, 53, 37, device=devices)
         src = _src(r, 3, 2, 3)
         dst = _dst(r, dcam, 47, 41, 3)
         reused = dst.reproject_from(src)
         outs.append((reused,) + dst.pixel_stats())
+        for b in (src, dst):
+            b.close()
         r.close()
-    for o in outs[1:]:
-        assert o[0] == outs[0][0] and all(np.array_equal(x, y) for x, y in zip(o[1:], outs[0][1:]))
+    for devices, o in zip(lists[1:], outs[1:]):
+        assert o[0] == outs[0][0] and all(np.array_equal(x, y) for x, y in zip(o[1:], outs[0][1:])), devices
 
 
 def test_a_reprojected_buffer_renders_its_holes_first(gpu_ok):
@@ -165,7 +170,8 @@ def _rc(dst, src, prm=None):
     return capi.lib().rptb_buffer_reproject(dst.handle, src.handle, C.byref(c), None), capi.lib().rptb_last_error().decode()
 
 
-def test_errors(gpu_ok):
+def test_errors(gpu_ok, monkeypatch):
+    monkeypatch.setenv(util.REPEATED_DEVICES, "1")
     cfg, cam = _setup("sphere")
     other = orbit(cam, CENTER["sphere"], 0.1)
     w, h = 16, 12
@@ -217,13 +223,20 @@ def test_errors(gpu_ok):
     assert rc[0] == capi.ERR_UNSUPPORTED and "aperture" in rc[1]
     rc = _rc(src_with([], [focused]), good)
     assert rc[0] == capi.ERR_UNSUPPORTED and "aperture" in rc[1]
-    # buffers of scenes with other device lists
-    if gpu_ok >= 2:
-        r1 = _renderer(cfg, other, w, h, device=1)
+    # buffers of scenes with other device lists: two replicas on one device against one, and another GPU
+    for devices in [[0, 0]] + ([[1]] if gpu_ok >= 2 else []):
+        r1 = _renderer(cfg, other, w, h, device=devices)
         on1 = r1.device_buffer()
         r1.sample_features(1, on1)
         rc = _rc(on1, good)
-        assert rc[0] == capi.ERR_BAD_ARG and "device lists" in rc[1]
+        assert rc[0] == capi.ERR_BAD_ARG and "device lists" in rc[1], devices
+        r1.camera = cam
+        src1 = _src(r1, 2, 1, 1)
+        rc = _rc(fresh, src1)
+        assert rc[0] == capi.ERR_BAD_ARG and "device lists" in rc[1], devices
+        for b in (on1, src1):
+            b.close()
+        r1.close()
     # and nothing it refused touched dst
     assert fresh.reproject_from(good) > 0
 

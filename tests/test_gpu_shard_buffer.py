@@ -11,6 +11,7 @@ import torch
 from rpt_b200 import _capi as capi
 from rpt_b200 import api, scenes
 from rpt_b200.distributed import ShardBuffer, shard_block_layout, shard_tiles
+from tests import util
 
 pytestmark = pytest.mark.gpu
 
@@ -262,10 +263,9 @@ def test_errors(gpu_ok):
         b.close()
 
 
-def test_multi_replica_scene_is_unsupported(gpu_ok):
-    if gpu_ok < 2:
-        pytest.skip("a scene with two replicas needs two GPUs")
-    r = _renderer(32, 16, F32).device([0, 1])
+def test_multi_replica_scene_is_unsupported(gpu_ok, monkeypatch):
+    monkeypatch.setenv(util.REPEATED_DEVICES, "1")
+    r = _renderer(32, 16, F32).device([0, 0])
     hd = C.c_void_p()
     rc = capi.lib().rptb_buffer_create_shard(r.device_scene().handle, 32, 16, 0, 0, 2, C.byref(hd))
     assert rc == capi.ERR_UNSUPPORTED and not hd

@@ -110,6 +110,20 @@ def rmse(a, b):
     return float(np.sqrt(np.mean((np.asarray(a) - np.asarray(b)) ** 2)))
 
 
+REPEATED_DEVICES = "RPTB_ALLOW_REPEATED_DEVICES"
+
+
+def replica_lists(gpu_ok):
+    """Device lists for the tests that must give the same bits for every replica count.  A repeated device is a replica
+    of its own (under RPTB_ALLOW_REPEATED_DEVICES=1, which the caller sets with monkeypatch.setenv), so one GPU runs every
+    multi-part path; with two or more GPUs the lists also cross devices, and [0, 1, 0, 1] mixes same-device and
+    cross-device copies in one buffer."""
+    lists = [[0], [0, 0], [0, 0, 0], [0] * 5, [0] * 8]
+    if gpu_ok >= 2:
+        lists += [[0, 1], [0, 1, 0, 1], list(range(min(gpu_ok, 8)))]
+    return lists
+
+
 def golden_config(name):
     """The scene behind each committed fixture of tests/golden (tools/make_golden.py builds it the same way)."""
     from rpt_b200 import scenes

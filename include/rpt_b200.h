@@ -536,7 +536,8 @@ int rptb_buffer_reproject(rptb_buffer* dst, rptb_buffer* src, const rptb_reproje
  * no-ops), in one part on scene's device.  rptb_sample_into, rptb_sample_into_adaptive and rptb_buffer_add_features
  * take it when params->shard_index / shard_count are its own (else RPTB_ERR_BAD_ARG); out_active counts this shard's
  * pixels.  Its whole-image calls -- image, variance, sums, pixel_stats, features, denoise, reproject (as dst or src)
- * and add_samples -- are RPTB_ERR_UNSUPPORTED: gather the shards first.  RPTB_ERR_BAD_ARG: shard_index >=
+ * and add_samples -- are RPTB_ERR_UNSUPPORTED: gather the shards first.  It is reprojected into with
+ * rptb_buffer_reproject_shard.  RPTB_ERR_BAD_ARG: shard_index >=
  * shard_count, and the checks of rptb_buffer_create; RPTB_ERR_UNSUPPORTED: a scene with more than one replica.   */
 int rptb_buffer_create_shard(rptb_scene* scene, uint32_t width, uint32_t height, uint32_t box_radius, uint32_t shard_index,
                              uint32_t shard_count, rptb_buffer** out);
@@ -547,19 +548,30 @@ int rptb_buffer_create_shard(rptb_scene* scene, uint32_t width, uint32_t height,
 uint64_t rptb_buffer_shard_bytes(const rptb_buffer* buffer, uint32_t with_features);
 /* Writes the shard buffer's block (rptb_buffer_shard_bytes) to dst_device, on `stream` (a cudaStream_t, behind the
  * buffer's earlier calls; NULL = the buffer's own stream, and the call then synchronises).  The header holds the
- * image size, shard_index, shard_count, with_features, the entry count, the feature rays and the recorded entry and
- * feature cameras; the planes are device-to-device copies of the shard's own.  Slots past the shard's own are not
+ * image size, shard_index, shard_count, with_features, the entry count, whether the shard was reprojected
+ * (rptb_buffer_reproject_shard), the feature rays and the recorded entry and feature cameras; the planes are device-to-device copies of the shard's own.  Slots past the shard's own are not
  * written.  RPTB_ERR_BAD_ARG: a null pointer, a whole buffer, or with_features on a buffer holding no features.  */
 int rptb_buffer_export_shard(rptb_buffer* buffer, void* dst_device, uint32_t with_features, void* stream);
 /* Replaces the state of `dst`, a whole buffer, with the shards gathered in `gathered_device` on dst's first device:
  * shard_count blocks of rptb_buffer_shard_bytes each, shard 0 first -- what an all-gather of every shard's export
  * gives.  The bytes must be complete when the call is made; it returns once it has read them.  Afterwards dst holds
  * the shards' entries, counts and recorded cameras -- and their features with with_features, none without -- and is
- * indistinguishable from a whole buffer that received the same calls (it may be reprojected from or into).
+ * indistinguishable from a whole buffer that received the same calls (it may be reprojected from or into; gathered
+ * from reprojected shards, it is a reprojected buffer, whose image, variance and denoise check the least count).
  * RPTB_ERR_BAD_ARG: a null pointer or shard_count 0; dst a shard buffer; a block that is not an export, or was made
  * for another image size, shard count or with_features; shards out of order (block i must hold shard i); shards that
- * received different calls (entry counts, feature rays or cameras differ).                                        */
+ * received different calls (entry counts, reprojection, feature rays or cameras differ).                          */
 int rptb_buffer_import_shards(rptb_buffer* dst, const void* gathered_device, uint32_t shard_count, uint32_t with_features);
+/* rptb_buffer_reproject into a shard buffer: `dst`, a shard, takes the history of its own pixels from `src`, a whole
+ * buffer on the shard's device -- in a frame loop, the previous frame's shards gathered with features.  Each pixel
+ * gets the bits rptb_buffer_reproject gives it in a whole dst of the same size, features and camera, so the shards'
+ * blocks, gathered, are that whole dst.  The checks and refusals are rptb_buffer_reproject's, and the two buffers may
+ * differ in size; besides, RPTB_ERR_BAD_ARG: dst a whole buffer, or src's first device not the shard's;
+ * RPTB_ERR_UNSUPPORTED: src a shard buffer (gather the shards first).  Afterwards dst is reprojected as by
+ * rptb_buffer_reproject, and its block says so (rptb_buffer_export_shard).  A shard that owns no tile does no device
+ * work and takes the same state.  out_reused counts this shard's pixels: summed over the shards, the whole call's. */
+int rptb_buffer_reproject_shard(rptb_buffer* dst, rptb_buffer* src, const rptb_reproject* params,
+                                uint64_t* out_reused /* nullable, forces sync: this shard's pixels that got history */);
 
 #ifdef __cplusplus
 }

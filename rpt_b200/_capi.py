@@ -285,6 +285,7 @@ SYMBOLS = [
     ("rptb_buffer_shard_bytes", C.c_uint64, [C.c_void_p, C.c_uint32]),
     ("rptb_buffer_export_shard", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p]),
     ("rptb_buffer_import_shards", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32]),
+    ("rptb_buffer_reproject_shard", C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(Reproject), C.POINTER(C.c_uint64)]),
 ]
 
 _lib = None

@@ -1232,6 +1232,13 @@ class Renderer:
             self.sample_features(feature_samples, buf)
             return buf.denoised_image(denoise)
 
+    def _check_frames(self, entries: int, adaptive: Optional[Adaptive], denoise: Optional[Denoise]) -> None:
+        """The arguments render_frames and distributed.render_frames_distributed refuse."""
+        if entries < 1 or self._num_samples % entries:
+            raise ValueError(f"num_samples {self._num_samples} must be a multiple of entries {entries} (and entries >= 1)")
+        if denoise is not None and entries < 2 and adaptive is None:
+            raise ValueError("a denoised frame needs entries >= 2 (or adaptive entries)")
+
     def render_frames(self, cameras, entries: int = 8, feature_samples: int = 16, reproject: Optional[Reproject] = Reproject(),
                       adaptive: Optional[Adaptive] = None, denoise: Optional[Denoise] = None):
         """Renders one frame per camera of a static scene and yields each as (height, width, 3) uint8.  Per frame: a new
@@ -1239,10 +1246,7 @@ class Renderer:
         reprojected into it (unless `reproject` is None), and `entries` entries of num_samples / entries samples each are
         added -- adaptive ones with `adaptive` -- continuing the renderer's sample streams; the frame is image(), or
         denoised_image(denoise).  The device scene is uploaded once for all frames."""
-        if entries < 1 or self._num_samples % entries:
-            raise ValueError(f"num_samples {self._num_samples} must be a multiple of entries {entries} (and entries >= 1)")
-        if denoise is not None and entries < 2 and adaptive is None:
-            raise ValueError("a denoised frame needs entries >= 2 (or adaptive entries)")
+        self._check_frames(entries, adaptive, denoise)
         own, prev = self.camera, None
         try:
             for cam in cameras:

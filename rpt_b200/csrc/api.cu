@@ -62,6 +62,9 @@ cudaError_t launch_denoise(const double* sums, const double* m2, const uint32_t*
 cudaError_t launch_reproject(const ReprojectView& dv, const ReprojectView& sv, const ReprojectSource& s, const double* dnrm,
                              const double* ddepth, const double* dfrac, const rptb_reproject& prm, double* sums, double* m2,
                              uint32_t* counts, unsigned long long* reused, cudaStream_t stream);
+cudaError_t launch_reproject_part(const ReprojectView& dv, const ReprojectView& sv, const ReprojectSource& s, const FeaturePlanes& f,
+                                  double rays, uint32_t index, uint32_t count, uint64_t nelem, const rptb_reproject& prm, double* sums,
+                                  double* m2, uint32_t* counts, unsigned long long* reused, cudaStream_t stream);
 cudaError_t launch_buffer_min_count(const uint32_t* counts, uint64_t npix, uint32_t* out, cudaStream_t stream);
 int parse_obj_text(const char* text, size_t len, std::vector<double>& tris, std::string& err);
 struct ObjGroup {
@@ -914,8 +917,10 @@ struct ShardCamera {
     uint32_t state, _pad;  // CameraRecord::State
     rptb_camera cam;       // zero unless state is ONE
 };
+// ShardHeader::flags: the shard was reprojected (rptb_buffer_reproject_shard), so its pixels may hold 0 or 1 entries
+constexpr uint32_t kShardReprojected = 1u;
 struct ShardHeader {
-    uint32_t magic, with_features, width, height, shard_index, shard_count, entries, _pad;
+    uint32_t magic, with_features, width, height, shard_index, shard_count, entries, flags;
     uint64_t feature_rays;
     ShardCamera entry_cam, feat_cam;
 };
@@ -1885,18 +1890,20 @@ int rptb_buffer_denoise(rptb_buffer* b, const rptb_denoise* d, double* out_rgb, 
     return RPTB_OK;
 }
 
-int rptb_buffer_reproject(rptb_buffer* dst, rptb_buffer* src, const rptb_reproject* prm, uint64_t* out_reused) {
+// What a reprojection checks before it looks at the buffers: its arguments and parameters.
+static int check_reproject_params(const rptb_buffer* dst, const rptb_buffer* src, const rptb_reproject* prm) {
     if (!dst || !src || !prm) return fail(RPTB_ERR_BAD_ARG, "null argument");
     if (dst == src) return fail(RPTB_ERR_BAD_ARG, "src and dst are the same buffer");
     if (!(std::isfinite(prm->depth_tol) && prm->depth_tol >= 0.0))
         return fail(RPTB_ERR_BAD_ARG, "depth_tol must be finite and >= 0 (%g)", prm->depth_tol);
     if (!(prm->normal_cos >= -1.0 && prm->normal_cos <= 1.0)) return fail(RPTB_ERR_BAD_ARG, "normal_cos must lie in [-1, 1] (%g)", prm->normal_cos);
     if (prm->max_history < 2) return fail(RPTB_ERR_BAD_ARG, "max_history %u < 2 (a pixel's variance needs two entries)", prm->max_history);
-    if (dst->shard || src->shard) return refuse_shard("reproject");
-    std::scoped_lock both(dst->lock, src->lock);
-    bool same = dst->parts.size() == src->parts.size();
-    for (size_t i = 0; same && i < dst->parts.size(); i++) same = dst->parts[i].device == src->parts[i].device;
-    if (!same) return fail(RPTB_ERR_BAD_ARG, "the buffers were created on scenes with different device lists");
+    return RPTB_OK;
+}
+
+// What a reprojection checks of the buffers (both locked): dst has features and no entries, src has entries and
+// features made through one camera, and neither camera has an open aperture.
+static int check_reproject_buffers(const rptb_buffer* dst, const rptb_buffer* src) {
     if (dst->entries) return fail(RPTB_ERR_BAD_ARG, "dst already holds entries");
     if (dst->feature_rays == 0) return fail(RPTB_ERR_BAD_ARG, "dst holds no features (rptb_buffer_add_features)");
     if (src->entries == 0) return fail(RPTB_ERR_BAD_ARG, "src holds no entries");
@@ -1912,31 +1919,73 @@ int rptb_buffer_reproject(rptb_buffer* dst, rptb_buffer* src, const rptb_reproje
         return fail(RPTB_ERR_BAD_ARG, "src's entries and features were made through different cameras");
     if (src->feat_cam.cam.aperture > 0.0 || dst->feat_cam.cam.aperture > 0.0)
         return fail(RPTB_ERR_UNSUPPORTED, "an open aperture: depth of field blurs the first hits, no one point to reproject");
+    return RPTB_OK;
+}
+
+// src's state and resolved features, row-major on its parts[0]'s device (current), enqueued on that part's stream with
+// its `done` recorded behind them.
+static int reproject_source(rptb_buffer* src, ReprojectSource* out) {
+    BufferPart& s0 = src->parts[0];
+    const size_t snpix = (size_t)src->width * src->height;
+    const int rc = buffer_gather(src, COLOUR | FEATURES);
+    if (rc != RPTB_OK) return rc;
+    const Aov sa = buffer_aov(src);
+    CU(launch_features_resolve(feature_planes(src->rows.feat, snpix), snpix, (double)src->feature_rays, sa, s0.stream));
+    CU(cudaEventRecord(s0.done, s0.stream));
+    *out = {src->rows.sums, src->rows.m2, src->rows.counts, sa.normal, sa.depth, sa.frac};
+    return RPTB_OK;
+}
+
+// The reused-pixel counter and the least count of a reprojected buffer, on parts[0]'s device (current).
+static int reproject_scratch_alloc(rptb_buffer* dst) {
+    if (!dst->reused) CU(own(dst->mem, &dst->reused, sizeof(unsigned long long)));
+    if (!dst->min_count) CU(own(dst->mem, &dst->min_count, sizeof(uint32_t)));
+    return RPTB_OK;
+}
+
+// The state a reprojection leaves dst in, and its reused count (waited for on `stream`) when asked.
+static int reproject_finish(rptb_buffer* dst, const rptb_reproject* prm, uint64_t* out_reused, cudaStream_t stream) {
+    dst->entries = prm->max_history;
+    dst->reprojected = true;
+    dst->entry_cam = dst->feat_cam;
+    if (out_reused) {
+        unsigned long long n = 0;
+        CU(cudaMemcpyAsync(&n, dst->reused, sizeof(n), cudaMemcpyDeviceToHost, stream));
+        CU(cudaStreamSynchronize(stream));
+        *out_reused = n;
+    }
+    return RPTB_OK;
+}
+
+int rptb_buffer_reproject(rptb_buffer* dst, rptb_buffer* src, const rptb_reproject* prm, uint64_t* out_reused) {
+    int rc = check_reproject_params(dst, src, prm);
+    if (rc != RPTB_OK) return rc;
+    if (dst->shard || src->shard) return refuse_shard("reproject");
+    std::scoped_lock both(dst->lock, src->lock);
+    bool same = dst->parts.size() == src->parts.size();
+    for (size_t i = 0; same && i < dst->parts.size(); i++) same = dst->parts[i].device == src->parts[i].device;
+    if (!same) return fail(RPTB_ERR_BAD_ARG, "the buffers were created on scenes with different device lists");
+    rc = check_reproject_buffers(dst, src);
+    if (rc != RPTB_OK) return rc;
     BufferPart& d0 = dst->parts[0];
     BufferPart& s0 = src->parts[0];
     DeviceGuard g(d0.device);
     if (!g.ok) return fail(RPTB_ERR_CUDA, "cudaSetDevice(%d) failed", d0.device);
     // src's state and both buffers' features, row-major on parts[0]'s device
-    const size_t snpix = (size_t)src->width * src->height, dnpix = (size_t)dst->width * dst->height;
-    int rc = buffer_gather(src, COLOUR | FEATURES);
-    if (rc != RPTB_OK) return rc;
-    const Aov sa = buffer_aov(src);
-    CU(launch_features_resolve(feature_planes(src->rows.feat, snpix), snpix, (double)src->feature_rays, sa, s0.stream));
-    CU(cudaEventRecord(s0.done, s0.stream));
-    rc = buffer_rows_alloc(dst, COLOUR);
+    const size_t dnpix = (size_t)dst->width * dst->height;
+    ReprojectSource sp;
+    rc = reproject_source(src, &sp);
+    if (rc == RPTB_OK) rc = buffer_rows_alloc(dst, COLOUR);
     if (rc == RPTB_OK) rc = buffer_gather(dst, FEATURES);
     if (rc != RPTB_OK) return rc;
     const Aov da = buffer_aov(dst);
     CU(launch_features_resolve(feature_planes(dst->rows.feat, dnpix), dnpix, (double)dst->feature_rays, da, d0.stream));
-    if (!dst->reused) {
-        CU(own(dst->mem, &dst->reused, sizeof(unsigned long long)));
-        CU(own(dst->mem, &dst->min_count, sizeof(uint32_t)));
-    }
+    rc = reproject_scratch_alloc(dst);
+    if (rc != RPTB_OK) return rc;
     CU(cudaStreamWaitEvent(d0.stream, s0.done, 0));
     if (out_reused) CU(cudaMemsetAsync(dst->reused, 0, sizeof(unsigned long long), d0.stream));
     const ReprojectView dv = reproject_view(dst->feat_cam.cam, dst->width, dst->height);
     const ReprojectView sv = reproject_view(src->feat_cam.cam, src->width, src->height);
-    const ReprojectSource sp = {src->rows.sums, src->rows.m2, src->rows.counts, sa.normal, sa.depth, sa.frac};
     CU(launch_reproject(dv, sv, sp, da.normal, da.depth, da.frac, *prm, dst->rows.sums, dst->rows.m2, dst->rows.counts,
                         out_reused ? dst->reused : nullptr, d0.stream));
     // back to every dst part's compact tiles; every later call on either buffer is ordered behind this one
@@ -1944,16 +1993,44 @@ int rptb_buffer_reproject(rptb_buffer* dst, rptb_buffer* src, const rptb_reproje
     if (rc == RPTB_OK) rc = buffer_order_behind(dst, d0.stream);
     if (rc == RPTB_OK) rc = buffer_order_behind(src, d0.stream);
     if (rc != RPTB_OK) return rc;
-    dst->entries = prm->max_history;
-    dst->reprojected = true;
-    dst->entry_cam = dst->feat_cam;
-    if (out_reused) {
-        unsigned long long n = 0;
-        CU(cudaMemcpyAsync(&n, dst->reused, sizeof(n), cudaMemcpyDeviceToHost, d0.stream));
-        CU(cudaStreamSynchronize(d0.stream));
-        *out_reused = n;
+    return reproject_finish(dst, prm, out_reused, d0.stream);
+}
+
+int rptb_buffer_reproject_shard(rptb_buffer* dst, rptb_buffer* src, const rptb_reproject* prm, uint64_t* out_reused) {
+    int rc = check_reproject_params(dst, src, prm);
+    if (rc != RPTB_OK) return rc;
+    if (!dst->shard) return fail(RPTB_ERR_BAD_ARG, "dst is not a shard buffer (rptb_buffer_create_shard): a whole one reprojects with rptb_buffer_reproject");
+    if (src->shard) return refuse_shard("reproject");
+    std::scoped_lock both(dst->lock, src->lock);
+    BufferPart& d0 = dst->parts[0];
+    BufferPart& s0 = src->parts[0];
+    if (s0.device != d0.device) return fail(RPTB_ERR_BAD_ARG, "src's first device %d is not the shard's device %d", s0.device, d0.device);
+    rc = check_reproject_buffers(dst, src);
+    if (rc != RPTB_OK) return rc;
+    DeviceGuard g(d0.device);
+    if (!g.ok) return fail(RPTB_ERR_CUDA, "cudaSetDevice(%d) failed", d0.device);
+    rc = reproject_scratch_alloc(dst);
+    if (rc != RPTB_OK) return rc;
+    if (!d0.tiles) {  // no pixel to reproject: the state alone, so that the shard's exchange block agrees with the others'
+        if (out_reused) *out_reused = 0;
+        return reproject_finish(dst, prm, nullptr, d0.stream);
     }
-    return RPTB_OK;
+    ReprojectSource sp;
+    rc = reproject_source(src, &sp);
+    if (rc != RPTB_OK) return rc;
+    // the shard's own elements, in place in its compact planes; every later call on either buffer is ordered behind them
+    CU(cudaStreamWaitEvent(d0.stream, s0.done, 0));
+    CU(cudaStreamWaitEvent(d0.stream, d0.done, 0));
+    if (out_reused) CU(cudaMemsetAsync(dst->reused, 0, sizeof(unsigned long long), d0.stream));
+    const ReprojectView dv = reproject_view(dst->feat_cam.cam, dst->width, dst->height);
+    const ReprojectView sv = reproject_view(src->feat_cam.cam, src->width, src->height);
+    const Planes& q = d0.planes;
+    CU(launch_reproject_part(dv, sv, sp, feature_planes(q.feat, q.n), (double)dst->feature_rays, d0.index, d0.count, q.n, *prm, q.sums,
+                             q.m2, q.counts, out_reused ? dst->reused : nullptr, d0.stream));
+    rc = buffer_order_behind(dst, d0.stream);
+    if (rc == RPTB_OK) rc = buffer_order_behind(src, d0.stream);
+    if (rc != RPTB_OK) return rc;
+    return reproject_finish(dst, prm, out_reused, d0.stream);
 }
 
 uint64_t rptb_buffer_shard_bytes(const rptb_buffer* b, uint32_t with_features) {
@@ -1979,6 +2056,7 @@ int rptb_buffer_export_shard(rptb_buffer* b, void* dst_device, uint32_t with_fea
     h.shard_index = q.index;
     h.shard_count = q.count;
     h.entries = b->entries;
+    h.flags = b->reprojected ? kShardReprojected : 0u;
     h.feature_rays = b->feature_rays;
     h.entry_cam = shard_camera(b->entry_cam);
     h.feat_cam = shard_camera(b->feat_cam);
@@ -2018,6 +2096,7 @@ int rptb_buffer_import_shards(rptb_buffer* dst, const void* gathered_device, uin
     if (h0.shard_count != shard_count) return fail(RPTB_ERR_BAD_ARG, "the shards are %u but shard_count is %u", h0.shard_count, shard_count);
     if (h0.with_features != (with_features ? 1u : 0u))
         return fail(RPTB_ERR_BAD_ARG, "the shards were exported %s features", h0.with_features ? "with" : "without");
+    if (h0.flags & ~kShardReprojected) return fail(RPTB_ERR_BAD_ARG, "block 0 carries unknown flags 0x%x", h0.flags);
     if (shard_count > 1)
         CU(cudaMemcpy2DAsync(hs.data() + 1, sizeof(ShardHeader), in + l.bytes, l.bytes, sizeof(ShardHeader), shard_count - 1,
                              cudaMemcpyDeviceToHost, d0.stream));
@@ -2028,11 +2107,14 @@ int rptb_buffer_import_shards(rptb_buffer* dst, const void* gathered_device, uin
         if (h.shard_index != i) return fail(RPTB_ERR_BAD_ARG, "block %u holds shard %u: the shards must be in order 0..%u", i, h.shard_index, shard_count - 1);
         if (h.width != W || h.height != H || h.shard_count != shard_count || h.with_features != h0.with_features)
             return fail(RPTB_ERR_BAD_ARG, "block %u was exported from another image, shard count or feature choice", i);
-        if (h.entries != h0.entries || h.feature_rays != h0.feature_rays ||
+        if (h.entries != h0.entries || h.flags != h0.flags || h.feature_rays != h0.feature_rays ||
             std::memcmp(&h.entry_cam, &h0.entry_cam, sizeof(ShardCamera)) != 0 ||
             std::memcmp(&h.feat_cam, &h0.feat_cam, sizeof(ShardCamera)) != 0)
-            return fail(RPTB_ERR_BAD_ARG, "shard %u received other calls than shard 0 (entries %u / %u, feature rays %llu / %llu, or cameras)",
-                        i, h.entries, h0.entries, (unsigned long long)h.feature_rays, (unsigned long long)h0.feature_rays);
+            return fail(RPTB_ERR_BAD_ARG,
+                        "shard %u received other calls than shard 0 (entries %u / %u, reprojected %u / %u, feature rays %llu / %llu, or "
+                        "cameras)",
+                        i, h.entries, h0.entries, h.flags & kShardReprojected, h0.flags & kShardReprojected,
+                        (unsigned long long)h.feature_rays, (unsigned long long)h0.feature_rays);
     }
     // everything dst holds is overwritten: its earlier work finishes first
     for (BufferPart& q : dst->parts) CU(cudaStreamWaitEvent(d0.stream, q.done, 0));
@@ -2050,7 +2132,9 @@ int rptb_buffer_import_shards(rptb_buffer* dst, const void* gathered_device, uin
     }
     // every block row-major on dst's first device, then back into dst's own parts; every later call on dst is ordered
     // behind this one
+    const bool reprojected = (h0.flags & kShardReprojected) != 0;
     int rc = buffer_rows_alloc(dst, l.mask);
+    if (rc == RPTB_OK && reprojected) rc = reproject_scratch_alloc(dst);
     for (uint32_t i = 0; rc == RPTB_OK && i < shard_count; i++)
         rc = buffer_scatter(dst, shard_planes(l, in + (size_t)i * l.bytes), l.mask, i, shard_count);
     if (rc == RPTB_OK) rc = buffer_write_back(dst, l.mask);
@@ -2059,7 +2143,7 @@ int rptb_buffer_import_shards(rptb_buffer* dst, const void* gathered_device, uin
     // the caller may reuse the gathered bytes when the call returns
     CU(cudaStreamSynchronize(d0.stream));
     dst->entries = h0.entries;
-    dst->reprojected = false;
+    dst->reprojected = reprojected;
     dst->entry_cam = camera_record(h0.entry_cam);
     dst->feature_rays = with_features ? h0.feature_rays : 0;
     dst->feat_cam = with_features ? camera_record(h0.feat_cam) : CameraRecord();

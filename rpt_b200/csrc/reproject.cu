@@ -2,6 +2,9 @@
 // (reproject.h) over the gathered row-major state of both buffers on parts[0]'s device.  Compiled with -fmad=false:
 // reproject.h rounds every operation on its own, as its host emulation and tests/reproject_ref.py do.
 //
+// rptb_buffer_reproject_shard: one thread per element of a shard part's compact tiles runs reproject_slot against the
+// same gathered source and writes the part's colour planes in place -- no row-major destination, no write-back.
+//
 // Also the per-pixel minimum of a buffer's counts, which image / variance / denoise of a reprojected buffer check.
 #include <cuda_runtime.h>
 
@@ -28,6 +31,23 @@ __global__ void __launch_bounds__(256) reproject_kernel(const ReprojectView dv, 
     }
 }
 
+__global__ void __launch_bounds__(256) reproject_part_kernel(const ReprojectView dv, const ReprojectView sv, const ReprojectSource s,
+                                                             const FeaturePlanes f, double rays, uint32_t index, uint32_t count,
+                                                             uint64_t nelem, const rptb_reproject prm, double* __restrict__ sums,
+                                                             double* __restrict__ m2, uint32_t* __restrict__ counts,
+                                                             unsigned long long* __restrict__ reused) {
+    const uint64_t e = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    uint32_t n = 0;
+    if (e < nelem) {
+        n = reproject_slot(dv, sv, s, f, rays, index, count, e, prm, sums + 3 * e, m2 + e);
+        counts[e] = n;
+    }
+    if (reused) {  // every lane reaches the ballot: no early return above
+        const unsigned got = __ballot_sync(0xffffffffu, n > 0u);
+        if ((threadIdx.x & 31u) == 0u && got) atomicAdd(reused, (unsigned long long)__popc(got));
+    }
+}
+
 // *out = min(*out, counts[0..npix)); the caller sets *out to UINT32_MAX first.
 __global__ void __launch_bounds__(256) buffer_min_count_kernel(const uint32_t* __restrict__ counts, uint64_t npix, uint32_t* out) {
     uint32_t m = 0xFFFFFFFFu;
@@ -42,6 +62,15 @@ cudaError_t launch_reproject(const ReprojectView& dv, const ReprojectView& sv, c
                              uint32_t* counts, unsigned long long* reused, cudaStream_t stream) {
     const uint64_t npix = (uint64_t)dv.width * dv.height;
     reproject_kernel<<<(unsigned)((npix + 255) / 256), 256, 0, stream>>>(dv, sv, s, dnrm, ddepth, dfrac, prm, sums, m2, counts, reused);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_reproject_part(const ReprojectView& dv, const ReprojectView& sv, const ReprojectSource& s, const FeaturePlanes& f,
+                                  double rays, uint32_t index, uint32_t count, uint64_t nelem, const rptb_reproject& prm, double* sums,
+                                  double* m2, uint32_t* counts, unsigned long long* reused, cudaStream_t stream) {
+    if (nelem == 0) return cudaSuccess;
+    reproject_part_kernel<<<(unsigned)((nelem + 255) / 256), 256, 0, stream>>>(dv, sv, s, f, rays, index, count, nelem, prm, sums, m2,
+                                                                               counts, reused);
     return cudaGetLastError();
 }
 

@@ -29,10 +29,17 @@
 //     mu_c = sum w^_q * (S_qc / n_q),   s2 = sum w^_q * (M2_q / (n_q - 1)),   n_h = min(max_history, min over valid q of n_q)
 // and the pixel gets sums mu_c * n_h, M2 s2 * (n_h - 1) and count n_h: the mean and the per-entry variance of its
 // neighbourhood, carried as if n_h entries had made them.
+//
+// A shard buffer (rptb_buffer_reproject_shard) runs the same function per element of its compact tiles (reproject_slot):
+// the element's pixel is tile_pixel's, its features resolve from the element's own feature sums (features_resolve,
+// denoise.h), and the source is whole and row-major as above.  So every pixel gets the bits the whole buffer's gets.
 #pragma once
 #include <cmath>
 
 #include "../../include/rpt_b200.h"
+#include "denoise.h"
+#include "planes.h"
+#include "tile.h"
 #include "vec.cuh"
 
 namespace rptb {
@@ -173,6 +180,26 @@ RPTB_HD uint32_t reproject_pixel(const ReprojectView& dv, const ReprojectView& s
     out_sums[2] = mu2 * dh;
     *out_m2 = s2 * (double)(nh - 1u);
     return nh;
+}
+
+// The history of element `slot` of the compact tiles of shard `index` of `count` of view dv: its pixel is
+// tile_pixel(dv.width, dv.height, index + (slot / 128) * count, slot % 128), and its features resolve from the element's
+// sums in f (the part's feature planes) over `rays` camera rays.  Writes out_sums[3] and *out_m2, returns the count; an
+// element past a ragged edge gets sums 0, M2 0 and count 0.
+RPTB_HD uint32_t reproject_slot(const ReprojectView& dv, const ReprojectView& sv, const ReprojectSource& s, const FeaturePlanes& f,
+                                double rays, uint32_t index, uint32_t count, uint64_t slot, const rptb_reproject& prm,
+                                double* out_sums, double* out_m2) {
+    const int64_t p = tile_pixel(dv.width, dv.height, index + (uint32_t)(slot >> 7) * count, (uint32_t)(slot & 127u));
+    if (p < 0) {
+        out_sums[0] = 0.0;
+        out_sums[1] = 0.0;
+        out_sums[2] = 0.0;
+        *out_m2 = 0.0;
+        return 0u;
+    }
+    double N[3], z, a[3], fp;
+    features_resolve(f.h[slot], f.n + 3 * slot, f.z[slot], f.a + 3 * slot, rays, N, &z, a, &fp);
+    return reproject_pixel(dv, sv, s, (uint32_t)(p % dv.width), (uint32_t)(p / dv.width), N, z, fp, prm, out_sums, out_m2);
 }
 
 }  // namespace rptb

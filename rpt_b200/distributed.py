@@ -21,6 +21,11 @@ features into its own tiles with no exchange, and `ShardBuffer.gather` -- one al
 -- gives every rank an ordinary whole DeviceBuffer, the same bits for any world size.  `render_iterative_distributed`
 is Renderer.iterative_render over a ShardBuffer; with adaptive sampling it adds one collective per batch, an
 all-reduce of the ranks' active pixel counts that ends the loop.  Nothing else is exchanged.
+
+`render_frames_distributed` is Renderer.render_frames over ShardBuffers.  A reprojected pixel needs only its own
+features and the whole previous frame, which every rank already holds: the frame's gather, with features, gave it.  So
+each rank reprojects that gathered buffer into its own shard (ShardBuffer.reproject_from), and a frame costs one
+all-gather, the one that makes its image.
 """
 from __future__ import annotations
 
@@ -186,9 +191,10 @@ def _rank_world(group=None):
 class ShardBuffer(api.DeviceBuffer):
     """A DeviceBuffer holding one rank's shard of the image (rptb_buffer_create_shard): the 16x8 tiles t with
     t % world == rank, on the scene's one device.  Renderer.sample and Renderer.sample_features render and add only
-    those tiles, with no exchange; an adaptive sample() returns this rank's active pixel count.  Whole-image reads
-    (image, variance, sums, pixel_stats, counts, features, denoise, reproject_from, add_samples) are refused: gather()
-    first.  `entries` counts the calls (a bound on any pixel's count) until the gather reads the counts."""
+    those tiles, with no exchange; an adaptive sample() returns this rank's active pixel count, and reproject_from
+    takes this rank's pixels' history from a whole buffer.  Whole-image reads (image, variance, sums, pixel_stats,
+    counts, features, denoise, add_samples) are refused: gather() first.  `entries` counts the calls (a bound on any
+    pixel's count) until the gather reads the counts."""
 
     def __init__(self, scene: "api.DeviceScene", width: int, height: int, filter: Optional["api.Filter"] = None, group=None,
                  rank: Optional[int] = None, world: Optional[int] = None):
@@ -219,6 +225,20 @@ class ShardBuffer(api.DeviceBuffer):
             stream = torch.cuda.current_stream(out.device).cuda_stream
         capi.check(capi.lib().rptb_buffer_export_shard(self.handle, C.c_void_p(out.data_ptr()), 1 if with_features else 0,
                                                        C.c_void_p(stream or 1)), "rptb_buffer_export_shard")
+
+    def reproject_from(self, src: "api.DeviceBuffer", params: Optional["api.Reproject"] = None) -> int:
+        """DeviceBuffer.reproject_from into this shard (rptb_buffer_reproject_shard): this rank's pixels take their history
+        from `src`, a whole DeviceBuffer on this rank's device -- typically the previous frame's shards gathered with
+        features, prev.gather(with_features=True).  Every pixel gets the bits a whole buffer's reprojection gives it.
+        Returns this rank's reused pixels; summed over the ranks, they are the whole call's."""
+        if isinstance(src, ShardBuffer):
+            raise TypeError("src is a ShardBuffer: gather() the shards into a whole buffer first")
+        c = (params or api.Reproject()).to_c()
+        n = C.c_uint64(0)
+        capi.check(capi.lib().rptb_buffer_reproject_shard(self.handle, src.handle, C.byref(c), C.byref(n)),
+                   "rptb_buffer_reproject_shard")
+        self.entries = int(c.max_history)  # the bound a reprojected pixel's count keeps
+        return int(n.value)
 
     def gather(self, group=None, with_features: bool = False) -> "api.DeviceBuffer":
         """All ranks call this: export every shard's block, one all_gather_into_tensor, and import the blocks into a new
@@ -287,3 +307,40 @@ def render_iterative_distributed(renderer, callback_interval: int, callback: Cal
                 break
         callback(iteration, buffer)
     return buffer
+
+
+def render_frames_distributed(renderer, cameras, entries: int = 8, feature_samples: int = 16,
+                              reproject: Optional["api.Reproject"] = api.Reproject(), adaptive: Optional["api.Adaptive"] = None,
+                              denoise: Optional["api.Denoise"] = None, group=None):
+    """All ranks call this: Renderer.render_frames over one ShardBuffer per frame, yielding each frame's (height, width,
+    3) uint8 on every rank -- the bytes of render_frames on one whole buffer, for any world size.  Per frame: this
+    rank's shard gets `feature_samples` feature rays through the frame's camera, the previous frame's gathered buffer is
+    reprojected into it (unless `reproject` is None), and `entries` plain or adaptive entries are added, continuing
+    the renderer's sample streams; then one gather (with features when `reproject` or `denoise` needs them) makes the
+    whole buffer the frame's image() or denoised_image(denoise) comes from, and which the next frame reprojects.  That
+    gather is the frame's only collective."""
+    renderer._check_frames(entries, adaptive, denoise)
+    with_features = reproject is not None or denoise is not None
+    own, prev = renderer.camera, None
+    try:
+        for cam in cameras:
+            renderer.camera = cam
+            buf = ShardBuffer(renderer.device_scene(), renderer._width, renderer._height, renderer._filter, group=group)
+            try:
+                renderer.sample_features(feature_samples, buf)
+                if prev is not None and reproject is not None:
+                    buf.reproject_from(prev, reproject)
+                for _ in range(entries):
+                    renderer.sample(renderer._num_samples // entries, buf, want_stats=False, adaptive=adaptive)
+                whole = buf.gather(group, with_features)
+            finally:
+                buf.close()
+            img = whole.image() if denoise is None else whole.denoised_image(denoise)
+            if prev is not None:
+                prev.close()
+            prev = whole
+            yield img
+    finally:
+        renderer.camera = own
+        if prev is not None:
+            prev.close()

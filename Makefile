@@ -82,7 +82,8 @@ HOSTEMU_DENOISE := tests/hostemu/_build/libhostemu_denoise.so
 # the same emulation plus the renders given no counters (the packed-table F_NOCOUNT twins; tests/hostemu/hostemu_slim.cu)
 HOSTEMU_SLIM := tests/hostemu/_build/libhostemu_slim.so
 # the denoiser's emulation plus the reprojection's per-pixel function (reproject.h; tests/hostemu/hostemu_reproject.cu) and
-# its per-element form for a shard's compact tiles (tests/hostemu/hostemu_reproject_part.cu)
+# its per-element form for a shard's compact tiles (tests/hostemu/hostemu_reproject_part.cu), and the history test of
+# the merge, per pixel and per element (tests/hostemu/hostemu_reproject_merge.cu)
 HOSTEMU_REPROJECT := tests/hostemu/_build/libhostemu_reproject.so
 hostemu: $(HOSTEMU) $(HOSTEMU_LIST) $(HOSTEMU_DENOISE) $(HOSTEMU_SLIM) $(HOSTEMU_REPROJECT)
 $(HOSTEMU): tests/hostemu/hostemu.cu $(CSRC)/kdbuild.cpp $(CSRC)/bvhbuild.cpp $(HDRS)
@@ -97,9 +98,9 @@ $(HOSTEMU_DENOISE): tests/hostemu/hostemu_denoise.cu tests/hostemu/hostemu.cu $(
 $(HOSTEMU_SLIM): tests/hostemu/hostemu_slim.cu tests/hostemu/hostemu.cu $(CSRC)/kdbuild.cpp $(CSRC)/bvhbuild.cpp $(HDRS)
 	@mkdir -p $(dir $@)
 	nvcc -std=c++17 -O2 -DRPTB_HOST_EMU -DRPTB_BUILD_BVH8=1 -DRPTB_BUILD_BVH4=1 -gencode arch=compute_90a,code=sm_90a -Xcompiler -fPIC,-fopenmp,-ffp-contract=off -shared -Xlinker -Bsymbolic -o $@ tests/hostemu/hostemu_slim.cu $(CSRC)/kdbuild.cpp $(CSRC)/bvhbuild.cpp -lgomp
-$(HOSTEMU_REPROJECT): tests/hostemu/hostemu_reproject.cu tests/hostemu/hostemu_reproject_part.cu tests/hostemu/hostemu_denoise.cu tests/hostemu/hostemu.cu $(CSRC)/kdbuild.cpp $(CSRC)/bvhbuild.cpp $(HDRS)
+$(HOSTEMU_REPROJECT): tests/hostemu/hostemu_reproject.cu tests/hostemu/hostemu_reproject_part.cu tests/hostemu/hostemu_reproject_merge.cu tests/hostemu/hostemu_denoise.cu tests/hostemu/hostemu.cu $(CSRC)/kdbuild.cpp $(CSRC)/bvhbuild.cpp $(HDRS)
 	@mkdir -p $(dir $@)
-	nvcc -std=c++17 -O2 -DRPTB_HOST_EMU -DRPTB_BUILD_BVH8=1 -DRPTB_BUILD_BVH4=1 -gencode arch=compute_90a,code=sm_90a -Xcompiler -fPIC,-fopenmp,-ffp-contract=off -shared -Xlinker -Bsymbolic -o $@ tests/hostemu/hostemu_reproject.cu tests/hostemu/hostemu_reproject_part.cu $(CSRC)/kdbuild.cpp $(CSRC)/bvhbuild.cpp -lgomp
+	nvcc -std=c++17 -O2 -DRPTB_HOST_EMU -DRPTB_BUILD_BVH8=1 -DRPTB_BUILD_BVH4=1 -gencode arch=compute_90a,code=sm_90a -Xcompiler -fPIC,-fopenmp,-ffp-contract=off -shared -Xlinker -Bsymbolic -o $@ tests/hostemu/hostemu_reproject.cu tests/hostemu/hostemu_reproject_part.cu tests/hostemu/hostemu_reproject_merge.cu $(CSRC)/kdbuild.cpp $(CSRC)/bvhbuild.cpp -lgomp
 
 clean:
 	rm -rf build $(LIB) $(ORACLE) tests/hostemu/_build

@@ -19,6 +19,7 @@
 #include <sstream>
 #include <stdexcept>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "rpt_b200.h"
@@ -337,6 +338,13 @@ public:
         uint64_t n = 0;
         check(rptb_buffer_reproject(handle_, src.handle_, &params, &n));
         return n;
+    }
+    // Tests src's reprojected history against this buffer's own fresh entries (>= 2 calls through its feature camera)
+    // and merges it where they agree (rptb_buffer_reproject_merge).  Returns {reused, rejected} pixel counts.
+    std::pair<uint64_t, uint64_t> merge_history_from(const DeviceBuffer& src, const rptb_reproject& params, double gamma) {
+        uint64_t reused = 0, rejected = 0;
+        check(rptb_buffer_reproject_merge(handle_, src.handle_, &params, gamma, &reused, &rejected));
+        return {reused, rejected};
     }
     rptb_buffer* handle() const { return handle_; }
 

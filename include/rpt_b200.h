@@ -573,6 +573,32 @@ int rptb_buffer_import_shards(rptb_buffer* dst, const void* gathered_device, uin
 int rptb_buffer_reproject_shard(rptb_buffer* dst, rptb_buffer* src, const rptb_reproject* params,
                                 uint64_t* out_reused /* nullable, forces sync: this shard's pixels that got history */);
 
+/* ---- Testing reprojected history against fresh entries ----------------------------------------------------
+ * rptb_buffer_reproject writes history into an empty buffer, and nothing checks that the new view agrees with it:
+ * stale history (a view-dependent highlight, glass) looks converged to the adaptive criterion and to the denoiser.
+ * rptb_buffer_reproject_merge instead takes a dst that already holds >= 2 fresh entry calls through its own feature
+ * camera, and tests each pixel's history (the one rptb_buffer_reproject would give it) against that pixel's own fresh
+ * mean and variance: with delta the difference of the two means, d2 = |delta|^2 and v the channel-summed variance of
+ * that difference, history with d2 > gamma^2 v is rejected and the pixel keeps its bits; agreeing history is merged
+ * by the parallel (Chan) combination, whose between-means term d2 n_f n_h / n goes into M2.  gamma = +inf accepts
+ * every history, gamma = 0 rejects any whose mean differs.  rpt_b200/csrc/reproject.h gives every formula.  A pixel
+ * with no history is left as it is and counted in neither total; out_reused + out_rejected is what out_reused of
+ * rptb_buffer_reproject into a fresh buffer with the same features counts.
+ *
+ * The checks and refusals are rptb_buffer_reproject's for src, the parameters and the device lists; for dst,
+ * RPTB_ERR_BAD_ARG: fewer than 2 entry calls, already reprojected, or entries whose camera is not exactly its feature
+ * camera (or mixed or unknown); gamma NaN or negative.  Afterwards dst is reprojected, its entry count is its fresh
+ * calls plus max_history (a bound), and its entry camera is unchanged, so the next frame can reproject from it.  */
+int rptb_buffer_reproject_merge(rptb_buffer* dst, rptb_buffer* src, const rptb_reproject* params, double gamma,
+                                uint64_t* out_reused /* nullable, forces sync: pixels whose history was merged */,
+                                uint64_t* out_rejected /* nullable, forces sync: pixels whose history was rejected */);
+/* rptb_buffer_reproject_merge into a shard buffer, in place in its own tiles: what rptb_buffer_reproject_shard is to
+ * rptb_buffer_reproject, with its extra refusals.  The counts are this shard's pixels; summed over the shards, the
+ * whole call's.  A shard that owns no tile does no device work and takes the same state.                         */
+int rptb_buffer_reproject_merge_shard(rptb_buffer* dst, rptb_buffer* src, const rptb_reproject* params, double gamma,
+                                      uint64_t* out_reused /* nullable, forces sync */,
+                                      uint64_t* out_rejected /* nullable, forces sync */);
+
 #ifdef __cplusplus
 }
 #endif

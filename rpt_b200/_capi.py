@@ -286,6 +286,10 @@ SYMBOLS = [
     ("rptb_buffer_export_shard", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p]),
     ("rptb_buffer_import_shards", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32]),
     ("rptb_buffer_reproject_shard", C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(Reproject), C.POINTER(C.c_uint64)]),
+    ("rptb_buffer_reproject_merge", C.c_int,
+     [C.c_void_p, C.c_void_p, C.POINTER(Reproject), C.c_double, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
+    ("rptb_buffer_reproject_merge_shard", C.c_int,
+     [C.c_void_p, C.c_void_p, C.POINTER(Reproject), C.c_double, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
 ]
 
 _lib = None

@@ -893,6 +893,20 @@ class Reproject:
         return capi.Reproject(self.depth_tol, self.normal_cos, self.max_history, 0)
 
 
+class HistoryTest:
+    """Testing reprojected history against fresh entries (DeviceBuffer.merge_history_from, rptb_buffer_reproject_merge;
+    render_frames(history_test=...)).  A frame first renders `fresh_entries` plain entries (>= 2: a mean and a
+    variance per pixel), then each pixel's history is merged in only where it agrees with them: it is rejected when
+    the squared distance of the two means exceeds gamma^2 times the variance of their difference.  gamma = inf accepts
+    every history, 0 rejects any that differs.  Default gamma 4: of tools/reproject_measure.py's sweep over gamma in
+    {2, 3, 4, 6} on 16-frame orbits of the sphere, Cornell, the teapot and glass at 4 and 16 fresh spp, it gives the best
+    geometric mean of the denoised gains over fresh frames (DESIGN.md section 6c).  rpt_b200/csrc/reproject.h gives
+    every formula."""
+
+    def __init__(self, gamma: float = 4.0, fresh_entries: int = 2):
+        self.gamma, self.fresh_entries = float(gamma), int(fresh_entries)
+
+
 class Buffer:
     """src/buffer.rs:6-93.  Holds one equally weighted entry per pixel per
     `add_samples` call, like the reference's Vec<Vec<Color>>."""
@@ -1034,6 +1048,21 @@ class DeviceBuffer:
         capi.check(capi.lib().rptb_buffer_reproject(self.handle, src.handle, C.byref(c), C.byref(n)), "rptb_buffer_reproject")
         self.entries = int(self.counts().max())
         return int(n.value)
+
+    def merge_history_from(self, src: "DeviceBuffer", reproject: Optional[Reproject] = None,
+                           test: Optional[HistoryTest] = None) -> tuple:
+        """Tests the history reproject_from would carry from `src` against this buffer's own fresh entries, and merges it
+        only where they agree (rptb_buffer_reproject_merge).  This buffer must hold features and >= 2 entry calls, all
+        through its feature camera, and must not be reprojected; `src` as for reproject_from.  A merged pixel holds both
+        groups' entries, and the gap between their means goes into its variance; a rejected one keeps its fresh entries
+        only.  Returns (reused, rejected) pixel counts; pixels with no history are in neither."""
+        c = (reproject or Reproject()).to_c()
+        gamma = (test or HistoryTest()).gamma
+        n, j = C.c_uint64(0), C.c_uint64(0)
+        capi.check(capi.lib().rptb_buffer_reproject_merge(self.handle, src.handle, C.byref(c), gamma, C.byref(n), C.byref(j)),
+                   "rptb_buffer_reproject_merge")
+        self.entries = int(self.counts().max())
+        return int(n.value), int(j.value)
 
     def close(self) -> None:
         if self.handle:
@@ -1232,31 +1261,55 @@ class Renderer:
             self.sample_features(feature_samples, buf)
             return buf.denoised_image(denoise)
 
-    def _check_frames(self, entries: int, adaptive: Optional[Adaptive], denoise: Optional[Denoise]) -> None:
+    def _check_frames(self, entries: int, adaptive: Optional[Adaptive], denoise: Optional[Denoise],
+                      reproject: Optional[Reproject] = None, history_test: Optional[HistoryTest] = None) -> None:
         """The arguments render_frames and distributed.render_frames_distributed refuse."""
         if entries < 1 or self._num_samples % entries:
             raise ValueError(f"num_samples {self._num_samples} must be a multiple of entries {entries} (and entries >= 1)")
         if denoise is not None and entries < 2 and adaptive is None:
             raise ValueError("a denoised frame needs entries >= 2 (or adaptive entries)")
+        if history_test is not None:
+            if history_test.fresh_entries < 2 or history_test.fresh_entries > entries:
+                raise ValueError(f"history_test.fresh_entries {history_test.fresh_entries} must lie in [2, entries {entries}]")
+            if reproject is None:
+                raise ValueError("history_test tests reprojected history: it needs reproject")
+
+    def _frame_entries(self, buf: DeviceBuffer, prev: Optional[DeviceBuffer], entries: int, reproject: Optional[Reproject],
+                       adaptive: Optional[Adaptive], history_test: Optional[HistoryTest]) -> None:
+        """A frame's entries after its feature pass, for render_frames and distributed.render_frames_distributed: the
+        previous frame's history reprojected, then `entries` entries -- or, with `history_test`, its fresh_entries plain
+        entries first, the history merged where they agree with it, then the other entries."""
+        n, fresh = self._num_samples // entries, 0
+        if history_test is not None:
+            fresh = history_test.fresh_entries
+            for _ in range(fresh):
+                self.sample(n, buf, want_stats=False)
+            if prev is not None:
+                buf.merge_history_from(prev, reproject, history_test)
+        elif prev is not None and reproject is not None:
+            buf.reproject_from(prev, reproject)
+        for _ in range(entries - fresh):
+            self.sample(n, buf, want_stats=False, adaptive=adaptive)
 
     def render_frames(self, cameras, entries: int = 8, feature_samples: int = 16, reproject: Optional[Reproject] = Reproject(),
-                      adaptive: Optional[Adaptive] = None, denoise: Optional[Denoise] = None):
+                      adaptive: Optional[Adaptive] = None, denoise: Optional[Denoise] = None,
+                      history_test: Optional[HistoryTest] = None):
         """Renders one frame per camera of a static scene and yields each as (height, width, 3) uint8.  Per frame: a new
         DeviceBuffer gets `feature_samples` feature rays through the frame's camera, the previous frame's buffer is
         reprojected into it (unless `reproject` is None), and `entries` entries of num_samples / entries samples each are
         added -- adaptive ones with `adaptive` -- continuing the renderer's sample streams; the frame is image(), or
-        denoised_image(denoise).  The device scene is uploaded once for all frames."""
-        self._check_frames(entries, adaptive, denoise)
+        denoised_image(denoise).  The device scene is uploaded once for all frames.
+        With `history_test` (which needs `reproject`), a frame renders history_test.fresh_entries plain entries before
+        it takes the previous frame's history, merges that history only where it agrees with them
+        (DeviceBuffer.merge_history_from), and then adds the other entries."""
+        self._check_frames(entries, adaptive, denoise, reproject, history_test)
         own, prev = self.camera, None
         try:
             for cam in cameras:
                 self.camera = cam
                 buf = self.device_buffer()
                 self.sample_features(feature_samples, buf)
-                if prev is not None and reproject is not None:
-                    buf.reproject_from(prev, reproject)
-                for _ in range(entries):
-                    self.sample(self._num_samples // entries, buf, want_stats=False, adaptive=adaptive)
+                self._frame_entries(buf, prev, entries, reproject, adaptive, history_test)
                 img = buf.image() if denoise is None else buf.denoised_image(denoise)
                 if prev is not None:
                     prev.close()

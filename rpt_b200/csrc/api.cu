@@ -65,6 +65,13 @@ cudaError_t launch_reproject(const ReprojectView& dv, const ReprojectView& sv, c
 cudaError_t launch_reproject_part(const ReprojectView& dv, const ReprojectView& sv, const ReprojectSource& s, const FeaturePlanes& f,
                                   double rays, uint32_t index, uint32_t count, uint64_t nelem, const rptb_reproject& prm, double* sums,
                                   double* m2, uint32_t* counts, unsigned long long* reused, cudaStream_t stream);
+cudaError_t launch_reproject_merge(const ReprojectView& dv, const ReprojectView& sv, const ReprojectSource& s, const double* dnrm,
+                                   const double* ddepth, const double* dfrac, const rptb_reproject& prm, double gamma, double* sums,
+                                   double* m2, uint32_t* counts, unsigned long long* tally, cudaStream_t stream);
+cudaError_t launch_reproject_merge_part(const ReprojectView& dv, const ReprojectView& sv, const ReprojectSource& s,
+                                        const FeaturePlanes& f, double rays, uint32_t index, uint32_t count, uint64_t nelem,
+                                        const rptb_reproject& prm, double gamma, double* sums, double* m2, uint32_t* counts,
+                                        unsigned long long* tally, cudaStream_t stream);
 cudaError_t launch_buffer_min_count(const uint32_t* counts, uint64_t npix, uint32_t* out, cudaStream_t stream);
 int parse_obj_text(const char* text, size_t len, std::vector<double>& tris, std::string& err);
 struct ObjGroup {
@@ -1901,10 +1908,10 @@ static int check_reproject_params(const rptb_buffer* dst, const rptb_buffer* src
     return RPTB_OK;
 }
 
-// What a reprojection checks of the buffers (both locked): dst has features and no entries, src has entries and
-// features made through one camera, and neither camera has an open aperture.
-static int check_reproject_buffers(const rptb_buffer* dst, const rptb_buffer* src) {
-    if (dst->entries) return fail(RPTB_ERR_BAD_ARG, "dst already holds entries");
+// What a reprojection checks of the buffers (both locked): dst has features and no entries (a merge's dst: see
+// check_merge_dst instead), src has entries and features made through one camera, and neither camera has an open aperture.
+static int check_reproject_buffers(const rptb_buffer* dst, const rptb_buffer* src, bool merge) {
+    if (!merge && dst->entries) return fail(RPTB_ERR_BAD_ARG, "dst already holds entries");
     if (dst->feature_rays == 0) return fail(RPTB_ERR_BAD_ARG, "dst holds no features (rptb_buffer_add_features)");
     if (src->entries == 0) return fail(RPTB_ERR_BAD_ARG, "src holds no entries");
     if (src->feature_rays == 0) return fail(RPTB_ERR_BAD_ARG, "src holds no features (rptb_buffer_add_features)");
@@ -1922,6 +1929,22 @@ static int check_reproject_buffers(const rptb_buffer* dst, const rptb_buffer* sr
     return RPTB_OK;
 }
 
+// What a merge checks of dst (locked) after check_reproject_buffers: fresh entries of its own view to test the history
+// against -- at least 2 calls, so that every pixel of a never-reprojected buffer holds n_f >= 2 (rptb_buffer_denoise),
+// none of them reprojected, all through dst's feature camera -- and room for the history's count.
+static int check_merge_dst(const rptb_buffer* dst, const rptb_reproject* prm) {
+    if (dst->entries < 2)
+        return fail(RPTB_ERR_BAD_ARG, "dst holds %u entry calls: testing history needs >= 2 fresh ones (a mean and a variance)", dst->entries);
+    if (dst->reprojected) return fail(RPTB_ERR_BAD_ARG, "dst is already reprojected: its entries are not all fresh");
+    const char* why[] = {"none", "one", "mixed (several cameras)", "unknown (a host entry)"};
+    if (dst->entry_cam.state != CameraRecord::ONE)
+        return fail(RPTB_ERR_BAD_ARG, "dst's entries have no single camera: %s", why[dst->entry_cam.state]);
+    if (std::memcmp(&dst->entry_cam.cam, &dst->feat_cam.cam, sizeof(rptb_camera)) != 0)
+        return fail(RPTB_ERR_BAD_ARG, "dst's entries and features were made through different cameras");
+    if (dst->entries > UINT32_MAX - prm->max_history) return fail(RPTB_ERR_UNSUPPORTED, "too many entries");
+    return RPTB_OK;
+}
+
 // src's state and resolved features, row-major on its parts[0]'s device (current), enqueued on that part's stream with
 // its `done` recorded behind them.
 static int reproject_source(rptb_buffer* src, ReprojectSource* out) {
@@ -1936,76 +1959,95 @@ static int reproject_source(rptb_buffer* src, ReprojectSource* out) {
     return RPTB_OK;
 }
 
-// The reused-pixel counter and the least count of a reprojected buffer, on parts[0]'s device (current).
+// The counters (reused pixels, then a merge's rejected ones) and the least count of a reprojected buffer, on parts[0]'s
+// device (current).
 static int reproject_scratch_alloc(rptb_buffer* dst) {
-    if (!dst->reused) CU(own(dst->mem, &dst->reused, sizeof(unsigned long long)));
+    if (!dst->reused) CU(own(dst->mem, &dst->reused, 2 * sizeof(unsigned long long)));
     if (!dst->min_count) CU(own(dst->mem, &dst->min_count, sizeof(uint32_t)));
     return RPTB_OK;
 }
 
-// The state a reprojection leaves dst in, and its reused count (waited for on `stream`) when asked.
-static int reproject_finish(rptb_buffer* dst, const rptb_reproject* prm, uint64_t* out_reused, cudaStream_t stream) {
-    dst->entries = prm->max_history;
+// The state a reprojection leaves dst in, and its counts (waited for on `stream`) when asked: a reprojection's entries
+// are max_history, a merge adds max_history to the fresh ones (both bounds); dst's entries now belong to its feature camera.
+static int reproject_finish(rptb_buffer* dst, const rptb_reproject* prm, bool merge, uint64_t* out_reused, uint64_t* out_rejected,
+                            cudaStream_t stream) {
+    dst->entries = merge ? dst->entries + prm->max_history : prm->max_history;
     dst->reprojected = true;
     dst->entry_cam = dst->feat_cam;
-    if (out_reused) {
-        unsigned long long n = 0;
-        CU(cudaMemcpyAsync(&n, dst->reused, sizeof(n), cudaMemcpyDeviceToHost, stream));
+    if (out_reused || out_rejected) {
+        unsigned long long n[2] = {0, 0};
+        CU(cudaMemcpyAsync(n, dst->reused, (merge ? 2 : 1) * sizeof(unsigned long long), cudaMemcpyDeviceToHost, stream));
         CU(cudaStreamSynchronize(stream));
-        *out_reused = n;
+        if (out_reused) *out_reused = n[0];
+        if (out_rejected) *out_rejected = n[1];
     }
     return RPTB_OK;
 }
 
-int rptb_buffer_reproject(rptb_buffer* dst, rptb_buffer* src, const rptb_reproject* prm, uint64_t* out_reused) {
+// rptb_buffer_reproject (gamma null) and rptb_buffer_reproject_merge (*gamma the test's threshold).
+static int reproject_whole(rptb_buffer* dst, rptb_buffer* src, const rptb_reproject* prm, const double* gamma, uint64_t* out_reused,
+                           uint64_t* out_rejected) {
     int rc = check_reproject_params(dst, src, prm);
     if (rc != RPTB_OK) return rc;
-    if (dst->shard || src->shard) return refuse_shard("reproject");
+    if (gamma && !(*gamma >= 0.0)) return fail(RPTB_ERR_BAD_ARG, "gamma must be >= 0 (%g)", *gamma);
+    if (dst->shard || src->shard) return refuse_shard(gamma ? "reproject_merge" : "reproject");
     std::scoped_lock both(dst->lock, src->lock);
     bool same = dst->parts.size() == src->parts.size();
     for (size_t i = 0; same && i < dst->parts.size(); i++) same = dst->parts[i].device == src->parts[i].device;
     if (!same) return fail(RPTB_ERR_BAD_ARG, "the buffers were created on scenes with different device lists");
-    rc = check_reproject_buffers(dst, src);
+    rc = check_reproject_buffers(dst, src, gamma != nullptr);
+    if (rc == RPTB_OK && gamma) rc = check_merge_dst(dst, prm);
     if (rc != RPTB_OK) return rc;
     BufferPart& d0 = dst->parts[0];
     BufferPart& s0 = src->parts[0];
     DeviceGuard g(d0.device);
     if (!g.ok) return fail(RPTB_ERR_CUDA, "cudaSetDevice(%d) failed", d0.device);
-    // src's state and both buffers' features, row-major on parts[0]'s device
+    // src's state and both buffers' features (and a merge's fresh dst state), row-major on parts[0]'s device
     const size_t dnpix = (size_t)dst->width * dst->height;
+    const bool count = out_reused || out_rejected;
     ReprojectSource sp;
     rc = reproject_source(src, &sp);
     if (rc == RPTB_OK) rc = buffer_rows_alloc(dst, COLOUR);
-    if (rc == RPTB_OK) rc = buffer_gather(dst, FEATURES);
+    if (rc == RPTB_OK) rc = buffer_gather(dst, gamma ? COLOUR | FEATURES : FEATURES);
     if (rc != RPTB_OK) return rc;
     const Aov da = buffer_aov(dst);
     CU(launch_features_resolve(feature_planes(dst->rows.feat, dnpix), dnpix, (double)dst->feature_rays, da, d0.stream));
     rc = reproject_scratch_alloc(dst);
     if (rc != RPTB_OK) return rc;
     CU(cudaStreamWaitEvent(d0.stream, s0.done, 0));
-    if (out_reused) CU(cudaMemsetAsync(dst->reused, 0, sizeof(unsigned long long), d0.stream));
+    if (count) CU(cudaMemsetAsync(dst->reused, 0, (gamma ? 2 : 1) * sizeof(unsigned long long), d0.stream));
     const ReprojectView dv = reproject_view(dst->feat_cam.cam, dst->width, dst->height);
     const ReprojectView sv = reproject_view(src->feat_cam.cam, src->width, src->height);
-    CU(launch_reproject(dv, sv, sp, da.normal, da.depth, da.frac, *prm, dst->rows.sums, dst->rows.m2, dst->rows.counts,
-                        out_reused ? dst->reused : nullptr, d0.stream));
+    if (gamma)
+        CU(launch_reproject_merge(dv, sv, sp, da.normal, da.depth, da.frac, *prm, *gamma, dst->rows.sums, dst->rows.m2, dst->rows.counts,
+                                  count ? dst->reused : nullptr, d0.stream));
+    else
+        CU(launch_reproject(dv, sv, sp, da.normal, da.depth, da.frac, *prm, dst->rows.sums, dst->rows.m2, dst->rows.counts,
+                            count ? dst->reused : nullptr, d0.stream));
     // back to every dst part's compact tiles; every later call on either buffer is ordered behind this one
     rc = buffer_write_back(dst, COLOUR);
     if (rc == RPTB_OK) rc = buffer_order_behind(dst, d0.stream);
     if (rc == RPTB_OK) rc = buffer_order_behind(src, d0.stream);
     if (rc != RPTB_OK) return rc;
-    return reproject_finish(dst, prm, out_reused, d0.stream);
+    return reproject_finish(dst, prm, gamma != nullptr, out_reused, out_rejected, d0.stream);
 }
 
-int rptb_buffer_reproject_shard(rptb_buffer* dst, rptb_buffer* src, const rptb_reproject* prm, uint64_t* out_reused) {
+// rptb_buffer_reproject_shard (gamma null) and rptb_buffer_reproject_merge_shard.
+static int reproject_shard(rptb_buffer* dst, rptb_buffer* src, const rptb_reproject* prm, const double* gamma, uint64_t* out_reused,
+                           uint64_t* out_rejected) {
     int rc = check_reproject_params(dst, src, prm);
     if (rc != RPTB_OK) return rc;
-    if (!dst->shard) return fail(RPTB_ERR_BAD_ARG, "dst is not a shard buffer (rptb_buffer_create_shard): a whole one reprojects with rptb_buffer_reproject");
-    if (src->shard) return refuse_shard("reproject");
+    if (gamma && !(*gamma >= 0.0)) return fail(RPTB_ERR_BAD_ARG, "gamma must be >= 0 (%g)", *gamma);
+    if (!dst->shard)
+        return fail(RPTB_ERR_BAD_ARG, "dst is not a shard buffer (rptb_buffer_create_shard): a whole one reprojects with %s",
+                    gamma ? "rptb_buffer_reproject_merge" : "rptb_buffer_reproject");
+    if (src->shard) return refuse_shard(gamma ? "reproject_merge" : "reproject");
     std::scoped_lock both(dst->lock, src->lock);
     BufferPart& d0 = dst->parts[0];
     BufferPart& s0 = src->parts[0];
     if (s0.device != d0.device) return fail(RPTB_ERR_BAD_ARG, "src's first device %d is not the shard's device %d", s0.device, d0.device);
-    rc = check_reproject_buffers(dst, src);
+    rc = check_reproject_buffers(dst, src, gamma != nullptr);
+    if (rc == RPTB_OK && gamma) rc = check_merge_dst(dst, prm);
     if (rc != RPTB_OK) return rc;
     DeviceGuard g(d0.device);
     if (!g.ok) return fail(RPTB_ERR_CUDA, "cudaSetDevice(%d) failed", d0.device);
@@ -2013,24 +2055,49 @@ int rptb_buffer_reproject_shard(rptb_buffer* dst, rptb_buffer* src, const rptb_r
     if (rc != RPTB_OK) return rc;
     if (!d0.tiles) {  // no pixel to reproject: the state alone, so that the shard's exchange block agrees with the others'
         if (out_reused) *out_reused = 0;
-        return reproject_finish(dst, prm, nullptr, d0.stream);
+        if (out_rejected) *out_rejected = 0;
+        return reproject_finish(dst, prm, gamma != nullptr, nullptr, nullptr, d0.stream);
     }
+    const bool count = out_reused || out_rejected;
     ReprojectSource sp;
     rc = reproject_source(src, &sp);
     if (rc != RPTB_OK) return rc;
     // the shard's own elements, in place in its compact planes; every later call on either buffer is ordered behind them
     CU(cudaStreamWaitEvent(d0.stream, s0.done, 0));
     CU(cudaStreamWaitEvent(d0.stream, d0.done, 0));
-    if (out_reused) CU(cudaMemsetAsync(dst->reused, 0, sizeof(unsigned long long), d0.stream));
+    if (count) CU(cudaMemsetAsync(dst->reused, 0, (gamma ? 2 : 1) * sizeof(unsigned long long), d0.stream));
     const ReprojectView dv = reproject_view(dst->feat_cam.cam, dst->width, dst->height);
     const ReprojectView sv = reproject_view(src->feat_cam.cam, src->width, src->height);
     const Planes& q = d0.planes;
-    CU(launch_reproject_part(dv, sv, sp, feature_planes(q.feat, q.n), (double)dst->feature_rays, d0.index, d0.count, q.n, *prm, q.sums,
-                             q.m2, q.counts, out_reused ? dst->reused : nullptr, d0.stream));
+    const FeaturePlanes f = feature_planes(q.feat, q.n);
+    if (gamma)
+        CU(launch_reproject_merge_part(dv, sv, sp, f, (double)dst->feature_rays, d0.index, d0.count, q.n, *prm, *gamma, q.sums, q.m2,
+                                       q.counts, count ? dst->reused : nullptr, d0.stream));
+    else
+        CU(launch_reproject_part(dv, sv, sp, f, (double)dst->feature_rays, d0.index, d0.count, q.n, *prm, q.sums, q.m2, q.counts,
+                                 count ? dst->reused : nullptr, d0.stream));
     rc = buffer_order_behind(dst, d0.stream);
     if (rc == RPTB_OK) rc = buffer_order_behind(src, d0.stream);
     if (rc != RPTB_OK) return rc;
-    return reproject_finish(dst, prm, out_reused, d0.stream);
+    return reproject_finish(dst, prm, gamma != nullptr, out_reused, out_rejected, d0.stream);
+}
+
+int rptb_buffer_reproject(rptb_buffer* dst, rptb_buffer* src, const rptb_reproject* prm, uint64_t* out_reused) {
+    return reproject_whole(dst, src, prm, nullptr, out_reused, nullptr);
+}
+
+int rptb_buffer_reproject_shard(rptb_buffer* dst, rptb_buffer* src, const rptb_reproject* prm, uint64_t* out_reused) {
+    return reproject_shard(dst, src, prm, nullptr, out_reused, nullptr);
+}
+
+int rptb_buffer_reproject_merge(rptb_buffer* dst, rptb_buffer* src, const rptb_reproject* prm, double gamma, uint64_t* out_reused,
+                                uint64_t* out_rejected) {
+    return reproject_whole(dst, src, prm, &gamma, out_reused, out_rejected);
+}
+
+int rptb_buffer_reproject_merge_shard(rptb_buffer* dst, rptb_buffer* src, const rptb_reproject* prm, double gamma, uint64_t* out_reused,
+                                      uint64_t* out_rejected) {
+    return reproject_shard(dst, src, prm, &gamma, out_reused, out_rejected);
 }
 
 uint64_t rptb_buffer_shard_bytes(const rptb_buffer* b, uint32_t with_features) {

@@ -5,6 +5,9 @@
 // rptb_buffer_reproject_shard: one thread per element of a shard part's compact tiles runs reproject_slot against the
 // same gathered source and writes the part's colour planes in place -- no row-major destination, no write-back.
 //
+// rptb_buffer_reproject_merge / _merge_shard: the same two shapes, but each thread merges the history into the pixel's
+// (element's) fresh colour planes in place when reproject_merge accepts it, and counts reused and rejected pixels.
+//
 // Also the per-pixel minimum of a buffer's counts, which image / variance / denoise of a reprojected buffer check.
 #include <cuda_runtime.h>
 
@@ -48,6 +51,43 @@ __global__ void __launch_bounds__(256) reproject_part_kernel(const ReprojectView
     }
 }
 
+// tally[0] += the warp's reused pixels, tally[1] += its rejected ones (verdicts of reproject_merge: 1, 2).
+__device__ __forceinline__ void merge_tally(int verdict, unsigned long long* tally) {
+    const unsigned reused = __ballot_sync(0xffffffffu, verdict == 1), rejected = __ballot_sync(0xffffffffu, verdict == 2);
+    if ((threadIdx.x & 31u) == 0u) {
+        if (reused) atomicAdd(tally, (unsigned long long)__popc(reused));
+        if (rejected) atomicAdd(tally + 1, (unsigned long long)__popc(rejected));
+    }
+}
+
+__global__ void __launch_bounds__(256) reproject_merge_kernel(const ReprojectView dv, const ReprojectView sv, const ReprojectSource s,
+                                                              const double* __restrict__ dnrm, const double* __restrict__ ddepth,
+                                                              const double* __restrict__ dfrac, const rptb_reproject prm, double gamma,
+                                                              double* __restrict__ sums, double* __restrict__ m2,
+                                                              uint32_t* __restrict__ counts, unsigned long long* __restrict__ tally) {
+    const uint64_t p = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const uint64_t npix = (uint64_t)dv.width * dv.height;
+    int verdict = 0;
+    if (p < npix) {
+        const uint32_t x = (uint32_t)(p % dv.width), y = (uint32_t)(p / dv.width);
+        double sh[3], m2h;
+        const uint32_t nh = reproject_pixel(dv, sv, s, x, y, dnrm + 3 * p, ddepth[p], dfrac[p], prm, sh, &m2h);
+        verdict = reproject_merge(sh, m2h, nh, gamma, sums + 3 * p, m2 + p, counts + p);
+    }
+    if (tally) merge_tally(verdict, tally);  // every lane reaches the ballots: no early return above
+}
+
+__global__ void __launch_bounds__(256) reproject_merge_part_kernel(const ReprojectView dv, const ReprojectView sv, const ReprojectSource s,
+                                                                   const FeaturePlanes f, double rays, uint32_t index, uint32_t count,
+                                                                   uint64_t nelem, const rptb_reproject prm, double gamma,
+                                                                   double* __restrict__ sums, double* __restrict__ m2,
+                                                                   uint32_t* __restrict__ counts, unsigned long long* __restrict__ tally) {
+    const uint64_t e = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    int verdict = 0;
+    if (e < nelem) verdict = reproject_merge_slot(dv, sv, s, f, rays, index, count, e, prm, gamma, sums + 3 * e, m2 + e, counts + e);
+    if (tally) merge_tally(verdict, tally);  // every lane reaches the ballots: no early return above
+}
+
 // *out = min(*out, counts[0..npix)); the caller sets *out to UINT32_MAX first.
 __global__ void __launch_bounds__(256) buffer_min_count_kernel(const uint32_t* __restrict__ counts, uint64_t npix, uint32_t* out) {
     uint32_t m = 0xFFFFFFFFu;
@@ -71,6 +111,25 @@ cudaError_t launch_reproject_part(const ReprojectView& dv, const ReprojectView& 
     if (nelem == 0) return cudaSuccess;
     reproject_part_kernel<<<(unsigned)((nelem + 255) / 256), 256, 0, stream>>>(dv, sv, s, f, rays, index, count, nelem, prm, sums, m2,
                                                                                counts, reused);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_reproject_merge(const ReprojectView& dv, const ReprojectView& sv, const ReprojectSource& s, const double* dnrm,
+                                   const double* ddepth, const double* dfrac, const rptb_reproject& prm, double gamma, double* sums,
+                                   double* m2, uint32_t* counts, unsigned long long* tally, cudaStream_t stream) {
+    const uint64_t npix = (uint64_t)dv.width * dv.height;
+    reproject_merge_kernel<<<(unsigned)((npix + 255) / 256), 256, 0, stream>>>(dv, sv, s, dnrm, ddepth, dfrac, prm, gamma, sums, m2,
+                                                                               counts, tally);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_reproject_merge_part(const ReprojectView& dv, const ReprojectView& sv, const ReprojectSource& s,
+                                        const FeaturePlanes& f, double rays, uint32_t index, uint32_t count, uint64_t nelem,
+                                        const rptb_reproject& prm, double gamma, double* sums, double* m2, uint32_t* counts,
+                                        unsigned long long* tally, cudaStream_t stream) {
+    if (nelem == 0) return cudaSuccess;
+    reproject_merge_part_kernel<<<(unsigned)((nelem + 255) / 256), 256, 0, stream>>>(dv, sv, s, f, rays, index, count, nelem, prm, gamma,
+                                                                                     sums, m2, counts, tally);
     return cudaGetLastError();
 }
 

@@ -33,6 +33,20 @@
 // A shard buffer (rptb_buffer_reproject_shard) runs the same function per element of its compact tiles (reproject_slot):
 // the element's pixel is tile_pixel's, its features resolve from the element's own feature sums (features_resolve,
 // denoise.h), and the source is whole and row-major as above.  So every pixel gets the bits the whole buffer's gets.
+//
+// Testing history against fresh entries (rptb_buffer_reproject_merge): dst already holds fresh entries S_f (3), M2_f, n_f
+// of its own view, and the history S_h, M2_h, n_h that reproject_pixel gives the pixel is merged in only where the two
+// agree.  Nothing happens (and the pixel is not counted) when n_h = 0 or n_f < 2.  Otherwise
+//     delta_c = S_hc / n_h - S_fc / n_f,   d2 = (delta_0 delta_0 + delta_1 delta_1) + delta_2 delta_2,
+//     v = M2_f / ((n_f - 1) n_f) + M2_h / ((n_h - 1) n_h)      (the channel-summed variance of the difference of the means)
+// and the history is rejected -- the pixel keeps its bits -- iff d2 > gamma^2 v (gamma^2 = gamma * gamma).  gamma = +inf
+// accepts every history (inf * 0 is NaN, and a comparison with NaN is false); gamma = 0 rejects any history whose mean
+// differs.  Accepted, the pixel becomes the parallel (Chan et al.) combination of the two groups:
+//     n = n_f + n_h,   S_c = S_fc + S_hc,   M2 = (M2_f + M2_h) + d2 ((double)n_f (double)n_h / (double)n)
+// whose between-means term carries the disagreement into the variance the adaptive criterion and the denoiser read.  The
+// test reads the pixel's own fresh state only, no neighbourhood: a 3x3 window would cross tile borders into other shards,
+// and per pixel the shards' merges stay the whole buffer's bits with no exchange.  reproject_merge_slot is the per-element
+// form for a shard's compact tiles, as reproject_slot is reproject_pixel's.
 #pragma once
 #include <cmath>
 
@@ -200,6 +214,37 @@ RPTB_HD uint32_t reproject_slot(const ReprojectView& dv, const ReprojectView& sv
     double N[3], z, a[3], fp;
     features_resolve(f.h[slot], f.n + 3 * slot, f.z[slot], f.a + 3 * slot, rays, N, &z, a, &fp);
     return reproject_pixel(dv, sv, s, (uint32_t)(p % dv.width), (uint32_t)(p / dv.width), N, z, fp, prm, out_sums, out_m2);
+}
+
+// Merges the history sh[3], m2h, nh into the fresh state sums[3], *m2, *count in place when the test above accepts it.
+// Returns 0 for no test (nh = 0 or n_f < 2), 1 for reused, 2 for rejected.
+RPTB_HD int reproject_merge(const double* sh, double m2h, uint32_t nh, double gamma, double* sums, double* m2, uint32_t* count) {
+    const uint32_t nf = *count;
+    if (nh == 0u || nf < 2u) return 0;
+    const double dnf = (double)nf, dnh = (double)nh;
+    const double d0 = sh[0] / dnh - sums[0] / dnf;
+    const double d1 = sh[1] / dnh - sums[1] / dnf;
+    const double d2c = sh[2] / dnh - sums[2] / dnf;
+    const double d2 = (d0 * d0 + d1 * d1) + d2c * d2c;
+    const double v = *m2 / ((double)(nf - 1u) * dnf) + m2h / ((double)(nh - 1u) * dnh);
+    if (d2 > (gamma * gamma) * v) return 2;
+    const uint32_t n = nf + nh;
+    sums[0] = sums[0] + sh[0];
+    sums[1] = sums[1] + sh[1];
+    sums[2] = sums[2] + sh[2];
+    *m2 = (*m2 + m2h) + d2 * ((dnf * dnh) / (double)n);
+    *count = n;
+    return 1;
+}
+
+// reproject_merge at element `slot` of shard `index` of `count`'s compact tiles: the history reproject_slot gives it,
+// merged into the element's fresh sums[3], *m2, *n.  An element past a ragged edge is left untouched (and returns 0).
+RPTB_HD int reproject_merge_slot(const ReprojectView& dv, const ReprojectView& sv, const ReprojectSource& s, const FeaturePlanes& f,
+                                 double rays, uint32_t index, uint32_t count, uint64_t slot, const rptb_reproject& prm, double gamma,
+                                 double* sums, double* m2, uint32_t* n) {
+    double sh[3], m2h;
+    const uint32_t nh = reproject_slot(dv, sv, s, f, rays, index, count, slot, prm, sh, &m2h);
+    return reproject_merge(sh, m2h, nh, gamma, sums, m2, n);
 }
 
 }  // namespace rptb

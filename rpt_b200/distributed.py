@@ -25,7 +25,8 @@ all-reduce of the ranks' active pixel counts that ends the loop.  Nothing else i
 `render_frames_distributed` is Renderer.render_frames over ShardBuffers.  A reprojected pixel needs only its own
 features and the whole previous frame, which every rank already holds: the frame's gather, with features, gave it.  So
 each rank reprojects that gathered buffer into its own shard (ShardBuffer.reproject_from), and a frame costs one
-all-gather, the one that makes its image.
+all-gather, the one that makes its image.  Testing the history against fresh entries (history_test,
+ShardBuffer.merge_history_from) reads each pixel's own fresh state only, so it adds no exchange either.
 """
 from __future__ import annotations
 
@@ -240,6 +241,22 @@ class ShardBuffer(api.DeviceBuffer):
         self.entries = int(c.max_history)  # the bound a reprojected pixel's count keeps
         return int(n.value)
 
+    def merge_history_from(self, src: "api.DeviceBuffer", reproject: Optional["api.Reproject"] = None,
+                           test: Optional["api.HistoryTest"] = None) -> tuple:
+        """DeviceBuffer.merge_history_from into this shard (rptb_buffer_reproject_merge_shard): this rank's pixels test
+        the history of `src`, a whole DeviceBuffer on this rank's device (the previous frame gathered with features),
+        against their own fresh entries.  Every pixel gets the bits a whole buffer's merge gives it.  Returns this rank's
+        (reused, rejected) pixels; summed over the ranks, they are the whole call's."""
+        if isinstance(src, ShardBuffer):
+            raise TypeError("src is a ShardBuffer: gather() the shards into a whole buffer first")
+        c = (reproject or api.Reproject()).to_c()
+        gamma = (test or api.HistoryTest()).gamma
+        n, j = C.c_uint64(0), C.c_uint64(0)
+        capi.check(capi.lib().rptb_buffer_reproject_merge_shard(self.handle, src.handle, C.byref(c), gamma, C.byref(n), C.byref(j)),
+                   "rptb_buffer_reproject_merge_shard")
+        self.entries += int(c.max_history)  # the fresh calls plus the history's bound
+        return int(n.value), int(j.value)
+
     def gather(self, group=None, with_features: bool = False) -> "api.DeviceBuffer":
         """All ranks call this: export every shard's block, one all_gather_into_tensor, and import the blocks into a new
         whole DeviceBuffer on this rank's device -- the same bits on every rank, and those of one whole buffer given the
@@ -311,15 +328,16 @@ def render_iterative_distributed(renderer, callback_interval: int, callback: Cal
 
 def render_frames_distributed(renderer, cameras, entries: int = 8, feature_samples: int = 16,
                               reproject: Optional["api.Reproject"] = api.Reproject(), adaptive: Optional["api.Adaptive"] = None,
-                              denoise: Optional["api.Denoise"] = None, group=None):
+                              denoise: Optional["api.Denoise"] = None, group=None,
+                              history_test: Optional["api.HistoryTest"] = None):
     """All ranks call this: Renderer.render_frames over one ShardBuffer per frame, yielding each frame's (height, width,
     3) uint8 on every rank -- the bytes of render_frames on one whole buffer, for any world size.  Per frame: this
     rank's shard gets `feature_samples` feature rays through the frame's camera, the previous frame's gathered buffer is
     reprojected into it (unless `reproject` is None), and `entries` plain or adaptive entries are added, continuing
     the renderer's sample streams; then one gather (with features when `reproject` or `denoise` needs them) makes the
     whole buffer the frame's image() or denoised_image(denoise) comes from, and which the next frame reprojects.  That
-    gather is the frame's only collective."""
-    renderer._check_frames(entries, adaptive, denoise)
+    gather is the frame's only collective.  `history_test` as in render_frames: each rank tests its own pixels."""
+    renderer._check_frames(entries, adaptive, denoise, reproject, history_test)
     with_features = reproject is not None or denoise is not None
     own, prev = renderer.camera, None
     try:
@@ -328,10 +346,7 @@ def render_frames_distributed(renderer, cameras, entries: int = 8, feature_sampl
             buf = ShardBuffer(renderer.device_scene(), renderer._width, renderer._height, renderer._filter, group=group)
             try:
                 renderer.sample_features(feature_samples, buf)
-                if prev is not None and reproject is not None:
-                    buf.reproject_from(prev, reproject)
-                for _ in range(entries):
-                    renderer.sample(renderer._num_samples // entries, buf, want_stats=False, adaptive=adaptive)
+                renderer._frame_entries(buf, prev, entries, reproject, adaptive, history_test)
                 whole = buf.gather(group, with_features)
             finally:
                 buf.close()

@@ -40,6 +40,10 @@ $(OBJDIR)/denoise.o: $(CSRC)/denoise.cu $(HDRS)
 $(OBJDIR)/reproject.o: $(CSRC)/reproject.cu $(HDRS)
 	@mkdir -p $(OBJDIR)
 	$(NVCC) $(NVFLAGS) -fmad=false -c $< -o $@ 2> $(OBJDIR)/reproject.ptxas.log || (cat $(OBJDIR)/reproject.ptxas.log; false)
+# the guided criterion (guided.h) likewise: its numpy restatement and host emulation round every operation on its own
+$(OBJDIR)/guided.o: $(CSRC)/guided.cu $(HDRS)
+	@mkdir -p $(OBJDIR)
+	$(NVCC) $(NVFLAGS) -fmad=false -c $< -o $@ 2> $(OBJDIR)/guided.ptxas.log || (cat $(OBJDIR)/guided.ptxas.log; false)
 $(OBJDIR)/film.o: $(CSRC)/film.cu $(HDRS)
 	@mkdir -p $(OBJDIR)
 	$(NVCC) $(NVFLAGS) -c $< -o $@ 2> $(OBJDIR)/film.ptxas.log || (cat $(OBJDIR)/film.ptxas.log; false)
@@ -56,7 +60,7 @@ $(OBJDIR)/objparse.o: $(CSRC)/objparse.cpp
 	@mkdir -p $(OBJDIR)
 	$(CXX) -std=c++17 -O3 -fPIC -Wall -c $< -o $@
 
-$(LIB): $(OBJDIR)/kernels_f32.o $(OBJDIR)/kernels_vx.o $(OBJDIR)/kernels_f64.o $(OBJDIR)/film.o $(OBJDIR)/adaptive.o $(OBJDIR)/denoise.o $(OBJDIR)/reproject.o $(OBJDIR)/api.o $(OBJDIR)/kdbuild.o $(OBJDIR)/bvhbuild.o $(OBJDIR)/objparse.o
+$(LIB): $(OBJDIR)/kernels_f32.o $(OBJDIR)/kernels_vx.o $(OBJDIR)/kernels_f64.o $(OBJDIR)/film.o $(OBJDIR)/adaptive.o $(OBJDIR)/denoise.o $(OBJDIR)/guided.o $(OBJDIR)/reproject.o $(OBJDIR)/api.o $(OBJDIR)/kdbuild.o $(OBJDIR)/bvhbuild.o $(OBJDIR)/objparse.o
 	@mkdir -p rpt_b200/lib
 	$(NVCC) -shared $(ARCH) -o $@ $^ -Xcompiler -fopenmp -lgomp -cudart shared
 
@@ -85,7 +89,10 @@ HOSTEMU_SLIM := tests/hostemu/_build/libhostemu_slim.so
 # its per-element form for a shard's compact tiles (tests/hostemu/hostemu_reproject_part.cu), and the history test of
 # the merge, per pixel and per element (tests/hostemu/hostemu_reproject_merge.cu)
 HOSTEMU_REPROJECT := tests/hostemu/_build/libhostemu_reproject.so
-hostemu: $(HOSTEMU) $(HOSTEMU_LIST) $(HOSTEMU_DENOISE) $(HOSTEMU_SLIM) $(HOSTEMU_REPROJECT)
+# the denoiser's emulation plus the guided adaptive criterion, per pixel and per slot of a part (guided.h;
+# tests/hostemu/hostemu_guided.cu)
+HOSTEMU_GUIDED := tests/hostemu/_build/libhostemu_guided.so
+hostemu: $(HOSTEMU) $(HOSTEMU_LIST) $(HOSTEMU_DENOISE) $(HOSTEMU_SLIM) $(HOSTEMU_REPROJECT) $(HOSTEMU_GUIDED)
 $(HOSTEMU): tests/hostemu/hostemu.cu $(CSRC)/kdbuild.cpp $(CSRC)/bvhbuild.cpp $(HDRS)
 	@mkdir -p $(dir $@)
 	nvcc -std=c++17 -O2 -DRPTB_HOST_EMU -DRPTB_BUILD_BVH8=1 -DRPTB_BUILD_BVH4=1 -gencode arch=compute_90a,code=sm_90a -Xcompiler -fPIC,-fopenmp,-ffp-contract=off -shared -Xlinker -Bsymbolic -o $@ tests/hostemu/hostemu.cu $(CSRC)/kdbuild.cpp $(CSRC)/bvhbuild.cpp -lgomp
@@ -101,6 +108,9 @@ $(HOSTEMU_SLIM): tests/hostemu/hostemu_slim.cu tests/hostemu/hostemu.cu $(CSRC)/
 $(HOSTEMU_REPROJECT): tests/hostemu/hostemu_reproject.cu tests/hostemu/hostemu_reproject_part.cu tests/hostemu/hostemu_reproject_merge.cu tests/hostemu/hostemu_denoise.cu tests/hostemu/hostemu.cu $(CSRC)/kdbuild.cpp $(CSRC)/bvhbuild.cpp $(HDRS)
 	@mkdir -p $(dir $@)
 	nvcc -std=c++17 -O2 -DRPTB_HOST_EMU -DRPTB_BUILD_BVH8=1 -DRPTB_BUILD_BVH4=1 -gencode arch=compute_90a,code=sm_90a -Xcompiler -fPIC,-fopenmp,-ffp-contract=off -shared -Xlinker -Bsymbolic -o $@ tests/hostemu/hostemu_reproject.cu tests/hostemu/hostemu_reproject_part.cu tests/hostemu/hostemu_reproject_merge.cu $(CSRC)/kdbuild.cpp $(CSRC)/bvhbuild.cpp -lgomp
+$(HOSTEMU_GUIDED): tests/hostemu/hostemu_guided.cu tests/hostemu/hostemu_denoise.cu tests/hostemu/hostemu.cu $(CSRC)/kdbuild.cpp $(CSRC)/bvhbuild.cpp $(HDRS)
+	@mkdir -p $(dir $@)
+	nvcc -std=c++17 -O2 -DRPTB_HOST_EMU -DRPTB_BUILD_BVH8=1 -DRPTB_BUILD_BVH4=1 -gencode arch=compute_90a,code=sm_90a -Xcompiler -fPIC,-fopenmp,-ffp-contract=off -shared -Xlinker -Bsymbolic -o $@ tests/hostemu/hostemu_guided.cu $(CSRC)/kdbuild.cpp $(CSRC)/bvhbuild.cpp -lgomp
 
 clean:
 	rm -rf build $(LIB) $(ORACLE) tests/hostemu/_build

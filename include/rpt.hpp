@@ -332,6 +332,13 @@ public:
         check(rptb_buffer_denoise(handle_, &d, nullptr, out.data()));
         return out;
     }
+    // The variance of each pixel of denoise(d) as the filter estimates it (rptb_buffer_denoise_variance): one double per
+    // pixel, row-major.
+    std::vector<double> denoised_variance(const rptb_denoise& d) const {
+        std::vector<double> out((size_t)width_ * height_);
+        check(rptb_buffer_denoise_variance(handle_, &d, out.data()));
+        return out;
+    }
     // Carries src's entries over a camera move into this buffer, which holds features and no entries
     // (rptb_buffer_reproject).  Returns the number of pixels that got history.
     uint64_t reproject_from(const DeviceBuffer& src, const rptb_reproject& params) {
@@ -431,6 +438,19 @@ public:
         next_sample_ += iterations;
         return active;
     }
+    // Adaptive sampling guided by the denoiser (rptb_sample_into_guided): `criterion` tests the variance of each pixel's
+    // denoised value under `guide`.  The buffer needs features through this renderer's camera.  Returns how many pixels
+    // got the entry (which waits for the call).
+    uint64_t sample(uint32_t iterations, DeviceBuffer& buffer, const rptb_adaptive& criterion, const rptb_denoise& guide) {
+        ensure_scene();
+        const rptb_render_params p = params(iterations);
+        const rptb_camera c = camera();
+        uint64_t active = 0;
+        if (rptb_sample_into_guided(handle_, &c, &p, &criterion, &guide, buffer.handle(), &active, nullptr) != RPTB_OK)
+            throw std::runtime_error(rptb_last_error());
+        next_sample_ += iterations;
+        return active;
+    }
     // Adds the first hits of `iterations` more camera rays per pixel to the buffer's features: the samples after those
     // its features already hold (0 .. iterations-1 on the first call).
     void sample_features(uint32_t iterations, DeviceBuffer& buffer) {
@@ -448,6 +468,19 @@ public:
         while (iteration < num_samples_) {
             const uint32_t steps = std::min(num_samples_ - iteration, interval);
             const uint64_t active = sample(steps, buffer, criterion);
+            iteration += steps;
+            if (active == 0) break;
+            cb(iteration, buffer);
+        }
+    }
+    // The same loop guided by the denoiser; a buffer without features first gets `feature_samples` feature rays per pixel.
+    void iterative_render(uint32_t interval, DeviceBuffer& buffer, const rptb_adaptive& criterion, const rptb_denoise& guide,
+                          const std::function<void(uint32_t, const DeviceBuffer&)>& cb, uint32_t feature_samples = 16) {
+        if (buffer.feature_rays() == 0) sample_features(feature_samples, buffer);
+        uint32_t iteration = 0;
+        while (iteration < num_samples_) {
+            const uint32_t steps = std::min(num_samples_ - iteration, interval);
+            const uint64_t active = sample(steps, buffer, criterion, guide);
             iteration += steps;
             if (active == 0) break;
             cb(iteration, buffer);

@@ -496,6 +496,38 @@ typedef struct rptb_denoise {
  * negative or not finite.                                                                                     */
 int rptb_buffer_denoise(rptb_buffer* buffer, const rptb_denoise* params, double* out_rgb /* nullable */,
                         uint8_t* out_rgb8 /* nullable */);
+/* Stands beside rptb_buffer_denoise: the variance v' of each pixel's denoised value, the filter's own estimate carried
+ * through its passes, v'_p = sum w^2 v_q / (sum w)^2 (rpt_b200/csrc/denoise.h) -- a per-pixel error map of the denoised
+ * image, in the filter's radiance units.  With iterations == 0 it is each pixel's variance of the mean,
+ * M2 / ((n-1) n 3).  The passes treat their inputs as independent, so after the first pass v' underestimates the true
+ * variance (DESIGN.md section 6e measures by how much).  out_var: width*height doubles, row-major.  Refusals as
+ * rptb_buffer_denoise.                                                                                        */
+int rptb_buffer_denoise_variance(rptb_buffer* buffer, const rptb_denoise* params, double* out_var);
+
+/* ---- Adaptive sampling guided by the denoiser --------------------------------------------------------------
+ * Stands beside rptb_sample_into_adaptive: the same entry for the active pixels, but the test looks at the value the
+ * denoiser will show instead of the raw mean.  Before rendering, the filter of rptb_buffer_denoise runs with `guide`
+ * over the buffer, and a pixel with n entries is active iff
+ *     n < min_entries   or   NOT( v' <= (rel_tol * m' + abs_tol)^2 ),
+ * where c' is the pixel's denoised colour (rptb_buffer_denoise's output, bit for bit), m' = ((c'_0 + c'_1) + c'_2) / 3
+ * and v' its variance after the last pass (rptb_buffer_denoise_variance), every operation a double rounded on its own
+ * in the order rpt_b200/csrc/guided.h documents.  So flat regions, which the filter averages over many neighbours,
+ * stop early, and pixels at edges, which it leaves almost alone, render on.  A pixel with 0 or 1 entries (after a
+ * reprojection) has a NaN v' and stays active; it gives its neighbours no weight.  The decision is a pure function of
+ * the gathered state: the same bits for any device count.
+ * guide->iterations == 0 is rptb_sample_into_adaptive exactly and needs no features.  While no pixel can hold
+ * min_entries (the buffer has had fewer calls), every pixel is active, and the filter is skipped (stats->launches
+ * shows it).  The filter runs on the buffer's first device; only each other part's mask and flags (132 bytes a 16x8
+ * tile) go to that part's device.  stats->gpu_ms times each part's select, render and accumulate, as
+ * rptb_sample_into_adaptive's does; stats->launches counts the filter's kernels too.
+ * RPTB_ERR_BAD_ARG: as rptb_sample_into_adaptive, as rptb_denoise's parameters in rptb_buffer_denoise, and, when
+ * guide->iterations > 0, a buffer with no features, features not made through exactly `camera`, or entries made
+ * through another camera, through several, or from the host (rptb_buffer_add_samples); a reprojected buffer's
+ * entries count as its feature camera's.  RPTB_ERR_UNSUPPORTED: a shard buffer (gather the shards first), and the
+ * wavefront engine.  out_active and stats as rptb_sample_into_adaptive.                                        */
+int rptb_sample_into_guided(rptb_scene* scene, const rptb_camera* camera, const rptb_render_params* params,
+                            const rptb_adaptive* criterion, const rptb_denoise* guide, rptb_buffer* buffer,
+                            uint64_t* out_active /* nullable, forces sync */, rptb_stats* stats /* nullable, forces sync */);
 
 /* ---- Reprojecting the device Buffer across a camera move ---------------------------------------------------
  * The temporal half of SVGF for a static scene: each pixel of `dst`'s view finds, through its own first-hit depth,

@@ -279,6 +279,10 @@ SYMBOLS = [
      [C.c_void_p, C.POINTER(Camera), C.POINTER(RenderParams), C.c_void_p, C.POINTER(Stats)]),
     ("rptb_buffer_features", C.c_int, [C.c_void_p, c_double_p, c_double_p, c_double_p, c_double_p]),
     ("rptb_buffer_denoise", C.c_int, [C.c_void_p, C.POINTER(Denoise), c_double_p, c_u8_p]),
+    ("rptb_buffer_denoise_variance", C.c_int, [C.c_void_p, C.POINTER(Denoise), c_double_p]),
+    ("rptb_sample_into_guided", C.c_int,
+     [C.c_void_p, C.POINTER(Camera), C.POINTER(RenderParams), C.POINTER(Adaptive), C.POINTER(Denoise), C.c_void_p,
+      C.POINTER(C.c_uint64), C.POINTER(Stats)]),
     ("rptb_buffer_reproject", C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(Reproject), C.POINTER(C.c_uint64)]),
     ("rptb_buffer_create_shard", C.c_int,
      [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(C.c_void_p)]),

@@ -839,10 +839,19 @@ class Adaptive:
     renders only the pixels that are still active.  A pixel with n entries is active while n < min_entries, or while
     the channel-mean variance of its mean, M2 / ((n - 1) n 3), exceeds (rel_tol * mean + abs_tol)^2.  Defaults: stop
     at 2 % relative error of the mean or 1/1000 absolute, and never before 4 entries (the guard against a dark pixel
-    whose first entries happen to agree)."""
+    whose first entries happen to agree).
+    `guide` (a Denoise): test the value the denoiser will show instead of the raw mean (rptb_sample_into_guided).  Each
+    call first runs the filter with those parameters over the buffer, and a pixel is active while n < min_entries, or
+    while the variance of its denoised value, v' (DeviceBuffer.denoised_variance), exceeds (rel_tol * m' + abs_tol)^2,
+    m' the channel mean of its denoised colour.  The buffer needs features (Renderer.sample_features) and entries made
+    through the renderer's camera alone; guide.iterations == 0 is the plain criterion.  rpt_b200/csrc/guided.h gives
+    every formula; DESIGN.md section 6e what it buys and where it loses."""
 
-    def __init__(self, rel_tol: float = 0.02, abs_tol: float = 1e-3, min_entries: int = 4):
+    def __init__(self, rel_tol: float = 0.02, abs_tol: float = 1e-3, min_entries: int = 4, guide: Optional["Denoise"] = None):
         self.rel_tol, self.abs_tol, self.min_entries = float(rel_tol), float(abs_tol), int(min_entries)
+        if guide is not None and not isinstance(guide, Denoise):
+            raise TypeError(f"guide must be an api.Denoise, not {type(guide).__name__}")
+        self.guide = guide
 
     def to_c(self) -> capi.Adaptive:
         return capi.Adaptive(self.rel_tol, self.abs_tol, self.min_entries, 0)
@@ -1030,6 +1039,16 @@ class DeviceBuffer:
                    "rptb_buffer_denoise")
         return out
 
+    def denoised_variance(self, d: Optional[Denoise] = None) -> np.ndarray:
+        """The variance of each pixel of denoise(d), as the filter estimates it (rptb_buffer_denoise_variance): (H, W)
+        float64, in the filter's radiance units -- an error map of the denoised image.  It treats each pass's inputs as
+        independent, so it underestimates the true variance (DESIGN.md section 6e).  Refusals as denoise()."""
+        out = np.empty((self.height, self.width))
+        c = (d or Denoise()).to_c()
+        capi.check(capi.lib().rptb_buffer_denoise_variance(self.handle, C.byref(c), out.ctypes.data_as(capi.c_double_p)),
+                   "rptb_buffer_denoise_variance")
+        return out
+
     def denoised_image(self, d: Optional[Denoise] = None) -> np.ndarray:
         """denoise() through Buffer::image's clamp, gamma and cast (no box filter): (H, W, 3) uint8."""
         out = np.empty((self.height, self.width, 3), np.uint8)
@@ -1190,7 +1209,8 @@ class Renderer:
         host memory; a DeviceBuffer gets it on the device, and the call returns once the work is enqueued unless
         `want_stats` (then last_stats is filled, which waits for the render).
         `adaptive` (DeviceBuffer only): add the entry only to the pixels the criterion leaves active
-        (rptb_sample_into_adaptive); returns how many pixels got it, which waits for the call.
+        (rptb_sample_into_adaptive, or rptb_sample_into_guided with adaptive.guide); returns how many pixels got it,
+        which waits for the call.
         A distributed.ShardBuffer renders and adds its own shard's tiles only; `adaptive` then counts its pixels."""
         ds = self.device_scene()
         shard = getattr(buffer, "shard", None) or (0, 1)
@@ -1200,9 +1220,14 @@ class Renderer:
             if not isinstance(buffer, DeviceBuffer):
                 raise TypeError("adaptive sampling needs a DeviceBuffer (Renderer.device_buffer())")
             stats, active, crit = capi.Stats(), C.c_uint64(0), adaptive.to_c()
-            capi.check(capi.lib().rptb_sample_into_adaptive(ds.handle, C.byref(cam), C.byref(p), C.byref(crit), buffer.handle,
-                                                            C.byref(active), C.byref(stats) if want_stats else None),
-                       "rptb_sample_into_adaptive")
+            st = C.byref(stats) if want_stats else None
+            if adaptive.guide is not None:
+                guide = adaptive.guide.to_c()
+                capi.check(capi.lib().rptb_sample_into_guided(ds.handle, C.byref(cam), C.byref(p), C.byref(crit), C.byref(guide),
+                                                              buffer.handle, C.byref(active), st), "rptb_sample_into_guided")
+            else:
+                capi.check(capi.lib().rptb_sample_into_adaptive(ds.handle, C.byref(cam), C.byref(p), C.byref(crit), buffer.handle,
+                                                                C.byref(active), st), "rptb_sample_into_adaptive")
             self._next_sample += int(iterations)
             if buffer.shard is not None:  # a shard's counts are read after the gather; the calls bound them
                 buffer.entries += 1
@@ -1321,15 +1346,20 @@ class Renderer:
                 prev.close()
 
     def iterative_render(self, callback_interval: int, callback: Callable[[int, Buffer], None],
-                         buffer: Optional[DeviceBuffer] = None, adaptive: Optional[Adaptive] = None) -> None:  # :103-115
+                         buffer: Optional[DeviceBuffer] = None, adaptive: Optional[Adaptive] = None,
+                         feature_samples: int = 16) -> None:  # :103-115
         """`buffer`: a DeviceBuffer (Renderer.device_buffer()) to accumulate into on the device; None keeps a
         host Buffer.  The callback receives whichever it is.  `adaptive` (needs a DeviceBuffer): every batch renders
-        only the pixels the criterion leaves active, and the render stops early after a batch that rendered none."""
+        only the pixels the criterion leaves active, and the render stops early after a batch that rendered none.  A
+        guided criterion (adaptive.guide) needs features: a buffer that holds none first gets `feature_samples` feature
+        rays per pixel through this renderer's camera."""
         device = buffer is not None
         if adaptive is not None and not device:
             raise TypeError("adaptive sampling needs a DeviceBuffer (Renderer.device_buffer())")
         if buffer is None:
             buffer = Buffer(self._width, self._height, self._filter, self._first_device())
+        elif adaptive is not None and adaptive.guide is not None and buffer.feature_rays == 0:
+            self.sample_features(feature_samples, buffer)
         iteration = 0
         while iteration < self._num_samples:
             steps = min(self._num_samples - iteration, callback_interval)

@@ -39,6 +39,14 @@ size_t adaptive_temp_bytes(uint32_t tiles) {
     return bytes;
 }
 
+// The ids of the flagged warp blocks of marked flags (tiles*4) and their number *len.
+cudaError_t launch_adaptive_list(const uint8_t* flags, uint32_t tiles, uint32_t* ids, uint32_t* len, void* temp, size_t temp_bytes,
+                                 cudaStream_t stream) {
+    if (tiles == 0) return cudaMemsetAsync(len, 0, sizeof(uint32_t), stream);
+    return cub::DeviceSelect::Flagged(temp, temp_bytes, cub::CountingInputIterator<uint32_t>(0u), flags, ids, len, (int)(tiles * 4u),
+                                      stream);
+}
+
 // mask: tiles*128, flags / ids: tiles*4, *len: listed blocks, *active_pixels: pixels that take the entry.
 cudaError_t launch_adaptive_select(const double* sums, const double* m2, const uint32_t* counts, uint32_t tiles, uint32_t width,
                                    uint32_t height, uint32_t shard_index, uint32_t shard_count, const rptb_adaptive& crit,
@@ -46,13 +54,13 @@ cudaError_t launch_adaptive_select(const double* sums, const double* m2, const u
                                    void* temp, size_t temp_bytes, cudaStream_t stream) {
     cudaError_t e = cudaMemsetAsync(active_pixels, 0, sizeof(unsigned long long), stream);
     if (e != cudaSuccess) return e;
-    if (tiles == 0) return cudaMemsetAsync(len, 0, sizeof(uint32_t), stream);
-    adaptive_mark_kernel<<<tiles, 128, 0, stream>>>(sums, m2, counts, width, height, shard_index, shard_count, crit, mask, flags,
-                                                    active_pixels);
-    e = cudaGetLastError();
-    if (e != cudaSuccess) return e;
-    return cub::DeviceSelect::Flagged(temp, temp_bytes, cub::CountingInputIterator<uint32_t>(0u), (const uint8_t*)flags, ids, len,
-                                      (int)(tiles * 4u), stream);
+    if (tiles) {
+        adaptive_mark_kernel<<<tiles, 128, 0, stream>>>(sums, m2, counts, width, height, shard_index, shard_count, crit, mask, flags,
+                                                        active_pixels);
+        e = cudaGetLastError();
+        if (e != cudaSuccess) return e;
+    }
+    return launch_adaptive_list(flags, tiles, ids, len, temp, temp_bytes, stream);
 }
 
 }  // namespace rptb

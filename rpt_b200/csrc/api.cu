@@ -53,11 +53,21 @@ cudaError_t launch_adaptive_select(const double* sums, const double* m2, const u
                                    uint32_t height, uint32_t shard_index, uint32_t shard_count, const rptb_adaptive& crit,
                                    uint8_t* mask, uint8_t* flags, uint32_t* ids, uint32_t* len, unsigned long long* active_pixels,
                                    void* temp, size_t temp_bytes, cudaStream_t stream);
+cudaError_t launch_adaptive_list(const uint8_t* flags, uint32_t tiles, uint32_t* ids, uint32_t* len, void* temp, size_t temp_bytes,
+                                 cudaStream_t stream);
+// the mask of a guided adaptive call: guided.cu
+cudaError_t launch_guided_mark(const double* col, const double* var, const double* albedo, const uint32_t* counts, uint32_t width,
+                               uint32_t height, uint32_t index, uint32_t count, uint32_t tiles, double eps_a, const rptb_adaptive& crit,
+                               uint8_t* mask, uint8_t* flags, unsigned long long* active_pixels, cudaStream_t stream);
 // the feature planes and the denoiser: denoise.cu
 cudaError_t launch_features_resolve(const FeaturePlanes& f, uint64_t npix, double rays, const Aov& out, cudaStream_t stream);
 cudaError_t launch_denoise(const double* sums, const double* m2, const uint32_t* counts, const double* nrm,
                            const double* depth, const double* albedo, uint32_t width, uint32_t height, const rptb_denoise& d,
                            double* const col[2], double* const var[2], double* out, cudaStream_t stream, uint32_t* launches);
+cudaError_t launch_denoise_passes(const double* sums, const double* m2, const uint32_t* counts, const double* nrm, const double* depth,
+                                  const double* albedo, uint32_t width, uint32_t height, const rptb_denoise& d, double* const col[2],
+                                  double* const var[2], const double** out_col, const double** out_var, cudaStream_t stream,
+                                  uint32_t* launches);
 // the reprojection and the least count: reproject.cu
 cudaError_t launch_reproject(const ReprojectView& dv, const ReprojectView& sv, const ReprojectSource& s, const double* dnrm,
                              const double* ddepth, const double* dfrac, const rptb_reproject& prm, double* sums, double* m2,
@@ -662,6 +672,10 @@ struct rptb_buffer {
     uint64_t feature_rays = 0;       // camera rays per pixel in the feature sums
     double* aov = nullptr;           // with the feature rows, width*height*8: the resolved features (buffer_aov)
     double* dn = nullptr;            // the denoiser's, width*height*11: colour (3) and variance ping-pong planes, then c' (3)
+    // allocated by the first guided adaptive call on a buffer of several parts: the mask and flags of parts[1..] (as many
+    // tiles as the largest holds, *132 bytes) marked here before they go to the part, and their active pixel count
+    uint8_t* guide_mask = nullptr;
+    unsigned long long* guide_active = nullptr;
     // allocated by the first reprojection into the buffer: the reused-pixel counter and the least count
     unsigned long long* reused = nullptr;
     uint32_t* min_count = nullptr;
@@ -870,9 +884,10 @@ int render_list_launch(rptb_scene* s, const rptb_camera* cam, const rptb_render_
 // Enqueues one buffer part's share of one rptb_sample_into on replica r's own stream: render the part's tiles (its
 // index of its count) into the compact out32/out64 scratch, then add them to the part as one more entry of every
 // pixel.  No host synchronise.  `crit` (rptb_sample_into_adaptive): first decide which pixels and warp blocks are
-// active, render those through the list schedule and add the entry to them alone.
+// active, render those through the list schedule and add the entry to them alone.  `marked` (a guided call): the
+// part's mask, flags and active count are already written (guide_mark), and only the list is selected from the flags.
 int sample_part(rptb_scene* r, const rptb_camera* cam, const rptb_render_params* p, BufferPart& q, bool want_stats,
-                uint32_t* launches, const rptb_adaptive* crit = nullptr) {
+                uint32_t* launches, const rptb_adaptive* crit = nullptr, bool marked = false) {
     DeviceGuard g(r->device);
     if (!g.ok) return fail(RPTB_ERR_CUDA, "cudaSetDevice(%d) failed", r->device);
     int rc = wait_busy(r, r->stream);
@@ -891,11 +906,14 @@ int sample_part(rptb_scene* r, const rptb_camera* cam, const rptb_render_params*
     }
     if (want_stats) CU(cudaEventRecord(r->ev0, r->stream));
     if (crit) {
-        CU(launch_adaptive_select(q.planes.sums, q.planes.m2, q.planes.counts, q.tiles, p->width, p->height, index, nparts, *crit, q.mask, q.flags, q.ids,
-                                  q.len, q.active, q.temp, q.temp_bytes, r->stream));
+        if (marked)
+            CU(launch_adaptive_list(q.flags, q.tiles, q.ids, q.len, q.temp, q.temp_bytes, r->stream));
+        else
+            CU(launch_adaptive_select(q.planes.sums, q.planes.m2, q.planes.counts, q.tiles, p->width, p->height, index, nparts, *crit, q.mask,
+                                      q.flags, q.ids, q.len, q.active, q.temp, q.temp_bytes, r->stream));
         const RenderList list = {q.ids, q.len, q.mask};
         rc = render_list_launch(r, cam, &qp, list, r->stream, want_stats, launches);
-        *launches += q.tiles ? 3u : 0u;  // the mark kernel and the select's two
+        *launches += q.tiles ? (marked ? 2u : 3u) : 0u;  // the mark kernel (unless marked) and the select's two
     } else {
         rc = render_launch(r, cam, &qp, r->out32, r->out64, r->stream, want_stats, true, launches);
     }
@@ -1590,22 +1608,110 @@ void rptb_buffer_destroy(rptb_buffer* b) {
     if (b) buffer_free(b);
 }
 
+// What a guided call checks of the buffer (locked) when its filter runs: features, and entries and features made
+// through `cam` alone, so that the filter's features describe what the entries saw.
+static int check_guide_buffer(const rptb_buffer* b, const rptb_camera* cam) {
+    if (b->feature_rays == 0) return fail(RPTB_ERR_BAD_ARG, "the buffer holds no features (rptb_buffer_add_features)");
+    const char* why[] = {"none", "one", "mixed (several cameras)", "unknown (a host entry)"};
+    if (b->feat_cam.state != CameraRecord::ONE) return fail(RPTB_ERR_BAD_ARG, "the buffer's features have no single camera: %s", why[b->feat_cam.state]);
+    if (std::memcmp(&b->feat_cam.cam, cam, sizeof(rptb_camera)) != 0)
+        return fail(RPTB_ERR_BAD_ARG, "the buffer's features were made through another camera");
+    if (b->entry_cam.state != CameraRecord::NONE && b->entry_cam.state != CameraRecord::ONE)
+        return fail(RPTB_ERR_BAD_ARG, "the buffer's entries have no single camera: %s", why[b->entry_cam.state]);
+    if (b->entry_cam.state == CameraRecord::ONE && std::memcmp(&b->entry_cam.cam, cam, sizeof(rptb_camera)) != 0)
+        return fail(RPTB_ERR_BAD_ARG, "the buffer's entries were made through another camera");
+    return RPTB_OK;
+}
+
+// A guided call's decision (rptb_sample_into_guided), enqueued on parts[0]'s stream: the buffer's colour and features
+// gathered row-major, the features resolved and the filter's passes run into b->dn, then the guided mark kernel once
+// per part -- into parts[0]'s own mask, flags and active count, and for every other part into the guide staging, whose
+// mask and flags (tiles*132 bytes) and count then go to the part's device.  Every part's later work is ordered behind
+// it.  Every part holds its select scratch.  *launches: kernels enqueued.
+static int guide_mark(rptb_buffer* b, const rptb_adaptive& crit, const rptb_denoise& d, uint32_t* launches) {
+    BufferPart& q0 = b->parts[0];
+    DeviceGuard g(q0.device);
+    if (!g.ok) return fail(RPTB_ERR_CUDA, "cudaSetDevice(%d) failed", q0.device);
+    const size_t npix = (size_t)b->width * b->height;
+    uint32_t most = 0, nl = 0;
+    for (size_t i = 0; i < b->parts.size(); i++) {
+        if (i > 0) most = std::max(most, b->parts[i].tiles);
+        nl += b->parts[i].tiles ? 1u : 0u;  // the gather's scatter
+    }
+    int rc = buffer_gather(b, COLOUR | FEATURES);
+    if (rc != RPTB_OK) return rc;
+    const Aov a = buffer_aov(b);
+    CU(launch_features_resolve(feature_planes(b->rows.feat, npix), npix, (double)b->feature_rays, a, q0.stream));
+    if (!b->dn) CU(own(b->mem, &b->dn, npix * 11 * sizeof(double)));
+    if (most && !b->guide_mask) {
+        CU(own(b->mem, &b->guide_mask, (size_t)most * 132u));
+        CU(own(b->mem, &b->guide_active, sizeof(unsigned long long)));
+    }
+    double* const col[2] = {b->dn, b->dn + 3 * npix};
+    double* const var[2] = {b->dn + 6 * npix, b->dn + 7 * npix};
+    const double *icol, *ivar;
+    uint32_t passes = 0;
+    CU(launch_denoise_passes(b->rows.sums, b->rows.m2, b->rows.counts, a.normal, a.depth, a.albedo, b->width, b->height, d, col, var,
+                             &icol, &ivar, q0.stream, &passes));
+    nl += 1u + passes;
+    for (size_t i = 0; i < b->parts.size(); i++) {
+        BufferPart& q = b->parts[i];
+        uint8_t* mask = i == 0 ? q.mask : b->guide_mask;
+        uint8_t* flags = i == 0 ? q.flags : b->guide_mask + (size_t)most * 128u;
+        unsigned long long* active = i == 0 ? q.active : b->guide_active;
+        CU(launch_guided_mark(icol, ivar, a.albedo, b->rows.counts, b->width, b->height, q.index, q.count, q.tiles, d.albedo_eps, crit,
+                              mask, flags, active, q0.stream));
+        nl += q.tiles ? 1u : 0u;
+        if (i == 0) continue;
+        if (q.tiles) {
+            CU(cudaMemcpyPeerAsync(q.mask, q.device, mask, q0.device, (size_t)q.tiles * 128u, q0.stream));
+            CU(cudaMemcpyPeerAsync(q.flags, q.device, flags, q0.device, (size_t)q.tiles * 4u, q0.stream));
+        }
+        CU(cudaMemcpyPeerAsync(q.active, q.device, active, q0.device, sizeof(unsigned long long), q0.stream));
+    }
+    *launches = nl;
+    return buffer_order_behind(b, q0.stream);
+}
+
+// rptb_sample_into (crit null), rptb_sample_into_adaptive (crit) and rptb_sample_into_guided (crit and guide; the
+// filter runs when guide->iterations > 0).
 static int sample_into_impl(rptb_scene* s, const rptb_camera* cam, const rptb_render_params* p, const rptb_adaptive* crit,
-                            rptb_buffer* b, uint64_t* out_active, rptb_stats* stats) {
+                            const rptb_denoise* guide, rptb_buffer* b, uint64_t* out_active, rptb_stats* stats) {
     int rc = check_render_into(s, cam, p, b);
     if (rc != RPTB_OK) return rc;
     if (crit && p->engine == RPTB_ENGINE_WAVEFRONT)
         return fail(RPTB_ERR_UNSUPPORTED, "adaptive sampling renders with the slot megakernel, not the wavefront engine");
+    if (guide && b->shard) return refuse_shard("guided adaptive sampling");
     const uint32_t nparts = (uint32_t)b->parts.size();
     std::lock_guard<std::mutex> bl(b->lock);
     if (b->entries == UINT32_MAX) return fail(RPTB_ERR_UNSUPPORTED, "too many entries");
+    const bool filter = guide && guide->iterations > 0;
+    if (filter) {
+        rc = check_guide_buffer(b, cam);
+        if (rc != RPTB_OK) return rc;
+    }
+    // While no pixel can hold min_entries (none holds more than b->entries), every pixel is active under either
+    // criterion: the plain mark decides that without the filter.
+    const bool marked = filter && b->entries >= crit->min_entries;
+    uint32_t guide_launches = 0;
+    if (marked) {
+        for (uint32_t i = 0; i < nparts; i++) {
+            BufferPart& q = b->parts[i];
+            DeviceGuard g(q.device);
+            if (!g.ok) return fail(RPTB_ERR_CUDA, "cudaSetDevice(%d) failed", q.device);
+            rc = buffer_part_select_alloc(q);
+            if (rc != RPTB_OK) return rc;
+        }
+        rc = guide_mark(b, *crit, *guide, &guide_launches);
+        if (rc != RPTB_OK) return rc;
+    }
     // every replica's share is enqueued before any is waited for, so the devices run concurrently
     std::vector<std::unique_lock<std::mutex>> locks;
     std::vector<uint32_t> launches(nparts, 0);
     for (uint32_t i = 0; i < nparts; i++) {
         rptb_scene* r = replica(s, i);
         locks.emplace_back(r->lock);
-        rc = sample_part(r, cam, p, b->parts[i], stats != nullptr, &launches[i], crit);
+        rc = sample_part(r, cam, p, b->parts[i], stats != nullptr, &launches[i], crit, marked);
         if (rc != RPTB_OK) return nparts > 1 ? fail(rc, "device %d: %s", r->device, g_error.c_str()) : rc;
     }
     b->entries++;
@@ -1645,21 +1751,47 @@ static int sample_into_impl(rptb_scene* s, const rptb_camera* cam, const rptb_re
         stats->gpu_ms = std::max(stats->gpu_ms, (double)ms);  // the devices run concurrently
         stats->launches += launches[i];
     }
+    stats->launches += guide_launches;
     stats->engine = !crit && use_wavefront(s, p) ? RPTB_ENGINE_WAVEFRONT : RPTB_ENGINE_MEGAKERNEL;
     return RPTB_OK;
 }
 
 int rptb_sample_into(rptb_scene* s, const rptb_camera* cam, const rptb_render_params* p, rptb_buffer* b, rptb_stats* stats) {
-    return sample_into_impl(s, cam, p, nullptr, b, nullptr, stats);
+    return sample_into_impl(s, cam, p, nullptr, nullptr, b, nullptr, stats);
 }
 
-int rptb_sample_into_adaptive(rptb_scene* s, const rptb_camera* cam, const rptb_render_params* p, const rptb_adaptive* crit,
-                              rptb_buffer* b, uint64_t* out_active, rptb_stats* stats) {
+static int check_adaptive(const rptb_adaptive* crit) {
     if (!crit) return fail(RPTB_ERR_BAD_ARG, "null argument");
     if (crit->min_entries < 2) return fail(RPTB_ERR_BAD_ARG, "min_entries %u < 2 (a pixel's variance needs two entries)", crit->min_entries);
     if (!(std::isfinite(crit->rel_tol) && crit->rel_tol >= 0.0) || !(std::isfinite(crit->abs_tol) && crit->abs_tol >= 0.0))
         return fail(RPTB_ERR_BAD_ARG, "tolerances must be finite and >= 0 (rel_tol %g, abs_tol %g)", crit->rel_tol, crit->abs_tol);
-    return sample_into_impl(s, cam, p, crit, b, out_active, stats);
+    return RPTB_OK;
+}
+
+static int check_denoise(const rptb_denoise* d) {
+    if (!d) return fail(RPTB_ERR_BAD_ARG, "null argument");
+    if (d->iterations > kDenoiseMaxIterations)
+        return fail(RPTB_ERR_BAD_ARG, "iterations %u > %u", d->iterations, kDenoiseMaxIterations);
+    if (!(std::isfinite(d->sigma_depth) && d->sigma_depth >= 0.0) || !(std::isfinite(d->sigma_luminance) && d->sigma_luminance >= 0.0) ||
+        !(std::isfinite(d->albedo_eps) && d->albedo_eps >= 0.0))
+        return fail(RPTB_ERR_BAD_ARG, "sigma_depth, sigma_luminance and albedo_eps must be finite and >= 0 (%g, %g, %g)", d->sigma_depth,
+                    d->sigma_luminance, d->albedo_eps);
+    return RPTB_OK;
+}
+
+int rptb_sample_into_adaptive(rptb_scene* s, const rptb_camera* cam, const rptb_render_params* p, const rptb_adaptive* crit,
+                              rptb_buffer* b, uint64_t* out_active, rptb_stats* stats) {
+    const int rc = check_adaptive(crit);
+    if (rc != RPTB_OK) return rc;
+    return sample_into_impl(s, cam, p, crit, nullptr, b, out_active, stats);
+}
+
+int rptb_sample_into_guided(rptb_scene* s, const rptb_camera* cam, const rptb_render_params* p, const rptb_adaptive* crit,
+                            const rptb_denoise* guide, rptb_buffer* b, uint64_t* out_active, rptb_stats* stats) {
+    int rc = check_adaptive(crit);
+    if (rc == RPTB_OK) rc = check_denoise(guide);
+    if (rc != RPTB_OK) return rc;
+    return sample_into_impl(s, cam, p, crit, guide, b, out_active, stats);
 }
 
 int rptb_buffer_add_samples(rptb_buffer* b, const double* rgb) {
@@ -1853,16 +1985,10 @@ int rptb_buffer_features(rptb_buffer* b, double* normal, double* depth, double* 
     return RPTB_OK;
 }
 
-int rptb_buffer_denoise(rptb_buffer* b, const rptb_denoise* d, double* out_rgb, uint8_t* out_rgb8) {
-    if (!b || !d) return fail(RPTB_ERR_BAD_ARG, "null argument");
-    if (d->iterations > kDenoiseMaxIterations)
-        return fail(RPTB_ERR_BAD_ARG, "iterations %u > %u", d->iterations, kDenoiseMaxIterations);
-    if (!(std::isfinite(d->sigma_depth) && d->sigma_depth >= 0.0) || !(std::isfinite(d->sigma_luminance) && d->sigma_luminance >= 0.0) ||
-        !(std::isfinite(d->albedo_eps) && d->albedo_eps >= 0.0))
-        return fail(RPTB_ERR_BAD_ARG, "sigma_depth, sigma_luminance and albedo_eps must be finite and >= 0 (%g, %g, %g)", d->sigma_depth,
-                    d->sigma_luminance, d->albedo_eps);
-    if (b->shard) return refuse_shard("denoise");
-    std::lock_guard<std::mutex> bl(b->lock);
+// What rptb_buffer_denoise and rptb_buffer_denoise_variance share, on the locked buffer with parts[0]'s device
+// current: the refusals, then the gathered colour and features, the resolved features and the filter's planes, enqueued
+// on parts[0]'s stream.
+static int denoise_prepare(rptb_buffer* b, Aov* a) {
     if (b->entries == 0) return fail(RPTB_ERR_BAD_ARG, "Pixel found with no samples");  // buffer.rs:89
     // Every pixel holds at least min(entries, 2) entries, so this is exact for any mix of calls: the first call of any
     // kind reaches every pixel (an adaptive one because n = 0 < min_entries); plain calls and add_samples reach every
@@ -1870,7 +1996,6 @@ int rptb_buffer_denoise(rptb_buffer* b, const rptb_denoise* d, double* out_rgb, 
     if (b->entries < 2) return fail(RPTB_ERR_BAD_ARG, "a pixel has fewer than 2 entries (no variance to guide the filter)");
     if (b->feature_rays == 0) return fail(RPTB_ERR_BAD_ARG, "the buffer holds no features (rptb_buffer_add_features)");
     BufferPart& q0 = b->parts[0];
-    DeviceGuard g(q0.device);
     const size_t npix = (size_t)b->width * b->height;
     uint32_t least = 0;  // a reprojected buffer does not keep the invariant above: look at the counts
     int rc = buffer_gather(b, COLOUR | FEATURES);
@@ -1878,9 +2003,24 @@ int rptb_buffer_denoise(rptb_buffer* b, const rptb_denoise* d, double* out_rgb, 
     if (rc != RPTB_OK) return rc;
     if (least == 0) return fail(RPTB_ERR_BAD_ARG, "Pixel found with no samples");  // buffer.rs:89
     if (least < 2) return fail(RPTB_ERR_BAD_ARG, "a pixel has fewer than 2 entries (no variance to guide the filter)");
-    const Aov a = buffer_aov(b);
-    CU(launch_features_resolve(feature_planes(b->rows.feat, npix), npix, (double)b->feature_rays, a, q0.stream));
+    *a = buffer_aov(b);
+    CU(launch_features_resolve(feature_planes(b->rows.feat, npix), npix, (double)b->feature_rays, *a, q0.stream));
     if (!b->dn) CU(own(b->mem, &b->dn, npix * 11 * sizeof(double)));
+    return RPTB_OK;
+}
+
+int rptb_buffer_denoise(rptb_buffer* b, const rptb_denoise* d, double* out_rgb, uint8_t* out_rgb8) {
+    if (!b) return fail(RPTB_ERR_BAD_ARG, "null argument");
+    int rc = check_denoise(d);
+    if (rc != RPTB_OK) return rc;
+    if (b->shard) return refuse_shard("denoise");
+    std::lock_guard<std::mutex> bl(b->lock);
+    BufferPart& q0 = b->parts[0];
+    DeviceGuard g(q0.device);
+    Aov a;
+    rc = denoise_prepare(b, &a);
+    if (rc != RPTB_OK) return rc;
+    const size_t npix = (size_t)b->width * b->height;
     double* const col[2] = {b->dn, b->dn + 3 * npix};
     double* const var[2] = {b->dn + 6 * npix, b->dn + 7 * npix};
     double* out = b->dn + 8 * npix;
@@ -1893,6 +2033,29 @@ int rptb_buffer_denoise(rptb_buffer* b, const rptb_denoise* d, double* out_rgb, 
         CU(launch_film_resolve(out, 1u, b->width, b->height, 0u, b->rgb8, q0.stream));
         CU(cudaMemcpyAsync(out_rgb8, b->rgb8, npix * 3, cudaMemcpyDeviceToHost, q0.stream));
     }
+    CU(cudaStreamSynchronize(q0.stream));
+    return RPTB_OK;
+}
+
+int rptb_buffer_denoise_variance(rptb_buffer* b, const rptb_denoise* d, double* out_var) {
+    if (!b || !out_var) return fail(RPTB_ERR_BAD_ARG, "null argument");
+    int rc = check_denoise(d);
+    if (rc != RPTB_OK) return rc;
+    if (b->shard) return refuse_shard("denoise_variance");
+    std::lock_guard<std::mutex> bl(b->lock);
+    BufferPart& q0 = b->parts[0];
+    DeviceGuard g(q0.device);
+    Aov a;
+    rc = denoise_prepare(b, &a);
+    if (rc != RPTB_OK) return rc;
+    const size_t npix = (size_t)b->width * b->height;
+    double* const col[2] = {b->dn, b->dn + 3 * npix};
+    double* const var[2] = {b->dn + 6 * npix, b->dn + 7 * npix};
+    const double *icol, *ivar;
+    uint32_t launches = 0;
+    CU(launch_denoise_passes(b->rows.sums, b->rows.m2, b->rows.counts, a.normal, a.depth, a.albedo, b->width, b->height, *d, col, var,
+                             &icol, &ivar, q0.stream, &launches));
+    CU(cudaMemcpyAsync(out_var, ivar, npix * sizeof(double), cudaMemcpyDeviceToHost, q0.stream));
     CU(cudaStreamSynchronize(q0.stream));
     return RPTB_OK;
 }

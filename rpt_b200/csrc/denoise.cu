@@ -59,6 +59,28 @@ cudaError_t launch_features_resolve(const FeaturePlanes& f, uint64_t npix, doubl
     return cudaGetLastError();
 }
 
+// The filter without its remodulation: demodulate, then d.iterations passes (none: the demodulated planes themselves).
+// col[2] / var[2]: the ping-pong planes; *out_col / *out_var: which of them holds the last pass's i' and v' (the
+// variance of the denoised value, rptb_buffer_denoise_variance; what a guided adaptive call tests).  *launches:
+// kernels enqueued.
+cudaError_t launch_denoise_passes(const double* sums, const double* m2, const uint32_t* counts, const double* nrm, const double* depth,
+                                  const double* albedo, uint32_t width, uint32_t height, const rptb_denoise& d, double* const col[2],
+                                  double* const var[2], const double** out_col, const double** out_var, cudaStream_t stream,
+                                  uint32_t* launches) {
+    const uint64_t npix = (uint64_t)width * height;
+    denoise_demodulate_kernel<<<(unsigned)((npix + 255) / 256), 256, 0, stream>>>(sums, m2, counts, npix, albedo, d.albedo_eps, col[0],
+                                                                                  var[0]);
+    const dim3 block(32, 8), grid2((width + 31) / 32, (height + 7) / 8);
+    uint32_t cur = 0;
+    for (uint32_t k = 0; k < d.iterations; k++, cur ^= 1u)
+        denoise_pass_kernel<<<grid2, block, 0, stream>>>(col[cur], var[cur], nrm, depth, albedo, width, height, 1u << k, d, col[cur ^ 1u],
+                                                         var[cur ^ 1u]);
+    *out_col = col[cur];
+    *out_var = var[cur];
+    *launches = 1u + d.iterations;
+    return cudaGetLastError();
+}
+
 // The whole filter: sums / m2 / counts and the resolved features in, c' (width*height*3) out.
 // col[2] / var[2]: the ping-pong planes.  *launches: kernels enqueued.
 cudaError_t launch_denoise(const double* sums, const double* m2, const uint32_t* counts, const double* nrm,
@@ -66,24 +88,17 @@ cudaError_t launch_denoise(const double* sums, const double* m2, const uint32_t*
                            double* const col[2], double* const var[2], double* out, cudaStream_t stream, uint32_t* launches) {
     const uint64_t npix = (uint64_t)width * height;
     const unsigned grid = (unsigned)((npix + 255) / 256);
-    uint32_t nl = 0;
     if (d.iterations == 0) {
         denoise_finish_kernel<<<grid, 256, 0, stream>>>(nullptr, albedo, d.albedo_eps, sums, counts, npix, out);
         *launches = 1;
         return cudaGetLastError();
     }
-    denoise_demodulate_kernel<<<grid, 256, 0, stream>>>(sums, m2, counts, npix, albedo, d.albedo_eps, col[0], var[0]);
-    nl++;
-    const dim3 block(32, 8), grid2((width + 31) / 32, (height + 7) / 8);
-    uint32_t cur = 0;
-    for (uint32_t k = 0; k < d.iterations; k++, cur ^= 1u) {
-        denoise_pass_kernel<<<grid2, block, 0, stream>>>(col[cur], var[cur], nrm, depth, albedo, width, height, 1u << k, d, col[cur ^ 1u],
-                                                         var[cur ^ 1u]);
-        nl++;
-    }
-    denoise_finish_kernel<<<grid, 256, 0, stream>>>(col[cur], albedo, d.albedo_eps, sums, counts, npix, out);
-    nl++;
-    *launches = nl;
+    const double *icol, *ivar;
+    const cudaError_t e = launch_denoise_passes(sums, m2, counts, nrm, depth, albedo, width, height, d, col, var, &icol, &ivar, stream,
+                                                launches);
+    if (e != cudaSuccess) return e;
+    denoise_finish_kernel<<<grid, 256, 0, stream>>>(icol, albedo, d.albedo_eps, sums, counts, npix, out);
+    (*launches)++;
     return cudaGetLastError();
 }
 

@@ -293,6 +293,14 @@ class ShardBuffer(api.DeviceBuffer):
         return whole
 
 
+def _refuse_guided(adaptive) -> None:
+    """A guided criterion's filter reaches across other ranks' tiles, so a shard cannot decide on its own: refused here,
+    before any collective, so that no rank is left waiting."""
+    if adaptive is not None and adaptive.guide is not None:
+        raise ValueError("guided adaptive sampling (Adaptive(guide=...)) needs the whole image: it is not supported on "
+                         "shards; use a plain Adaptive criterion")
+
+
 def render_iterative_distributed(renderer, callback_interval: int, callback: Callable[[int, ShardBuffer], None],
                                  adaptive: Optional["api.Adaptive"] = None, group=None,
                                  buffer: Optional[ShardBuffer] = None) -> ShardBuffer:
@@ -301,6 +309,7 @@ def render_iterative_distributed(renderer, callback_interval: int, callback: Cal
     the callback receives the ShardBuffer and calls its gather() when it wants an image, so a batch exchanges nothing
     unless asked.  With `adaptive`, the loop ends after a batch in which no rank rendered a pixel: one all-reduce(sum)
     of the ranks' active counts per batch.  Returns the ShardBuffer."""
+    _refuse_guided(adaptive)
     import torch
     import torch.distributed as dist
 
@@ -337,6 +346,7 @@ def render_frames_distributed(renderer, cameras, entries: int = 8, feature_sampl
     the renderer's sample streams; then one gather (with features when `reproject` or `denoise` needs them) makes the
     whole buffer the frame's image() or denoised_image(denoise) comes from, and which the next frame reprojects.  That
     gather is the frame's only collective.  `history_test` as in render_frames: each rank tests its own pixels."""
+    _refuse_guided(adaptive)
     renderer._check_frames(entries, adaptive, denoise, reproject, history_test)
     with_features = reproject is not None or denoise is not None
     own, prev = renderer.camera, None

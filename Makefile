@@ -44,6 +44,10 @@ $(OBJDIR)/reproject.o: $(CSRC)/reproject.cu $(HDRS)
 $(OBJDIR)/guided.o: $(CSRC)/guided.cu $(HDRS)
 	@mkdir -p $(OBJDIR)
 	$(NVCC) $(NVFLAGS) -fmad=false -c $< -o $@ 2> $(OBJDIR)/guided.ptxas.log || (cat $(OBJDIR)/guided.ptxas.log; false)
+# the delta exchange (delta.h) only moves doubles; compiled like its neighbours all the same
+$(OBJDIR)/delta.o: $(CSRC)/delta.cu $(HDRS)
+	@mkdir -p $(OBJDIR)
+	$(NVCC) $(NVFLAGS) -fmad=false -c $< -o $@ 2> $(OBJDIR)/delta.ptxas.log || (cat $(OBJDIR)/delta.ptxas.log; false)
 $(OBJDIR)/film.o: $(CSRC)/film.cu $(HDRS)
 	@mkdir -p $(OBJDIR)
 	$(NVCC) $(NVFLAGS) -c $< -o $@ 2> $(OBJDIR)/film.ptxas.log || (cat $(OBJDIR)/film.ptxas.log; false)
@@ -60,7 +64,7 @@ $(OBJDIR)/objparse.o: $(CSRC)/objparse.cpp
 	@mkdir -p $(OBJDIR)
 	$(CXX) -std=c++17 -O3 -fPIC -Wall -c $< -o $@
 
-$(LIB): $(OBJDIR)/kernels_f32.o $(OBJDIR)/kernels_vx.o $(OBJDIR)/kernels_f64.o $(OBJDIR)/film.o $(OBJDIR)/adaptive.o $(OBJDIR)/denoise.o $(OBJDIR)/guided.o $(OBJDIR)/reproject.o $(OBJDIR)/api.o $(OBJDIR)/kdbuild.o $(OBJDIR)/bvhbuild.o $(OBJDIR)/objparse.o
+$(LIB): $(OBJDIR)/kernels_f32.o $(OBJDIR)/kernels_vx.o $(OBJDIR)/kernels_f64.o $(OBJDIR)/film.o $(OBJDIR)/adaptive.o $(OBJDIR)/denoise.o $(OBJDIR)/guided.o $(OBJDIR)/delta.o $(OBJDIR)/reproject.o $(OBJDIR)/api.o $(OBJDIR)/kdbuild.o $(OBJDIR)/bvhbuild.o $(OBJDIR)/objparse.o
 	@mkdir -p rpt_b200/lib
 	$(NVCC) -shared $(ARCH) -o $@ $^ -Xcompiler -fopenmp -lgomp -cudart shared
 
@@ -92,7 +96,9 @@ HOSTEMU_REPROJECT := tests/hostemu/_build/libhostemu_reproject.so
 # the denoiser's emulation plus the guided adaptive criterion, per pixel and per slot of a part (guided.h;
 # tests/hostemu/hostemu_guided.cu)
 HOSTEMU_GUIDED := tests/hostemu/_build/libhostemu_guided.so
-hostemu: $(HOSTEMU) $(HOSTEMU_LIST) $(HOSTEMU_DENOISE) $(HOSTEMU_SLIM) $(HOSTEMU_REPROJECT) $(HOSTEMU_GUIDED)
+# the delta exchange's per-element export and import (delta.h; tests/hostemu/hostemu_delta.cu)
+HOSTEMU_DELTA := tests/hostemu/_build/libhostemu_delta.so
+hostemu: $(HOSTEMU) $(HOSTEMU_LIST) $(HOSTEMU_DENOISE) $(HOSTEMU_SLIM) $(HOSTEMU_REPROJECT) $(HOSTEMU_GUIDED) $(HOSTEMU_DELTA)
 $(HOSTEMU): tests/hostemu/hostemu.cu $(CSRC)/kdbuild.cpp $(CSRC)/bvhbuild.cpp $(HDRS)
 	@mkdir -p $(dir $@)
 	nvcc -std=c++17 -O2 -DRPTB_HOST_EMU -DRPTB_BUILD_BVH8=1 -DRPTB_BUILD_BVH4=1 -gencode arch=compute_90a,code=sm_90a -Xcompiler -fPIC,-fopenmp,-ffp-contract=off -shared -Xlinker -Bsymbolic -o $@ tests/hostemu/hostemu.cu $(CSRC)/kdbuild.cpp $(CSRC)/bvhbuild.cpp -lgomp
@@ -111,6 +117,9 @@ $(HOSTEMU_REPROJECT): tests/hostemu/hostemu_reproject.cu tests/hostemu/hostemu_r
 $(HOSTEMU_GUIDED): tests/hostemu/hostemu_guided.cu tests/hostemu/hostemu_denoise.cu tests/hostemu/hostemu.cu $(CSRC)/kdbuild.cpp $(CSRC)/bvhbuild.cpp $(HDRS)
 	@mkdir -p $(dir $@)
 	nvcc -std=c++17 -O2 -DRPTB_HOST_EMU -DRPTB_BUILD_BVH8=1 -DRPTB_BUILD_BVH4=1 -gencode arch=compute_90a,code=sm_90a -Xcompiler -fPIC,-fopenmp,-ffp-contract=off -shared -Xlinker -Bsymbolic -o $@ tests/hostemu/hostemu_guided.cu $(CSRC)/kdbuild.cpp $(CSRC)/bvhbuild.cpp -lgomp
+$(HOSTEMU_DELTA): tests/hostemu/hostemu_delta.cu $(HDRS)
+	@mkdir -p $(dir $@)
+	nvcc -std=c++17 -O2 -DRPTB_HOST_EMU -gencode arch=compute_90a,code=sm_90a -Xcompiler -fPIC,-ffp-contract=off -shared -Xlinker -Bsymbolic -o $@ tests/hostemu/hostemu_delta.cu
 
 clean:
 	rm -rf build $(LIB) $(ORACLE) tests/hostemu/_build

@@ -631,6 +631,53 @@ int rptb_buffer_reproject_merge_shard(rptb_buffer* dst, rptb_buffer* src, const 
                                       uint64_t* out_reused /* nullable, forces sync */,
                                       uint64_t* out_rejected /* nullable, forces sync */);
 
+/* ---- Guided adaptive sampling on shards: a gathered whole buffer kept current by deltas -------------------------
+ * The guided criterion's filter reaches across other shards' tiles, so a shard decides from a whole buffer on its own
+ * device that holds every shard's state: one full gather (rptb_buffer_export_shard with features, an all-gather,
+ * rptb_buffer_import_shards), then, after each adaptive or guided call, one delta per shard carrying only the pixels
+ * that call changed, imported in place.  The decisions, and so the shards' entries, are those of the whole buffer's
+ * rptb_sample_into_guided, bit for bit, for any shard count.
+ *
+ * A delta block of capacity m (the same on every shard): a 256-byte header (the image size, shard_index, shard_count,
+ * the entry count before and after the call, the reprojected flag, the feature rays, the recorded entry and feature
+ * cameras, the pixel count n <= m and m), then sums (3m doubles), M2 (m doubles), counts (m uint32) and the slots (m
+ * uint32: each pixel's compact slot in the shard, ascending).  256 + 40 m bytes; only n entries of each plane are
+ * written.  No device needed.                                                                                    */
+uint64_t rptb_delta_bytes(uint32_t capacity);
+/* Writes the shard buffer's delta block of `capacity` (rptb_delta_bytes) to dst_device, on `stream` as
+ * rptb_buffer_export_shard does; out_pixels (nullable) receives n.  It reads n, the call's active count, first (one
+ * synchronising 8-byte copy).  A delta exists only when the shard's last call was rptb_sample_into_adaptive or
+ * rptb_sample_into_guided_shard, that call came right after an export (full or delta), and it kept the shard's entry
+ * camera (or made its first entry).  RPTB_ERR_BAD_ARG: a null pointer, a
+ * whole buffer, no delta (any other call since the last export -- an entry of another kind, a feature pass, a
+ * reprojection or merge, or two calls: gather the full block), or a capacity below n.  A shard with no tile exports
+ * n = 0.                                                                                                         */
+int rptb_buffer_export_delta(rptb_buffer* buffer, void* dst_device, uint32_t capacity, void* stream, uint32_t* out_pixels);
+/* Applies shard_count delta blocks of `capacity`, shard 0 first (an all-gather of every shard's export), in place to
+ * `dst`, on dst's device; the bytes must be complete when the call is made, and it returns once it has read them.
+ * Afterwards dst holds the shards' state after the call, and its image, variance, pixel_stats, features, denoise and
+ * later gathers are those of a full import of the same shards.  RPTB_ERR_BAD_ARG: a null pointer or shard_count 0; dst
+ * a shard buffer; a block that is not a delta block, or was made for another image size, shard count or capacity;
+ * shards out of order; shards that received different calls (entry counts, reprojection, feature rays or cameras);
+ * n > capacity; and a dst that is not at the blocks' state before the call -- one not last written by an import (full
+ * or delta) of shard_count shards, or at another entry count, reprojection, feature rays or cameras.
+ * RPTB_ERR_UNSUPPORTED: a dst of more than one part.                                                           */
+int rptb_buffer_import_deltas(rptb_buffer* dst, const void* gathered_device, uint32_t shard_count, uint32_t capacity);
+/* rptb_sample_into_guided for a shard buffer: the filter runs over `whole`, a one-part whole buffer on the shard's
+ * device holding the gathered state of every shard at the shard's current state, and the mark writes this shard's
+ * pixels only.  Each shard renders exactly the pixels the whole buffer's call renders among its tiles; out_active
+ * counts them, and summed over the shards it is the whole call's.  While the shard holds fewer than min_entries entry
+ * calls the plain mark decides, as in the whole call, and `whole` may be NULL.  Refusals as rptb_sample_into_guided on
+ * the shard (its features and entry camera included), and, once the filter runs, RPTB_ERR_BAD_ARG: `whole` NULL, a
+ * shard buffer, on another device or of another size; the shard changed since its last export; `whole` not last
+ * written by an import (full or delta) of shard_count shards, or not at the shard's entries, reprojection, feature
+ * rays and cameras; `whole` failing rptb_sample_into_guided's feature and camera checks.  RPTB_ERR_UNSUPPORTED: a
+ * `whole` of more than one part.  RPTB_ERR_BAD_ARG: `shard` a whole buffer.                                     */
+int rptb_sample_into_guided_shard(rptb_scene* scene, const rptb_camera* camera, const rptb_render_params* params,
+                                  const rptb_adaptive* criterion, const rptb_denoise* guide, rptb_buffer* shard,
+                                  rptb_buffer* whole /* nullable while shard entries < min_entries */,
+                                  uint64_t* out_active /* nullable, forces sync */, rptb_stats* stats /* nullable, forces sync */);
+
 #ifdef __cplusplus
 }
 #endif

@@ -294,6 +294,12 @@ SYMBOLS = [
      [C.c_void_p, C.c_void_p, C.POINTER(Reproject), C.c_double, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
     ("rptb_buffer_reproject_merge_shard", C.c_int,
      [C.c_void_p, C.c_void_p, C.POINTER(Reproject), C.c_double, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
+    ("rptb_delta_bytes", C.c_uint64, [C.c_uint32]),
+    ("rptb_buffer_export_delta", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.POINTER(C.c_uint32)]),
+    ("rptb_buffer_import_deltas", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32]),
+    ("rptb_sample_into_guided_shard", C.c_int,
+     [C.c_void_p, C.POINTER(Camera), C.POINTER(RenderParams), C.POINTER(Adaptive), C.POINTER(Denoise), C.c_void_p, C.c_void_p,
+      C.POINTER(C.c_uint64), C.POINTER(Stats)]),
 ]
 
 _lib = None

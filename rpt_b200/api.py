@@ -1203,15 +1203,21 @@ class Renderer:
         return DeviceBuffer(self.device_scene(), self._width, self._height, self._filter)
 
     # ---- the seam: Renderer::sample (:117-129) ---------------------------------
+    _NO_GUIDE_BUFFER = object()
+
     def sample(self, iterations: int, buffer, collect_stats: int = 0, want_stats: bool = True,
-               adaptive: Optional[Adaptive] = None) -> Optional[int]:
+               adaptive: Optional[Adaptive] = None, guide_buffer=_NO_GUIDE_BUFFER) -> Optional[int]:
         """Adds one entry of `iterations` samples per pixel to `buffer`.  A host Buffer gets the image through
         host memory; a DeviceBuffer gets it on the device, and the call returns once the work is enqueued unless
         `want_stats` (then last_stats is filled, which waits for the render).
         `adaptive` (DeviceBuffer only): add the entry only to the pixels the criterion leaves active
         (rptb_sample_into_adaptive, or rptb_sample_into_guided with adaptive.guide); returns how many pixels got it,
         which waits for the call.
-        A distributed.ShardBuffer renders and adds its own shard's tiles only; `adaptive` then counts its pixels."""
+        A distributed.ShardBuffer renders and adds its own shard's tiles only; `adaptive` then counts its pixels.
+        `guide_buffer` (a ShardBuffer with a guided `adaptive`; rptb_sample_into_guided_shard): the whole DeviceBuffer the
+        shard's filter runs over -- every shard gathered with features on this rank's device, at the shard's current state
+        (ShardBuffer.gather, then ShardBuffer.gather_delta after each call).  None is allowed while the shard has fewer
+        than adaptive.min_entries calls, when the plain mark decides."""
         ds = self.device_scene()
         shard = getattr(buffer, "shard", None) or (0, 1)
         p = self.params(iterations, self._next_sample, *shard, collect_stats=collect_stats)
@@ -1221,7 +1227,12 @@ class Renderer:
                 raise TypeError("adaptive sampling needs a DeviceBuffer (Renderer.device_buffer())")
             stats, active, crit = capi.Stats(), C.c_uint64(0), adaptive.to_c()
             st = C.byref(stats) if want_stats else None
-            if adaptive.guide is not None:
+            if adaptive.guide is not None and guide_buffer is not Renderer._NO_GUIDE_BUFFER:
+                guide = adaptive.guide.to_c()
+                capi.check(capi.lib().rptb_sample_into_guided_shard(ds.handle, C.byref(cam), C.byref(p), C.byref(crit), C.byref(guide),
+                                                                    buffer.handle, guide_buffer.handle if guide_buffer is not None else None,
+                                                                    C.byref(active), st), "rptb_sample_into_guided_shard")
+            elif adaptive.guide is not None:
                 guide = adaptive.guide.to_c()
                 capi.check(capi.lib().rptb_sample_into_guided(ds.handle, C.byref(cam), C.byref(p), C.byref(crit), C.byref(guide),
                                                               buffer.handle, C.byref(active), st), "rptb_sample_into_guided")
@@ -1300,10 +1311,12 @@ class Renderer:
                 raise ValueError("history_test tests reprojected history: it needs reproject")
 
     def _frame_entries(self, buf: DeviceBuffer, prev: Optional[DeviceBuffer], entries: int, reproject: Optional[Reproject],
-                       adaptive: Optional[Adaptive], history_test: Optional[HistoryTest]) -> None:
+                       adaptive: Optional[Adaptive], history_test: Optional[HistoryTest],
+                       entry: Optional[Callable[[int], None]] = None) -> None:
         """A frame's entries after its feature pass, for render_frames and distributed.render_frames_distributed: the
         previous frame's history reprojected, then `entries` entries -- or, with `history_test`, its fresh_entries plain
-        entries first, the history merged where they agree with it, then the other entries."""
+        entries first, the history merged where they agree with it, then the other entries.  `entry(samples)`, when
+        given, adds each of those last entries instead of sample()."""
         n, fresh = self._num_samples // entries, 0
         if history_test is not None:
             fresh = history_test.fresh_entries
@@ -1314,7 +1327,10 @@ class Renderer:
         elif prev is not None and reproject is not None:
             buf.reproject_from(prev, reproject)
         for _ in range(entries - fresh):
-            self.sample(n, buf, want_stats=False, adaptive=adaptive)
+            if entry is None:
+                self.sample(n, buf, want_stats=False, adaptive=adaptive)
+            else:
+                entry(n)
 
     def render_frames(self, cameras, entries: int = 8, feature_samples: int = 16, reproject: Optional[Reproject] = Reproject(),
                       adaptive: Optional[Adaptive] = None, denoise: Optional[Denoise] = None,

@@ -24,6 +24,7 @@
 #include <vector>
 
 #include "../../include/rpt_b200.h"
+#include "delta.h"
 #include "denoise.h"
 #include "flatten.h"
 #include "launch.h"
@@ -59,6 +60,13 @@ cudaError_t launch_adaptive_list(const uint8_t* flags, uint32_t tiles, uint32_t*
 cudaError_t launch_guided_mark(const double* col, const double* var, const double* albedo, const uint32_t* counts, uint32_t width,
                                uint32_t height, uint32_t index, uint32_t count, uint32_t tiles, double eps_a, const rptb_adaptive& crit,
                                uint8_t* mask, uint8_t* flags, unsigned long long* active_pixels, cudaStream_t stream);
+// the delta exchange of a shard buffer: delta.cu
+size_t delta_temp_bytes(uint64_t nelem);
+cudaError_t launch_delta_export(const uint8_t* mask, uint64_t nelem, const double* sums, const double* m2, const uint32_t* counts,
+                                void* block, uint32_t capacity, uint32_t pixels, uint32_t* selected, void* temp, size_t temp_bytes,
+                                cudaStream_t stream);
+cudaError_t launch_delta_import(const void* blocks, uint32_t shard_count, uint32_t capacity, double* sums, double* m2, uint32_t* counts,
+                                cudaStream_t stream);
 // the feature planes and the denoiser: denoise.cu
 cudaError_t launch_features_resolve(const FeaturePlanes& f, uint64_t npix, double rays, const Aov& out, cudaStream_t stream);
 cudaError_t launch_denoise(const double* sums, const double* m2, const uint32_t* counts, const double* nrm,
@@ -632,6 +640,10 @@ struct BufferPart {
     unsigned long long* active = nullptr;
     void* temp = nullptr;
     size_t temp_bytes = 0;
+    // from a shard's first rptb_buffer_export_delta on: the select's count of listed slots and its temporary storage
+    uint32_t* delta_len = nullptr;
+    void* delta_temp = nullptr;
+    size_t delta_temp_bytes = 0;
     std::vector<void*> mem;      // everything above that cudaMalloc gave, on the part's device
 };
 
@@ -662,6 +674,13 @@ struct rptb_buffer {
     // reads are refused until the shards are gathered into a whole buffer (rptb_buffer_import_shards)
     bool shard = false;
     CameraRecord entry_cam, feat_cam;
+    // The delta exchange (rptb_buffer_export_delta, rptb_buffer_import_deltas) checks against `state`, which every call
+    // that changes the buffer bumps: an entry, a feature pass, a host entry, a reprojection or merge, an import.
+    // exported: a shard's state at its last export (full or delta).  masked: a shard's state right after its last
+    // adaptive or guided call, whose mask (parts[0].mask) is then exactly the pixels that call changed.  imported /
+    // imported_shards: a whole buffer's state right after an import (full or delta), and of how many shards.
+    uint64_t state = 0, exported = UINT64_MAX, masked = UINT64_MAX, imported = UINT64_MAX;
+    uint32_t imported_shards = 0;
     std::vector<BufferPart> parts;
     // on parts[0]'s device, each group allocated by its first gather: the image's planes row-major (width*height
     // elements), and the staging another part's planes are copied into (as many elements as the largest such part)
@@ -938,10 +957,6 @@ int sample_part(rptb_scene* r, const rptb_camera* cam, const rptb_render_params*
 // the shard's own are not written.
 constexpr uint32_t kShardMagic = 0x44524853u;  // "SHRD"
 constexpr size_t kShardHeaderBytes = 256;
-struct ShardCamera {
-    uint32_t state, _pad;  // CameraRecord::State
-    rptb_camera cam;       // zero unless state is ONE
-};
 // ShardHeader::flags: the shard was reprojected (rptb_buffer_reproject_shard), so its pixels may hold 0 or 1 entries
 constexpr uint32_t kShardReprojected = 1u;
 struct ShardHeader {
@@ -1628,7 +1643,9 @@ static int check_guide_buffer(const rptb_buffer* b, const rptb_camera* cam) {
 // per part -- into parts[0]'s own mask, flags and active count, and for every other part into the guide staging, whose
 // mask and flags (tiles*132 bytes) and count then go to the part's device.  Every part's later work is ordered behind
 // it.  Every part holds its select scratch.  *launches: kernels enqueued.
-static int guide_mark(rptb_buffer* b, const rptb_adaptive& crit, const rptb_denoise& d, uint32_t* launches) {
+// `shard` (rptb_sample_into_guided_shard): the filter runs over b, the gathered whole buffer, and the mark kernel once,
+// for the shard's one part on parts[0]'s device, whose later work is ordered behind it; b's parts are not marked.
+static int guide_mark(rptb_buffer* b, const rptb_adaptive& crit, const rptb_denoise& d, uint32_t* launches, BufferPart* shard = nullptr) {
     BufferPart& q0 = b->parts[0];
     DeviceGuard g(q0.device);
     if (!g.ok) return fail(RPTB_ERR_CUDA, "cudaSetDevice(%d) failed", q0.device);
@@ -1654,7 +1671,14 @@ static int guide_mark(rptb_buffer* b, const rptb_adaptive& crit, const rptb_deno
     CU(launch_denoise_passes(b->rows.sums, b->rows.m2, b->rows.counts, a.normal, a.depth, a.albedo, b->width, b->height, d, col, var,
                              &icol, &ivar, q0.stream, &passes));
     nl += 1u + passes;
-    for (size_t i = 0; i < b->parts.size(); i++) {
+    if (shard) {
+        CU(cudaStreamWaitEvent(q0.stream, shard->done, 0));  // the shard's last accumulate and export read its mask
+        CU(launch_guided_mark(icol, ivar, a.albedo, b->rows.counts, b->width, b->height, shard->index, shard->count, shard->tiles,
+                              d.albedo_eps, crit, shard->mask, shard->flags, shard->active, q0.stream));
+        nl += shard->tiles ? 1u : 0u;
+        CU(cudaEventRecord(shard->done, q0.stream));
+    }
+    for (size_t i = 0; !shard && i < b->parts.size(); i++) {
         BufferPart& q = b->parts[i];
         uint8_t* mask = i == 0 ? q.mask : b->guide_mask;
         uint8_t* flags = i == 0 ? q.flags : b->guide_mask + (size_t)most * 128u;
@@ -1673,15 +1697,52 @@ static int guide_mark(rptb_buffer* b, const rptb_adaptive& crit, const rptb_deno
     return buffer_order_behind(b, q0.stream);
 }
 
+static bool same_camera(const CameraRecord& a, const CameraRecord& b) {
+    const ShardCamera x = shard_camera(a), y = shard_camera(b);
+    return std::memcmp(&x, &y, sizeof(x)) == 0;
+}
+
+// What rptb_sample_into_guided_shard checks of `whole` (locked) once the filter runs: a one-part whole buffer on the
+// shard's device, of its size, last written by an import of all the shards at the shard's current state -- which the
+// shard still has, not having changed since its last export -- and check_guide_buffer's conditions.
+static int check_guide_whole(const rptb_buffer* shard, const rptb_buffer* whole, const rptb_camera* cam) {
+    if (!whole) return fail(RPTB_ERR_BAD_ARG, "null whole buffer: the shard has reached min_entries, so the filter runs over its gathered image");
+    if (whole->shard) return fail(RPTB_ERR_BAD_ARG, "whole is a shard buffer: the filter needs every shard gathered (rptb_buffer_import_shards)");
+    if (whole->parts.size() != 1)
+        return fail(RPTB_ERR_UNSUPPORTED, "whole has %zu parts: a shard's filter runs over a one-part whole buffer", whole->parts.size());
+    const BufferPart& q = shard->parts[0];
+    if (whole->parts[0].device != q.device)
+        return fail(RPTB_ERR_BAD_ARG, "whole is on device %d but the shard on device %d", whole->parts[0].device, q.device);
+    if (whole->width != shard->width || whole->height != shard->height)
+        return fail(RPTB_ERR_BAD_ARG, "whole is %ux%u but the shard %ux%u", whole->width, whole->height, shard->width, shard->height);
+    if (shard->exported != shard->state)
+        return fail(RPTB_ERR_BAD_ARG, "the shard changed since its last export: gather it into whole first (rptb_buffer_export_shard or "
+                                      "rptb_buffer_export_delta)");
+    if (whole->imported != whole->state || whole->imported_shards != q.count)
+        return fail(RPTB_ERR_BAD_ARG, "whole was not last written by an import of the %u shards (rptb_buffer_import_shards or "
+                                      "rptb_buffer_import_deltas)", q.count);
+    if (whole->entries != shard->entries || whole->reprojected != shard->reprojected || whole->feature_rays != shard->feature_rays ||
+        !same_camera(whole->entry_cam, shard->entry_cam) || !same_camera(whole->feat_cam, shard->feat_cam))
+        return fail(RPTB_ERR_BAD_ARG,
+                    "whole does not hold the shard's current state (entries %u / %u, reprojected %d / %d, feature rays %llu / %llu, or "
+                    "cameras)", whole->entries, shard->entries, (int)whole->reprojected, (int)shard->reprojected,
+                    (unsigned long long)whole->feature_rays, (unsigned long long)shard->feature_rays);
+    return check_guide_buffer(whole, cam);
+}
+
 // rptb_sample_into (crit null), rptb_sample_into_adaptive (crit) and rptb_sample_into_guided (crit and guide; the
-// filter runs when guide->iterations > 0).
+// filter runs when guide->iterations > 0).  shard_entry (rptb_sample_into_guided_shard): b is a shard buffer and the
+// filter runs over `whole`.
 static int sample_into_impl(rptb_scene* s, const rptb_camera* cam, const rptb_render_params* p, const rptb_adaptive* crit,
-                            const rptb_denoise* guide, rptb_buffer* b, uint64_t* out_active, rptb_stats* stats) {
+                            const rptb_denoise* guide, rptb_buffer* b, uint64_t* out_active, rptb_stats* stats, bool shard_entry = false,
+                            rptb_buffer* whole = nullptr) {
     int rc = check_render_into(s, cam, p, b);
     if (rc != RPTB_OK) return rc;
     if (crit && p->engine == RPTB_ENGINE_WAVEFRONT)
         return fail(RPTB_ERR_UNSUPPORTED, "adaptive sampling renders with the slot megakernel, not the wavefront engine");
-    if (guide && b->shard) return refuse_shard("guided adaptive sampling");
+    if (guide && b->shard && !shard_entry) return refuse_shard("guided adaptive sampling");
+    if (shard_entry && !b->shard)
+        return fail(RPTB_ERR_BAD_ARG, "not a shard buffer (rptb_buffer_create_shard): a whole buffer samples with rptb_sample_into_guided");
     const uint32_t nparts = (uint32_t)b->parts.size();
     std::lock_guard<std::mutex> bl(b->lock);
     if (b->entries == UINT32_MAX) return fail(RPTB_ERR_UNSUPPORTED, "too many entries");
@@ -1693,8 +1754,20 @@ static int sample_into_impl(rptb_scene* s, const rptb_camera* cam, const rptb_re
     // While no pixel can hold min_entries (none holds more than b->entries), every pixel is active under either
     // criterion: the plain mark decides that without the filter.
     const bool marked = filter && b->entries >= crit->min_entries;
+    std::unique_lock<std::mutex> wl;
+    if (marked && shard_entry) {
+        if (whole && whole != b) wl = std::unique_lock<std::mutex>(whole->lock);
+        rc = check_guide_whole(b, whole, cam);
+        if (rc != RPTB_OK) return rc;
+    }
     uint32_t guide_launches = 0;
-    if (marked) {
+    if (marked && shard_entry) {
+        DeviceGuard g(b->parts[0].device);
+        if (!g.ok) return fail(RPTB_ERR_CUDA, "cudaSetDevice(%d) failed", b->parts[0].device);
+        rc = buffer_part_select_alloc(b->parts[0]);
+        if (rc == RPTB_OK) rc = guide_mark(whole, *crit, *guide, &guide_launches, &b->parts[0]);
+        if (rc != RPTB_OK) return rc;
+    } else if (marked) {
         for (uint32_t i = 0; i < nparts; i++) {
             BufferPart& q = b->parts[i];
             DeviceGuard g(q.device);
@@ -1714,8 +1787,15 @@ static int sample_into_impl(rptb_scene* s, const rptb_camera* cam, const rptb_re
         rc = sample_part(r, cam, p, b->parts[i], stats != nullptr, &launches[i], crit, marked);
         if (rc != RPTB_OK) return nparts > 1 ? fail(rc, "device %d: %s", r->device, g_error.c_str()) : rc;
     }
+    const CameraRecord cam_before = b->entry_cam;
+    const uint32_t entries_before = b->entries;
     b->entries++;
     b->entry_cam.note(*cam);
+    b->state++;
+    // A delta block can carry this call when it was adaptive, and either kept the entry camera or made the first entry: an
+    // importer then knows the camera before the call from the one after (rptb_buffer_import_deltas).
+    const bool cam_known = same_camera(cam_before, b->entry_cam) || (cam_before.state == CameraRecord::NONE && entries_before == 0);
+    b->masked = crit && cam_known ? b->state : UINT64_MAX;
     if (out_active) {
         uint64_t total = 0;
         for (uint32_t i = 0; i < nparts; i++) {
@@ -1794,6 +1874,15 @@ int rptb_sample_into_guided(rptb_scene* s, const rptb_camera* cam, const rptb_re
     return sample_into_impl(s, cam, p, crit, guide, b, out_active, stats);
 }
 
+int rptb_sample_into_guided_shard(rptb_scene* s, const rptb_camera* cam, const rptb_render_params* p, const rptb_adaptive* crit,
+                                  const rptb_denoise* guide, rptb_buffer* shard, rptb_buffer* whole, uint64_t* out_active,
+                                  rptb_stats* stats) {
+    int rc = check_adaptive(crit);
+    if (rc == RPTB_OK) rc = check_denoise(guide);
+    if (rc != RPTB_OK) return rc;
+    return sample_into_impl(s, cam, p, crit, guide, shard, out_active, stats, true, whole);
+}
+
 int rptb_buffer_add_samples(rptb_buffer* b, const double* rgb) {
     if (!b || !rgb) return fail(RPTB_ERR_BAD_ARG, "null argument");
     if (b->shard) return refuse_shard("add_samples");
@@ -1815,6 +1904,7 @@ int rptb_buffer_add_samples(rptb_buffer* b, const double* rgb) {
     }
     b->entries++;
     b->entry_cam.state = CameraRecord::UNKNOWN;
+    b->state++;
     return RPTB_OK;
 }
 
@@ -1939,6 +2029,7 @@ int rptb_buffer_add_features(rptb_scene* s, const rptb_camera* cam, const rptb_r
     }
     b->feature_rays += p->iterations;
     b->feat_cam.note(*cam);
+    b->state++;
     if (!stats) return RPTB_OK;
     std::memset(stats, 0, sizeof(*stats));
     for (uint32_t i = 0; i < nparts; i++) {
@@ -2137,6 +2228,7 @@ static int reproject_finish(rptb_buffer* dst, const rptb_reproject* prm, bool me
     dst->entries = merge ? dst->entries + prm->max_history : prm->max_history;
     dst->reprojected = true;
     dst->entry_cam = dst->feat_cam;
+    dst->state++;
     if (out_reused || out_rejected) {
         unsigned long long n[2] = {0, 0};
         CU(cudaMemcpyAsync(n, dst->reused, (merge ? 2 : 1) * sizeof(unsigned long long), cudaMemcpyDeviceToHost, stream));
@@ -2301,6 +2393,7 @@ int rptb_buffer_export_shard(rptb_buffer* b, void* dst_device, uint32_t with_fea
     // a later accumulate into the part waits until the block is read
     CU(cudaEventRecord(q.done, st));
     if (!stream) CU(cudaStreamSynchronize(st));
+    b->exported = b->state;
     return RPTB_OK;
 }
 
@@ -2347,6 +2440,7 @@ int rptb_buffer_import_shards(rptb_buffer* dst, const void* gathered_device, uin
                         (unsigned long long)h.feature_rays, (unsigned long long)h0.feature_rays);
     }
     // everything dst holds is overwritten: its earlier work finishes first
+    dst->state++;
     for (BufferPart& q : dst->parts) CU(cudaStreamWaitEvent(d0.stream, q.done, 0));
     for (BufferPart& q : dst->parts) {
         DeviceGuard gq(q.device);
@@ -2377,6 +2471,130 @@ int rptb_buffer_import_shards(rptb_buffer* dst, const void* gathered_device, uin
     dst->entry_cam = camera_record(h0.entry_cam);
     dst->feature_rays = with_features ? h0.feature_rays : 0;
     dst->feat_cam = with_features ? camera_record(h0.feat_cam) : CameraRecord();
+    dst->imported = dst->state;
+    dst->imported_shards = shard_count;
+    return RPTB_OK;
+}
+
+uint64_t rptb_delta_bytes(uint32_t capacity) { return delta_bytes(capacity); }
+
+int rptb_buffer_export_delta(rptb_buffer* b, void* dst_device, uint32_t capacity, void* stream, uint32_t* out_pixels) {
+    if (!b || !dst_device) return fail(RPTB_ERR_BAD_ARG, "null argument");
+    if (!b->shard) return fail(RPTB_ERR_BAD_ARG, "not a shard buffer (rptb_buffer_create_shard)");
+    std::lock_guard<std::mutex> bl(b->lock);
+    if (b->masked != b->state || b->exported + 1 != b->state)
+        return fail(RPTB_ERR_BAD_ARG, "no delta to export: the shard's last call must be an adaptive or guided entry made right after an "
+                                      "export, keeping its entry camera; gather the full block (rptb_buffer_export_shard)");
+    BufferPart& q = b->parts[0];
+    DeviceGuard g(q.device);
+    if (!g.ok) return fail(RPTB_ERR_CUDA, "cudaSetDevice(%d) failed", q.device);
+    cudaStream_t st = stream ? (cudaStream_t)stream : q.stream;
+    CU(cudaStreamWaitEvent(st, q.done, 0));
+    unsigned long long n = 0;  // the pixels the call changed: its active count
+    CU(cudaMemcpyAsync(&n, q.active, sizeof(n), cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    if (n > capacity) return fail(RPTB_ERR_BAD_ARG, "capacity %u is below the %llu pixels the shard's last call changed", capacity, n);
+    const uint64_t nelem = (uint64_t)q.tiles * 128u;
+    if (nelem && !q.delta_len) {
+        q.delta_temp_bytes = delta_temp_bytes(nelem);
+        CU(own(q.mem, &q.delta_len, sizeof(uint32_t)));
+        CU(own(q.mem, &q.delta_temp, q.delta_temp_bytes ? q.delta_temp_bytes : 1));
+    }
+    DeltaHeader h;
+    std::memset(&h, 0, sizeof(h));
+    h.magic = kDeltaMagic;
+    h.width = b->width;
+    h.height = b->height;
+    h.shard_index = q.index;
+    h.shard_count = q.count;
+    h.entries_before = b->entries - 1;
+    h.entries_after = b->entries;
+    h.flags = b->reprojected ? kShardReprojected : 0u;
+    h.feature_rays = b->feature_rays;
+    h.entry_cam = shard_camera(b->entry_cam);
+    h.feat_cam = shard_camera(b->feat_cam);
+    h.pixels = (uint32_t)n;
+    h.capacity = capacity;
+    // pageable source: the call returns once the header is staged
+    CU(cudaMemcpyAsync(dst_device, &h, sizeof(h), cudaMemcpyHostToDevice, st));
+    CU(launch_delta_export(q.mask, nelem, q.planes.sums, q.planes.m2, q.planes.counts, dst_device, capacity, (uint32_t)n, q.delta_len,
+                           q.delta_temp, q.delta_temp_bytes, st));
+    // a later mark or accumulate into the part waits until the block is written
+    CU(cudaEventRecord(q.done, st));
+    if (!stream) CU(cudaStreamSynchronize(st));
+    b->exported = b->state;
+    if (out_pixels) *out_pixels = (uint32_t)n;
+    return RPTB_OK;
+}
+
+int rptb_buffer_import_deltas(rptb_buffer* dst, const void* gathered_device, uint32_t shard_count, uint32_t capacity) {
+    if (!dst || !gathered_device) return fail(RPTB_ERR_BAD_ARG, "null argument");
+    if (shard_count == 0) return fail(RPTB_ERR_BAD_ARG, "shard_count 0");
+    if (dst->shard) return fail(RPTB_ERR_BAD_ARG, "dst is a shard buffer: the deltas go into the shards' gathered whole buffer");
+    if (dst->parts.size() != 1)
+        return fail(RPTB_ERR_UNSUPPORTED, "dst has %zu parts: deltas are imported into a one-part whole buffer", dst->parts.size());
+    std::lock_guard<std::mutex> bl(dst->lock);
+    BufferPart& d0 = dst->parts[0];
+    DeviceGuard g(d0.device);
+    if (!g.ok) return fail(RPTB_ERR_CUDA, "cudaSetDevice(%d) failed", d0.device);
+    const uint32_t W = dst->width, H = dst->height;
+    const uint64_t bytes = delta_bytes(capacity);
+    const char* in = (const char*)gathered_device;
+    // header 0 first: only once it names dst's size, shard_count and capacity is the block stride known to be right
+    std::vector<DeltaHeader> hs(shard_count);
+    CU(cudaMemcpyAsync(hs.data(), in, sizeof(DeltaHeader), cudaMemcpyDeviceToHost, d0.stream));
+    CU(cudaStreamSynchronize(d0.stream));
+    const DeltaHeader& h0 = hs[0];
+    if (h0.magic != kDeltaMagic) return fail(RPTB_ERR_BAD_ARG, "block 0 is not a delta block (rptb_buffer_export_delta)");
+    if (h0.width != W || h0.height != H) return fail(RPTB_ERR_BAD_ARG, "the deltas are %ux%u but dst is %ux%u", h0.width, h0.height, W, H);
+    if (h0.shard_count != shard_count) return fail(RPTB_ERR_BAD_ARG, "the deltas are of %u shards but shard_count is %u", h0.shard_count, shard_count);
+    if (h0.capacity != capacity) return fail(RPTB_ERR_BAD_ARG, "the deltas have capacity %u but capacity is %u", h0.capacity, capacity);
+    if (shard_count > 1)
+        CU(cudaMemcpy2DAsync(hs.data() + 1, sizeof(DeltaHeader), in + bytes, bytes, sizeof(DeltaHeader), shard_count - 1,
+                             cudaMemcpyDeviceToHost, d0.stream));
+    CU(cudaStreamSynchronize(d0.stream));
+    for (uint32_t i = 0; i < shard_count; i++) {
+        const DeltaHeader& h = hs[i];
+        if (h.magic != kDeltaMagic) return fail(RPTB_ERR_BAD_ARG, "block %u is not a delta block (rptb_buffer_export_delta)", i);
+        if (h.shard_index != i)
+            return fail(RPTB_ERR_BAD_ARG, "block %u holds shard %u: the shards must be in order 0..%u", i, h.shard_index, shard_count - 1);
+        if (h.width != W || h.height != H || h.shard_count != shard_count || h.capacity != capacity)
+            return fail(RPTB_ERR_BAD_ARG, "block %u was exported for another image, shard count or capacity", i);
+        if (h.pixels > capacity) return fail(RPTB_ERR_BAD_ARG, "block %u holds %u pixels, more than its capacity %u", i, h.pixels, capacity);
+        if (h.entries_before != h0.entries_before || h.entries_after != h0.entries_after || h.flags != h0.flags ||
+            h.feature_rays != h0.feature_rays || std::memcmp(&h.entry_cam, &h0.entry_cam, sizeof(ShardCamera)) != 0 ||
+            std::memcmp(&h.feat_cam, &h0.feat_cam, sizeof(ShardCamera)) != 0)
+            return fail(RPTB_ERR_BAD_ARG,
+                        "shard %u received other calls than shard 0 (entries %u -> %u / %u -> %u, reprojected %u / %u, feature rays "
+                        "%llu / %llu, or cameras)",
+                        i, h.entries_before, h.entries_after, h0.entries_before, h0.entries_after, h.flags & kShardReprojected,
+                        h0.flags & kShardReprojected, (unsigned long long)h.feature_rays, (unsigned long long)h0.feature_rays);
+    }
+    // dst must hold the shards' state before the call: an import of them, untouched since.  The entry camera before the call
+    // is the one after it, or none before the first entry (rptb_buffer_export_delta refuses any other change).
+    const CameraRecord after_cam = camera_record(h0.entry_cam);
+    const CameraRecord before_cam = h0.entries_before == 0 ? CameraRecord() : after_cam;
+    const bool reprojected = (h0.flags & kShardReprojected) != 0;
+    if (dst->imported != dst->state || dst->imported_shards != shard_count)
+        return fail(RPTB_ERR_BAD_ARG, "dst was not last written by an import of the %u shards (rptb_buffer_import_shards or "
+                                      "rptb_buffer_import_deltas); gather the full blocks", shard_count);
+    if (dst->entries != h0.entries_before || dst->reprojected != reprojected || dst->feature_rays != h0.feature_rays ||
+        !same_camera(dst->entry_cam, before_cam) || !same_camera(dst->feat_cam, camera_record(h0.feat_cam)))
+        return fail(RPTB_ERR_BAD_ARG,
+                    "dst is not at the shards' state before the call (entries %u / %u, reprojected %d / %d, feature rays %llu / %llu, or "
+                    "cameras); gather the full blocks",
+                    dst->entries, h0.entries_before, (int)dst->reprojected, (int)reprojected, (unsigned long long)dst->feature_rays,
+                    (unsigned long long)h0.feature_rays);
+    // in place in dst's compact planes; every later call on dst is ordered behind it
+    dst->state++;
+    CU(cudaStreamWaitEvent(d0.stream, d0.done, 0));
+    CU(launch_delta_import(in, shard_count, capacity, d0.planes.sums, d0.planes.m2, d0.planes.counts, d0.stream));
+    CU(cudaEventRecord(d0.done, d0.stream));
+    // the caller may reuse the gathered bytes when the call returns
+    CU(cudaStreamSynchronize(d0.stream));
+    dst->entries = h0.entries_after;
+    dst->entry_cam = after_cam;
+    dst->imported = dst->state;
     return RPTB_OK;
 }
 

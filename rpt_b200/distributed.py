@@ -27,6 +27,13 @@ features and the whole previous frame, which every rank already holds: the frame
 each rank reprojects that gathered buffer into its own shard (ShardBuffer.reproject_from), and a frame costs one
 all-gather, the one that makes its image.  Testing the history against fresh entries (history_test,
 ShardBuffer.merge_history_from) reads each pixel's own fresh state only, so it adds no exchange either.
+
+Guided adaptive sampling (Adaptive(guide=...)) is the exception: its filter reaches about 62 pixels at 5 passes, across
+other ranks' tiles, so every rank needs the whole image's state before each guided call.  A rank keeps a gathered whole
+buffer current instead of re-gathering it: one full gather with features when the filter is first needed, then after
+every call one all-gather of delta blocks (ShardBuffer.gather_delta) -- only the pixels that call changed, with their
+new state -- applied in place.  Each rank's filter and decisions are then those of the whole buffer's call, bit for
+bit, and so are its entries.
 """
 from __future__ import annotations
 
@@ -181,6 +188,39 @@ def shard_block_layout(width: int, height: int, shard_count: int, with_features:
     return {"slots": slots, "sums": sums, "m2": m2, "features": features, "counts": counts, "bytes": counts + slots * 4}
 
 
+DELTA_HEADER_BYTES = 256  # must match rpt_b200/csrc/delta.h (kDeltaHeaderBytes)
+DELTA_PIXELS_AT = 248  # the byte offset of the header's pixel count (DeltaHeader::pixels, a uint32)
+
+
+def delta_block_layout(capacity: int) -> dict:
+    """Byte offsets of the planes in one shard's delta block of `capacity` pixels (rptb_buffer_export_delta), the same for
+    every shard: a header, then sums (3 doubles a pixel), M2 (1 double), counts (1 uint32) and slots (1 uint32: the
+    pixel's compact slot in its shard, ascending).  Only the header's pixel count of each plane is written."""
+    m = int(capacity)
+    sums = DELTA_HEADER_BYTES
+    m2 = sums + 24 * m
+    counts = m2 + 8 * m
+    slots = counts + 4 * m
+    return {"capacity": m, "sums": sums, "m2": m2, "counts": counts, "slots": slots, "bytes": slots + 4 * m}
+
+
+def _all_gather_bytes(mine, world: int, group):
+    """Every rank's uint8 block (the same size on every rank), concatenated in rank order: (on mine's device, on the host
+    or None).  NCCL gathers GPU to GPU; any other backend (gloo) through a host tensor, which is also returned."""
+    import torch
+    import torch.distributed as dist
+
+    if world == 1:
+        return mine, None
+    if dist.get_backend(group) == "nccl":
+        gathered = torch.empty(mine.numel() * world, dtype=torch.uint8, device=mine.device)
+        dist.all_gather_into_tensor(gathered, mine, group=group)
+        return gathered, None
+    staged = torch.empty(mine.numel() * world, dtype=torch.uint8)
+    dist.all_gather_into_tensor(staged, mine.cpu(), group=group)
+    return staged.to(mine.device), staged
+
+
 def _rank_world(group=None):
     import torch.distributed as dist
 
@@ -263,7 +303,6 @@ class ShardBuffer(api.DeviceBuffer):
         same calls.  NCCL gathers GPU to GPU; any other backend (gloo) through a host tensor.  `with_features` carries
         the feature sums too (denoise and reproject need them), 100 instead of 36 bytes per pixel."""
         import torch
-        import torch.distributed as dist
 
         group = self.group if group is None else group
         rank, world = self.shard
@@ -275,15 +314,7 @@ class ShardBuffer(api.DeviceBuffer):
             stream = torch.cuda.current_stream(dev)
             mine = torch.empty(nbytes, dtype=torch.uint8, device=dev)
             self.export(mine, with_features, stream.cuda_stream)
-            if world == 1:
-                gathered = mine
-            elif dist.get_backend(group) == "nccl":
-                gathered = torch.empty(nbytes * world, dtype=torch.uint8, device=dev)
-                dist.all_gather_into_tensor(gathered, mine, group=group)
-            else:
-                staged = torch.empty(nbytes * world, dtype=torch.uint8)
-                dist.all_gather_into_tensor(staged, mine.cpu(), group=group)
-                gathered = staged.to(dev)
+            gathered, _ = _all_gather_bytes(mine, world, group)
             stream.synchronize()  # the import reads the gathered bytes on the library's stream
             whole = api.DeviceBuffer(self._scene, self.width, self.height, self.filter)
             capi.check(capi.lib().rptb_buffer_import_shards(whole.handle, C.c_void_p(gathered.data_ptr()), world,
@@ -292,33 +323,141 @@ class ShardBuffer(api.DeviceBuffer):
         whole.feature_rays = self.feature_rays if with_features else 0
         return whole
 
+    def export_delta(self, out, capacity: int, stream: Optional[int] = None) -> int:
+        """Writes this shard's delta block of `capacity` pixels (delta_block_layout; rptb_buffer_export_delta) into `out`, a
+        CUDA uint8 tensor on the buffer's device, on `stream` (a raw cudaStream_t; the current torch stream when None):
+        the pixels this shard's last call changed, which must be an adaptive or guided call made right after an export
+        (gather or gather_delta).  Returns their number."""
+        import torch
 
-def _refuse_guided(adaptive) -> None:
-    """A guided criterion's filter reaches across other ranks' tiles, so a shard cannot decide on its own: refused here,
-    before any collective, so that no rank is left waiting."""
-    if adaptive is not None and adaptive.guide is not None:
-        raise ValueError("guided adaptive sampling (Adaptive(guide=...)) needs the whole image: it is not supported on "
-                         "shards; use a plain Adaptive criterion")
+        if stream is None:
+            stream = torch.cuda.current_stream(out.device).cuda_stream
+        n = C.c_uint32(0)
+        capi.check(capi.lib().rptb_buffer_export_delta(self.handle, C.c_void_p(out.data_ptr()), int(capacity), C.c_void_p(stream or 1),
+                                                       C.byref(n)), "rptb_buffer_export_delta")
+        return int(n.value)
+
+    def gather_delta(self, whole: "api.DeviceBuffer", capacity: int, group=None) -> None:
+        """All ranks call this after an adaptive or guided call: export this shard's delta block, one
+        all_gather_into_tensor (as gather() does), and apply every rank's block in place to `whole`
+        (rptb_buffer_import_deltas) -- this rank's gathered buffer, brought to the shards' state before the call by
+        gather(with_features=True) or the previous gather_delta.  Afterwards `whole` is what a new gather would give.
+        `capacity`, the same on every rank: at least the largest active count of the call over the ranks."""
+        import torch
+
+        group = self.group if group is None else group
+        rank, world = self.shard
+        if world > 1 and _rank_world(group) != (rank, world):
+            raise ValueError(f"the shard is {rank} of {world} but the process group has rank/world {_rank_world(group)}")
+        lay = delta_block_layout(capacity)
+        dev = torch.device("cuda", self.devices[0])
+        with torch.cuda.device(dev):
+            stream = torch.cuda.current_stream(dev)
+            mine = torch.empty(lay["bytes"], dtype=torch.uint8, device=dev)
+            self.export_delta(mine, capacity, stream.cuda_stream)
+            gathered, staged = _all_gather_bytes(mine, world, group)
+            stream.synchronize()  # the import reads the gathered bytes on the library's stream
+            capi.check(capi.lib().rptb_buffer_import_deltas(whole.handle, C.c_void_p(gathered.data_ptr()), world, lay["capacity"]),
+                       "rptb_buffer_import_deltas")
+            # a delta only raises counts: the largest is the old one or one of the counts the blocks carry
+            blocks = (staged if staged is not None else gathered).view(world, lay["bytes"])
+            pixels = blocks[:, DELTA_PIXELS_AT:DELTA_PIXELS_AT + 4].contiguous().view(torch.int32)
+            counts = blocks[:, lay["counts"]:lay["slots"]].contiguous().view(torch.int32)
+            written = torch.arange(lay["capacity"], device=blocks.device).unsqueeze(0) < pixels
+            if bool(written.any()):
+                whole.entries = max(whole.entries, int(counts[written].max()))
+
+
+def _count_device(buffer: ShardBuffer, group=None):
+    """Where the per-batch active counts are exchanged: on the GPU under NCCL, on the host otherwise."""
+    import torch
+    import torch.distributed as dist
+
+    if dist.is_available() and dist.is_initialized() and buffer.shard[1] > 1 and dist.get_backend(group) == "nccl":
+        return torch.device("cuda", buffer.devices[0])
+    return "cpu"
+
+
+class _GuidedShard:
+    """A rank's guided calls on its ShardBuffer and the gathered whole buffer its filter runs over, kept current: one full
+    gather with features before the first call that runs the filter, then after every call one gather_delta of that
+    call.  Every rank makes the same calls, and so the same collectives."""
+
+    def __init__(self, renderer, shard: ShardBuffer, adaptive: "api.Adaptive", group=None):
+        self.renderer, self.shard, self.adaptive, self.group = renderer, shard, adaptive, group
+        self.whole: Optional[api.DeviceBuffer] = None
+        self.count_dev = _count_device(shard, group)
+
+    def sample(self, samples: int) -> int:
+        """One guided call of `samples` samples on every rank, and its delta once the whole buffer exists; returns the
+        active pixels summed over the ranks."""
+        import torch
+        import torch.distributed as dist
+
+        a, s = self.adaptive, self.shard
+        if self.whole is None and a.guide.iterations > 0 and s.entries >= a.min_entries:
+            self.whole = s.gather(self.group, with_features=True)
+        active = self.renderer.sample(samples, s, want_stats=False, adaptive=a, guide_buffer=self.whole)
+        counts = [active]
+        if s.shard[1] > 1:  # every rank's count: their sum ends a loop, their largest is the delta's capacity
+            out = torch.empty(s.shard[1], dtype=torch.int64, device=self.count_dev)
+            dist.all_gather_into_tensor(out, torch.tensor([active], dtype=torch.int64, device=self.count_dev), group=self.group)
+            counts = out.tolist()
+        if self.whole is not None:
+            s.gather_delta(self.whole, max(counts), self.group)
+        return sum(counts)
+
+    def close(self) -> None:
+        if self.whole is not None:
+            self.whole.close()
+            self.whole = None
+
+
+def _check_guided_world(adaptive, world: int) -> None:
+    """A guided loop on shards keeps a gathered whole buffer on every rank and exchanges the ranks' deltas.  On one rank
+    the shard is already the whole image, so that copy and that exchange would only add work to what the whole-buffer
+    loop does: refused, before any device work or collective, with the loop to use instead."""
+    if adaptive is not None and adaptive.guide is not None and world < 2:
+        raise ValueError("guided adaptive sampling (Adaptive(guide=...)) on shards needs two or more ranks (torch.distributed "
+                         "initialized); one process renders it on one whole buffer: Renderer.iterative_render / render_frames")
 
 
 def render_iterative_distributed(renderer, callback_interval: int, callback: Callable[[int, ShardBuffer], None],
                                  adaptive: Optional["api.Adaptive"] = None, group=None,
-                                 buffer: Optional[ShardBuffer] = None) -> ShardBuffer:
+                                 buffer: Optional[ShardBuffer] = None, feature_samples: int = 16) -> ShardBuffer:
     """All ranks call this: Renderer.iterative_render over this rank's ShardBuffer (`buffer`, e.g. one given features
     first; None creates one for the renderer's size and filter).  Every batch renders and adds this rank's tiles only;
     the callback receives the ShardBuffer and calls its gather() when it wants an image, so a batch exchanges nothing
     unless asked.  With `adaptive`, the loop ends after a batch in which no rank rendered a pixel: one all-reduce(sum)
-    of the ranks' active counts per batch.  Returns the ShardBuffer."""
-    _refuse_guided(adaptive)
+    of the ranks' active counts per batch.  Returns the ShardBuffer.
+    A guided criterion (adaptive.guide) mirrors iterative_render: a shard with no features first gets `feature_samples`
+    feature rays per pixel; the first batch that runs the filter is preceded by one gather with features, and every
+    batch after that by the gather_delta of the batch before, which runs right after it, ahead of the callback.  The
+    active counts are all-gathered instead of all-reduced: their sum ends the loop, their largest is the delta's
+    capacity.  With one rank, a guided criterion is refused (ValueError): the whole-buffer loop does the same work."""
     import torch
     import torch.distributed as dist
 
+    _check_guided_world(adaptive, buffer.shard[1] if buffer is not None else _rank_world(group)[1])
     if buffer is None:
         buffer = ShardBuffer(renderer.device_scene(), renderer._width, renderer._height, renderer._filter, group=group)
+    if adaptive is not None and adaptive.guide is not None:
+        if buffer.feature_rays == 0:
+            renderer.sample_features(feature_samples, buffer)
+        guided = _GuidedShard(renderer, buffer, adaptive, group)
+        try:
+            iteration = 0
+            while iteration < renderer._num_samples:
+                steps = min(renderer._num_samples - iteration, callback_interval)
+                iteration += steps
+                if guided.sample(steps) == 0:
+                    break
+                callback(iteration, buffer)
+        finally:
+            guided.close()
+        return buffer
     on = dist.is_available() and dist.is_initialized() and buffer.shard[1] > 1
-    count_dev = "cpu"
-    if on and dist.get_backend(group) == "nccl":
-        count_dev = torch.device("cuda", buffer.devices[0])
+    count_dev = _count_device(buffer, group)
     iteration = 0
     while iteration < renderer._num_samples:
         steps = min(renderer._num_samples - iteration, callback_interval)
@@ -345,8 +484,14 @@ def render_frames_distributed(renderer, cameras, entries: int = 8, feature_sampl
     reprojected into it (unless `reproject` is None), and `entries` plain or adaptive entries are added, continuing
     the renderer's sample streams; then one gather (with features when `reproject` or `denoise` needs them) makes the
     whole buffer the frame's image() or denoised_image(denoise) comes from, and which the next frame reprojects.  That
-    gather is the frame's only collective.  `history_test` as in render_frames: each rank tests its own pixels."""
-    _refuse_guided(adaptive)
+    gather is the frame's only all-gather of full blocks.  `history_test` as in render_frames: each rank tests its own
+    pixels.
+    A guided criterion (adaptive.guide): the frame's guided entries run as in render_iterative_distributed, with one
+    gather with features before the first that runs the filter and a gather_delta after each.  The whole buffer they keep
+    current is the frame's image and the next frame's source, so a frame still makes one full gather (at its end, as
+    without guidance, when no entry ran the filter).  With one rank, a guided criterion is refused (ValueError), as in
+    render_iterative_distributed."""
+    _check_guided_world(adaptive, _rank_world(group)[1])
     renderer._check_frames(entries, adaptive, denoise, reproject, history_test)
     with_features = reproject is not None or denoise is not None
     own, prev = renderer.camera, None
@@ -354,11 +499,18 @@ def render_frames_distributed(renderer, cameras, entries: int = 8, feature_sampl
         for cam in cameras:
             renderer.camera = cam
             buf = ShardBuffer(renderer.device_scene(), renderer._width, renderer._height, renderer._filter, group=group)
+            guided = _GuidedShard(renderer, buf, adaptive, group) if adaptive is not None and adaptive.guide is not None else None
             try:
                 renderer.sample_features(feature_samples, buf)
-                renderer._frame_entries(buf, prev, entries, reproject, adaptive, history_test)
-                whole = buf.gather(group, with_features)
+                renderer._frame_entries(buf, prev, entries, reproject, adaptive, history_test,
+                                        None if guided is None else guided.sample)
+                if guided is not None and guided.whole is not None:
+                    whole, guided.whole = guided.whole, None
+                else:
+                    whole = buf.gather(group, with_features)
             finally:
+                if guided is not None:
+                    guided.close()
                 buf.close()
             img = whole.image() if denoise is None else whole.denoised_image(denoise)
             if prev is not None:

@@ -44,6 +44,11 @@ $(OBJDIR)/reproject.o: $(CSRC)/reproject.cu $(HDRS)
 $(OBJDIR)/guided.o: $(CSRC)/guided.cu $(HDRS)
 	@mkdir -p $(OBJDIR)
 	$(NVCC) $(NVFLAGS) -fmad=false -c $< -o $@ 2> $(OBJDIR)/guided.ptxas.log || (cat $(OBJDIR)/guided.ptxas.log; false)
+# the error estimate from two half buffers (halves.h) likewise: its numpy restatement and host emulation round every
+# operation on its own
+$(OBJDIR)/halves.o: $(CSRC)/halves.cu $(HDRS)
+	@mkdir -p $(OBJDIR)
+	$(NVCC) $(NVFLAGS) -fmad=false -c $< -o $@ 2> $(OBJDIR)/halves.ptxas.log || (cat $(OBJDIR)/halves.ptxas.log; false)
 # the delta exchange (delta.h) only moves doubles; compiled like its neighbours all the same
 $(OBJDIR)/delta.o: $(CSRC)/delta.cu $(HDRS)
 	@mkdir -p $(OBJDIR)
@@ -64,7 +69,7 @@ $(OBJDIR)/objparse.o: $(CSRC)/objparse.cpp
 	@mkdir -p $(OBJDIR)
 	$(CXX) -std=c++17 -O3 -fPIC -Wall -c $< -o $@
 
-$(LIB): $(OBJDIR)/kernels_f32.o $(OBJDIR)/kernels_vx.o $(OBJDIR)/kernels_f64.o $(OBJDIR)/film.o $(OBJDIR)/adaptive.o $(OBJDIR)/denoise.o $(OBJDIR)/guided.o $(OBJDIR)/delta.o $(OBJDIR)/reproject.o $(OBJDIR)/api.o $(OBJDIR)/kdbuild.o $(OBJDIR)/bvhbuild.o $(OBJDIR)/objparse.o
+$(LIB): $(OBJDIR)/kernels_f32.o $(OBJDIR)/kernels_vx.o $(OBJDIR)/kernels_f64.o $(OBJDIR)/film.o $(OBJDIR)/adaptive.o $(OBJDIR)/denoise.o $(OBJDIR)/guided.o $(OBJDIR)/halves.o $(OBJDIR)/delta.o $(OBJDIR)/reproject.o $(OBJDIR)/api.o $(OBJDIR)/kdbuild.o $(OBJDIR)/bvhbuild.o $(OBJDIR)/objparse.o
 	@mkdir -p rpt_b200/lib
 	$(NVCC) -shared $(ARCH) -o $@ $^ -Xcompiler -fopenmp -lgomp -cudart shared
 
@@ -98,7 +103,9 @@ HOSTEMU_REPROJECT := tests/hostemu/_build/libhostemu_reproject.so
 HOSTEMU_GUIDED := tests/hostemu/_build/libhostemu_guided.so
 # the delta exchange's per-element export and import (delta.h; tests/hostemu/hostemu_delta.cu)
 HOSTEMU_DELTA := tests/hostemu/_build/libhostemu_delta.so
-hostemu: $(HOSTEMU) $(HOSTEMU_LIST) $(HOSTEMU_DENOISE) $(HOSTEMU_SLIM) $(HOSTEMU_REPROJECT) $(HOSTEMU_GUIDED) $(HOSTEMU_DELTA)
+# the error estimate's per-pixel functions (halves.h; tests/hostemu/hostemu_halves.cu)
+HOSTEMU_HALVES := tests/hostemu/_build/libhostemu_halves.so
+hostemu: $(HOSTEMU) $(HOSTEMU_LIST) $(HOSTEMU_DENOISE) $(HOSTEMU_SLIM) $(HOSTEMU_REPROJECT) $(HOSTEMU_GUIDED) $(HOSTEMU_DELTA) $(HOSTEMU_HALVES)
 $(HOSTEMU): tests/hostemu/hostemu.cu $(CSRC)/kdbuild.cpp $(CSRC)/bvhbuild.cpp $(HDRS)
 	@mkdir -p $(dir $@)
 	nvcc -std=c++17 -O2 -DRPTB_HOST_EMU -DRPTB_BUILD_BVH8=1 -DRPTB_BUILD_BVH4=1 -gencode arch=compute_90a,code=sm_90a -Xcompiler -fPIC,-fopenmp,-ffp-contract=off -shared -Xlinker -Bsymbolic -o $@ tests/hostemu/hostemu.cu $(CSRC)/kdbuild.cpp $(CSRC)/bvhbuild.cpp -lgomp
@@ -120,6 +127,9 @@ $(HOSTEMU_GUIDED): tests/hostemu/hostemu_guided.cu tests/hostemu/hostemu_denoise
 $(HOSTEMU_DELTA): tests/hostemu/hostemu_delta.cu $(HDRS)
 	@mkdir -p $(dir $@)
 	nvcc -std=c++17 -O2 -DRPTB_HOST_EMU -gencode arch=compute_90a,code=sm_90a -Xcompiler -fPIC,-ffp-contract=off -shared -Xlinker -Bsymbolic -o $@ tests/hostemu/hostemu_delta.cu
+$(HOSTEMU_HALVES): tests/hostemu/hostemu_halves.cu $(HDRS)
+	@mkdir -p $(dir $@)
+	nvcc -std=c++17 -O2 -DRPTB_HOST_EMU -gencode arch=compute_90a,code=sm_90a -Xcompiler -fPIC,-fopenmp,-ffp-contract=off -shared -Xlinker -Bsymbolic -o $@ tests/hostemu/hostemu_halves.cu -lgomp
 
 clean:
 	rm -rf build $(LIB) $(ORACLE) tests/hostemu/_build

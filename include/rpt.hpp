@@ -262,8 +262,11 @@ private:
 // Owns its device memory; it may outlive the Renderer that made it.
 class DeviceBuffer {
 public:
-    DeviceBuffer(rptb_scene* scene, uint32_t w, uint32_t h, Filter f = {}) : width_(w), height_(h) {
-        if (rptb_buffer_create(scene, w, h, f.radius, &handle_) != RPTB_OK) throw std::runtime_error(rptb_last_error());
+    // halves: also keep the sums of each pixel's odd entries (rptb_buffer_create_halves), from which denoised_error()
+    // estimates the denoised image's error; everything else is the same bits either way.
+    DeviceBuffer(rptb_scene* scene, uint32_t w, uint32_t h, Filter f = {}, bool halves = false) : width_(w), height_(h) {
+        const int rc = halves ? rptb_buffer_create_halves(scene, w, h, f.radius, &handle_) : rptb_buffer_create(scene, w, h, f.radius, &handle_);
+        if (rc != RPTB_OK) throw std::runtime_error(rptb_last_error());
     }
     ~DeviceBuffer() { if (handle_) rptb_buffer_destroy(handle_); }
     DeviceBuffer(const DeviceBuffer&) = delete;
@@ -337,6 +340,19 @@ public:
     std::vector<double> denoised_variance(const rptb_denoise& d) const {
         std::vector<double> out((size_t)width_ * height_);
         check(rptb_buffer_denoise_variance(handle_, &d, out.data()));
+        return out;
+    }
+    // A buffer with halves: the sums of each pixel's odd entries (rptb_buffer_half_sums), 3 per pixel, row-major.
+    std::vector<double> half_sums() const {
+        std::vector<double> out((size_t)width_ * height_ * 3);
+        check(rptb_buffer_half_sums(handle_, out.data()));
+        return out;
+    }
+    // A buffer with halves: E, the variance of each pixel of denoise(d) estimated from the two halves
+    // (rptb_buffer_denoise_error), one double per pixel, row-major; d.iterations >= 1.
+    std::vector<double> denoised_error(const rptb_denoise& d) const {
+        std::vector<double> out((size_t)width_ * height_);
+        check(rptb_buffer_denoise_error(handle_, &d, out.data()));
         return out;
     }
     // Carries src's entries over a camera move into this buffer, which holds features and no entries
@@ -447,6 +463,18 @@ public:
         const rptb_camera c = camera();
         uint64_t active = 0;
         if (rptb_sample_into_guided(handle_, &c, &p, &criterion, &guide, buffer.handle(), &active, nullptr) != RPTB_OK)
+            throw std::runtime_error(rptb_last_error());
+        next_sample_ += iterations;
+        return active;
+    }
+    // The same on E, the error estimate from two half buffers (rptb_sample_into_guided_error): the buffer needs halves and
+    // guide.iterations >= 1.
+    uint64_t sample_on_error(uint32_t iterations, DeviceBuffer& buffer, const rptb_adaptive& criterion, const rptb_denoise& guide) {
+        ensure_scene();
+        const rptb_render_params p = params(iterations);
+        const rptb_camera c = camera();
+        uint64_t active = 0;
+        if (rptb_sample_into_guided_error(handle_, &c, &p, &criterion, &guide, buffer.handle(), &active, nullptr) != RPTB_OK)
             throw std::runtime_error(rptb_last_error());
         next_sample_ += iterations;
         return active;

@@ -529,6 +529,36 @@ int rptb_sample_into_guided(rptb_scene* scene, const rptb_camera* camera, const 
                             const rptb_adaptive* criterion, const rptb_denoise* guide, rptb_buffer* buffer,
                             uint64_t* out_active /* nullable, forces sync */, rptb_stats* stats /* nullable, forces sync */);
 
+/* ---- The denoised image's error from two half buffers ------------------------------------------------------
+ * v' (rptb_buffer_denoise_variance) treats each pass's inputs as independent and underestimates the variance of the
+ * denoised value.  A buffer with halves keeps one more plane, HALF: the sums of each pixel's odd entries (entry k,
+ * k the pixel's count before the add, for odd k) -- 24 more bytes a pixel.  Every way an entry arrives (rptb_sample_into,
+ * the adaptive and guided calls, rptb_buffer_add_samples) follows the rule, and everything else a buffer returns is
+ * the same bits as a plain buffer's given the same calls, for any device count.
+ * The filter runs over the scaled difference of the two halves' means with the weights it computes from the whole
+ * buffer, and the square of the result, remodulated, averaged over the channels and smoothed over 3x3, is E: an
+ * estimate of each pixel's variance of the denoised value that accounts for the correlation between passes.
+ * rpt_b200/csrc/halves.h gives every formula and its order of operations.
+ * A buffer with halves is not a reprojection's or merge's dst, nor an import's (RPTB_ERR_UNSUPPORTED): history and
+ * shards carry no halves.  It may be a reprojection's src.  There is no shard buffer with halves.
+ * Arguments and refusals of create as rptb_buffer_create.                                                      */
+int rptb_buffer_create_halves(rptb_scene* scene, uint32_t width, uint32_t height, uint32_t box_radius, rptb_buffer** out);
+/* The HALF plane: width*height*3 doubles, row-major.  RPTB_ERR_BAD_ARG: a buffer without halves.              */
+int rptb_buffer_half_sums(rptb_buffer* buffer, double* out);
+/* E, the error estimate of rptb_buffer_denoise(params)'s output, in the units of v': width*height doubles, row-major.
+ * A pixel with fewer than 2 entries in either half's sense (n_B = 0) gives no difference and no weight; where no
+ * finite tap is left, E is NaN.  Refusals as rptb_buffer_denoise, and RPTB_ERR_BAD_ARG: a buffer without halves,
+ * params->iterations == 0 (there is no filter to estimate).                                                  */
+int rptb_buffer_denoise_error(rptb_buffer* buffer, const rptb_denoise* params, double* out);
+/* rptb_sample_into_guided with E in place of v': a pixel with n entries is active iff
+ *     n < min_entries   or   NOT( E <= (rel_tol * m' + abs_tol)^2 ),
+ * m' as in rptb_sample_into_guided.  The same flow, checks, refusals, plain mark while no pixel can hold min_entries,
+ * out_active and stats.  Besides: RPTB_ERR_BAD_ARG: a buffer without halves, guide->iterations == 0;
+ * RPTB_ERR_UNSUPPORTED: a shard buffer, the wavefront engine.                                                    */
+int rptb_sample_into_guided_error(rptb_scene* scene, const rptb_camera* camera, const rptb_render_params* params,
+                                  const rptb_adaptive* criterion, const rptb_denoise* guide, rptb_buffer* buffer,
+                                  uint64_t* out_active /* nullable, forces sync */, rptb_stats* stats /* nullable, forces sync */);
+
 /* ---- Reprojecting the device Buffer across a camera move ---------------------------------------------------
  * The temporal half of SVGF for a static scene: each pixel of `dst`'s view finds, through its own first-hit depth,
  * the world point it sees, projects it into `src`'s view and takes the history of the (up to four, bilinear) src

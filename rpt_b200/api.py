@@ -845,13 +845,25 @@ class Adaptive:
     while the variance of its denoised value, v' (DeviceBuffer.denoised_variance), exceeds (rel_tol * m' + abs_tol)^2,
     m' the channel mean of its denoised colour.  The buffer needs features (Renderer.sample_features) and entries made
     through the renderer's camera alone; guide.iterations == 0 is the plain criterion.  rpt_b200/csrc/guided.h gives
-    every formula; DESIGN.md section 6e what it buys and where it loses."""
+    every formula; DESIGN.md section 6e what it buys and where it loses.
+    `estimate` (with a guide): which variance of the denoised value the test uses.  "filter" (the default) is v', the
+    filter's own; "halves" is E (DeviceBuffer.denoised_error, rptb_sample_into_guided_error), estimated from two half
+    buffers, which needs a buffer with halves (Renderer.device_buffer(halves=True)) and guide.iterations >= 1.  v'
+    underestimates the variance 10-31x, E 4-7x; with E, rel_tol 0.05 is the recommended setting (DESIGN.md section 6g,
+    BASELINE.md section 3.0h)."""
 
-    def __init__(self, rel_tol: float = 0.02, abs_tol: float = 1e-3, min_entries: int = 4, guide: Optional["Denoise"] = None):
+    ESTIMATES = ("filter", "halves")
+
+    def __init__(self, rel_tol: float = 0.02, abs_tol: float = 1e-3, min_entries: int = 4, guide: Optional["Denoise"] = None,
+                 estimate: str = "filter"):
         self.rel_tol, self.abs_tol, self.min_entries = float(rel_tol), float(abs_tol), int(min_entries)
         if guide is not None and not isinstance(guide, Denoise):
             raise TypeError(f"guide must be an api.Denoise, not {type(guide).__name__}")
-        self.guide = guide
+        if estimate not in Adaptive.ESTIMATES:
+            raise ValueError(f"estimate must be one of {Adaptive.ESTIMATES}, not {estimate!r}")
+        if estimate == "halves" and guide is None:
+            raise ValueError('estimate="halves" estimates the denoised value\'s error: it needs a guide (Denoise)')
+        self.guide, self.estimate = guide, estimate
 
     def to_c(self) -> capi.Adaptive:
         return capi.Adaptive(self.rel_tol, self.abs_tol, self.min_entries, 0)
@@ -965,15 +977,19 @@ class DeviceBuffer:
 
     shard: Optional[tuple] = None  # (shard_index, shard_count) of a distributed.ShardBuffer; None = the whole image
 
-    def __init__(self, scene: DeviceScene, width: int, height: int, filter: Optional[Filter] = None):
+    def __init__(self, scene: DeviceScene, width: int, height: int, filter: Optional[Filter] = None, halves: bool = False):
+        """`halves`: also keep the sums of each pixel's odd entries (rptb_buffer_create_halves, 24 more bytes a pixel),
+        from which denoised_error() estimates the denoised image's error.  Everything else is the same bits either way."""
         self.width, self.height = int(width), int(height)
         self.filter = filter or Filter()
         self.devices = list(scene.devices)
         self.entries = 0  # the most entries any pixel holds (every pixel, without adaptive calls)
         self.feature_rays = 0  # camera rays per pixel in the features (Renderer.sample_features)
+        self.halves = bool(halves)
         self.handle = C.c_void_p()
-        capi.check(capi.lib().rptb_buffer_create(scene.handle, self.width, self.height, self.filter.radius,
-                                                 C.byref(self.handle)), "rptb_buffer_create")
+        create = capi.lib().rptb_buffer_create_halves if self.halves else capi.lib().rptb_buffer_create
+        capi.check(create(scene.handle, self.width, self.height, self.filter.radius, C.byref(self.handle)),
+                   "rptb_buffer_create_halves" if self.halves else "rptb_buffer_create")
 
     def add_samples(self, samples) -> None:  # :32-40
         samples = np.ascontiguousarray(np.asarray(samples, dtype=np.float64).reshape(-1, 3))
@@ -1047,6 +1063,23 @@ class DeviceBuffer:
         c = (d or Denoise()).to_c()
         capi.check(capi.lib().rptb_buffer_denoise_variance(self.handle, C.byref(c), out.ctypes.data_as(capi.c_double_p)),
                    "rptb_buffer_denoise_variance")
+        return out
+
+    def half_sums(self) -> np.ndarray:
+        """(width * height, 3) per-pixel sums of the odd entries (entry k, counted from 0, for odd k), row-major.  Needs
+        a buffer with halves."""
+        out = np.empty((self.width * self.height, 3), np.float64)
+        capi.check(capi.lib().rptb_buffer_half_sums(self.handle, out.ctypes.data_as(capi.c_double_p)), "rptb_buffer_half_sums")
+        return out
+
+    def denoised_error(self, d: Optional[Denoise] = None) -> np.ndarray:
+        """E, the variance of each pixel of denoise(d) estimated from two half buffers (rptb_buffer_denoise_error): (H, W)
+        float64, in the units of denoised_variance().  Unlike v' it accounts for the correlation between the filter's
+        passes (DESIGN.md section 6g).  Needs a buffer with halves and d.iterations >= 1; otherwise refusals as denoise()."""
+        out = np.empty((self.height, self.width))
+        c = (d or Denoise()).to_c()
+        capi.check(capi.lib().rptb_buffer_denoise_error(self.handle, C.byref(c), out.ctypes.data_as(capi.c_double_p)),
+                   "rptb_buffer_denoise_error")
         return out
 
     def denoised_image(self, d: Optional[Denoise] = None) -> np.ndarray:
@@ -1198,9 +1231,10 @@ class Renderer:
             self._dev_scene.close()
             self._dev_scene = None
 
-    def device_buffer(self) -> DeviceBuffer:
-        """A DeviceBuffer of this renderer's size and filter on the GPUs of its device scene."""
-        return DeviceBuffer(self.device_scene(), self._width, self._height, self._filter)
+    def device_buffer(self, halves: bool = False) -> DeviceBuffer:
+        """A DeviceBuffer of this renderer's size and filter on the GPUs of its device scene; `halves`: one with halves
+        (DeviceBuffer), which Adaptive(estimate="halves") needs."""
+        return DeviceBuffer(self.device_scene(), self._width, self._height, self._filter, halves=halves)
 
     # ---- the seam: Renderer::sample (:117-129) ---------------------------------
     _NO_GUIDE_BUFFER = object()
@@ -1211,8 +1245,8 @@ class Renderer:
         host memory; a DeviceBuffer gets it on the device, and the call returns once the work is enqueued unless
         `want_stats` (then last_stats is filled, which waits for the render).
         `adaptive` (DeviceBuffer only): add the entry only to the pixels the criterion leaves active
-        (rptb_sample_into_adaptive, or rptb_sample_into_guided with adaptive.guide); returns how many pixels got it,
-        which waits for the call.
+        (rptb_sample_into_adaptive, or rptb_sample_into_guided with adaptive.guide, or rptb_sample_into_guided_error with
+        estimate="halves"); returns how many pixels got it, which waits for the call.
         A distributed.ShardBuffer renders and adds its own shard's tiles only; `adaptive` then counts its pixels.
         `guide_buffer` (a ShardBuffer with a guided `adaptive`; rptb_sample_into_guided_shard): the whole DeviceBuffer the
         shard's filter runs over -- every shard gathered with features on this rank's device, at the shard's current state
@@ -1227,7 +1261,13 @@ class Renderer:
                 raise TypeError("adaptive sampling needs a DeviceBuffer (Renderer.device_buffer())")
             stats, active, crit = capi.Stats(), C.c_uint64(0), adaptive.to_c()
             st = C.byref(stats) if want_stats else None
-            if adaptive.guide is not None and guide_buffer is not Renderer._NO_GUIDE_BUFFER:
+            if adaptive.estimate == "halves" and guide_buffer is not Renderer._NO_GUIDE_BUFFER:
+                raise ValueError('estimate="halves" is not supported on shards')
+            if adaptive.estimate == "halves":
+                guide = adaptive.guide.to_c()
+                capi.check(capi.lib().rptb_sample_into_guided_error(ds.handle, C.byref(cam), C.byref(p), C.byref(crit), C.byref(guide),
+                                                                    buffer.handle, C.byref(active), st), "rptb_sample_into_guided_error")
+            elif adaptive.guide is not None and guide_buffer is not Renderer._NO_GUIDE_BUFFER:
                 guide = adaptive.guide.to_c()
                 capi.check(capi.lib().rptb_sample_into_guided_shard(ds.handle, C.byref(cam), C.byref(p), C.byref(crit), C.byref(guide),
                                                                     buffer.handle, guide_buffer.handle if guide_buffer is not None else None,
@@ -1304,6 +1344,8 @@ class Renderer:
             raise ValueError(f"num_samples {self._num_samples} must be a multiple of entries {entries} (and entries >= 1)")
         if denoise is not None and entries < 2 and adaptive is None:
             raise ValueError("a denoised frame needs entries >= 2 (or adaptive entries)")
+        if adaptive is not None and adaptive.estimate == "halves":
+            raise ValueError('estimate="halves" is not supported in frame loops: reprojected history has no halves')
         if history_test is not None:
             if history_test.fresh_entries < 2 or history_test.fresh_entries > entries:
                 raise ValueError(f"history_test.fresh_entries {history_test.fresh_entries} must lie in [2, entries {entries}]")
@@ -1368,7 +1410,18 @@ class Renderer:
         host Buffer.  The callback receives whichever it is.  `adaptive` (needs a DeviceBuffer): every batch renders
         only the pixels the criterion leaves active, and the render stops early after a batch that rendered none.  A
         guided criterion (adaptive.guide) needs features: a buffer that holds none first gets `feature_samples` feature
-        rays per pixel through this renderer's camera."""
+        rays per pixel through this renderer's camera.  With estimate="halves" and no buffer, the loop makes its own
+        DeviceBuffer with halves (destroyed when it returns)."""
+        own = None
+        if buffer is None and adaptive is not None and adaptive.estimate == "halves":
+            buffer = own = self.device_buffer(halves=True)
+        try:
+            self._iterate(callback_interval, callback, buffer, adaptive, feature_samples)
+        finally:
+            if own is not None:
+                own.close()
+
+    def _iterate(self, callback_interval, callback, buffer, adaptive, feature_samples) -> None:
         device = buffer is not None
         if adaptive is not None and not device:
             raise TypeError("adaptive sampling needs a DeviceBuffer (Renderer.device_buffer())")

@@ -40,7 +40,9 @@ cudaError_t launch_film_variance(const double* batches, uint32_t nbatches, uint6
 // the device Buffer: film.cu
 cudaError_t launch_buffer_accumulate(const float* in32, const double* in64, bool rowmajor, const uint8_t* mask, uint64_t nelem,
                                      uint32_t width, uint32_t height, uint32_t shard_index, uint32_t shard_count, double* sums,
-                                     double* m2, uint32_t* counts, cudaStream_t stream);
+                                     double* m2, uint32_t* counts, double* half, cudaStream_t stream);
+cudaError_t launch_buffer_half_scatter(const double* src, double* dst, uint64_t nelem, uint32_t width, uint32_t height, uint32_t shard_index,
+                                       uint32_t shard_count, cudaStream_t stream);
 cudaError_t launch_buffer_move(bool compact, const PlaneSet& src, const PlaneSet& dst, uint64_t nelem, uint32_t width, uint32_t height,
                                uint32_t shard_index, uint32_t shard_count, cudaStream_t stream);
 uint32_t buffer_variance_blocks(uint64_t npixels);
@@ -76,6 +78,11 @@ cudaError_t launch_denoise_passes(const double* sums, const double* m2, const ui
                                   const double* albedo, uint32_t width, uint32_t height, const rptb_denoise& d, double* const col[2],
                                   double* const var[2], const double** out_col, const double** out_var, cudaStream_t stream,
                                   uint32_t* launches);
+// the error estimate from two half buffers: halves.cu
+cudaError_t launch_halves_error(const double* sums, const double* m2, const double* half, const uint32_t* counts, const double* nrm,
+                                const double* depth, const double* albedo, uint32_t width, uint32_t height, const rptb_denoise& d,
+                                double* const col[2], double* const var[2], double* const u[2], double* E, const double** out_col,
+                                cudaStream_t stream, uint32_t* launches);
 // the reprojection and the least count: reproject.cu
 cudaError_t launch_reproject(const ReprojectView& dv, const ReprojectView& sv, const ReprojectSource& s, const double* dnrm,
                              const double* ddepth, const double* dfrac, const rptb_reproject& prm, double* sums, double* m2,
@@ -601,13 +608,15 @@ void destroy_replica(rptb_scene* s) {
 // or on the part's own (rptb_buffer_add_samples) -- and every later operation on the part waits for it.
 
 // One copy of a buffer's per-pixel planes (planes.h), n elements a plane.  Each group is null until allocated: the
-// colour planes, one allocation each, and the feature sums, one allocation of FEATURE_SUMS doubles an element.
+// colour planes, one allocation each, the feature sums, one allocation of FEATURE_SUMS doubles an element, and the HALF
+// plane of a buffer with halves (not in a PlaneSet: it moves by its own kernel).
 struct Planes {
     size_t n = 0;
     double* sums = nullptr;
     double* m2 = nullptr;
     uint32_t* counts = nullptr;
     double* feat = nullptr;
+    double* half = nullptr;
     // the allocated planes of `mask`
     PlaneSet set(uint32_t mask) const {
         const FeaturePlanes f = feat ? feature_planes(feat, n) : FeaturePlanes{};
@@ -673,6 +682,8 @@ struct rptb_buffer {
     // rptb_buffer_create_shard: the buffer holds one shard of the image (parts[0]'s index and count), and its whole-image
     // reads are refused until the shards are gathered into a whole buffer (rptb_buffer_import_shards)
     bool shard = false;
+    // rptb_buffer_create_halves: every part holds the HALF plane, and every accumulate adds a pixel's odd entries to it
+    bool halves = false;
     CameraRecord entry_cam, feat_cam;
     // The delta exchange (rptb_buffer_export_delta, rptb_buffer_import_deltas) checks against `state`, which every call
     // that changes the buffer bumps: an entry, a feature pass, a host entry, a reprojection or merge, an import.
@@ -691,6 +702,7 @@ struct rptb_buffer {
     uint64_t feature_rays = 0;       // camera rays per pixel in the feature sums
     double* aov = nullptr;           // with the feature rows, width*height*8: the resolved features (buffer_aov)
     double* dn = nullptr;            // the denoiser's, width*height*11: colour (3) and variance ping-pong planes, then c' (3)
+    double* hv = nullptr;            // the error estimate's (halves.cu), width*height*7: u (3) ping-pong planes, then E
     // allocated by the first guided adaptive call on a buffer of several parts: the mask and flags of parts[1..] (as many
     // tiles as the largest holds, *132 bytes) marked here before they go to the part, and their active pixel count
     uint8_t* guide_mask = nullptr;
@@ -743,18 +755,21 @@ int planes_alloc(std::vector<void*>& mem, Planes& s, size_t n, uint32_t mask) {
         CU(own(mem, &s.counts, plane_bytes(COUNTS, n)));
     }
     if ((mask & FEATURES) && !s.feat) CU(own(mem, &s.feat, n * FEATURE_SUMS * sizeof(double)));
+    if ((mask >> HALF & 1u) && !s.half) CU(own(mem, &s.half, plane_bytes(HALF, n)));
     return RPTB_OK;
 }
 
-int buffer_part_alloc(BufferPart& q) {
+// halves: the part also holds the HALF plane (rptb_buffer_create_halves).
+int buffer_part_alloc(BufferPart& q, bool halves) {
     CU(cudaStreamCreateWithFlags(&q.stream, cudaStreamNonBlocking));
     CU(cudaEventCreateWithFlags(&q.done, cudaEventDisableTiming));
     if (q.tiles) {
-        const int rc = planes_alloc(q.mem, q.planes, (size_t)q.tiles * 128u, COLOUR);
+        const int rc = planes_alloc(q.mem, q.planes, (size_t)q.tiles * 128u, COLOUR | (halves ? 1u << HALF : 0u));
         if (rc != RPTB_OK) return rc;
         const PlaneSet s = q.planes.set(COLOUR);  // sums() of an empty buffer reads zero
         for (int k = 0; k < NPLANES; k++)
             if (s.p[k]) CU(cudaMemsetAsync(s.p[k], 0, plane_bytes(k, q.planes.n), q.stream));
+        if (halves) CU(cudaMemsetAsync(q.planes.half, 0, plane_bytes(HALF, q.planes.n), q.stream));
     }
     CU(cudaEventRecord(q.done, q.stream));
     return RPTB_OK;
@@ -799,7 +814,8 @@ int buffer_scatter(rptb_buffer* b, const PlaneSet& src, uint32_t mask, uint32_t 
 }
 
 // Brings the planes of `mask` from every part to parts[0]'s device in row-major order, on parts[0]'s stream (the caller
-// has made that device current): part 0 straight from its own planes, the others through the staging.
+// has made that device current): part 0 straight from its own planes, the others through the staging.  HALF in `mask`:
+// a buffer with halves only.
 int buffer_gather(rptb_buffer* b, uint32_t mask) {
     const BufferPart& q0 = b->parts[0];
     int rc = buffer_rows_alloc(b, mask);
@@ -810,6 +826,10 @@ int buffer_gather(rptb_buffer* b, uint32_t mask) {
         const PlaneSet src = i == 0 ? q.planes.set(mask) : b->staging.set(mask);
         if (i > 0) rc = copy_planes(src, q0.device, q.planes.set(mask), q.device, q.planes.n, q0.stream);
         if (rc == RPTB_OK) rc = buffer_scatter(b, src, mask, q.index, q.count);
+        if (rc != RPTB_OK || !(mask >> HALF & 1u)) continue;
+        const double* half = i == 0 ? q.planes.half : b->staging.half;
+        if (i > 0) CU(cudaMemcpyPeerAsync(b->staging.half, q0.device, q.planes.half, q.device, plane_bytes(HALF, q.planes.n), q0.stream));
+        CU(launch_buffer_half_scatter(half, b->rows.half, q.planes.n, b->width, b->height, q.index, q.count, q0.stream));
     }
     return rc;
 }
@@ -940,7 +960,7 @@ int sample_part(rptb_scene* r, const rptb_camera* cam, const rptb_render_params*
     if (want_stats && !crit) CU(cudaEventRecord(r->ev1, r->stream));
     const bool f32 = p->precision == RPTB_PRECISION_F32;
     CU(launch_buffer_accumulate(f32 ? r->out32 : nullptr, f32 ? nullptr : r->out64, false, crit ? q.mask : nullptr, nelem, p->width,
-                                p->height, index, nparts, q.planes.sums, q.planes.m2, q.planes.counts, r->stream));
+                                p->height, index, nparts, q.planes.sums, q.planes.m2, q.planes.counts, q.planes.half, r->stream));
     // (an adaptive call times the whole entry: select, render and accumulate; a plain one its render)
     if (want_stats && crit) CU(cudaEventRecord(r->ev1, r->stream));
     (*launches)++;
@@ -1568,15 +1588,17 @@ int rptb_film_resolve(const double* sums, uint32_t nbatches, uint32_t width, uin
 }
 
 // A whole buffer (shard_count == 0: one part per replica of s, part i dealt (i, nparts)) or the one-part shard buffer of
-// (shard_index, shard_count) on s's device.  The arguments are checked by the callers.
+// (shard_index, shard_count) on s's device; `halves`: a whole buffer with the HALF plane.  The arguments are checked by
+// the callers.
 static int buffer_create_impl(rptb_scene* s, uint32_t width, uint32_t height, uint32_t box_radius, uint32_t shard_index,
-                              uint32_t shard_count, rptb_buffer** out) {
+                              uint32_t shard_count, rptb_buffer** out, bool halves = false) {
     rptb_buffer* b = new (std::nothrow) rptb_buffer();
     if (!b) return fail(RPTB_ERR_OOM, "host allocation failed");
     b->width = width;
     b->height = height;
     b->radius = box_radius;
     b->shard = shard_count > 0;
+    b->halves = halves;
     const uint32_t nparts = b->shard ? 1u : 1u + (uint32_t)s->peers.size();
     b->parts.resize(nparts);
     int rc = RPTB_OK;
@@ -1587,7 +1609,7 @@ static int buffer_create_impl(rptb_scene* s, uint32_t width, uint32_t height, ui
         q.count = b->shard ? shard_count : nparts;
         q.tiles = buffer_tiles(width, height, q.index, q.count);
         DeviceGuard g(q.device);
-        rc = g.ok ? buffer_part_alloc(q) : fail(RPTB_ERR_CUDA, "cudaSetDevice(%d) failed", q.device);
+        rc = g.ok ? buffer_part_alloc(q, halves) : fail(RPTB_ERR_CUDA, "cudaSetDevice(%d) failed", q.device);
     }
     if (rc != RPTB_OK) {
         const std::string keep = g_error;
@@ -1605,6 +1627,14 @@ int rptb_buffer_create(rptb_scene* s, uint32_t width, uint32_t height, uint32_t 
     if (width == 0 || height == 0) return fail(RPTB_ERR_BAD_ARG, "empty image %ux%u", width, height);
     if ((uint64_t)width * height > 0x7FFFFFFFull / 4) return fail(RPTB_ERR_UNSUPPORTED, "image too large");
     return buffer_create_impl(s, width, height, box_radius, 0, 0, out);
+}
+
+int rptb_buffer_create_halves(rptb_scene* s, uint32_t width, uint32_t height, uint32_t box_radius, rptb_buffer** out) {
+    if (!s || !out) return fail(RPTB_ERR_BAD_ARG, "null argument");
+    *out = nullptr;
+    if (width == 0 || height == 0) return fail(RPTB_ERR_BAD_ARG, "empty image %ux%u", width, height);
+    if ((uint64_t)width * height > 0x7FFFFFFFull / 4) return fail(RPTB_ERR_UNSUPPORTED, "image too large");
+    return buffer_create_impl(s, width, height, box_radius, 0, 0, out, true);
 }
 
 int rptb_buffer_create_shard(rptb_scene* s, uint32_t width, uint32_t height, uint32_t box_radius, uint32_t shard_index,
@@ -1645,7 +1675,10 @@ static int check_guide_buffer(const rptb_buffer* b, const rptb_camera* cam) {
 // it.  Every part holds its select scratch.  *launches: kernels enqueued.
 // `shard` (rptb_sample_into_guided_shard): the filter runs over b, the gathered whole buffer, and the mark kernel once,
 // for the shard's one part on parts[0]'s device, whose later work is ordered behind it; b's parts are not marked.
-static int guide_mark(rptb_buffer* b, const rptb_adaptive& crit, const rptb_denoise& d, uint32_t* launches, BufferPart* shard = nullptr) {
+// `error` (rptb_sample_into_guided_error, a buffer with halves): the HALF plane is gathered too, the filter runs with the
+// error estimate (halves.cu), and the mark tests E in place of v'.
+static int guide_mark(rptb_buffer* b, const rptb_adaptive& crit, const rptb_denoise& d, uint32_t* launches, BufferPart* shard = nullptr,
+                      bool error = false) {
     BufferPart& q0 = b->parts[0];
     DeviceGuard g(q0.device);
     if (!g.ok) return fail(RPTB_ERR_CUDA, "cudaSetDevice(%d) failed", q0.device);
@@ -1655,11 +1688,12 @@ static int guide_mark(rptb_buffer* b, const rptb_adaptive& crit, const rptb_deno
         if (i > 0) most = std::max(most, b->parts[i].tiles);
         nl += b->parts[i].tiles ? 1u : 0u;  // the gather's scatter
     }
-    int rc = buffer_gather(b, COLOUR | FEATURES);
+    int rc = buffer_gather(b, COLOUR | FEATURES | (error ? 1u << HALF : 0u));
     if (rc != RPTB_OK) return rc;
     const Aov a = buffer_aov(b);
     CU(launch_features_resolve(feature_planes(b->rows.feat, npix), npix, (double)b->feature_rays, a, q0.stream));
     if (!b->dn) CU(own(b->mem, &b->dn, npix * 11 * sizeof(double)));
+    if (error && !b->hv) CU(own(b->mem, &b->hv, npix * 7 * sizeof(double)));
     if (most && !b->guide_mask) {
         CU(own(b->mem, &b->guide_mask, (size_t)most * 132u));
         CU(own(b->mem, &b->guide_active, sizeof(unsigned long long)));
@@ -1668,9 +1702,16 @@ static int guide_mark(rptb_buffer* b, const rptb_adaptive& crit, const rptb_deno
     double* const var[2] = {b->dn + 6 * npix, b->dn + 7 * npix};
     const double *icol, *ivar;
     uint32_t passes = 0;
-    CU(launch_denoise_passes(b->rows.sums, b->rows.m2, b->rows.counts, a.normal, a.depth, a.albedo, b->width, b->height, d, col, var,
-                             &icol, &ivar, q0.stream, &passes));
-    nl += 1u + passes;
+    if (error) {
+        double* const u[2] = {b->hv, b->hv + 3 * npix};
+        ivar = b->hv + 6 * npix;  // E
+        CU(launch_halves_error(b->rows.sums, b->rows.m2, b->rows.half, b->rows.counts, a.normal, a.depth, a.albedo, b->width, b->height, d,
+                               col, var, u, b->hv + 6 * npix, &icol, q0.stream, &passes));
+    } else {
+        CU(launch_denoise_passes(b->rows.sums, b->rows.m2, b->rows.counts, a.normal, a.depth, a.albedo, b->width, b->height, d, col, var,
+                                 &icol, &ivar, q0.stream, &passes));
+    }
+    nl += 1u + passes;  // the features' resolve and the filter
     if (shard) {
         CU(cudaStreamWaitEvent(q0.stream, shard->done, 0));  // the shard's last accumulate and export read its mask
         CU(launch_guided_mark(icol, ivar, a.albedo, b->rows.counts, b->width, b->height, shard->index, shard->count, shard->tiles,
@@ -1732,15 +1773,16 @@ static int check_guide_whole(const rptb_buffer* shard, const rptb_buffer* whole,
 
 // rptb_sample_into (crit null), rptb_sample_into_adaptive (crit) and rptb_sample_into_guided (crit and guide; the
 // filter runs when guide->iterations > 0).  shard_entry (rptb_sample_into_guided_shard): b is a shard buffer and the
-// filter runs over `whole`.
+// filter runs over `whole`.  error (rptb_sample_into_guided_error): b has halves, and the mark tests E.
 static int sample_into_impl(rptb_scene* s, const rptb_camera* cam, const rptb_render_params* p, const rptb_adaptive* crit,
                             const rptb_denoise* guide, rptb_buffer* b, uint64_t* out_active, rptb_stats* stats, bool shard_entry = false,
-                            rptb_buffer* whole = nullptr) {
+                            rptb_buffer* whole = nullptr, bool error = false) {
     int rc = check_render_into(s, cam, p, b);
     if (rc != RPTB_OK) return rc;
     if (crit && p->engine == RPTB_ENGINE_WAVEFRONT)
         return fail(RPTB_ERR_UNSUPPORTED, "adaptive sampling renders with the slot megakernel, not the wavefront engine");
     if (guide && b->shard && !shard_entry) return refuse_shard("guided adaptive sampling");
+    if (error && !b->halves) return fail(RPTB_ERR_BAD_ARG, "the buffer has no halves (rptb_buffer_create_halves): no error estimate");
     if (shard_entry && !b->shard)
         return fail(RPTB_ERR_BAD_ARG, "not a shard buffer (rptb_buffer_create_shard): a whole buffer samples with rptb_sample_into_guided");
     const uint32_t nparts = (uint32_t)b->parts.size();
@@ -1775,7 +1817,7 @@ static int sample_into_impl(rptb_scene* s, const rptb_camera* cam, const rptb_re
             rc = buffer_part_select_alloc(q);
             if (rc != RPTB_OK) return rc;
         }
-        rc = guide_mark(b, *crit, *guide, &guide_launches);
+        rc = guide_mark(b, *crit, *guide, &guide_launches, nullptr, error);
         if (rc != RPTB_OK) return rc;
     }
     // every replica's share is enqueued before any is waited for, so the devices run concurrently
@@ -1874,6 +1916,15 @@ int rptb_sample_into_guided(rptb_scene* s, const rptb_camera* cam, const rptb_re
     return sample_into_impl(s, cam, p, crit, guide, b, out_active, stats);
 }
 
+int rptb_sample_into_guided_error(rptb_scene* s, const rptb_camera* cam, const rptb_render_params* p, const rptb_adaptive* crit,
+                                  const rptb_denoise* guide, rptb_buffer* b, uint64_t* out_active, rptb_stats* stats) {
+    int rc = check_adaptive(crit);
+    if (rc == RPTB_OK) rc = check_denoise(guide);
+    if (rc != RPTB_OK) return rc;
+    if (guide->iterations == 0) return fail(RPTB_ERR_BAD_ARG, "iterations 0: the error estimate needs at least one filter pass");
+    return sample_into_impl(s, cam, p, crit, guide, b, out_active, stats, false, nullptr, true);
+}
+
 int rptb_sample_into_guided_shard(rptb_scene* s, const rptb_camera* cam, const rptb_render_params* p, const rptb_adaptive* crit,
                                   const rptb_denoise* guide, rptb_buffer* shard, rptb_buffer* whole, uint64_t* out_active,
                                   rptb_stats* stats) {
@@ -1899,7 +1950,7 @@ int rptb_buffer_add_samples(rptb_buffer* b, const double* rgb) {
         // pageable source: the call returns once the bytes are staged, `rgb` may be reused afterwards
         CU(cudaMemcpyAsync(q.upload, rgb, nvals * sizeof(double), cudaMemcpyHostToDevice, q.stream));
         CU(launch_buffer_accumulate(nullptr, q.upload, true, nullptr, (uint64_t)q.tiles * 128u, b->width, b->height, q.index, q.count,
-                                    q.planes.sums, q.planes.m2, q.planes.counts, q.stream));
+                                    q.planes.sums, q.planes.m2, q.planes.counts, q.planes.half, q.stream));
         CU(cudaEventRecord(q.done, q.stream));
     }
     b->entries++;
@@ -2151,6 +2202,48 @@ int rptb_buffer_denoise_variance(rptb_buffer* b, const rptb_denoise* d, double* 
     return RPTB_OK;
 }
 
+int rptb_buffer_half_sums(rptb_buffer* b, double* out) {
+    if (!b || !out) return fail(RPTB_ERR_BAD_ARG, "null argument");
+    if (!b->halves) return fail(RPTB_ERR_BAD_ARG, "the buffer has no halves (rptb_buffer_create_halves)");
+    std::lock_guard<std::mutex> bl(b->lock);
+    BufferPart& q0 = b->parts[0];
+    DeviceGuard g(q0.device);
+    const int rc = buffer_gather(b, 1u << HALF);
+    if (rc != RPTB_OK) return rc;
+    CU(cudaMemcpyAsync(out, b->rows.half, plane_bytes(HALF, (size_t)b->width * b->height), cudaMemcpyDeviceToHost, q0.stream));
+    CU(cudaStreamSynchronize(q0.stream));
+    return RPTB_OK;
+}
+
+int rptb_buffer_denoise_error(rptb_buffer* b, const rptb_denoise* d, double* out) {
+    if (!b || !out) return fail(RPTB_ERR_BAD_ARG, "null argument");
+    int rc = check_denoise(d);
+    if (rc != RPTB_OK) return rc;
+    if (d->iterations == 0) return fail(RPTB_ERR_BAD_ARG, "iterations 0: the error estimate needs at least one filter pass");
+    if (b->shard) return refuse_shard("denoise_error");
+    if (!b->halves) return fail(RPTB_ERR_BAD_ARG, "the buffer has no halves (rptb_buffer_create_halves)");
+    std::lock_guard<std::mutex> bl(b->lock);
+    BufferPart& q0 = b->parts[0];
+    DeviceGuard g(q0.device);
+    Aov a;
+    rc = denoise_prepare(b, &a);
+    if (rc == RPTB_OK) rc = buffer_gather(b, 1u << HALF);
+    if (rc != RPTB_OK) return rc;
+    const size_t npix = (size_t)b->width * b->height;
+    if (!b->hv) CU(own(b->mem, &b->hv, npix * 7 * sizeof(double)));
+    double* const col[2] = {b->dn, b->dn + 3 * npix};
+    double* const var[2] = {b->dn + 6 * npix, b->dn + 7 * npix};
+    double* const u[2] = {b->hv, b->hv + 3 * npix};
+    double* E = b->hv + 6 * npix;
+    const double* icol;
+    uint32_t launches = 0;
+    CU(launch_halves_error(b->rows.sums, b->rows.m2, b->rows.half, b->rows.counts, a.normal, a.depth, a.albedo, b->width, b->height, *d,
+                           col, var, u, E, &icol, q0.stream, &launches));
+    CU(cudaMemcpyAsync(out, E, npix * sizeof(double), cudaMemcpyDeviceToHost, q0.stream));
+    CU(cudaStreamSynchronize(q0.stream));
+    return RPTB_OK;
+}
+
 // What a reprojection checks before it looks at the buffers: its arguments and parameters.
 static int check_reproject_params(const rptb_buffer* dst, const rptb_buffer* src, const rptb_reproject* prm) {
     if (!dst || !src || !prm) return fail(RPTB_ERR_BAD_ARG, "null argument");
@@ -2162,9 +2255,11 @@ static int check_reproject_params(const rptb_buffer* dst, const rptb_buffer* src
     return RPTB_OK;
 }
 
-// What a reprojection checks of the buffers (both locked): dst has features and no entries (a merge's dst: see
-// check_merge_dst instead), src has entries and features made through one camera, and neither camera has an open aperture.
+// What a reprojection checks of the buffers (both locked): dst has no halves (history has none; a halves src is fine),
+// features and no entries (a merge's dst: see check_merge_dst instead), src has entries and features made through one
+// camera, and neither camera has an open aperture.
 static int check_reproject_buffers(const rptb_buffer* dst, const rptb_buffer* src, bool merge) {
+    if (dst->halves) return fail(RPTB_ERR_UNSUPPORTED, "dst has halves: reprojected history has no halves (a halves src is fine)");
     if (!merge && dst->entries) return fail(RPTB_ERR_BAD_ARG, "dst already holds entries");
     if (dst->feature_rays == 0) return fail(RPTB_ERR_BAD_ARG, "dst holds no features (rptb_buffer_add_features)");
     if (src->entries == 0) return fail(RPTB_ERR_BAD_ARG, "src holds no entries");
@@ -2401,6 +2496,7 @@ int rptb_buffer_import_shards(rptb_buffer* dst, const void* gathered_device, uin
     if (!dst || !gathered_device) return fail(RPTB_ERR_BAD_ARG, "null argument");
     if (shard_count == 0) return fail(RPTB_ERR_BAD_ARG, "shard_count 0");
     if (dst->shard) return fail(RPTB_ERR_BAD_ARG, "dst is a shard buffer: the shards gather into a whole buffer (rptb_buffer_create)");
+    if (dst->halves) return fail(RPTB_ERR_UNSUPPORTED, "dst has halves: shards carry no halves");
     std::lock_guard<std::mutex> bl(dst->lock);
     BufferPart& d0 = dst->parts[0];
     DeviceGuard g(d0.device);
@@ -2531,6 +2627,7 @@ int rptb_buffer_import_deltas(rptb_buffer* dst, const void* gathered_device, uin
     if (!dst || !gathered_device) return fail(RPTB_ERR_BAD_ARG, "null argument");
     if (shard_count == 0) return fail(RPTB_ERR_BAD_ARG, "shard_count 0");
     if (dst->shard) return fail(RPTB_ERR_BAD_ARG, "dst is a shard buffer: the deltas go into the shards' gathered whole buffer");
+    if (dst->halves) return fail(RPTB_ERR_UNSUPPORTED, "dst has halves: shards carry no halves");
     if (dst->parts.size() != 1)
         return fail(RPTB_ERR_UNSUPPORTED, "dst has %zu parts: deltas are imported into a one-part whole buffer", dst->parts.size());
     std::lock_guard<std::mutex> bl(dst->lock);

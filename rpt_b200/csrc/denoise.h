@@ -99,18 +99,19 @@ RPTB_HD void denoise_grad(const double* __restrict__ depth, uint32_t width, uint
     gy = denoise_grad1(y > 0 ? depth[p - width] : 0.0, y > 0, z, y + 1 < height ? depth[p + width] : 0.0, y + 1 < height);
 }
 
-// One a-trous pass at pixel (x, y) with step h over row-major planes: col (3 per pixel) and var the current demodulated
-// colour and variance, nrm (3 per pixel), depth and albedo (3 per pixel) the resolved features.  Writes out_col[3], *out_var.
-RPTB_HD void denoise_pixel(const double* __restrict__ col, const double* __restrict__ var, const double* __restrict__ nrm,
-                           const double* __restrict__ depth, const double* __restrict__ albedo, uint32_t width, uint32_t height,
-                           uint32_t x, uint32_t y, uint32_t h, const rptb_denoise& d, double* out_col, double* out_var) {
+// The taps of one a-trous pass at pixel (x, y) with step h over row-major planes: col (3 per pixel) and var the current
+// demodulated colour and variance, nrm (3 per pixel), depth and albedo (3 per pixel) the resolved features.  Calls
+// tap(q, w, i_q (3), v_q) for every tap with its weight w, in tap order (a neighbour with w = 0 because its i or v is not
+// finite is not called), then tap.finish(p).  When p's own i or v is not finite it calls tap.keep(p, i_p (3), v_p) alone.
+// denoise_pixel and halves_pixel (halves.h) share it, so the error estimate runs over exactly the filter's weights.
+template <class Tap>
+RPTB_HD void denoise_taps(const double* __restrict__ col, const double* __restrict__ var, const double* __restrict__ nrm,
+                          const double* __restrict__ depth, const double* __restrict__ albedo, uint32_t width, uint32_t height,
+                          uint32_t x, uint32_t y, uint32_t h, const rptb_denoise& d, Tap& tap) {
     const size_t p = (size_t)y * width + x;
     const double ip0 = col[3 * p], ip1 = col[3 * p + 1], ip2 = col[3 * p + 2], vp = var[p];
     if (!(denoise_finite(ip0) && denoise_finite(ip1) && denoise_finite(ip2) && denoise_finite(vp))) {
-        out_col[0] = ip0;
-        out_col[1] = ip1;
-        out_col[2] = ip2;
-        *out_var = vp;
+        tap.keep(p, ip0, ip1, ip2, vp);
         return;
     }
     const double k5[5] = {1.0 / 16.0, 1.0 / 4.0, 3.0 / 8.0, 1.0 / 4.0, 1.0 / 16.0};
@@ -139,7 +140,6 @@ RPTB_HD void denoise_pixel(const double* __restrict__ col, const double* __restr
     const double A0 = albedo[3 * p] + d.albedo_eps, A1 = albedo[3 * p + 1] + d.albedo_eps, A2 = albedo[3 * p + 2] + d.albedo_eps;
     const double lp = denoise_lum(ip0 * A0, ip1 * A1, ip2 * A2);
     const double lden = d.sigma_luminance * ::sqrt(g) + kDenoiseEpsL;
-    double sw = 0.0, sww = 0.0, s0 = 0.0, s1 = 0.0, s2 = 0.0;
     for (int v = -2; v <= 2; v++)
         for (int u = -2; u <= 2; u++) {
             const int64_t dx = (int64_t)u * h, dy = (int64_t)v * h;
@@ -178,16 +178,45 @@ RPTB_HD void denoise_pixel(const double* __restrict__ col, const double* __restr
                 const double wl = ::exp(-(::fabs(lp - lq) / lden));
                 w = ((K * wn) * wz) * wl;
             }
-            sw = sw + w;
-            sww = sww + (w * w) * vq;
-            s0 = s0 + w * iq0;
-            s1 = s1 + w * iq1;
-            s2 = s2 + w * iq2;
+            tap(q, w, iq0, iq1, iq2, vq);
         }
-    out_col[0] = s0 / sw;
-    out_col[1] = s1 / sw;
-    out_col[2] = s2 / sw;
-    *out_var = sww / (sw * sw);
+    tap.finish(p);
+}
+
+// The filter's sums over the taps -- sum w, sum (w * w) v_q and sum w i_q, in tap order -- and its outputs out_col[3],
+// *out_var: i'_p = (sum w i_q) / (sum w), v'_p = (sum (w * w) v_q) / ((sum w) * (sum w)), or p's own i and v (keep).
+struct DenoiseSums {
+    double* out_col;
+    double* out_var;
+    double sw = 0.0, sww = 0.0, s0 = 0.0, s1 = 0.0, s2 = 0.0;
+    RPTB_HD DenoiseSums(double* c, double* v) : out_col(c), out_var(v) {}
+    RPTB_HD void operator()(size_t, double w, double iq0, double iq1, double iq2, double vq) {
+        sw = sw + w;
+        sww = sww + (w * w) * vq;
+        s0 = s0 + w * iq0;
+        s1 = s1 + w * iq1;
+        s2 = s2 + w * iq2;
+    }
+    RPTB_HD void keep(size_t, double ip0, double ip1, double ip2, double vp) {
+        out_col[0] = ip0;
+        out_col[1] = ip1;
+        out_col[2] = ip2;
+        *out_var = vp;
+    }
+    RPTB_HD void finish(size_t) {
+        out_col[0] = s0 / sw;
+        out_col[1] = s1 / sw;
+        out_col[2] = s2 / sw;
+        *out_var = sww / (sw * sw);
+    }
+};
+
+// One a-trous pass at pixel (x, y) with step h (planes as denoise_taps).  Writes out_col[3], *out_var.
+RPTB_HD void denoise_pixel(const double* __restrict__ col, const double* __restrict__ var, const double* __restrict__ nrm,
+                           const double* __restrict__ depth, const double* __restrict__ albedo, uint32_t width, uint32_t height,
+                           uint32_t x, uint32_t y, uint32_t h, const rptb_denoise& d, double* out_col, double* out_var) {
+    DenoiseSums s(out_col, out_var);
+    denoise_taps(col, var, nrm, depth, albedo, width, height, x, y, h, d, s);
 }
 
 }  // namespace rptb

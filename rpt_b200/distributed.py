@@ -416,7 +416,11 @@ class _GuidedShard:
 def _check_guided_world(adaptive, world: int) -> None:
     """A guided loop on shards keeps a gathered whole buffer on every rank and exchanges the ranks' deltas.  On one rank
     the shard is already the whole image, so that copy and that exchange would only add work to what the whole-buffer
-    loop does: refused, before any device work or collective, with the loop to use instead."""
+    loop does: refused, before any device work or collective, with the loop to use instead.  The error estimate from two
+    half buffers (estimate="halves") is refused on any world size: a shard buffer has no halves."""
+    if adaptive is not None and adaptive.estimate == "halves":
+        raise ValueError('estimate="halves" is not supported on shards: a shard buffer has no halves; one process renders it '
+                         "on one whole buffer: Renderer.iterative_render")
     if adaptive is not None and adaptive.guide is not None and world < 2:
         raise ValueError("guided adaptive sampling (Adaptive(guide=...)) on shards needs two or more ranks (torch.distributed "
                          "initialized); one process renders it on one whole buffer: Renderer.iterative_render / render_frames")

@@ -84,15 +84,9 @@ cudaError_t launch_halves_error(const double* sums, const double* m2, const doub
                                 double* const col[2], double* const var[2], double* const u[2], double* E, const double** out_col,
                                 cudaStream_t stream, uint32_t* launches);
 // the reprojection and the least count: reproject.cu
-cudaError_t launch_reproject(const ReprojectView& dv, const ReprojectView& sv, const ReprojectSource& s, const double* dnrm,
-                             const double* ddepth, const double* dfrac, const rptb_reproject& prm, double* sums, double* m2,
-                             uint32_t* counts, unsigned long long* reused, cudaStream_t stream);
 cudaError_t launch_reproject_part(const ReprojectView& dv, const ReprojectView& sv, const ReprojectSource& s, const FeaturePlanes& f,
                                   double rays, uint32_t index, uint32_t count, uint64_t nelem, const rptb_reproject& prm, double* sums,
                                   double* m2, uint32_t* counts, unsigned long long* reused, cudaStream_t stream);
-cudaError_t launch_reproject_merge(const ReprojectView& dv, const ReprojectView& sv, const ReprojectSource& s, const double* dnrm,
-                                   const double* ddepth, const double* dfrac, const rptb_reproject& prm, double gamma, double* sums,
-                                   double* m2, uint32_t* counts, unsigned long long* tally, cudaStream_t stream);
 cudaError_t launch_reproject_merge_part(const ReprojectView& dv, const ReprojectView& sv, const ReprojectSource& s,
                                         const FeaturePlanes& f, double rays, uint32_t index, uint32_t count, uint64_t nelem,
                                         const rptb_reproject& prm, double gamma, double* sums, double* m2, uint32_t* counts,
@@ -1668,63 +1662,87 @@ static int check_guide_buffer(const rptb_buffer* b, const rptb_camera* cam) {
     return RPTB_OK;
 }
 
-// A guided call's decision (rptb_sample_into_guided), enqueued on parts[0]'s stream: the buffer's colour and features
-// gathered row-major, the features resolved and the filter's passes run into b->dn, then the guided mark kernel once
-// per part -- into parts[0]'s own mask, flags and active count, and for every other part into the guide staging, whose
-// mask and flags (tiles*132 bytes) and count then go to the part's device.  Every part's later work is ordered behind
-// it.  Every part holds its select scratch.  *launches: kernels enqueued.
-// `shard` (rptb_sample_into_guided_shard): the filter runs over b, the gathered whole buffer, and the mark kernel once,
-// for the shard's one part on parts[0]'s device, whose later work is ordered behind it; b's parts are not marked.
-// `error` (rptb_sample_into_guided_error, a buffer with halves): the HALF plane is gathered too, the filter runs with the
-// error estimate (halves.cu), and the mark tests E in place of v'.
-static int guide_mark(rptb_buffer* b, const rptb_adaptive& crit, const rptb_denoise& d, uint32_t* launches, BufferPart* shard = nullptr,
-                      bool error = false) {
-    BufferPart& q0 = b->parts[0];
-    DeviceGuard g(q0.device);
-    if (!g.ok) return fail(RPTB_ERR_CUDA, "cudaSetDevice(%d) failed", q0.device);
+// The denoiser's planes: the resolved features, the colour and variance ping-pong planes and c' in b->dn, and the error
+// estimate's u ping-pong planes and E in b->hv.
+struct FilterPlanes {
+    Aov a;
+    double* col[2];
+    double* var[2];
+    double* out;
+    double* u[2];
+    double* E;
+};
+
+// What every run of the filter over b (locked, parts[0]'s device current) starts with, enqueued on parts[0]'s stream:
+// b's colour and features (and with `error` its HALF plane) gathered row-major and the features resolved; b->dn (and
+// b->hv) allocated on first use and carved into *f.
+static int filter_planes(rptb_buffer* b, bool error, FilterPlanes* f) {
     const size_t npix = (size_t)b->width * b->height;
-    uint32_t most = 0, nl = 0;
-    for (size_t i = 0; i < b->parts.size(); i++) {
-        if (i > 0) most = std::max(most, b->parts[i].tiles);
-        nl += b->parts[i].tiles ? 1u : 0u;  // the gather's scatter
-    }
-    int rc = buffer_gather(b, COLOUR | FEATURES | (error ? 1u << HALF : 0u));
+    const int rc = buffer_gather(b, COLOUR | FEATURES | (error ? 1u << HALF : 0u));
     if (rc != RPTB_OK) return rc;
     const Aov a = buffer_aov(b);
-    CU(launch_features_resolve(feature_planes(b->rows.feat, npix), npix, (double)b->feature_rays, a, q0.stream));
+    CU(launch_features_resolve(feature_planes(b->rows.feat, npix), npix, (double)b->feature_rays, a, b->parts[0].stream));
     if (!b->dn) CU(own(b->mem, &b->dn, npix * 11 * sizeof(double)));
-    if (error && !b->hv) CU(own(b->mem, &b->hv, npix * 7 * sizeof(double)));
+    *f = {a, {b->dn, b->dn + 3 * npix}, {b->dn + 6 * npix, b->dn + 7 * npix}, b->dn + 8 * npix, {nullptr, nullptr}, nullptr};
+    if (!error) return RPTB_OK;
+    if (!b->hv) CU(own(b->mem, &b->hv, npix * 7 * sizeof(double)));
+    f->u[0] = b->hv;
+    f->u[1] = b->hv + 3 * npix;
+    f->E = b->hv + 6 * npix;
+    return RPTB_OK;
+}
+
+// filter_planes, then the filter's passes (launch_denoise_passes), or with `error` the passes with the error estimate
+// (launch_halves_error, a buffer with halves).  *col: the plane holding the last pass's i'; *var: v', or with `error`
+// E; *launches: the filter's kernels.
+static int buffer_filter(rptb_buffer* b, const rptb_denoise& d, bool error, Aov* a, const double** col, const double** var,
+                         uint32_t* launches) {
+    FilterPlanes f;
+    const int rc = filter_planes(b, error, &f);
+    if (rc != RPTB_OK) return rc;
+    *a = f.a;
+    if (error) {
+        *var = f.E;
+        CU(launch_halves_error(b->rows.sums, b->rows.m2, b->rows.half, b->rows.counts, f.a.normal, f.a.depth, f.a.albedo, b->width,
+                               b->height, d, f.col, f.var, f.u, f.E, col, b->parts[0].stream, launches));
+    } else {
+        CU(launch_denoise_passes(b->rows.sums, b->rows.m2, b->rows.counts, f.a.normal, f.a.depth, f.a.albedo, b->width, b->height, d,
+                                 f.col, f.var, col, var, b->parts[0].stream, launches));
+    }
+    return RPTB_OK;
+}
+
+// A guided call's decision, enqueued on the stream of f's parts[0]: the filter over f (buffer_filter), then the guided
+// mark kernel once per part of b -- into parts[0]'s own mask, flags and active count, and for every other part into the
+// guide staging, whose mask and flags (tiles*132 bytes) and count then go to the part's device.  f is b itself
+// (rptb_sample_into_guided), or the gathered whole buffer on the device of b, a shard (rptb_sample_into_guided_shard).
+// Every later call on either buffer is ordered behind it.  Every part of b holds its select scratch.  `error`
+// (rptb_sample_into_guided_error, a buffer with halves): the filter runs with the error estimate, and the mark tests E
+// in place of v'.  *launches: kernels enqueued, the HALF plane's scatter aside.
+static int guide_mark(rptb_buffer* f, rptb_buffer* b, const rptb_adaptive& crit, const rptb_denoise& d, uint32_t* launches, bool error) {
+    BufferPart& q0 = f->parts[0];
+    DeviceGuard g(q0.device);
+    if (!g.ok) return fail(RPTB_ERR_CUDA, "cudaSetDevice(%d) failed", q0.device);
+    uint32_t most = 0, nl = 0;
+    for (const BufferPart& q : f->parts) nl += q.tiles ? 1u : 0u;  // the gather's scatter
+    for (size_t i = 1; i < b->parts.size(); i++) most = std::max(most, b->parts[i].tiles);
     if (most && !b->guide_mask) {
         CU(own(b->mem, &b->guide_mask, (size_t)most * 132u));
         CU(own(b->mem, &b->guide_active, sizeof(unsigned long long)));
     }
-    double* const col[2] = {b->dn, b->dn + 3 * npix};
-    double* const var[2] = {b->dn + 6 * npix, b->dn + 7 * npix};
+    Aov a;
     const double *icol, *ivar;
     uint32_t passes = 0;
-    if (error) {
-        double* const u[2] = {b->hv, b->hv + 3 * npix};
-        ivar = b->hv + 6 * npix;  // E
-        CU(launch_halves_error(b->rows.sums, b->rows.m2, b->rows.half, b->rows.counts, a.normal, a.depth, a.albedo, b->width, b->height, d,
-                               col, var, u, b->hv + 6 * npix, &icol, q0.stream, &passes));
-    } else {
-        CU(launch_denoise_passes(b->rows.sums, b->rows.m2, b->rows.counts, a.normal, a.depth, a.albedo, b->width, b->height, d, col, var,
-                                 &icol, &ivar, q0.stream, &passes));
-    }
+    int rc = buffer_filter(f, d, error, &a, &icol, &ivar, &passes);
+    if (rc != RPTB_OK) return rc;
     nl += 1u + passes;  // the features' resolve and the filter
-    if (shard) {
-        CU(cudaStreamWaitEvent(q0.stream, shard->done, 0));  // the shard's last accumulate and export read its mask
-        CU(launch_guided_mark(icol, ivar, a.albedo, b->rows.counts, b->width, b->height, shard->index, shard->count, shard->tiles,
-                              d.albedo_eps, crit, shard->mask, shard->flags, shard->active, q0.stream));
-        nl += shard->tiles ? 1u : 0u;
-        CU(cudaEventRecord(shard->done, q0.stream));
-    }
-    for (size_t i = 0; !shard && i < b->parts.size(); i++) {
+    for (size_t i = 0; i < b->parts.size(); i++) {
         BufferPart& q = b->parts[i];
         uint8_t* mask = i == 0 ? q.mask : b->guide_mask;
         uint8_t* flags = i == 0 ? q.flags : b->guide_mask + (size_t)most * 128u;
         unsigned long long* active = i == 0 ? q.active : b->guide_active;
-        CU(launch_guided_mark(icol, ivar, a.albedo, b->rows.counts, b->width, b->height, q.index, q.count, q.tiles, d.albedo_eps, crit,
+        CU(cudaStreamWaitEvent(q0.stream, q.done, 0));  // the part's last accumulate (and a shard's export) read its mask
+        CU(launch_guided_mark(icol, ivar, a.albedo, f->rows.counts, f->width, f->height, q.index, q.count, q.tiles, d.albedo_eps, crit,
                               mask, flags, active, q0.stream));
         nl += q.tiles ? 1u : 0u;
         if (i == 0) continue;
@@ -1735,7 +1753,9 @@ static int guide_mark(rptb_buffer* b, const rptb_adaptive& crit, const rptb_deno
         CU(cudaMemcpyPeerAsync(q.active, q.device, active, q0.device, sizeof(unsigned long long), q0.stream));
     }
     *launches = nl;
-    return buffer_order_behind(b, q0.stream);
+    rc = buffer_order_behind(b, q0.stream);
+    if (rc == RPTB_OK && f != b) rc = buffer_order_behind(f, q0.stream);
+    return rc;
 }
 
 static bool same_camera(const CameraRecord& a, const CameraRecord& b) {
@@ -1803,21 +1823,14 @@ static int sample_into_impl(rptb_scene* s, const rptb_camera* cam, const rptb_re
         if (rc != RPTB_OK) return rc;
     }
     uint32_t guide_launches = 0;
-    if (marked && shard_entry) {
-        DeviceGuard g(b->parts[0].device);
-        if (!g.ok) return fail(RPTB_ERR_CUDA, "cudaSetDevice(%d) failed", b->parts[0].device);
-        rc = buffer_part_select_alloc(b->parts[0]);
-        if (rc == RPTB_OK) rc = guide_mark(whole, *crit, *guide, &guide_launches, &b->parts[0]);
-        if (rc != RPTB_OK) return rc;
-    } else if (marked) {
-        for (uint32_t i = 0; i < nparts; i++) {
-            BufferPart& q = b->parts[i];
+    if (marked) {
+        for (BufferPart& q : b->parts) {
             DeviceGuard g(q.device);
             if (!g.ok) return fail(RPTB_ERR_CUDA, "cudaSetDevice(%d) failed", q.device);
             rc = buffer_part_select_alloc(q);
             if (rc != RPTB_OK) return rc;
         }
-        rc = guide_mark(b, *crit, *guide, &guide_launches, nullptr, error);
+        rc = guide_mark(shard_entry ? whole : b, b, *crit, *guide, &guide_launches, error);
         if (rc != RPTB_OK) return rc;
     }
     // every replica's share is enqueued before any is waited for, so the devices run concurrently
@@ -2127,27 +2140,25 @@ int rptb_buffer_features(rptb_buffer* b, double* normal, double* depth, double* 
     return RPTB_OK;
 }
 
-// What rptb_buffer_denoise and rptb_buffer_denoise_variance share, on the locked buffer with parts[0]'s device
-// current: the refusals, then the gathered colour and features, the resolved features and the filter's planes, enqueued
-// on parts[0]'s stream.
-static int denoise_prepare(rptb_buffer* b, Aov* a) {
+// What rptb_buffer_denoise, _variance and _error refuse before any device work.
+static int check_denoise_entries(const rptb_buffer* b) {
     if (b->entries == 0) return fail(RPTB_ERR_BAD_ARG, "Pixel found with no samples");  // buffer.rs:89
     // Every pixel holds at least min(entries, 2) entries, so this is exact for any mix of calls: the first call of any
     // kind reaches every pixel (an adaptive one because n = 0 < min_entries); plain calls and add_samples reach every
     // pixel; and rptb_sample_into_adaptive refuses min_entries < 2, so a pixel with one entry is always active.
     if (b->entries < 2) return fail(RPTB_ERR_BAD_ARG, "a pixel has fewer than 2 entries (no variance to guide the filter)");
     if (b->feature_rays == 0) return fail(RPTB_ERR_BAD_ARG, "the buffer holds no features (rptb_buffer_add_features)");
-    BufferPart& q0 = b->parts[0];
-    const size_t npix = (size_t)b->width * b->height;
-    uint32_t least = 0;  // a reprojected buffer does not keep the invariant above: look at the counts
-    int rc = buffer_gather(b, COLOUR | FEATURES);
-    if (rc == RPTB_OK) rc = buffer_least_count(b, &least);
+    return RPTB_OK;
+}
+
+// ... and once the filter's gather has brought the counts: a reprojected buffer does not keep the invariant above, so
+// its least count decides.
+static int check_denoise_counts(rptb_buffer* b) {
+    uint32_t least = 0;
+    const int rc = buffer_least_count(b, &least);
     if (rc != RPTB_OK) return rc;
     if (least == 0) return fail(RPTB_ERR_BAD_ARG, "Pixel found with no samples");  // buffer.rs:89
     if (least < 2) return fail(RPTB_ERR_BAD_ARG, "a pixel has fewer than 2 entries (no variance to guide the filter)");
-    *a = buffer_aov(b);
-    CU(launch_features_resolve(feature_planes(b->rows.feat, npix), npix, (double)b->feature_rays, *a, q0.stream));
-    if (!b->dn) CU(own(b->mem, &b->dn, npix * 11 * sizeof(double)));
     return RPTB_OK;
 }
 
@@ -2159,22 +2170,38 @@ int rptb_buffer_denoise(rptb_buffer* b, const rptb_denoise* d, double* out_rgb, 
     std::lock_guard<std::mutex> bl(b->lock);
     BufferPart& q0 = b->parts[0];
     DeviceGuard g(q0.device);
-    Aov a;
-    rc = denoise_prepare(b, &a);
+    FilterPlanes f;
+    rc = check_denoise_entries(b);
+    if (rc == RPTB_OK) rc = filter_planes(b, false, &f);
+    if (rc == RPTB_OK) rc = check_denoise_counts(b);
     if (rc != RPTB_OK) return rc;
     const size_t npix = (size_t)b->width * b->height;
-    double* const col[2] = {b->dn, b->dn + 3 * npix};
-    double* const var[2] = {b->dn + 6 * npix, b->dn + 7 * npix};
-    double* out = b->dn + 8 * npix;
     uint32_t launches = 0;
-    CU(launch_denoise(b->rows.sums, b->rows.m2, b->rows.counts, a.normal, a.depth, a.albedo, b->width, b->height, *d, col, var, out,
-                      q0.stream, &launches));
-    if (out_rgb) CU(cudaMemcpyAsync(out_rgb, out, npix * 3 * sizeof(double), cudaMemcpyDeviceToHost, q0.stream));
+    CU(launch_denoise(b->rows.sums, b->rows.m2, b->rows.counts, f.a.normal, f.a.depth, f.a.albedo, b->width, b->height, *d, f.col, f.var,
+                      f.out, q0.stream, &launches));
+    if (out_rgb) CU(cudaMemcpyAsync(out_rgb, f.out, npix * 3 * sizeof(double), cudaMemcpyDeviceToHost, q0.stream));
     if (out_rgb8) {
         // the film resolve of one entry at radius 0: clamp, gamma and the truncating cast of Buffer::image
-        CU(launch_film_resolve(out, 1u, b->width, b->height, 0u, b->rgb8, q0.stream));
+        CU(launch_film_resolve(f.out, 1u, b->width, b->height, 0u, b->rgb8, q0.stream));
         CU(cudaMemcpyAsync(out_rgb8, b->rgb8, npix * 3, cudaMemcpyDeviceToHost, q0.stream));
     }
+    CU(cudaStreamSynchronize(q0.stream));
+    return RPTB_OK;
+}
+
+// rptb_buffer_denoise_variance (v') and rptb_buffer_denoise_error (`error`: E), copied to out.
+static int denoise_read(rptb_buffer* b, const rptb_denoise& d, bool error, double* out) {
+    std::lock_guard<std::mutex> bl(b->lock);
+    BufferPart& q0 = b->parts[0];
+    DeviceGuard g(q0.device);
+    Aov a;
+    const double *icol, *ivar;
+    uint32_t launches = 0;
+    int rc = check_denoise_entries(b);
+    if (rc == RPTB_OK) rc = buffer_filter(b, d, error, &a, &icol, &ivar, &launches);
+    if (rc == RPTB_OK) rc = check_denoise_counts(b);
+    if (rc != RPTB_OK) return rc;
+    CU(cudaMemcpyAsync(out, ivar, (size_t)b->width * b->height * sizeof(double), cudaMemcpyDeviceToHost, q0.stream));
     CU(cudaStreamSynchronize(q0.stream));
     return RPTB_OK;
 }
@@ -2184,22 +2211,7 @@ int rptb_buffer_denoise_variance(rptb_buffer* b, const rptb_denoise* d, double* 
     int rc = check_denoise(d);
     if (rc != RPTB_OK) return rc;
     if (b->shard) return refuse_shard("denoise_variance");
-    std::lock_guard<std::mutex> bl(b->lock);
-    BufferPart& q0 = b->parts[0];
-    DeviceGuard g(q0.device);
-    Aov a;
-    rc = denoise_prepare(b, &a);
-    if (rc != RPTB_OK) return rc;
-    const size_t npix = (size_t)b->width * b->height;
-    double* const col[2] = {b->dn, b->dn + 3 * npix};
-    double* const var[2] = {b->dn + 6 * npix, b->dn + 7 * npix};
-    const double *icol, *ivar;
-    uint32_t launches = 0;
-    CU(launch_denoise_passes(b->rows.sums, b->rows.m2, b->rows.counts, a.normal, a.depth, a.albedo, b->width, b->height, *d, col, var,
-                             &icol, &ivar, q0.stream, &launches));
-    CU(cudaMemcpyAsync(out_var, ivar, npix * sizeof(double), cudaMemcpyDeviceToHost, q0.stream));
-    CU(cudaStreamSynchronize(q0.stream));
-    return RPTB_OK;
+    return denoise_read(b, *d, false, out_var);
 }
 
 int rptb_buffer_half_sums(rptb_buffer* b, double* out) {
@@ -2222,26 +2234,7 @@ int rptb_buffer_denoise_error(rptb_buffer* b, const rptb_denoise* d, double* out
     if (d->iterations == 0) return fail(RPTB_ERR_BAD_ARG, "iterations 0: the error estimate needs at least one filter pass");
     if (b->shard) return refuse_shard("denoise_error");
     if (!b->halves) return fail(RPTB_ERR_BAD_ARG, "the buffer has no halves (rptb_buffer_create_halves)");
-    std::lock_guard<std::mutex> bl(b->lock);
-    BufferPart& q0 = b->parts[0];
-    DeviceGuard g(q0.device);
-    Aov a;
-    rc = denoise_prepare(b, &a);
-    if (rc == RPTB_OK) rc = buffer_gather(b, 1u << HALF);
-    if (rc != RPTB_OK) return rc;
-    const size_t npix = (size_t)b->width * b->height;
-    if (!b->hv) CU(own(b->mem, &b->hv, npix * 7 * sizeof(double)));
-    double* const col[2] = {b->dn, b->dn + 3 * npix};
-    double* const var[2] = {b->dn + 6 * npix, b->dn + 7 * npix};
-    double* const u[2] = {b->hv, b->hv + 3 * npix};
-    double* E = b->hv + 6 * npix;
-    const double* icol;
-    uint32_t launches = 0;
-    CU(launch_halves_error(b->rows.sums, b->rows.m2, b->rows.half, b->rows.counts, a.normal, a.depth, a.albedo, b->width, b->height, *d,
-                           col, var, u, E, &icol, q0.stream, &launches));
-    CU(cudaMemcpyAsync(out, E, npix * sizeof(double), cudaMemcpyDeviceToHost, q0.stream));
-    CU(cudaStreamSynchronize(q0.stream));
-    return RPTB_OK;
+    return denoise_read(b, *d, true, out);
 }
 
 // What a reprojection checks before it looks at the buffers: its arguments and parameters.
@@ -2334,120 +2327,91 @@ static int reproject_finish(rptb_buffer* dst, const rptb_reproject* prm, bool me
     return RPTB_OK;
 }
 
-// rptb_buffer_reproject (gamma null) and rptb_buffer_reproject_merge (*gamma the test's threshold).
-static int reproject_whole(rptb_buffer* dst, rptb_buffer* src, const rptb_reproject* prm, const double* gamma, uint64_t* out_reused,
-                           uint64_t* out_rejected) {
+// rptb_buffer_reproject and rptb_buffer_reproject_shard (gamma null), rptb_buffer_reproject_merge and
+// rptb_buffer_reproject_merge_shard (*gamma the test's threshold); shard_entry: the _shard entry points, whose dst is a
+// shard buffer on src's first device.  Every dst part with tiles runs the per-element kernel over its own compact tiles
+// against src's gathered row-major state: part 0 in place, any other (on another device, no peer access assumed) through
+// the staging on parts[0]'s device.
+static int reproject_impl(rptb_buffer* dst, rptb_buffer* src, const rptb_reproject* prm, const double* gamma, uint64_t* out_reused,
+                          uint64_t* out_rejected, bool shard_entry) {
     int rc = check_reproject_params(dst, src, prm);
     if (rc != RPTB_OK) return rc;
     if (gamma && !(*gamma >= 0.0)) return fail(RPTB_ERR_BAD_ARG, "gamma must be >= 0 (%g)", *gamma);
-    if (dst->shard || src->shard) return refuse_shard(gamma ? "reproject_merge" : "reproject");
+    if (shard_entry && !dst->shard)
+        return fail(RPTB_ERR_BAD_ARG, "dst is not a shard buffer (rptb_buffer_create_shard): a whole one reprojects with %s",
+                    gamma ? "rptb_buffer_reproject_merge" : "rptb_buffer_reproject");
+    if ((dst->shard && !shard_entry) || src->shard) return refuse_shard(gamma ? "reproject_merge" : "reproject");
     std::scoped_lock both(dst->lock, src->lock);
+    BufferPart& d0 = dst->parts[0];
+    BufferPart& s0 = src->parts[0];
+    if (shard_entry && s0.device != d0.device)
+        return fail(RPTB_ERR_BAD_ARG, "src's first device %d is not the shard's device %d", s0.device, d0.device);
     bool same = dst->parts.size() == src->parts.size();
     for (size_t i = 0; same && i < dst->parts.size(); i++) same = dst->parts[i].device == src->parts[i].device;
-    if (!same) return fail(RPTB_ERR_BAD_ARG, "the buffers were created on scenes with different device lists");
+    if (!shard_entry && !same) return fail(RPTB_ERR_BAD_ARG, "the buffers were created on scenes with different device lists");
     rc = check_reproject_buffers(dst, src, gamma != nullptr);
     if (rc == RPTB_OK && gamma) rc = check_merge_dst(dst, prm);
     if (rc != RPTB_OK) return rc;
-    BufferPart& d0 = dst->parts[0];
-    BufferPart& s0 = src->parts[0];
     DeviceGuard g(d0.device);
     if (!g.ok) return fail(RPTB_ERR_CUDA, "cudaSetDevice(%d) failed", d0.device);
-    // src's state and both buffers' features (and a merge's fresh dst state), row-major on parts[0]'s device
-    const size_t dnpix = (size_t)dst->width * dst->height;
+    rc = reproject_scratch_alloc(dst);
+    if (rc != RPTB_OK) return rc;
+    if (!d0.tiles) {  // a shard with no pixel to reproject: the state alone, so that its exchange block agrees with the others'
+        if (out_reused) *out_reused = 0;
+        if (out_rejected) *out_rejected = 0;
+        return reproject_finish(dst, prm, gamma != nullptr, nullptr, nullptr, d0.stream);
+    }
+    size_t most = 0;  // the staging holds the largest other part
+    for (size_t i = 1; i < dst->parts.size(); i++) most = std::max(most, (size_t)dst->parts[i].tiles * 128u);
+    if (most) rc = planes_alloc(dst->mem, dst->staging, most, COLOUR | FEATURES);
     const bool count = out_reused || out_rejected;
     ReprojectSource sp;
-    rc = reproject_source(src, &sp);
-    if (rc == RPTB_OK) rc = buffer_rows_alloc(dst, COLOUR);
-    if (rc == RPTB_OK) rc = buffer_gather(dst, gamma ? COLOUR | FEATURES : FEATURES);
-    if (rc != RPTB_OK) return rc;
-    const Aov da = buffer_aov(dst);
-    CU(launch_features_resolve(feature_planes(dst->rows.feat, dnpix), dnpix, (double)dst->feature_rays, da, d0.stream));
-    rc = reproject_scratch_alloc(dst);
+    if (rc == RPTB_OK) rc = reproject_source(src, &sp);
     if (rc != RPTB_OK) return rc;
     CU(cudaStreamWaitEvent(d0.stream, s0.done, 0));
     if (count) CU(cudaMemsetAsync(dst->reused, 0, (gamma ? 2 : 1) * sizeof(unsigned long long), d0.stream));
     const ReprojectView dv = reproject_view(dst->feat_cam.cam, dst->width, dst->height);
     const ReprojectView sv = reproject_view(src->feat_cam.cam, src->width, src->height);
-    if (gamma)
-        CU(launch_reproject_merge(dv, sv, sp, da.normal, da.depth, da.frac, *prm, *gamma, dst->rows.sums, dst->rows.m2, dst->rows.counts,
-                                  count ? dst->reused : nullptr, d0.stream));
-    else
-        CU(launch_reproject(dv, sv, sp, da.normal, da.depth, da.frac, *prm, dst->rows.sums, dst->rows.m2, dst->rows.counts,
-                            count ? dst->reused : nullptr, d0.stream));
-    // back to every dst part's compact tiles; every later call on either buffer is ordered behind this one
-    rc = buffer_write_back(dst, COLOUR);
+    const uint32_t in = gamma ? COLOUR | FEATURES : FEATURES;  // a merge reads the fresh colour; a reprojection writes it all
+    for (size_t i = 0; rc == RPTB_OK && i < dst->parts.size(); i++) {
+        const BufferPart& q = dst->parts[i];
+        if (!q.tiles) continue;
+        CU(cudaStreamWaitEvent(d0.stream, q.done, 0));
+        const Planes& p = i == 0 ? q.planes : dst->staging;
+        if (i > 0) rc = copy_planes(p.set(in), d0.device, q.planes.set(in), q.device, q.planes.n, d0.stream);
+        if (rc != RPTB_OK) return rc;
+        const FeaturePlanes f = feature_planes(p.feat, p.n);
+        if (gamma)
+            CU(launch_reproject_merge_part(dv, sv, sp, f, (double)dst->feature_rays, q.index, q.count, q.planes.n, *prm, *gamma, p.sums,
+                                           p.m2, p.counts, count ? dst->reused : nullptr, d0.stream));
+        else
+            CU(launch_reproject_part(dv, sv, sp, f, (double)dst->feature_rays, q.index, q.count, q.planes.n, *prm, p.sums, p.m2, p.counts,
+                                     count ? dst->reused : nullptr, d0.stream));
+        if (i > 0) rc = copy_planes(q.planes.set(COLOUR), q.device, p.set(COLOUR), d0.device, q.planes.n, d0.stream);
+    }
+    // every later call on either buffer is ordered behind this one
     if (rc == RPTB_OK) rc = buffer_order_behind(dst, d0.stream);
     if (rc == RPTB_OK) rc = buffer_order_behind(src, d0.stream);
     if (rc != RPTB_OK) return rc;
     return reproject_finish(dst, prm, gamma != nullptr, out_reused, out_rejected, d0.stream);
 }
 
-// rptb_buffer_reproject_shard (gamma null) and rptb_buffer_reproject_merge_shard.
-static int reproject_shard(rptb_buffer* dst, rptb_buffer* src, const rptb_reproject* prm, const double* gamma, uint64_t* out_reused,
-                           uint64_t* out_rejected) {
-    int rc = check_reproject_params(dst, src, prm);
-    if (rc != RPTB_OK) return rc;
-    if (gamma && !(*gamma >= 0.0)) return fail(RPTB_ERR_BAD_ARG, "gamma must be >= 0 (%g)", *gamma);
-    if (!dst->shard)
-        return fail(RPTB_ERR_BAD_ARG, "dst is not a shard buffer (rptb_buffer_create_shard): a whole one reprojects with %s",
-                    gamma ? "rptb_buffer_reproject_merge" : "rptb_buffer_reproject");
-    if (src->shard) return refuse_shard(gamma ? "reproject_merge" : "reproject");
-    std::scoped_lock both(dst->lock, src->lock);
-    BufferPart& d0 = dst->parts[0];
-    BufferPart& s0 = src->parts[0];
-    if (s0.device != d0.device) return fail(RPTB_ERR_BAD_ARG, "src's first device %d is not the shard's device %d", s0.device, d0.device);
-    rc = check_reproject_buffers(dst, src, gamma != nullptr);
-    if (rc == RPTB_OK && gamma) rc = check_merge_dst(dst, prm);
-    if (rc != RPTB_OK) return rc;
-    DeviceGuard g(d0.device);
-    if (!g.ok) return fail(RPTB_ERR_CUDA, "cudaSetDevice(%d) failed", d0.device);
-    rc = reproject_scratch_alloc(dst);
-    if (rc != RPTB_OK) return rc;
-    if (!d0.tiles) {  // no pixel to reproject: the state alone, so that the shard's exchange block agrees with the others'
-        if (out_reused) *out_reused = 0;
-        if (out_rejected) *out_rejected = 0;
-        return reproject_finish(dst, prm, gamma != nullptr, nullptr, nullptr, d0.stream);
-    }
-    const bool count = out_reused || out_rejected;
-    ReprojectSource sp;
-    rc = reproject_source(src, &sp);
-    if (rc != RPTB_OK) return rc;
-    // the shard's own elements, in place in its compact planes; every later call on either buffer is ordered behind them
-    CU(cudaStreamWaitEvent(d0.stream, s0.done, 0));
-    CU(cudaStreamWaitEvent(d0.stream, d0.done, 0));
-    if (count) CU(cudaMemsetAsync(dst->reused, 0, (gamma ? 2 : 1) * sizeof(unsigned long long), d0.stream));
-    const ReprojectView dv = reproject_view(dst->feat_cam.cam, dst->width, dst->height);
-    const ReprojectView sv = reproject_view(src->feat_cam.cam, src->width, src->height);
-    const Planes& q = d0.planes;
-    const FeaturePlanes f = feature_planes(q.feat, q.n);
-    if (gamma)
-        CU(launch_reproject_merge_part(dv, sv, sp, f, (double)dst->feature_rays, d0.index, d0.count, q.n, *prm, *gamma, q.sums, q.m2,
-                                       q.counts, count ? dst->reused : nullptr, d0.stream));
-    else
-        CU(launch_reproject_part(dv, sv, sp, f, (double)dst->feature_rays, d0.index, d0.count, q.n, *prm, q.sums, q.m2, q.counts,
-                                 count ? dst->reused : nullptr, d0.stream));
-    rc = buffer_order_behind(dst, d0.stream);
-    if (rc == RPTB_OK) rc = buffer_order_behind(src, d0.stream);
-    if (rc != RPTB_OK) return rc;
-    return reproject_finish(dst, prm, gamma != nullptr, out_reused, out_rejected, d0.stream);
-}
-
 int rptb_buffer_reproject(rptb_buffer* dst, rptb_buffer* src, const rptb_reproject* prm, uint64_t* out_reused) {
-    return reproject_whole(dst, src, prm, nullptr, out_reused, nullptr);
+    return reproject_impl(dst, src, prm, nullptr, out_reused, nullptr, false);
 }
 
 int rptb_buffer_reproject_shard(rptb_buffer* dst, rptb_buffer* src, const rptb_reproject* prm, uint64_t* out_reused) {
-    return reproject_shard(dst, src, prm, nullptr, out_reused, nullptr);
+    return reproject_impl(dst, src, prm, nullptr, out_reused, nullptr, true);
 }
 
 int rptb_buffer_reproject_merge(rptb_buffer* dst, rptb_buffer* src, const rptb_reproject* prm, double gamma, uint64_t* out_reused,
                                 uint64_t* out_rejected) {
-    return reproject_whole(dst, src, prm, &gamma, out_reused, out_rejected);
+    return reproject_impl(dst, src, prm, &gamma, out_reused, out_rejected, false);
 }
 
 int rptb_buffer_reproject_merge_shard(rptb_buffer* dst, rptb_buffer* src, const rptb_reproject* prm, double gamma, uint64_t* out_reused,
                                       uint64_t* out_rejected) {
-    return reproject_shard(dst, src, prm, &gamma, out_reused, out_rejected);
+    return reproject_impl(dst, src, prm, &gamma, out_reused, out_rejected, true);
 }
 
 uint64_t rptb_buffer_shard_bytes(const rptb_buffer* b, uint32_t with_features) {

@@ -1,12 +1,10 @@
-// reproject.cu -- rptb_buffer_reproject on the device: one thread per destination pixel runs reproject_pixel
-// (reproject.h) over the gathered row-major state of both buffers on parts[0]'s device.  Compiled with -fmad=false:
-// reproject.h rounds every operation on its own, as its host emulation and tests/reproject_ref.py do.
+// reproject.cu -- rptb_buffer_reproject and rptb_buffer_reproject_shard on the device: one thread per element of a
+// destination part's compact tiles runs reproject_slot (reproject.h) against the source's gathered row-major state and
+// writes the part's colour planes in place.  Compiled with -fmad=false: reproject.h rounds every operation on its own,
+// as its host emulation and tests/reproject_ref.py do.
 //
-// rptb_buffer_reproject_shard: one thread per element of a shard part's compact tiles runs reproject_slot against the
-// same gathered source and writes the part's colour planes in place -- no row-major destination, no write-back.
-//
-// rptb_buffer_reproject_merge / _merge_shard: the same two shapes, but each thread merges the history into the pixel's
-// (element's) fresh colour planes in place when reproject_merge accepts it, and counts reused and rejected pixels.
+// rptb_buffer_reproject_merge / _merge_shard: the same, but each thread merges the history into the element's fresh
+// colour planes in place when reproject_merge accepts it, and counts reused and rejected pixels.
 //
 // Also the per-pixel minimum of a buffer's counts, which image / variance / denoise of a reprojected buffer check.
 #include <cuda_runtime.h>
@@ -14,25 +12,6 @@
 #include "reproject.h"
 
 namespace rptb {
-
-__global__ void __launch_bounds__(256) reproject_kernel(const ReprojectView dv, const ReprojectView sv, const ReprojectSource s,
-                                                        const double* __restrict__ dnrm, const double* __restrict__ ddepth,
-                                                        const double* __restrict__ dfrac, const rptb_reproject prm,
-                                                        double* __restrict__ sums, double* __restrict__ m2,
-                                                        uint32_t* __restrict__ counts, unsigned long long* __restrict__ reused) {
-    const uint64_t p = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    const uint64_t npix = (uint64_t)dv.width * dv.height;
-    uint32_t n = 0;
-    if (p < npix) {
-        const uint32_t x = (uint32_t)(p % dv.width), y = (uint32_t)(p / dv.width);
-        n = reproject_pixel(dv, sv, s, x, y, dnrm + 3 * p, ddepth[p], dfrac[p], prm, sums + 3 * p, m2 + p);
-        counts[p] = n;
-    }
-    if (reused) {  // every lane reaches the ballot: no early return above
-        const unsigned got = __ballot_sync(0xffffffffu, n > 0u);
-        if ((threadIdx.x & 31u) == 0u && got) atomicAdd(reused, (unsigned long long)__popc(got));
-    }
-}
 
 __global__ void __launch_bounds__(256) reproject_part_kernel(const ReprojectView dv, const ReprojectView sv, const ReprojectSource s,
                                                              const FeaturePlanes f, double rays, uint32_t index, uint32_t count,
@@ -60,23 +39,6 @@ __device__ __forceinline__ void merge_tally(int verdict, unsigned long long* tal
     }
 }
 
-__global__ void __launch_bounds__(256) reproject_merge_kernel(const ReprojectView dv, const ReprojectView sv, const ReprojectSource s,
-                                                              const double* __restrict__ dnrm, const double* __restrict__ ddepth,
-                                                              const double* __restrict__ dfrac, const rptb_reproject prm, double gamma,
-                                                              double* __restrict__ sums, double* __restrict__ m2,
-                                                              uint32_t* __restrict__ counts, unsigned long long* __restrict__ tally) {
-    const uint64_t p = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    const uint64_t npix = (uint64_t)dv.width * dv.height;
-    int verdict = 0;
-    if (p < npix) {
-        const uint32_t x = (uint32_t)(p % dv.width), y = (uint32_t)(p / dv.width);
-        double sh[3], m2h;
-        const uint32_t nh = reproject_pixel(dv, sv, s, x, y, dnrm + 3 * p, ddepth[p], dfrac[p], prm, sh, &m2h);
-        verdict = reproject_merge(sh, m2h, nh, gamma, sums + 3 * p, m2 + p, counts + p);
-    }
-    if (tally) merge_tally(verdict, tally);  // every lane reaches the ballots: no early return above
-}
-
 __global__ void __launch_bounds__(256) reproject_merge_part_kernel(const ReprojectView dv, const ReprojectView sv, const ReprojectSource s,
                                                                    const FeaturePlanes f, double rays, uint32_t index, uint32_t count,
                                                                    uint64_t nelem, const rptb_reproject prm, double gamma,
@@ -97,29 +59,12 @@ __global__ void __launch_bounds__(256) buffer_min_count_kernel(const uint32_t* _
     if ((threadIdx.x & 31u) == 0u) atomicMin(out, m);
 }
 
-cudaError_t launch_reproject(const ReprojectView& dv, const ReprojectView& sv, const ReprojectSource& s, const double* dnrm,
-                             const double* ddepth, const double* dfrac, const rptb_reproject& prm, double* sums, double* m2,
-                             uint32_t* counts, unsigned long long* reused, cudaStream_t stream) {
-    const uint64_t npix = (uint64_t)dv.width * dv.height;
-    reproject_kernel<<<(unsigned)((npix + 255) / 256), 256, 0, stream>>>(dv, sv, s, dnrm, ddepth, dfrac, prm, sums, m2, counts, reused);
-    return cudaGetLastError();
-}
-
 cudaError_t launch_reproject_part(const ReprojectView& dv, const ReprojectView& sv, const ReprojectSource& s, const FeaturePlanes& f,
                                   double rays, uint32_t index, uint32_t count, uint64_t nelem, const rptb_reproject& prm, double* sums,
                                   double* m2, uint32_t* counts, unsigned long long* reused, cudaStream_t stream) {
     if (nelem == 0) return cudaSuccess;
     reproject_part_kernel<<<(unsigned)((nelem + 255) / 256), 256, 0, stream>>>(dv, sv, s, f, rays, index, count, nelem, prm, sums, m2,
                                                                                counts, reused);
-    return cudaGetLastError();
-}
-
-cudaError_t launch_reproject_merge(const ReprojectView& dv, const ReprojectView& sv, const ReprojectSource& s, const double* dnrm,
-                                   const double* ddepth, const double* dfrac, const rptb_reproject& prm, double gamma, double* sums,
-                                   double* m2, uint32_t* counts, unsigned long long* tally, cudaStream_t stream) {
-    const uint64_t npix = (uint64_t)dv.width * dv.height;
-    reproject_merge_kernel<<<(unsigned)((npix + 255) / 256), 256, 0, stream>>>(dv, sv, s, dnrm, ddepth, dfrac, prm, gamma, sums, m2,
-                                                                               counts, tally);
     return cudaGetLastError();
 }
 

@@ -30,9 +30,10 @@
 // and the pixel gets sums mu_c * n_h, M2 s2 * (n_h - 1) and count n_h: the mean and the per-entry variance of its
 // neighbourhood, carried as if n_h entries had made them.
 //
-// A shard buffer (rptb_buffer_reproject_shard) runs the same function per element of its compact tiles (reproject_slot):
-// the element's pixel is tile_pixel's, its features resolve from the element's own feature sums (features_resolve,
-// denoise.h), and the source is whole and row-major as above.  So every pixel gets the bits the whole buffer's gets.
+// The device runs the function per element of each destination part's compact tiles (reproject_slot), for a whole
+// buffer and a shard buffer (rptb_buffer_reproject_shard) alike: the element's pixel is tile_pixel's, its features
+// resolve from the element's own feature sums (features_resolve, denoise.h), and the source is whole and row-major as
+// above.  So every pixel gets the bits reproject_pixel gives it over row-major features.
 //
 // Testing history against fresh entries (rptb_buffer_reproject_merge): dst already holds fresh entries S_f (3), M2_f, n_f
 // of its own view, and the history S_h, M2_h, n_h that reproject_pixel gives the pixel is merged in only where the two

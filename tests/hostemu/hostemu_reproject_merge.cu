@@ -21,9 +21,9 @@ void hostemu_merge_pixels(const double* hsums, const double* hm2, const uint32_t
         verdict[p] = reproject_merge(hsums + 3 * p, hm2[p], hcounts[p], gamma, sums + 3 * p, m2 + p, counts + p);
 }
 
-// reproject_merge_kernel on the host: at every pixel of a dw x dh view through dcam (resolved features dnrm, ddepth,
-// dfrac), the history reproject_pixel takes from the source (as hostemu_reproject's) merged into the fresh row-major
-// sums, m2, counts in place.  *out_reused / *out_rejected: the pixels of each verdict.
+// The merge over row-major pixels on the host: at every pixel of a dw x dh view through dcam (resolved features dnrm,
+// ddepth, dfrac), the history reproject_pixel takes from the source (as hostemu_reproject's) merged into the fresh
+// row-major sums, m2, counts in place.  *out_reused / *out_rejected: the pixels of each verdict.
 void hostemu_reproject_merge(const rptb_camera* dcam, uint32_t dw, uint32_t dh, const double* dnrm, const double* ddepth,
                              const double* dfrac, const rptb_camera* scam, uint32_t sw, uint32_t sh, const double* ssums, const double* sm2,
                              const uint32_t* scounts, const double* snrm, const double* sdepth, const double* sfrac,

@@ -15,9 +15,10 @@ card's name and power limit read in the same run).
   tsweep   the tested mode, raw and denoised, at 4 and 16 spp on the same orbits for HistoryTest gamma in {2, 3, 4, 6}
            x fresh_entries in {2, 4} (the default gamma's evidence), with the fresh spp rendered and the rejected fraction
   timing   rptb_buffer_reproject after warm-up, --reps calls, at 800x600 and 1920x1080 (Cornell): the device time of the
-           reprojection kernel, of the gather / feature-resolve kernels before it and of the copy back, per call, from
-           torch.profiler's CUDA kernel records; and the host clock of the whole call with out_reused (median).  The same
-           for rptb_buffer_reproject_merge into buffers holding two fresh entries (its kernel reproject_merge_kernel).
+           reprojection kernel (reproject_part_kernel), of the source's gather / feature-resolve kernels before it and of
+           the call's kernels together, per call, from torch.profiler's CUDA kernel records; and the host clock of the whole
+           call with out_reused (median).  The same for rptb_buffer_reproject_merge into buffers holding two fresh entries
+           (its kernel reproject_merge_part_kernel).
 
 python tools/reproject_measure.py [--quick] [--ref-spp N] [--frames N] [--step RAD] [--reps N]
                                   [--what timing,quality,sweep,tsweep]"""
@@ -185,17 +186,15 @@ def timing(args, gpu):
                 t = time.perf_counter()
                 capi.check(capi.lib().rptb_buffer_reproject(b.handle, src.handle, C.byref(prm), C.byref(n)), "rptb_buffer_reproject")
                 times.append((time.perf_counter() - t) * 1e3)
-        kern = gather = back = 0.0
+        kern = gather = 0.0
         for e in prof.key_averages():
             us = e.device_time_total if hasattr(e, "device_time_total") else e.cuda_time_total
-            if "reproject_kernel" in e.key:
+            if "reproject_part_kernel" in e.key:
                 kern += us
             elif "buffer_scatter" in e.key or "features_resolve" in e.key:
                 gather += us
-            elif "buffer_compact" in e.key:
-                back += us
-        print(json.dumps({"what": "timing", "size": [w, h], "reproject_kernel_ms": round(kern / 1e3 / args.reps, 4),
-                          "gather_resolve_kernels_ms": round(gather / 1e3 / args.reps, 4), "copy_back_kernel_ms": round(back / 1e3 / args.reps, 4),
+        print(json.dumps({"what": "timing", "size": [w, h], "reproject_part_kernel_ms": round(kern / 1e3 / args.reps, 4),
+                          "gather_resolve_kernels_ms": round(gather / 1e3 / args.reps, 4), "call_kernels_ms": round((kern + gather) / 1e3 / args.reps, 4),
                           "call_ms_host_clock": round(statistics.median(times), 3), "reused": int(n.value), "gpu": gpu}), flush=True)
         for b in dsts:
             b.close()
@@ -218,17 +217,15 @@ def timing(args, gpu):
                 capi.check(capi.lib().rptb_buffer_reproject_merge(b.handle, src.handle, C.byref(prm), gamma, C.byref(n), C.byref(j)),
                            "rptb_buffer_reproject_merge")
                 times.append((time.perf_counter() - t) * 1e3)
-        kern = gather = back = 0.0
+        kern = gather = 0.0
         for e in prof.key_averages():
             us = e.device_time_total if hasattr(e, "device_time_total") else e.cuda_time_total
-            if "reproject_merge_kernel" in e.key:
+            if "reproject_merge_part_kernel" in e.key:
                 kern += us
             elif "buffer_scatter" in e.key or "features_resolve" in e.key:
                 gather += us
-            elif "buffer_compact" in e.key:
-                back += us
-        print(json.dumps({"what": "timing_merge", "size": [w, h], "reproject_merge_kernel_ms": round(kern / 1e3 / args.reps, 4),
-                          "gather_resolve_kernels_ms": round(gather / 1e3 / args.reps, 4), "copy_back_kernel_ms": round(back / 1e3 / args.reps, 4),
+        print(json.dumps({"what": "timing_merge", "size": [w, h], "reproject_merge_part_kernel_ms": round(kern / 1e3 / args.reps, 4),
+                          "gather_resolve_kernels_ms": round(gather / 1e3 / args.reps, 4), "call_kernels_ms": round((kern + gather) / 1e3 / args.reps, 4),
                           "call_ms_host_clock": round(statistics.median(times), 3), "reused": int(n.value), "rejected": int(j.value),
                           "gamma": gamma, "gpu": gpu}), flush=True)
         for b in dsts:

@@ -2,7 +2,7 @@
 with the card's name and power limit read in the same run).
 
   kernels  single process: reproject_part_kernel summed over the n = 1, 2, 4, 8 shards of one destination (all
-           simulated in this process), against reproject_kernel on the whole destination, at 800x600 and 1920x1080
+           simulated in this process), against the same kernel on the whole destination, at 800x600 and 1920x1080
            (Cornell, a 0.02 rad orbit step), per call from torch.profiler's CUDA kernel records over --reps calls after
            warm-up.  Also the source's gather and feature-resolve kernels, which every shard's call runs once (one per
            rank in a real run; n times here).
@@ -48,16 +48,14 @@ def card(dev):
 
 
 def _kernel_ms(prof, reps):
-    part = whole = src = 0.0
+    part = src = 0.0
     for e in prof.key_averages():
         us = e.device_time_total if hasattr(e, "device_time_total") else e.cuda_time_total
         if "reproject_part_kernel" in e.key:
             part += us
-        elif "reproject_kernel" in e.key:
-            whole += us
         elif "buffer_scatter" in e.key or "features_resolve" in e.key:
             src += us
-    return part / 1e3 / reps, whole / 1e3 / reps, src / 1e3 / reps
+    return part / 1e3 / reps, src / 1e3 / reps
 
 
 def kernels(args, gpu):
@@ -86,7 +84,7 @@ def kernels(args, gpu):
             for b in wholes[3:]:
                 capi.check(capi.lib().rptb_buffer_reproject(b.handle, src.handle, C.byref(prm), C.byref(n_out)), "rptb_buffer_reproject")
         torch.cuda.synchronize()
-        _, whole_ms, whole_src_ms = _kernel_ms(prof, args.reps)
+        whole_ms, whole_src_ms = _kernel_ms(prof, args.reps)
         reused_whole = int(n_out.value)
         for b in wholes:
             b.close()
@@ -99,9 +97,9 @@ def kernels(args, gpu):
                 for shards in sets[3:]:
                     reused.append(sum(s.reproject_from(src) for s in shards))
             torch.cuda.synchronize()
-            part_ms, _, src_ms = _kernel_ms(prof, args.reps)
+            part_ms, src_ms = _kernel_ms(prof, args.reps)
             print(json.dumps({"what": "kernels", "size": [w, h], "shards": n, "reproject_part_kernel_ms_summed": round(part_ms, 4),
-                              "reproject_kernel_ms_whole": round(whole_ms, 4),
+                              "reproject_part_kernel_ms_whole": round(whole_ms, 4),
                               "source_gather_resolve_ms_per_shard_call": round(src_ms / n, 4),
                               "source_gather_resolve_ms_whole_call": round(whole_src_ms, 4),
                               "reused_sum_equals_whole": all(x == reused_whole for x in reused), "gpu": gpu}), flush=True)

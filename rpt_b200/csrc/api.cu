@@ -41,8 +41,6 @@ cudaError_t launch_film_variance(const double* batches, uint32_t nbatches, uint6
 cudaError_t launch_buffer_accumulate(const float* in32, const double* in64, bool rowmajor, const uint8_t* mask, uint64_t nelem,
                                      uint32_t width, uint32_t height, uint32_t shard_index, uint32_t shard_count, double* sums,
                                      double* m2, uint32_t* counts, double* half, cudaStream_t stream);
-cudaError_t launch_buffer_half_scatter(const double* src, double* dst, uint64_t nelem, uint32_t width, uint32_t height, uint32_t shard_index,
-                                       uint32_t shard_count, cudaStream_t stream);
 cudaError_t launch_buffer_move(bool compact, const PlaneSet& src, const PlaneSet& dst, uint64_t nelem, uint32_t width, uint32_t height,
                                uint32_t shard_index, uint32_t shard_count, cudaStream_t stream);
 uint32_t buffer_variance_blocks(uint64_t npixels);
@@ -603,7 +601,7 @@ void destroy_replica(rptb_scene* s) {
 
 // One copy of a buffer's per-pixel planes (planes.h), n elements a plane.  Each group is null until allocated: the
 // colour planes, one allocation each, the feature sums, one allocation of FEATURE_SUMS doubles an element, and the HALF
-// plane of a buffer with halves (not in a PlaneSet: it moves by its own kernel).
+// plane of a buffer with halves.
 struct Planes {
     size_t n = 0;
     double* sums = nullptr;
@@ -614,7 +612,7 @@ struct Planes {
     // the allocated planes of `mask`
     PlaneSet set(uint32_t mask) const {
         const FeaturePlanes f = feat ? feature_planes(feat, n) : FeaturePlanes{};
-        PlaneSet s = {{sums, m2, f.n, f.a, f.h, f.z, counts}};
+        PlaneSet s = {{sums, m2, f.n, f.a, f.h, f.z, counts, half}};
         for (int k = 0; k < NPLANES; k++)
             if (!(mask >> k & 1u)) s.p[k] = nullptr;
         return s;
@@ -664,6 +662,8 @@ struct CameraRecord {
         }
     }
 };
+// CameraRecord::State's names, for refusals
+const char* const camera_state_name[] = {"none", "one", "mixed (several cameras)", "unknown (a host entry)"};
 
 struct rptb_buffer {
     uint32_t width = 0, height = 0, radius = 0;
@@ -760,10 +760,9 @@ int buffer_part_alloc(BufferPart& q, bool halves) {
     if (q.tiles) {
         const int rc = planes_alloc(q.mem, q.planes, (size_t)q.tiles * 128u, COLOUR | (halves ? 1u << HALF : 0u));
         if (rc != RPTB_OK) return rc;
-        const PlaneSet s = q.planes.set(COLOUR);  // sums() of an empty buffer reads zero
+        const PlaneSet s = q.planes.set(COLOUR | 1u << HALF);  // sums() of an empty buffer reads zero
         for (int k = 0; k < NPLANES; k++)
             if (s.p[k]) CU(cudaMemsetAsync(s.p[k], 0, plane_bytes(k, q.planes.n), q.stream));
-        if (halves) CU(cudaMemsetAsync(q.planes.half, 0, plane_bytes(HALF, q.planes.n), q.stream));
     }
     CU(cudaEventRecord(q.done, q.stream));
     return RPTB_OK;
@@ -808,8 +807,7 @@ int buffer_scatter(rptb_buffer* b, const PlaneSet& src, uint32_t mask, uint32_t 
 }
 
 // Brings the planes of `mask` from every part to parts[0]'s device in row-major order, on parts[0]'s stream (the caller
-// has made that device current): part 0 straight from its own planes, the others through the staging.  HALF in `mask`:
-// a buffer with halves only.
+// has made that device current): part 0 straight from its own planes, the others through the staging.
 int buffer_gather(rptb_buffer* b, uint32_t mask) {
     const BufferPart& q0 = b->parts[0];
     int rc = buffer_rows_alloc(b, mask);
@@ -820,10 +818,6 @@ int buffer_gather(rptb_buffer* b, uint32_t mask) {
         const PlaneSet src = i == 0 ? q.planes.set(mask) : b->staging.set(mask);
         if (i > 0) rc = copy_planes(src, q0.device, q.planes.set(mask), q.device, q.planes.n, q0.stream);
         if (rc == RPTB_OK) rc = buffer_scatter(b, src, mask, q.index, q.count);
-        if (rc != RPTB_OK || !(mask >> HALF & 1u)) continue;
-        const double* half = i == 0 ? q.planes.half : b->staging.half;
-        if (i > 0) CU(cudaMemcpyPeerAsync(b->staging.half, q0.device, q.planes.half, q.device, plane_bytes(HALF, q.planes.n), q0.stream));
-        CU(launch_buffer_half_scatter(half, b->rows.half, q.planes.n, b->width, b->height, q.index, q.count, q0.stream));
     }
     return rc;
 }
@@ -974,11 +968,10 @@ constexpr size_t kShardHeaderBytes = 256;
 // ShardHeader::flags: the shard was reprojected (rptb_buffer_reproject_shard), so its pixels may hold 0 or 1 entries
 constexpr uint32_t kShardReprojected = 1u;
 struct ShardHeader {
-    uint32_t magic, with_features, width, height, shard_index, shard_count, entries, flags;
-    uint64_t feature_rays;
-    ShardCamera entry_cam, feat_cam;
+    uint32_t magic, with_features, width, height, shard_index, shard_count;
+    BlockState s;
 };
-static_assert(sizeof(ShardHeader) <= kShardHeaderBytes, "the shard header outgrew its slot");
+static_assert(offsetof(ShardHeader, s) == 24 && sizeof(ShardHeader) == 248, "the shard header's layout");
 
 struct ShardLayout {
     size_t slots;         // pixel slots of every plane: shard 0's tiles * 128
@@ -1020,6 +1013,28 @@ CameraRecord camera_record(const ShardCamera& c) {
     r.state = (CameraRecord::State)c.state;
     r.cam = c.cam;
     return r;
+}
+
+// b's state as an exchange header carries it
+BlockState block_state(const rptb_buffer* b) {
+    return {b->entries, b->reprojected ? kShardReprojected : 0u, b->feature_rays, shard_camera(b->entry_cam), shard_camera(b->feat_cam)};
+}
+
+bool same_state(const BlockState& x, const BlockState& y) { return std::memcmp(&x, &y, sizeof(BlockState)) == 0; }
+
+// The headers of the n blocks of `stride` bytes at `in` (device memory) into hs, waited for on `stream`: header 0 first,
+// and the others only once check0(hs[0]) has passed -- that it names the caller's size and count is what makes the
+// stride right.
+template <class H, class Check>
+int fetch_headers(const char* in, uint32_t n, uint64_t stride, cudaStream_t stream, std::vector<H>& hs, Check check0) {
+    hs.resize(n);
+    CU(cudaMemcpyAsync(hs.data(), in, sizeof(H), cudaMemcpyDeviceToHost, stream));
+    CU(cudaStreamSynchronize(stream));
+    const int rc = check0(hs[0]);
+    if (rc != RPTB_OK) return rc;
+    if (n > 1) CU(cudaMemcpy2DAsync(hs.data() + 1, sizeof(H), in + stride, stride, sizeof(H), n - 1, cudaMemcpyDeviceToHost, stream));
+    CU(cudaStreamSynchronize(stream));
+    return RPTB_OK;
 }
 
 // Whole-image reads need every tile: a shard buffer holds only its own.
@@ -1581,17 +1596,23 @@ int rptb_film_resolve(const double* sums, uint32_t nbatches, uint32_t width, uin
     return RPTB_OK;
 }
 
-// A whole buffer (shard_count == 0: one part per replica of s, part i dealt (i, nparts)) or the one-part shard buffer of
-// (shard_index, shard_count) on s's device; `halves`: a whole buffer with the HALF plane.  The arguments are checked by
-// the callers.
-static int buffer_create_impl(rptb_scene* s, uint32_t width, uint32_t height, uint32_t box_radius, uint32_t shard_index,
-                              uint32_t shard_count, rptb_buffer** out, bool halves = false) {
+// A whole buffer (one part per replica of s, part i dealt (i, nparts); `halves`: with the HALF plane) or, with `shard`,
+// the one-part shard buffer of (shard_index, shard_count) on s's device.
+static int buffer_create_impl(rptb_scene* s, uint32_t width, uint32_t height, uint32_t box_radius, rptb_buffer** out, bool halves,
+                              bool shard = false, uint32_t shard_index = 0, uint32_t shard_count = 0) {
+    if (!s || !out) return fail(RPTB_ERR_BAD_ARG, "null argument");
+    *out = nullptr;
+    if (width == 0 || height == 0) return fail(RPTB_ERR_BAD_ARG, "empty image %ux%u", width, height);
+    if ((uint64_t)width * height > 0x7FFFFFFFull / 4) return fail(RPTB_ERR_UNSUPPORTED, "image too large");
+    if (shard && shard_index >= shard_count) return fail(RPTB_ERR_BAD_ARG, "shard_index %u >= shard_count %u", shard_index, shard_count);
+    if (shard && !s->peers.empty())
+        return fail(RPTB_ERR_UNSUPPORTED, "a shard buffer lives on one device, but the scene has %u replicas", 1u + (uint32_t)s->peers.size());
     rptb_buffer* b = new (std::nothrow) rptb_buffer();
     if (!b) return fail(RPTB_ERR_OOM, "host allocation failed");
     b->width = width;
     b->height = height;
     b->radius = box_radius;
-    b->shard = shard_count > 0;
+    b->shard = shard;
     b->halves = halves;
     const uint32_t nparts = b->shard ? 1u : 1u + (uint32_t)s->peers.size();
     b->parts.resize(nparts);
@@ -1616,31 +1637,16 @@ static int buffer_create_impl(rptb_scene* s, uint32_t width, uint32_t height, ui
 }
 
 int rptb_buffer_create(rptb_scene* s, uint32_t width, uint32_t height, uint32_t box_radius, rptb_buffer** out) {
-    if (!s || !out) return fail(RPTB_ERR_BAD_ARG, "null argument");
-    *out = nullptr;
-    if (width == 0 || height == 0) return fail(RPTB_ERR_BAD_ARG, "empty image %ux%u", width, height);
-    if ((uint64_t)width * height > 0x7FFFFFFFull / 4) return fail(RPTB_ERR_UNSUPPORTED, "image too large");
-    return buffer_create_impl(s, width, height, box_radius, 0, 0, out);
+    return buffer_create_impl(s, width, height, box_radius, out, false);
 }
 
 int rptb_buffer_create_halves(rptb_scene* s, uint32_t width, uint32_t height, uint32_t box_radius, rptb_buffer** out) {
-    if (!s || !out) return fail(RPTB_ERR_BAD_ARG, "null argument");
-    *out = nullptr;
-    if (width == 0 || height == 0) return fail(RPTB_ERR_BAD_ARG, "empty image %ux%u", width, height);
-    if ((uint64_t)width * height > 0x7FFFFFFFull / 4) return fail(RPTB_ERR_UNSUPPORTED, "image too large");
-    return buffer_create_impl(s, width, height, box_radius, 0, 0, out, true);
+    return buffer_create_impl(s, width, height, box_radius, out, true);
 }
 
 int rptb_buffer_create_shard(rptb_scene* s, uint32_t width, uint32_t height, uint32_t box_radius, uint32_t shard_index,
                              uint32_t shard_count, rptb_buffer** out) {
-    if (!s || !out) return fail(RPTB_ERR_BAD_ARG, "null argument");
-    *out = nullptr;
-    if (width == 0 || height == 0) return fail(RPTB_ERR_BAD_ARG, "empty image %ux%u", width, height);
-    if ((uint64_t)width * height > 0x7FFFFFFFull / 4) return fail(RPTB_ERR_UNSUPPORTED, "image too large");
-    if (shard_index >= shard_count) return fail(RPTB_ERR_BAD_ARG, "shard_index %u >= shard_count %u", shard_index, shard_count);
-    if (!s->peers.empty())
-        return fail(RPTB_ERR_UNSUPPORTED, "a shard buffer lives on one device, but the scene has %u replicas", 1u + (uint32_t)s->peers.size());
-    return buffer_create_impl(s, width, height, box_radius, shard_index, shard_count, out);
+    return buffer_create_impl(s, width, height, box_radius, out, false, true, shard_index, shard_count);
 }
 
 void rptb_buffer_destroy(rptb_buffer* b) {
@@ -1651,12 +1657,11 @@ void rptb_buffer_destroy(rptb_buffer* b) {
 // through `cam` alone, so that the filter's features describe what the entries saw.
 static int check_guide_buffer(const rptb_buffer* b, const rptb_camera* cam) {
     if (b->feature_rays == 0) return fail(RPTB_ERR_BAD_ARG, "the buffer holds no features (rptb_buffer_add_features)");
-    const char* why[] = {"none", "one", "mixed (several cameras)", "unknown (a host entry)"};
-    if (b->feat_cam.state != CameraRecord::ONE) return fail(RPTB_ERR_BAD_ARG, "the buffer's features have no single camera: %s", why[b->feat_cam.state]);
+    if (b->feat_cam.state != CameraRecord::ONE) return fail(RPTB_ERR_BAD_ARG, "the buffer's features have no single camera: %s", camera_state_name[b->feat_cam.state]);
     if (std::memcmp(&b->feat_cam.cam, cam, sizeof(rptb_camera)) != 0)
         return fail(RPTB_ERR_BAD_ARG, "the buffer's features were made through another camera");
     if (b->entry_cam.state != CameraRecord::NONE && b->entry_cam.state != CameraRecord::ONE)
-        return fail(RPTB_ERR_BAD_ARG, "the buffer's entries have no single camera: %s", why[b->entry_cam.state]);
+        return fail(RPTB_ERR_BAD_ARG, "the buffer's entries have no single camera: %s", camera_state_name[b->entry_cam.state]);
     if (b->entry_cam.state == CameraRecord::ONE && std::memcmp(&b->entry_cam.cam, cam, sizeof(rptb_camera)) != 0)
         return fail(RPTB_ERR_BAD_ARG, "the buffer's entries were made through another camera");
     return RPTB_OK;
@@ -1718,7 +1723,7 @@ static int buffer_filter(rptb_buffer* b, const rptb_denoise& d, bool error, Aov*
 // (rptb_sample_into_guided), or the gathered whole buffer on the device of b, a shard (rptb_sample_into_guided_shard).
 // Every later call on either buffer is ordered behind it.  Every part of b holds its select scratch.  `error`
 // (rptb_sample_into_guided_error, a buffer with halves): the filter runs with the error estimate, and the mark tests E
-// in place of v'.  *launches: kernels enqueued, the HALF plane's scatter aside.
+// in place of v'.  *launches: kernels enqueued.
 static int guide_mark(rptb_buffer* f, rptb_buffer* b, const rptb_adaptive& crit, const rptb_denoise& d, uint32_t* launches, bool error) {
     BufferPart& q0 = f->parts[0];
     DeviceGuard g(q0.device);
@@ -1758,11 +1763,6 @@ static int guide_mark(rptb_buffer* f, rptb_buffer* b, const rptb_adaptive& crit,
     return rc;
 }
 
-static bool same_camera(const CameraRecord& a, const CameraRecord& b) {
-    const ShardCamera x = shard_camera(a), y = shard_camera(b);
-    return std::memcmp(&x, &y, sizeof(x)) == 0;
-}
-
 // What rptb_sample_into_guided_shard checks of `whole` (locked) once the filter runs: a one-part whole buffer on the
 // shard's device, of its size, last written by an import of all the shards at the shard's current state -- which the
 // shard still has, not having changed since its last export -- and check_guide_buffer's conditions.
@@ -1782,8 +1782,7 @@ static int check_guide_whole(const rptb_buffer* shard, const rptb_buffer* whole,
     if (whole->imported != whole->state || whole->imported_shards != q.count)
         return fail(RPTB_ERR_BAD_ARG, "whole was not last written by an import of the %u shards (rptb_buffer_import_shards or "
                                       "rptb_buffer_import_deltas)", q.count);
-    if (whole->entries != shard->entries || whole->reprojected != shard->reprojected || whole->feature_rays != shard->feature_rays ||
-        !same_camera(whole->entry_cam, shard->entry_cam) || !same_camera(whole->feat_cam, shard->feat_cam))
+    if (!same_state(block_state(whole), block_state(shard)))
         return fail(RPTB_ERR_BAD_ARG,
                     "whole does not hold the shard's current state (entries %u / %u, reprojected %d / %d, feature rays %llu / %llu, or "
                     "cameras)", whole->entries, shard->entries, (int)whole->reprojected, (int)shard->reprojected,
@@ -1842,14 +1841,15 @@ static int sample_into_impl(rptb_scene* s, const rptb_camera* cam, const rptb_re
         rc = sample_part(r, cam, p, b->parts[i], stats != nullptr, &launches[i], crit, marked);
         if (rc != RPTB_OK) return nparts > 1 ? fail(rc, "device %d: %s", r->device, g_error.c_str()) : rc;
     }
-    const CameraRecord cam_before = b->entry_cam;
+    const CameraRecord::State cam_before = b->entry_cam.state;
     const uint32_t entries_before = b->entries;
     b->entries++;
     b->entry_cam.note(*cam);
     b->state++;
     // A delta block can carry this call when it was adaptive, and either kept the entry camera or made the first entry: an
-    // importer then knows the camera before the call from the one after (rptb_buffer_import_deltas).
-    const bool cam_known = same_camera(cam_before, b->entry_cam) || (cam_before.state == CameraRecord::NONE && entries_before == 0);
+    // importer then knows the camera before the call from the one after (rptb_buffer_import_deltas).  note() keeps the
+    // camera exactly when it keeps the state.
+    const bool cam_known = b->entry_cam.state == cam_before || (cam_before == CameraRecord::NONE && entries_before == 0);
     b->masked = crit && cam_known ? b->state : UINT64_MAX;
     if (out_active) {
         uint64_t total = 0;
@@ -2257,13 +2257,12 @@ static int check_reproject_buffers(const rptb_buffer* dst, const rptb_buffer* sr
     if (dst->feature_rays == 0) return fail(RPTB_ERR_BAD_ARG, "dst holds no features (rptb_buffer_add_features)");
     if (src->entries == 0) return fail(RPTB_ERR_BAD_ARG, "src holds no entries");
     if (src->feature_rays == 0) return fail(RPTB_ERR_BAD_ARG, "src holds no features (rptb_buffer_add_features)");
-    const char* why[] = {"none", "one", "mixed (several cameras)", "unknown (a host entry)"};
     if (src->entry_cam.state != CameraRecord::ONE)
-        return fail(RPTB_ERR_BAD_ARG, "src's entries have no single camera: %s", why[src->entry_cam.state]);
+        return fail(RPTB_ERR_BAD_ARG, "src's entries have no single camera: %s", camera_state_name[src->entry_cam.state]);
     if (src->feat_cam.state != CameraRecord::ONE)
-        return fail(RPTB_ERR_BAD_ARG, "src's features have no single camera: %s", why[src->feat_cam.state]);
+        return fail(RPTB_ERR_BAD_ARG, "src's features have no single camera: %s", camera_state_name[src->feat_cam.state]);
     if (dst->feat_cam.state != CameraRecord::ONE)
-        return fail(RPTB_ERR_BAD_ARG, "dst's features have no single camera: %s", why[dst->feat_cam.state]);
+        return fail(RPTB_ERR_BAD_ARG, "dst's features have no single camera: %s", camera_state_name[dst->feat_cam.state]);
     if (std::memcmp(&src->entry_cam.cam, &src->feat_cam.cam, sizeof(rptb_camera)) != 0)
         return fail(RPTB_ERR_BAD_ARG, "src's entries and features were made through different cameras");
     if (src->feat_cam.cam.aperture > 0.0 || dst->feat_cam.cam.aperture > 0.0)
@@ -2278,9 +2277,8 @@ static int check_merge_dst(const rptb_buffer* dst, const rptb_reproject* prm) {
     if (dst->entries < 2)
         return fail(RPTB_ERR_BAD_ARG, "dst holds %u entry calls: testing history needs >= 2 fresh ones (a mean and a variance)", dst->entries);
     if (dst->reprojected) return fail(RPTB_ERR_BAD_ARG, "dst is already reprojected: its entries are not all fresh");
-    const char* why[] = {"none", "one", "mixed (several cameras)", "unknown (a host entry)"};
     if (dst->entry_cam.state != CameraRecord::ONE)
-        return fail(RPTB_ERR_BAD_ARG, "dst's entries have no single camera: %s", why[dst->entry_cam.state]);
+        return fail(RPTB_ERR_BAD_ARG, "dst's entries have no single camera: %s", camera_state_name[dst->entry_cam.state]);
     if (std::memcmp(&dst->entry_cam.cam, &dst->feat_cam.cam, sizeof(rptb_camera)) != 0)
         return fail(RPTB_ERR_BAD_ARG, "dst's entries and features were made through different cameras");
     if (dst->entries > UINT32_MAX - prm->max_history) return fail(RPTB_ERR_UNSUPPORTED, "too many entries");
@@ -2436,11 +2434,7 @@ int rptb_buffer_export_shard(rptb_buffer* b, void* dst_device, uint32_t with_fea
     h.height = b->height;
     h.shard_index = q.index;
     h.shard_count = q.count;
-    h.entries = b->entries;
-    h.flags = b->reprojected ? kShardReprojected : 0u;
-    h.feature_rays = b->feature_rays;
-    h.entry_cam = shard_camera(b->entry_cam);
-    h.feat_cam = shard_camera(b->feat_cam);
+    h.s = block_state(b);
     cudaStream_t st = stream ? (cudaStream_t)stream : q.stream;
     CU(cudaStreamWaitEvent(st, q.done, 0));
     // pageable source: the call returns once the header is staged
@@ -2468,36 +2462,31 @@ int rptb_buffer_import_shards(rptb_buffer* dst, const void* gathered_device, uin
     const uint32_t W = dst->width, H = dst->height;
     const ShardLayout l = shard_layout(W, H, shard_count, with_features != 0);
     const char* in = (const char*)gathered_device;
-    // header 0 first: only once it names dst's size, shard_count and with_features is the block stride known to be right
-    std::vector<ShardHeader> hs(shard_count);
-    CU(cudaMemcpyAsync(hs.data(), in, sizeof(ShardHeader), cudaMemcpyDeviceToHost, d0.stream));
-    CU(cudaStreamSynchronize(d0.stream));
+    std::vector<ShardHeader> hs;
+    int rc = fetch_headers(in, shard_count, l.bytes, d0.stream, hs, [&](const ShardHeader& h0) {
+        if (h0.magic != kShardMagic) return fail(RPTB_ERR_BAD_ARG, "block 0 is not a shard block (rptb_buffer_export_shard)");
+        if (h0.width != W || h0.height != H)
+            return fail(RPTB_ERR_BAD_ARG, "the shards are %ux%u but dst is %ux%u", h0.width, h0.height, W, H);
+        if (h0.shard_count != shard_count) return fail(RPTB_ERR_BAD_ARG, "the shards are %u but shard_count is %u", h0.shard_count, shard_count);
+        if (h0.with_features != (with_features ? 1u : 0u))
+            return fail(RPTB_ERR_BAD_ARG, "the shards were exported %s features", h0.with_features ? "with" : "without");
+        if (h0.s.flags & ~kShardReprojected) return fail(RPTB_ERR_BAD_ARG, "block 0 carries unknown flags 0x%x", h0.s.flags);
+        return (int)RPTB_OK;
+    });
+    if (rc != RPTB_OK) return rc;
     const ShardHeader& h0 = hs[0];
-    if (h0.magic != kShardMagic) return fail(RPTB_ERR_BAD_ARG, "block 0 is not a shard block (rptb_buffer_export_shard)");
-    if (h0.width != W || h0.height != H)
-        return fail(RPTB_ERR_BAD_ARG, "the shards are %ux%u but dst is %ux%u", h0.width, h0.height, W, H);
-    if (h0.shard_count != shard_count) return fail(RPTB_ERR_BAD_ARG, "the shards are %u but shard_count is %u", h0.shard_count, shard_count);
-    if (h0.with_features != (with_features ? 1u : 0u))
-        return fail(RPTB_ERR_BAD_ARG, "the shards were exported %s features", h0.with_features ? "with" : "without");
-    if (h0.flags & ~kShardReprojected) return fail(RPTB_ERR_BAD_ARG, "block 0 carries unknown flags 0x%x", h0.flags);
-    if (shard_count > 1)
-        CU(cudaMemcpy2DAsync(hs.data() + 1, sizeof(ShardHeader), in + l.bytes, l.bytes, sizeof(ShardHeader), shard_count - 1,
-                             cudaMemcpyDeviceToHost, d0.stream));
-    CU(cudaStreamSynchronize(d0.stream));
     for (uint32_t i = 0; i < shard_count; i++) {
         const ShardHeader& h = hs[i];
         if (h.magic != kShardMagic) return fail(RPTB_ERR_BAD_ARG, "block %u is not a shard block (rptb_buffer_export_shard)", i);
         if (h.shard_index != i) return fail(RPTB_ERR_BAD_ARG, "block %u holds shard %u: the shards must be in order 0..%u", i, h.shard_index, shard_count - 1);
         if (h.width != W || h.height != H || h.shard_count != shard_count || h.with_features != h0.with_features)
             return fail(RPTB_ERR_BAD_ARG, "block %u was exported from another image, shard count or feature choice", i);
-        if (h.entries != h0.entries || h.flags != h0.flags || h.feature_rays != h0.feature_rays ||
-            std::memcmp(&h.entry_cam, &h0.entry_cam, sizeof(ShardCamera)) != 0 ||
-            std::memcmp(&h.feat_cam, &h0.feat_cam, sizeof(ShardCamera)) != 0)
+        if (!same_state(h.s, h0.s))
             return fail(RPTB_ERR_BAD_ARG,
                         "shard %u received other calls than shard 0 (entries %u / %u, reprojected %u / %u, feature rays %llu / %llu, or "
                         "cameras)",
-                        i, h.entries, h0.entries, h.flags & kShardReprojected, h0.flags & kShardReprojected,
-                        (unsigned long long)h.feature_rays, (unsigned long long)h0.feature_rays);
+                        i, h.s.entries, h0.s.entries, h.s.flags & kShardReprojected, h0.s.flags & kShardReprojected,
+                        (unsigned long long)h.s.feature_rays, (unsigned long long)h0.s.feature_rays);
     }
     // everything dst holds is overwritten: its earlier work finishes first
     dst->state++;
@@ -2516,8 +2505,8 @@ int rptb_buffer_import_shards(rptb_buffer* dst, const void* gathered_device, uin
     }
     // every block row-major on dst's first device, then back into dst's own parts; every later call on dst is ordered
     // behind this one
-    const bool reprojected = (h0.flags & kShardReprojected) != 0;
-    int rc = buffer_rows_alloc(dst, l.mask);
+    const bool reprojected = (h0.s.flags & kShardReprojected) != 0;
+    rc = buffer_rows_alloc(dst, l.mask);
     if (rc == RPTB_OK && reprojected) rc = reproject_scratch_alloc(dst);
     for (uint32_t i = 0; rc == RPTB_OK && i < shard_count; i++)
         rc = buffer_scatter(dst, shard_planes(l, in + (size_t)i * l.bytes), l.mask, i, shard_count);
@@ -2526,11 +2515,11 @@ int rptb_buffer_import_shards(rptb_buffer* dst, const void* gathered_device, uin
     if (rc != RPTB_OK) return rc;
     // the caller may reuse the gathered bytes when the call returns
     CU(cudaStreamSynchronize(d0.stream));
-    dst->entries = h0.entries;
+    dst->entries = h0.s.entries;
     dst->reprojected = reprojected;
-    dst->entry_cam = camera_record(h0.entry_cam);
-    dst->feature_rays = with_features ? h0.feature_rays : 0;
-    dst->feat_cam = with_features ? camera_record(h0.feat_cam) : CameraRecord();
+    dst->entry_cam = camera_record(h0.s.entry_cam);
+    dst->feature_rays = with_features ? h0.s.feature_rays : 0;
+    dst->feat_cam = with_features ? camera_record(h0.s.feat_cam) : CameraRecord();
     dst->imported = dst->state;
     dst->imported_shards = shard_count;
     return RPTB_OK;
@@ -2568,11 +2557,7 @@ int rptb_buffer_export_delta(rptb_buffer* b, void* dst_device, uint32_t capacity
     h.shard_index = q.index;
     h.shard_count = q.count;
     h.entries_before = b->entries - 1;
-    h.entries_after = b->entries;
-    h.flags = b->reprojected ? kShardReprojected : 0u;
-    h.feature_rays = b->feature_rays;
-    h.entry_cam = shard_camera(b->entry_cam);
-    h.feat_cam = shard_camera(b->feat_cam);
+    h.s = block_state(b);
     h.pixels = (uint32_t)n;
     h.capacity = capacity;
     // pageable source: the call returns once the header is staged
@@ -2601,19 +2586,17 @@ int rptb_buffer_import_deltas(rptb_buffer* dst, const void* gathered_device, uin
     const uint32_t W = dst->width, H = dst->height;
     const uint64_t bytes = delta_bytes(capacity);
     const char* in = (const char*)gathered_device;
-    // header 0 first: only once it names dst's size, shard_count and capacity is the block stride known to be right
-    std::vector<DeltaHeader> hs(shard_count);
-    CU(cudaMemcpyAsync(hs.data(), in, sizeof(DeltaHeader), cudaMemcpyDeviceToHost, d0.stream));
-    CU(cudaStreamSynchronize(d0.stream));
+    std::vector<DeltaHeader> hs;
+    const int rc = fetch_headers(in, shard_count, bytes, d0.stream, hs, [&](const DeltaHeader& h0) {
+        if (h0.magic != kDeltaMagic) return fail(RPTB_ERR_BAD_ARG, "block 0 is not a delta block (rptb_buffer_export_delta)");
+        if (h0.width != W || h0.height != H) return fail(RPTB_ERR_BAD_ARG, "the deltas are %ux%u but dst is %ux%u", h0.width, h0.height, W, H);
+        if (h0.shard_count != shard_count)
+            return fail(RPTB_ERR_BAD_ARG, "the deltas are of %u shards but shard_count is %u", h0.shard_count, shard_count);
+        if (h0.capacity != capacity) return fail(RPTB_ERR_BAD_ARG, "the deltas have capacity %u but capacity is %u", h0.capacity, capacity);
+        return (int)RPTB_OK;
+    });
+    if (rc != RPTB_OK) return rc;
     const DeltaHeader& h0 = hs[0];
-    if (h0.magic != kDeltaMagic) return fail(RPTB_ERR_BAD_ARG, "block 0 is not a delta block (rptb_buffer_export_delta)");
-    if (h0.width != W || h0.height != H) return fail(RPTB_ERR_BAD_ARG, "the deltas are %ux%u but dst is %ux%u", h0.width, h0.height, W, H);
-    if (h0.shard_count != shard_count) return fail(RPTB_ERR_BAD_ARG, "the deltas are of %u shards but shard_count is %u", h0.shard_count, shard_count);
-    if (h0.capacity != capacity) return fail(RPTB_ERR_BAD_ARG, "the deltas have capacity %u but capacity is %u", h0.capacity, capacity);
-    if (shard_count > 1)
-        CU(cudaMemcpy2DAsync(hs.data() + 1, sizeof(DeltaHeader), in + bytes, bytes, sizeof(DeltaHeader), shard_count - 1,
-                             cudaMemcpyDeviceToHost, d0.stream));
-    CU(cudaStreamSynchronize(d0.stream));
     for (uint32_t i = 0; i < shard_count; i++) {
         const DeltaHeader& h = hs[i];
         if (h.magic != kDeltaMagic) return fail(RPTB_ERR_BAD_ARG, "block %u is not a delta block (rptb_buffer_export_delta)", i);
@@ -2622,30 +2605,28 @@ int rptb_buffer_import_deltas(rptb_buffer* dst, const void* gathered_device, uin
         if (h.width != W || h.height != H || h.shard_count != shard_count || h.capacity != capacity)
             return fail(RPTB_ERR_BAD_ARG, "block %u was exported for another image, shard count or capacity", i);
         if (h.pixels > capacity) return fail(RPTB_ERR_BAD_ARG, "block %u holds %u pixels, more than its capacity %u", i, h.pixels, capacity);
-        if (h.entries_before != h0.entries_before || h.entries_after != h0.entries_after || h.flags != h0.flags ||
-            h.feature_rays != h0.feature_rays || std::memcmp(&h.entry_cam, &h0.entry_cam, sizeof(ShardCamera)) != 0 ||
-            std::memcmp(&h.feat_cam, &h0.feat_cam, sizeof(ShardCamera)) != 0)
+        if (h.entries_before != h0.entries_before || !same_state(h.s, h0.s))
             return fail(RPTB_ERR_BAD_ARG,
                         "shard %u received other calls than shard 0 (entries %u -> %u / %u -> %u, reprojected %u / %u, feature rays "
                         "%llu / %llu, or cameras)",
-                        i, h.entries_before, h.entries_after, h0.entries_before, h0.entries_after, h.flags & kShardReprojected,
-                        h0.flags & kShardReprojected, (unsigned long long)h.feature_rays, (unsigned long long)h0.feature_rays);
+                        i, h.entries_before, h.s.entries, h0.entries_before, h0.s.entries, h.s.flags & kShardReprojected,
+                        h0.s.flags & kShardReprojected, (unsigned long long)h.s.feature_rays, (unsigned long long)h0.s.feature_rays);
     }
     // dst must hold the shards' state before the call: an import of them, untouched since.  The entry camera before the call
-    // is the one after it, or none before the first entry (rptb_buffer_export_delta refuses any other change).
-    const CameraRecord after_cam = camera_record(h0.entry_cam);
-    const CameraRecord before_cam = h0.entries_before == 0 ? CameraRecord() : after_cam;
-    const bool reprojected = (h0.flags & kShardReprojected) != 0;
+    // is the one after it, or none before the first entry (rptb_buffer_export_delta refuses any other change).  The state
+    // is compared as dst would record it from the header: the reprojected flag only, and each camera as its state keeps it.
+    const CameraRecord after_cam = camera_record(h0.s.entry_cam);
+    const BlockState before = {h0.entries_before, h0.s.flags & kShardReprojected, h0.s.feature_rays,
+                               shard_camera(h0.entries_before == 0 ? CameraRecord() : after_cam), shard_camera(camera_record(h0.s.feat_cam))};
     if (dst->imported != dst->state || dst->imported_shards != shard_count)
         return fail(RPTB_ERR_BAD_ARG, "dst was not last written by an import of the %u shards (rptb_buffer_import_shards or "
                                       "rptb_buffer_import_deltas); gather the full blocks", shard_count);
-    if (dst->entries != h0.entries_before || dst->reprojected != reprojected || dst->feature_rays != h0.feature_rays ||
-        !same_camera(dst->entry_cam, before_cam) || !same_camera(dst->feat_cam, camera_record(h0.feat_cam)))
+    if (!same_state(block_state(dst), before))
         return fail(RPTB_ERR_BAD_ARG,
                     "dst is not at the shards' state before the call (entries %u / %u, reprojected %d / %d, feature rays %llu / %llu, or "
                     "cameras); gather the full blocks",
-                    dst->entries, h0.entries_before, (int)dst->reprojected, (int)reprojected, (unsigned long long)dst->feature_rays,
-                    (unsigned long long)h0.feature_rays);
+                    dst->entries, h0.entries_before, (int)dst->reprojected, (int)before.flags, (unsigned long long)dst->feature_rays,
+                    (unsigned long long)h0.s.feature_rays);
     // in place in dst's compact planes; every later call on dst is ordered behind it
     dst->state++;
     CU(cudaStreamWaitEvent(d0.stream, d0.done, 0));
@@ -2653,7 +2634,7 @@ int rptb_buffer_import_deltas(rptb_buffer* dst, const void* gathered_device, uin
     CU(cudaEventRecord(d0.done, d0.stream));
     // the caller may reuse the gathered bytes when the call returns
     CU(cudaStreamSynchronize(d0.stream));
-    dst->entries = h0.entries_after;
+    dst->entries = h0.s.entries;
     dst->entry_cam = after_cam;
     dst->imported = dst->state;
     return RPTB_OK;

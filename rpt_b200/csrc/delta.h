@@ -25,15 +25,25 @@ struct ShardCamera {
     rptb_camera cam;
 };
 
-// The header of a delta block.  The entries and flags describe the shard before and after the call; the feature rays
-// and cameras are the shard's after the call (the call records its camera; see rptb_buffer_import_deltas).
-struct DeltaHeader {
-    uint32_t magic, width, height, shard_index, shard_count, entries_before, entries_after, flags;
+// A buffer's state as both exchange headers carry it, at the same offset: its entry calls, flags (kShardReprojected,
+// api.cu), feature rays per pixel and cameras.  Every byte is written (shard_camera zeroes what a state leaves unused),
+// so two states are the same when their bytes are.
+struct BlockState {
+    uint32_t entries, flags;
     uint64_t feature_rays;
     ShardCamera entry_cam, feat_cam;
+};
+
+// The header of a delta block.  `s` is the shard's state after the call, and entries_before its entry count before it
+// (rptb_buffer_import_deltas derives the rest of the state before the call from `s`).
+struct DeltaHeader {
+    uint32_t magic, width, height, shard_index, shard_count, entries_before;
+    BlockState s;
     uint32_t pixels, capacity;
 };
 static_assert(sizeof(DeltaHeader) <= kDeltaHeaderBytes, "the delta header outgrew its slot");
+static_assert(offsetof(DeltaHeader, s) == 24, "the state sits where the shard header's does");
+static_assert(offsetof(DeltaHeader, pixels) == 248, "distributed.DELTA_PIXELS_AT");
 
 RPTB_HD uint64_t delta_bytes(uint32_t capacity) { return kDeltaHeaderBytes + 40ull * capacity; }
 

@@ -123,31 +123,13 @@ __device__ __forceinline__ void welford_add(double x0, double x1, double x2, uin
     *m = first ? 0.0 : om + dm;
 }
 
-template <class T, bool ROWMAJOR>
+// HALVES (a buffer with halves, planes.h): entry k = counts[e] (the count before the add) also goes into half[3e..3e+3)
+// when k is odd, added in entry order.
+template <class T, bool ROWMAJOR, bool HALVES>
 __global__ void buffer_accumulate_kernel(const T* __restrict__ in, const uint8_t* __restrict__ mask, uint64_t nelem,
                                          uint32_t width, uint32_t height, uint32_t shard_index, uint32_t shard_count,
-                                         double* __restrict__ sums, double* __restrict__ m2, uint32_t* __restrict__ counts) {
-    const uint64_t e = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (e >= nelem) return;
-    if (mask && !mask[e]) return;
-    const T* src = in + 3 * e;
-    if (ROWMAJOR) {
-        const int64_t p = tile_pixel(width, height, shard_index + (uint32_t)(e >> 7) * shard_count, (uint32_t)(e & 127u));
-        if (p < 0) return;
-        src = in + 3 * p;
-    }
-    const uint32_t n = counts[e] + 1u;
-    welford_add((double)src[0], (double)src[1], (double)src[2], n, sums + 3 * e, m2 + e);
-    counts[e] = n;
-}
-
-// buffer_accumulate_kernel for a buffer with halves (planes.h): the same sums, M2 and counts, and entry k = counts[e]
-// (the count before the add) also goes into half[3e..3e+3) when k is odd, added in entry order.
-template <class T, bool ROWMAJOR>
-__global__ void buffer_accumulate_halves_kernel(const T* __restrict__ in, const uint8_t* __restrict__ mask, uint64_t nelem,
-                                                uint32_t width, uint32_t height, uint32_t shard_index, uint32_t shard_count,
-                                                double* __restrict__ sums, double* __restrict__ m2, uint32_t* __restrict__ counts,
-                                                double* __restrict__ half) {
+                                         double* __restrict__ sums, double* __restrict__ m2, uint32_t* __restrict__ counts,
+                                         double* __restrict__ half) {
     const uint64_t e = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (e >= nelem) return;
     if (mask && !mask[e]) return;
@@ -161,37 +143,31 @@ __global__ void buffer_accumulate_halves_kernel(const T* __restrict__ in, const 
     const double x0 = (double)src[0], x1 = (double)src[1], x2 = (double)src[2];
     welford_add(x0, x1, x2, k + 1u, sums + 3 * e, m2 + e);
     counts[e] = k + 1u;
-    if (k & 1u) {
-        half[3 * e] = half[3 * e] + x0;
-        half[3 * e + 1] = half[3 * e + 1] + x1;
-        half[3 * e + 2] = half[3 * e + 2] + x2;
+    if constexpr (HALVES) {
+        if (k & 1u) {
+            half[3 * e] = half[3 * e] + x0;
+            half[3 * e + 1] = half[3 * e + 1] + x1;
+            half[3 * e + 2] = half[3 * e + 2] + x2;
+        }
     }
 }
 
-// The HALF plane of a buffer with halves: the compact tiles of replica `shard_index` of `shard_count` -> the row-major
-// plane of the whole image, as buffer_scatter_kernel moves the planes of a PlaneSet.
-__global__ void buffer_half_scatter_kernel(const double* __restrict__ src, double* __restrict__ dst, uint64_t nelem, uint32_t width,
-                                           uint32_t height, uint32_t shard_index, uint32_t shard_count) {
-    const uint64_t e = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (e >= nelem) return;
-    const int64_t p = tile_pixel(width, height, shard_index + (uint32_t)(e >> 7) * shard_count, (uint32_t)(e & 127u));
-    if (p < 0) return;
-    for (int k = 0; k < 3; k++) dst[3 * p + k] = src[3 * e + k];
-}
-
-// Element `from` of every plane present in both sets (planes.h) -> element `to` of dst; from < 0 writes zeros.  Every
-// value is loaded before any is stored, so the loads of all planes are in flight together.
+// Element `from` of every plane k < NP present in both sets (planes.h) -> element `to` of dst; from < 0 writes zeros.
+// Every value is loaded before any is stored, so the loads of all planes are in flight together.  NP is HALF unless
+// the sets hold HALF (launch_buffer_move): the kernels that move the other planes alone keep the registers and the
+// instructions they have without it.
+template <int NP>
 __device__ __forceinline__ void move_planes(const PlaneSet& src, const PlaneSet& dst, int64_t from, uint64_t to) {
-    unsigned long long v[NPLANES][3];
+    unsigned long long v[NP][3];
 #pragma unroll
-    for (int k = 0; k < NPLANES; k++) {
+    for (int k = 0; k < NP; k++) {
         const PlaneShape s = plane_shape(k);
         if (!src.p[k] || !dst.p[k] || from < 0) continue;
         for (uint32_t j = 0; j < s.values; j++)
             v[k][j] = s.bytes == 8 ? ((const unsigned long long*)src.p[k])[s.values * from + j] : ((const uint32_t*)src.p[k])[s.values * from + j];
     }
 #pragma unroll
-    for (int k = 0; k < NPLANES; k++) {
+    for (int k = 0; k < NP; k++) {
         const PlaneShape s = plane_shape(k);
         if (!src.p[k] || !dst.p[k]) continue;
         for (uint32_t j = 0; j < s.values; j++) {
@@ -203,21 +179,23 @@ __device__ __forceinline__ void move_planes(const PlaneSet& src, const PlaneSet&
 }
 
 // The compact tiles of replica `shard_index` of `shard_count` -> the row-major planes of the whole image.
+template <int NP>
 __global__ void buffer_scatter_kernel(const PlaneSet src, const PlaneSet dst, uint64_t nelem, uint32_t width, uint32_t height,
                                       uint32_t shard_index, uint32_t shard_count) {
     const uint64_t e = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (e >= nelem) return;
     const int64_t p = tile_pixel(width, height, shard_index + (uint32_t)(e >> 7) * shard_count, (uint32_t)(e & 127u));
-    if (p >= 0) move_planes(src, dst, e, p);
+    if (p >= 0) move_planes<NP>(src, dst, e, p);
 }
 
 // The inverse: the row-major planes -> the compact tiles.  Elements past a ragged edge are zeroed, as a fresh buffer
 // holds them.
+template <int NP>
 __global__ void buffer_compact_kernel(const PlaneSet src, const PlaneSet dst, uint64_t nelem, uint32_t width, uint32_t height,
                                       uint32_t shard_index, uint32_t shard_count) {
     const uint64_t e = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (e >= nelem) return;
-    move_planes(src, dst, tile_pixel(width, height, shard_index + (uint32_t)(e >> 7) * shard_count, (uint32_t)(e & 127u)), e);
+    move_planes<NP>(src, dst, tile_pixel(width, height, shard_index + (uint32_t)(e >> 7) * shard_count, (uint32_t)(e & 127u)), e);
 }
 
 // Buffer::variance from the row-major M2 and counts: the sum over pixels of M2/(n-1), each pixel with its own n (a
@@ -256,31 +234,20 @@ __global__ void __launch_bounds__(kVarThreads) buffer_variance_final_kernel(cons
     if (threadIdx.x == 0) *out_sum = s;
 }
 
-// half: the HALF plane of a buffer with halves (buffer_accumulate_halves_kernel), else null.
+// half: the HALF plane of a buffer with halves (buffer_accumulate_kernel's HALVES), else null.
 cudaError_t launch_buffer_accumulate(const float* in32, const double* in64, bool rowmajor, const uint8_t* mask, uint64_t nelem,
                                      uint32_t width, uint32_t height, uint32_t shard_index, uint32_t shard_count, double* sums,
                                      double* m2, uint32_t* counts, double* half, cudaStream_t stream) {
     if (nelem == 0) return cudaSuccess;
     const unsigned grid = (unsigned)((nelem + 255) / 256);
-    if (half) {
-        if (in32)
-            buffer_accumulate_halves_kernel<float, false><<<grid, 256, 0, stream>>>(in32, mask, nelem, width, height, shard_index,
-                                                                                    shard_count, sums, m2, counts, half);
-        else if (rowmajor)
-            buffer_accumulate_halves_kernel<double, true><<<grid, 256, 0, stream>>>(in64, mask, nelem, width, height, shard_index,
-                                                                                    shard_count, sums, m2, counts, half);
-        else
-            buffer_accumulate_halves_kernel<double, false><<<grid, 256, 0, stream>>>(in64, mask, nelem, width, height, shard_index,
-                                                                                     shard_count, sums, m2, counts, half);
-    } else if (in32)
-        buffer_accumulate_kernel<float, false><<<grid, 256, 0, stream>>>(in32, mask, nelem, width, height, shard_index, shard_count,
-                                                                         sums, m2, counts);
-    else if (rowmajor)
-        buffer_accumulate_kernel<double, true><<<grid, 256, 0, stream>>>(in64, mask, nelem, width, height, shard_index, shard_count,
-                                                                         sums, m2, counts);
-    else
-        buffer_accumulate_kernel<double, false><<<grid, 256, 0, stream>>>(in64, mask, nelem, width, height, shard_index, shard_count,
-                                                                          sums, m2, counts);
+    if (in32) {
+        const auto k = half ? buffer_accumulate_kernel<float, false, true> : buffer_accumulate_kernel<float, false, false>;
+        k<<<grid, 256, 0, stream>>>(in32, mask, nelem, width, height, shard_index, shard_count, sums, m2, counts, half);
+    } else {
+        const auto k = rowmajor ? (half ? buffer_accumulate_kernel<double, true, true> : buffer_accumulate_kernel<double, true, false>)
+                                : (half ? buffer_accumulate_kernel<double, false, true> : buffer_accumulate_kernel<double, false, false>);
+        k<<<grid, 256, 0, stream>>>(in64, mask, nelem, width, height, shard_index, shard_count, sums, m2, counts, half);
+    }
     return cudaGetLastError();
 }
 
@@ -307,17 +274,13 @@ cudaError_t launch_buffer_move(bool compact, const PlaneSet& src, const PlaneSet
                                uint32_t shard_index, uint32_t shard_count, cudaStream_t stream) {
     if (nelem == 0) return cudaSuccess;
     const unsigned grid = (unsigned)((nelem + 255) / 256);
-    if (compact) buffer_compact_kernel<<<grid, 256, 0, stream>>>(src, dst, nelem, width, height, shard_index, shard_count);
-    else buffer_scatter_kernel<<<grid, 256, 0, stream>>>(src, dst, nelem, width, height, shard_index, shard_count);
-    return cudaGetLastError();
-}
-
-// launch_buffer_move's scatter for the HALF plane.
-cudaError_t launch_buffer_half_scatter(const double* src, double* dst, uint64_t nelem, uint32_t width, uint32_t height, uint32_t shard_index,
-                                       uint32_t shard_count, cudaStream_t stream) {
-    if (nelem == 0) return cudaSuccess;
-    buffer_half_scatter_kernel<<<(unsigned)((nelem + 255) / 256), 256, 0, stream>>>(src, dst, nelem, width, height, shard_index,
-                                                                                    shard_count);
+    const bool half = src.p[HALF] && dst.p[HALF];
+    if (compact)
+        (half ? buffer_compact_kernel<NPLANES> : buffer_compact_kernel<HALF>)<<<grid, 256, 0, stream>>>(src, dst, nelem, width, height,
+                                                                                                       shard_index, shard_count);
+    else
+        (half ? buffer_scatter_kernel<NPLANES> : buffer_scatter_kernel<HALF>)<<<grid, 256, 0, stream>>>(src, dst, nelem, width, height,
+                                                                                                       shard_index, shard_count);
     return cudaGetLastError();
 }
 

@@ -10,9 +10,9 @@
 namespace rptb {
 
 // HALF (rptb_buffer_create_halves): the sums of a pixel's odd entries (entry k, counted from 0, for odd k), 3 per
-// pixel.  It comes after the planes of the exchange block and of PlaneSet, which stay as they are: only a buffer with
-// halves holds it, and it moves between the compact tiles and the rows by its own kernel (film.cu).
-enum Plane { SUMS, M2, NORMAL, ALBEDO, HITS, DEPTH, COUNTS, NPLANES, HALF = NPLANES };
+// pixel.  Only a buffer with halves holds it.  It is in PlaneSet, so the scatter and compact kernels (film.cu) move it
+// like any other plane, but never in the exchange block, whose planes are COLOUR | FEATURES.
+enum Plane { SUMS, M2, NORMAL, ALBEDO, HITS, DEPTH, COUNTS, HALF, NPLANES };
 constexpr uint32_t COLOUR = 1u << SUMS | 1u << M2 | 1u << COUNTS;
 constexpr uint32_t FEATURES = 1u << NORMAL | 1u << ALBEDO | 1u << HITS | 1u << DEPTH;
 
@@ -20,7 +20,7 @@ struct PlaneShape {
     uint32_t values, bytes;  // per pixel, per value
 };
 RPTB_HD constexpr PlaneShape plane_shape(int k) {
-    constexpr PlaneShape t[NPLANES + 1] = {{3, 8}, {1, 8}, {3, 8}, {3, 8}, {1, 8}, {1, 8}, {1, 4}, {3, 8}};
+    constexpr PlaneShape t[NPLANES] = {{3, 8}, {1, 8}, {3, 8}, {3, 8}, {1, 8}, {1, 8}, {1, 4}, {3, 8}};
     return t[k];
 }
 

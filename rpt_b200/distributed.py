@@ -297,28 +297,34 @@ class ShardBuffer(api.DeviceBuffer):
         self.entries += int(c.max_history)  # the fresh calls plus the history's bound
         return int(n.value), int(j.value)
 
-    def gather(self, group=None, with_features: bool = False) -> "api.DeviceBuffer":
-        """All ranks call this: export every shard's block, one all_gather_into_tensor, and import the blocks into a new
-        whole DeviceBuffer on this rank's device -- the same bits on every rank, and those of one whole buffer given the
-        same calls.  NCCL gathers GPU to GPU; any other backend (gloo) through a host tensor.  `with_features` carries
-        the feature sums too (denoise and reproject need them), 100 instead of 36 bytes per pixel."""
+    def _exchange(self, group, nbytes: int, export) -> tuple:
+        """What gather and gather_delta share: check the process group against the shard, `export(out, stream)` this
+        shard's block into a new CUDA uint8 tensor of `nbytes` on the buffer's device, all-gather every rank's block and
+        wait for it.  Returns _all_gather_bytes' (gathered, staged)."""
         import torch
 
         group = self.group if group is None else group
         rank, world = self.shard
         if world > 1 and _rank_world(group) != (rank, world):
             raise ValueError(f"the shard is {rank} of {world} but the process group has rank/world {_rank_world(group)}")
-        nbytes = self.block_bytes(with_features)
         dev = torch.device("cuda", self.devices[0])
         with torch.cuda.device(dev):
             stream = torch.cuda.current_stream(dev)
             mine = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-            self.export(mine, with_features, stream.cuda_stream)
-            gathered, _ = _all_gather_bytes(mine, world, group)
+            export(mine, stream.cuda_stream)
+            out = _all_gather_bytes(mine, world, group)
             stream.synchronize()  # the import reads the gathered bytes on the library's stream
-            whole = api.DeviceBuffer(self._scene, self.width, self.height, self.filter)
-            capi.check(capi.lib().rptb_buffer_import_shards(whole.handle, C.c_void_p(gathered.data_ptr()), world,
-                                                            1 if with_features else 0), "rptb_buffer_import_shards")
+        return out
+
+    def gather(self, group=None, with_features: bool = False) -> "api.DeviceBuffer":
+        """All ranks call this: export every shard's block, one all_gather_into_tensor, and import the blocks into a new
+        whole DeviceBuffer on this rank's device -- the same bits on every rank, and those of one whole buffer given the
+        same calls.  NCCL gathers GPU to GPU; any other backend (gloo) through a host tensor.  `with_features` carries
+        the feature sums too (denoise and reproject need them), 100 instead of 36 bytes per pixel."""
+        gathered, _ = self._exchange(group, self.block_bytes(with_features), lambda out, stream: self.export(out, with_features, stream))
+        whole = api.DeviceBuffer(self._scene, self.width, self.height, self.filter)
+        capi.check(capi.lib().rptb_buffer_import_shards(whole.handle, C.c_void_p(gathered.data_ptr()), self.shard[1],
+                                                        1 if with_features else 0), "rptb_buffer_import_shards")
         whole.entries = int(whole.counts().max())
         whole.feature_rays = self.feature_rays if with_features else 0
         return whole
@@ -345,27 +351,18 @@ class ShardBuffer(api.DeviceBuffer):
         `capacity`, the same on every rank: at least the largest active count of the call over the ranks."""
         import torch
 
-        group = self.group if group is None else group
-        rank, world = self.shard
-        if world > 1 and _rank_world(group) != (rank, world):
-            raise ValueError(f"the shard is {rank} of {world} but the process group has rank/world {_rank_world(group)}")
+        world = self.shard[1]
         lay = delta_block_layout(capacity)
-        dev = torch.device("cuda", self.devices[0])
-        with torch.cuda.device(dev):
-            stream = torch.cuda.current_stream(dev)
-            mine = torch.empty(lay["bytes"], dtype=torch.uint8, device=dev)
-            self.export_delta(mine, capacity, stream.cuda_stream)
-            gathered, staged = _all_gather_bytes(mine, world, group)
-            stream.synchronize()  # the import reads the gathered bytes on the library's stream
-            capi.check(capi.lib().rptb_buffer_import_deltas(whole.handle, C.c_void_p(gathered.data_ptr()), world, lay["capacity"]),
-                       "rptb_buffer_import_deltas")
-            # a delta only raises counts: the largest is the old one or one of the counts the blocks carry
-            blocks = (staged if staged is not None else gathered).view(world, lay["bytes"])
-            pixels = blocks[:, DELTA_PIXELS_AT:DELTA_PIXELS_AT + 4].contiguous().view(torch.int32)
-            counts = blocks[:, lay["counts"]:lay["slots"]].contiguous().view(torch.int32)
-            written = torch.arange(lay["capacity"], device=blocks.device).unsqueeze(0) < pixels
-            if bool(written.any()):
-                whole.entries = max(whole.entries, int(counts[written].max()))
+        gathered, staged = self._exchange(group, lay["bytes"], lambda out, stream: self.export_delta(out, capacity, stream))
+        capi.check(capi.lib().rptb_buffer_import_deltas(whole.handle, C.c_void_p(gathered.data_ptr()), world, lay["capacity"]),
+                   "rptb_buffer_import_deltas")
+        # a delta only raises counts: the largest is the old one or one of the counts the blocks carry
+        blocks = (staged if staged is not None else gathered).view(world, lay["bytes"])
+        pixels = blocks[:, DELTA_PIXELS_AT:DELTA_PIXELS_AT + 4].contiguous().view(torch.int32)
+        counts = blocks[:, lay["counts"]:lay["slots"]].contiguous().view(torch.int32)
+        written = torch.arange(lay["capacity"], device=blocks.device).unsqueeze(0) < pixels
+        if bool(written.any()):
+            whole.entries = max(whole.entries, int(counts[written].max()))
 
 
 def _count_device(buffer: ShardBuffer, group=None):

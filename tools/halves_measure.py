@@ -66,16 +66,16 @@ def cost(gpu, quick, reps):
             r.sample(SPP, bufs[True], want_stats=False, adaptive=err)
             r.sample(SPP, bufs[True], want_stats=False, adaptive=filt)
             r.sample(SPP, bufs[False], want_stats=False)
-        acc = ["buffer_accumulate_kernel", "buffer_accumulate_halves_kernel"]
+        acc = ["buffer_accumulate_kernel"]  # plain or halves: the buffer decides the instantiation
         plain = _kernel_ms(lambda: r.sample(SPP, bufs[False], want_stats=False), reps, acc)
         halves = _kernel_ms(lambda: r.sample(SPP, bufs[True], want_stats=False), reps, acc)
-        guide = ["buffer_scatter", "buffer_half_scatter", "features_resolve", "denoise_demodulate", "denoise_pass", "halves_demodulate",
+        guide = ["buffer_scatter", "features_resolve", "denoise_demodulate", "denoise_pass", "halves_demodulate",
                  "halves_pass", "halves_error", "guided_mark"]
         on_v = _kernel_ms(lambda: r.sample(SPP, bufs[True], want_stats=False, adaptive=filt), reps, guide)
         on_e = _kernel_ms(lambda: r.sample(SPP, bufs[True], want_stats=False, adaptive=err), reps, guide)
         row = {"what": "cost", "size": [w, h], "iterations": GUIDE.iterations,
                "accumulate_ms_plain_buffer": plain["buffer_accumulate_kernel"],
-               "accumulate_ms_halves_buffer": halves["buffer_accumulate_halves_kernel"],
+               "accumulate_ms_halves_buffer": halves["buffer_accumulate_kernel"],
                "guide_kernels_ms_filter": on_v, "guide_total_ms_filter": round(sum(on_v.values()), 3),
                "guide_kernels_ms_halves": on_e, "guide_total_ms_halves": round(sum(on_e.values()), 3),
                "buffer_bytes_per_pixel": {"plain": 3 * 8 + 8 + 4, "halves": 3 * 8 + 8 + 4 + 24}, "gpu": gpu}

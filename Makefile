@@ -103,9 +103,11 @@ HOSTEMU_REPROJECT := tests/hostemu/_build/libhostemu_reproject.so
 HOSTEMU_GUIDED := tests/hostemu/_build/libhostemu_guided.so
 # the delta exchange's per-element export and import (delta.h; tests/hostemu/hostemu_delta.cu)
 HOSTEMU_DELTA := tests/hostemu/_build/libhostemu_delta.so
+# the same for the delta block of a shard with halves (delta.h; tests/hostemu/hostemu_delta_halves.cu)
+HOSTEMU_DELTA_HALVES := tests/hostemu/_build/libhostemu_delta_halves.so
 # the error estimate's per-pixel functions (halves.h; tests/hostemu/hostemu_halves.cu)
 HOSTEMU_HALVES := tests/hostemu/_build/libhostemu_halves.so
-hostemu: $(HOSTEMU) $(HOSTEMU_LIST) $(HOSTEMU_DENOISE) $(HOSTEMU_SLIM) $(HOSTEMU_REPROJECT) $(HOSTEMU_GUIDED) $(HOSTEMU_DELTA) $(HOSTEMU_HALVES)
+hostemu: $(HOSTEMU) $(HOSTEMU_LIST) $(HOSTEMU_DENOISE) $(HOSTEMU_SLIM) $(HOSTEMU_REPROJECT) $(HOSTEMU_GUIDED) $(HOSTEMU_DELTA) $(HOSTEMU_DELTA_HALVES) $(HOSTEMU_HALVES)
 $(HOSTEMU): tests/hostemu/hostemu.cu $(CSRC)/kdbuild.cpp $(CSRC)/bvhbuild.cpp $(HDRS)
 	@mkdir -p $(dir $@)
 	nvcc -std=c++17 -O2 -DRPTB_HOST_EMU -DRPTB_BUILD_BVH8=1 -DRPTB_BUILD_BVH4=1 -gencode arch=compute_90a,code=sm_90a -Xcompiler -fPIC,-fopenmp,-ffp-contract=off -shared -Xlinker -Bsymbolic -o $@ tests/hostemu/hostemu.cu $(CSRC)/kdbuild.cpp $(CSRC)/bvhbuild.cpp -lgomp
@@ -127,6 +129,9 @@ $(HOSTEMU_GUIDED): tests/hostemu/hostemu_guided.cu tests/hostemu/hostemu_denoise
 $(HOSTEMU_DELTA): tests/hostemu/hostemu_delta.cu $(HDRS)
 	@mkdir -p $(dir $@)
 	nvcc -std=c++17 -O2 -DRPTB_HOST_EMU -gencode arch=compute_90a,code=sm_90a -Xcompiler -fPIC,-ffp-contract=off -shared -Xlinker -Bsymbolic -o $@ tests/hostemu/hostemu_delta.cu
+$(HOSTEMU_DELTA_HALVES): tests/hostemu/hostemu_delta_halves.cu $(HDRS)
+	@mkdir -p $(dir $@)
+	nvcc -std=c++17 -O2 -DRPTB_HOST_EMU -gencode arch=compute_90a,code=sm_90a -Xcompiler -fPIC,-ffp-contract=off -shared -Xlinker -Bsymbolic -o $@ tests/hostemu/hostemu_delta_halves.cu
 $(HOSTEMU_HALVES): tests/hostemu/hostemu_halves.cu $(HDRS)
 	@mkdir -p $(dir $@)
 	nvcc -std=c++17 -O2 -DRPTB_HOST_EMU -gencode arch=compute_90a,code=sm_90a -Xcompiler -fPIC,-fopenmp,-ffp-contract=off -shared -Xlinker -Bsymbolic -o $@ tests/hostemu/hostemu_halves.cu -lgomp

@@ -539,11 +539,13 @@ int rptb_sample_into_guided(rptb_scene* scene, const rptb_camera* camera, const 
  * buffer, and the square of the result, remodulated, averaged over the channels and smoothed over 3x3, is E: an
  * estimate of each pixel's variance of the denoised value that accounts for the correlation between passes.
  * rpt_b200/csrc/halves.h gives every formula and its order of operations.
- * A buffer with halves is not a reprojection's or merge's dst, nor an import's (RPTB_ERR_UNSUPPORTED): history and
- * shards carry no halves.  It may be a reprojection's src.  There is no shard buffer with halves.
+ * A buffer with halves is not a reprojection's or merge's dst (RPTB_ERR_UNSUPPORTED): history carries no halves.  It
+ * may be a reprojection's src.  It imports the blocks of shards with halves (rptb_buffer_create_shard_halves), whose
+ * exchange blocks carry HALF, and only those.
  * Arguments and refusals of create as rptb_buffer_create.                                                      */
 int rptb_buffer_create_halves(rptb_scene* scene, uint32_t width, uint32_t height, uint32_t box_radius, rptb_buffer** out);
-/* The HALF plane: width*height*3 doubles, row-major.  RPTB_ERR_BAD_ARG: a buffer without halves.              */
+/* The HALF plane: width*height*3 doubles, row-major.  RPTB_ERR_BAD_ARG: a buffer without halves;
+ * RPTB_ERR_UNSUPPORTED: a shard buffer (gather the shards first).                                              */
 int rptb_buffer_half_sums(rptb_buffer* buffer, double* out);
 /* E, the error estimate of rptb_buffer_denoise(params)'s output, in the units of v': width*height doubles, row-major.
  * A pixel with fewer than 2 entries in either half's sense (n_B = 0) gives no difference and no weight; where no
@@ -554,7 +556,7 @@ int rptb_buffer_denoise_error(rptb_buffer* buffer, const rptb_denoise* params, d
  *     n < min_entries   or   NOT( E <= (rel_tol * m' + abs_tol)^2 ),
  * m' as in rptb_sample_into_guided.  The same flow, checks, refusals, plain mark while no pixel can hold min_entries,
  * out_active and stats.  Besides: RPTB_ERR_BAD_ARG: a buffer without halves, guide->iterations == 0;
- * RPTB_ERR_UNSUPPORTED: a shard buffer, the wavefront engine.                                                    */
+ * RPTB_ERR_UNSUPPORTED: a shard buffer (rptb_sample_into_guided_error_shard takes it), the wavefront engine.      */
 int rptb_sample_into_guided_error(rptb_scene* scene, const rptb_camera* camera, const rptb_render_params* params,
                                   const rptb_adaptive* criterion, const rptb_denoise* guide, rptb_buffer* buffer,
                                   uint64_t* out_active /* nullable, forces sync */, rptb_stats* stats /* nullable, forces sync */);
@@ -606,8 +608,19 @@ int rptb_buffer_create_shard(rptb_scene* scene, uint32_t width, uint32_t height,
 /* The size in bytes of the shard buffer's exchange block, the same for every shard of one image and shard count: a
  * 256-byte header, then the shard's planes, each padded to shard 0's pixel slots P = (its tiles) * 128 -- sums (3P
  * doubles), M2 (P doubles), with_features the feature sums (8P doubles: normal 3P, albedo 3P, hits P, depth P), then
- * counts (P uint32).  256 + 36 P bytes, 256 + 100 P with features.  0 for NULL or a whole buffer.           */
+ * counts (P uint32).  256 + 36 P bytes, 256 + 100 P with features; a shard with halves appends HALF (3P doubles):
+ * 256 + 60 P, 256 + 124 P with features.  0 for NULL or a whole buffer.                                      */
 uint64_t rptb_buffer_shard_bytes(const rptb_buffer* buffer, uint32_t with_features);
+/* rptb_buffer_create_shard with halves: the shard also keeps HALF (rptb_buffer_create_halves) for its own tiles.  Every
+ * entry, adaptive and guided call and feature pass takes it as it takes a plain shard, and entry k of a pixel (k its
+ * count before the add) goes into HALF iff k is odd, so a shard's HALF is the whole buffer's for its tiles.  Its
+ * exchange block appends HALF (3P doubles) after counts: 256 + 60 P bytes, 256 + 124 P with features, and its header's
+ * flags say so.  Such blocks import into a whole buffer with halves only (RPTB_ERR_BAD_ARG into a plain one), and a
+ * buffer with halves imports no plain blocks (RPTB_ERR_UNSUPPORTED).  It is not a reprojection's or merge's dst
+ * (RPTB_ERR_UNSUPPORTED: history carries no halves), and its half_sums and denoise_error are refused like every other
+ * whole-image read.  Arguments and refusals as rptb_buffer_create_shard.                                        */
+int rptb_buffer_create_shard_halves(rptb_scene* scene, uint32_t width, uint32_t height, uint32_t box_radius, uint32_t shard_index,
+                                    uint32_t shard_count, rptb_buffer** out);
 /* Writes the shard buffer's block (rptb_buffer_shard_bytes) to dst_device, on `stream` (a cudaStream_t, behind the
  * buffer's earlier calls; NULL = the buffer's own stream, and the call then synchronises).  The header holds the
  * image size, shard_index, shard_count, with_features, the entry count, whether the shard was reprojected
@@ -622,7 +635,8 @@ int rptb_buffer_export_shard(rptb_buffer* buffer, void* dst_device, uint32_t wit
  * from reprojected shards, it is a reprojected buffer, whose image, variance and denoise check the least count).
  * RPTB_ERR_BAD_ARG: a null pointer or shard_count 0; dst a shard buffer; a block that is not an export, or was made
  * for another image size, shard count or with_features; shards out of order (block i must hold shard i); shards that
- * received different calls (entry counts, reprojection, feature rays or cameras differ).                          */
+ * received different calls (entry counts, reprojection, feature rays or cameras differ); halves blocks into a plain
+ * dst.  RPTB_ERR_UNSUPPORTED: plain blocks into a dst with halves.  A dst with halves takes its HALF from the blocks. */
 int rptb_buffer_import_shards(rptb_buffer* dst, const void* gathered_device, uint32_t shard_count, uint32_t with_features);
 /* rptb_buffer_reproject into a shard buffer: `dst`, a shard, takes the history of its own pixels from `src`, a whole
  * buffer on the shard's device -- in a frame loop, the previous frame's shards gathered with features.  Each pixel
@@ -674,7 +688,11 @@ int rptb_buffer_reproject_merge_shard(rptb_buffer* dst, rptb_buffer* src, const 
  * uint32: each pixel's compact slot in the shard, ascending).  256 + 40 m bytes; only n entries of each plane are
  * written.  No device needed.                                                                                    */
 uint64_t rptb_delta_bytes(uint32_t capacity);
-/* Writes the shard buffer's delta block of `capacity` (rptb_delta_bytes) to dst_device, on `stream` as
+/* The delta block of a shard with halves (rptb_buffer_create_shard_halves): the block above, its header's flags saying
+ * halves, then HALF (3m doubles) at 256 + 40 m.  256 + 64 m bytes.  No device needed.                            */
+uint64_t rptb_delta_bytes_halves(uint32_t capacity);
+/* Writes the shard buffer's delta block of `capacity` (rptb_delta_bytes, or rptb_delta_bytes_halves for a shard with
+ * halves) to dst_device, on `stream` as
  * rptb_buffer_export_shard does; out_pixels (nullable) receives n.  It reads n, the call's active count, first (one
  * synchronising 8-byte copy).  A delta exists only when the shard's last call was rptb_sample_into_adaptive or
  * rptb_sample_into_guided_shard, that call came right after an export (full or delta), and it kept the shard's entry
@@ -691,7 +709,8 @@ int rptb_buffer_export_delta(rptb_buffer* buffer, void* dst_device, uint32_t cap
  * shards out of order; shards that received different calls (entry counts, reprojection, feature rays or cameras);
  * n > capacity; and a dst that is not at the blocks' state before the call -- one not last written by an import (full
  * or delta) of shard_count shards, or at another entry count, reprojection, feature rays or cameras.
- * RPTB_ERR_UNSUPPORTED: a dst of more than one part.                                                           */
+ * RPTB_ERR_UNSUPPORTED: a dst of more than one part.  A dst with halves takes halves blocks only, at the stride of
+ * rptb_delta_bytes_halves (RPTB_ERR_UNSUPPORTED: plain blocks); a plain dst plain ones (RPTB_ERR_BAD_ARG: halves blocks). */
 int rptb_buffer_import_deltas(rptb_buffer* dst, const void* gathered_device, uint32_t shard_count, uint32_t capacity);
 /* rptb_sample_into_guided for a shard buffer: the filter runs over `whole`, a one-part whole buffer on the shard's
  * device holding the gathered state of every shard at the shard's current state, and the mark writes this shard's
@@ -707,6 +726,16 @@ int rptb_sample_into_guided_shard(rptb_scene* scene, const rptb_camera* camera, 
                                   const rptb_adaptive* criterion, const rptb_denoise* guide, rptb_buffer* shard,
                                   rptb_buffer* whole /* nullable while shard entries < min_entries */,
                                   uint64_t* out_active /* nullable, forces sync */, rptb_stats* stats /* nullable, forces sync */);
+/* rptb_sample_into_guided_shard with E in place of v' (rptb_sample_into_guided_error): `shard` is a shard with halves
+ * (rptb_buffer_create_shard_halves), and once the filter runs, the error estimate runs over `whole`, a whole buffer
+ * with halves kept current by halves blocks, and the mark tests E for this shard's pixels.  Each shard renders exactly
+ * the pixels rptb_sample_into_guided_error renders among its tiles on a whole buffer with halves.  `whole` may be NULL
+ * while the shard holds fewer than min_entries entry calls.  Refusals as rptb_sample_into_guided_shard, and
+ * RPTB_ERR_BAD_ARG: the shard or `whole` without halves, guide->iterations == 0.                                 */
+int rptb_sample_into_guided_error_shard(rptb_scene* scene, const rptb_camera* camera, const rptb_render_params* params,
+                                        const rptb_adaptive* criterion, const rptb_denoise* guide, rptb_buffer* shard,
+                                        rptb_buffer* whole /* nullable while shard entries < min_entries */,
+                                        uint64_t* out_active /* nullable, forces sync */, rptb_stats* stats /* nullable, forces sync */);
 
 #ifdef __cplusplus
 }

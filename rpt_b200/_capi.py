@@ -306,6 +306,12 @@ SYMBOLS = [
     ("rptb_sample_into_guided_error", C.c_int,
      [C.c_void_p, C.POINTER(Camera), C.POINTER(RenderParams), C.POINTER(Adaptive), C.POINTER(Denoise), C.c_void_p,
       C.POINTER(C.c_uint64), C.POINTER(Stats)]),
+    ("rptb_buffer_create_shard_halves", C.c_int,
+     [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(C.c_void_p)]),
+    ("rptb_delta_bytes_halves", C.c_uint64, [C.c_uint32]),
+    ("rptb_sample_into_guided_error_shard", C.c_int,
+     [C.c_void_p, C.POINTER(Camera), C.POINTER(RenderParams), C.POINTER(Adaptive), C.POINTER(Denoise), C.c_void_p, C.c_void_p,
+      C.POINTER(C.c_uint64), C.POINTER(Stats)]),
 ]
 
 _lib = None

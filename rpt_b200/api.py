@@ -1251,7 +1251,8 @@ class Renderer:
         `guide_buffer` (a ShardBuffer with a guided `adaptive`; rptb_sample_into_guided_shard): the whole DeviceBuffer the
         shard's filter runs over -- every shard gathered with features on this rank's device, at the shard's current state
         (ShardBuffer.gather, then ShardBuffer.gather_delta after each call).  None is allowed while the shard has fewer
-        than adaptive.min_entries calls, when the plain mark decides."""
+        than adaptive.min_entries calls, when the plain mark decides.  With estimate="halves"
+        (rptb_sample_into_guided_error_shard) the shard and guide_buffer both have halves."""
         ds = self.device_scene()
         shard = getattr(buffer, "shard", None) or (0, 1)
         p = self.params(iterations, self._next_sample, *shard, collect_stats=collect_stats)
@@ -1262,8 +1263,11 @@ class Renderer:
             stats, active, crit = capi.Stats(), C.c_uint64(0), adaptive.to_c()
             st = C.byref(stats) if want_stats else None
             if adaptive.estimate == "halves" and guide_buffer is not Renderer._NO_GUIDE_BUFFER:
-                raise ValueError('estimate="halves" is not supported on shards')
-            if adaptive.estimate == "halves":
+                guide = adaptive.guide.to_c()
+                capi.check(capi.lib().rptb_sample_into_guided_error_shard(
+                    ds.handle, C.byref(cam), C.byref(p), C.byref(crit), C.byref(guide), buffer.handle,
+                    guide_buffer.handle if guide_buffer is not None else None, C.byref(active), st), "rptb_sample_into_guided_error_shard")
+            elif adaptive.estimate == "halves":
                 guide = adaptive.guide.to_c()
                 capi.check(capi.lib().rptb_sample_into_guided_error(ds.handle, C.byref(cam), C.byref(p), C.byref(crit), C.byref(guide),
                                                                     buffer.handle, C.byref(active), st), "rptb_sample_into_guided_error")

@@ -63,10 +63,10 @@ cudaError_t launch_guided_mark(const double* col, const double* var, const doubl
 // the delta exchange of a shard buffer: delta.cu
 size_t delta_temp_bytes(uint64_t nelem);
 cudaError_t launch_delta_export(const uint8_t* mask, uint64_t nelem, const double* sums, const double* m2, const uint32_t* counts,
-                                void* block, uint32_t capacity, uint32_t pixels, uint32_t* selected, void* temp, size_t temp_bytes,
-                                cudaStream_t stream);
+                                const double* half, void* block, uint32_t capacity, uint32_t pixels, uint32_t* selected, void* temp,
+                                size_t temp_bytes, cudaStream_t stream);
 cudaError_t launch_delta_import(const void* blocks, uint32_t shard_count, uint32_t capacity, double* sums, double* m2, uint32_t* counts,
-                                cudaStream_t stream);
+                                double* half, cudaStream_t stream);
 // the feature planes and the denoiser: denoise.cu
 cudaError_t launch_features_resolve(const FeaturePlanes& f, uint64_t npix, double rays, const Aov& out, cudaStream_t stream);
 cudaError_t launch_denoise(const double* sums, const double* m2, const uint32_t* counts, const double* nrm,
@@ -961,12 +961,15 @@ int sample_part(rptb_scene* r, const rptb_camera* cam, const rptb_render_params*
 
 // ---- the exchange block of a shard buffer (rptb_buffer_export_shard / rptb_buffer_import_shards) ----
 // A header of kShardHeaderBytes, then the shard's compact planes in Plane order (planes.h), the feature planes only
-// with features, each padded to shard 0's slots (the most any shard holds, as distributed.gather_tiles pads).  Slots past
-// the shard's own are not written.
+// with features and HALF only from a shard with halves, each padded to shard 0's slots (the most any shard holds, as
+// distributed.gather_tiles pads).  Slots past the shard's own are not written.
 constexpr uint32_t kShardMagic = 0x44524853u;  // "SHRD"
 constexpr size_t kShardHeaderBytes = 256;
-// ShardHeader::flags: the shard was reprojected (rptb_buffer_reproject_shard), so its pixels may hold 0 or 1 entries
+// BlockState::flags: the shard was reprojected (rptb_buffer_reproject_shard), so its pixels may hold 0 or 1 entries
 constexpr uint32_t kShardReprojected = 1u;
+// BlockState::flags: the buffer has halves (rptb_buffer_create_halves, rptb_buffer_create_shard_halves), and its exchange
+// blocks carry HALF
+constexpr uint32_t kShardHalves = 2u;
 struct ShardHeader {
     uint32_t magic, with_features, width, height, shard_index, shard_count;
     BlockState s;
@@ -979,10 +982,10 @@ struct ShardLayout {
     size_t at[NPLANES];   // their byte offsets in the block
     size_t bytes;         // the block's size
 };
-ShardLayout shard_layout(uint32_t width, uint32_t height, uint32_t count, bool with_features) {
+ShardLayout shard_layout(uint32_t width, uint32_t height, uint32_t count, bool with_features, bool halves) {
     ShardLayout l = {};
     l.slots = (size_t)buffer_tiles(width, height, 0, count) * 128u;
-    l.mask = COLOUR | (with_features ? FEATURES : 0u);
+    l.mask = COLOUR | (with_features ? FEATURES : 0u) | (halves ? 1u << HALF : 0u);
     l.bytes = kShardHeaderBytes;
     for (int k = 0; k < NPLANES; k++)
         if (l.mask >> k & 1u) {
@@ -1017,7 +1020,8 @@ CameraRecord camera_record(const ShardCamera& c) {
 
 // b's state as an exchange header carries it
 BlockState block_state(const rptb_buffer* b) {
-    return {b->entries, b->reprojected ? kShardReprojected : 0u, b->feature_rays, shard_camera(b->entry_cam), shard_camera(b->feat_cam)};
+    const uint32_t flags = (b->reprojected ? kShardReprojected : 0u) | (b->halves ? kShardHalves : 0u);
+    return {b->entries, flags, b->feature_rays, shard_camera(b->entry_cam), shard_camera(b->feat_cam)};
 }
 
 bool same_state(const BlockState& x, const BlockState& y) { return std::memcmp(&x, &y, sizeof(BlockState)) == 0; }
@@ -1034,6 +1038,19 @@ int fetch_headers(const char* in, uint32_t n, uint64_t stride, cudaStream_t stre
     if (rc != RPTB_OK) return rc;
     if (n > 1) CU(cudaMemcpy2DAsync(hs.data() + 1, sizeof(H), in + stride, stride, sizeof(H), n - 1, cudaMemcpyDeviceToHost, stream));
     CU(cudaStreamSynchronize(stream));
+    return RPTB_OK;
+}
+
+// What an import checks of block 0's state against dst before it reads the other blocks, whose stride depends on it:
+// halves blocks go into a dst with halves (rptb_buffer_create_halves), plain ones into a plain dst.
+int check_halves(const BlockState& s0, const rptb_buffer* dst, const char* what) {
+    const bool halves = (s0.flags & kShardHalves) != 0;
+    if (dst->halves && !halves)
+        return fail(RPTB_ERR_UNSUPPORTED, "dst has halves but the %s carry none: export them from shards with halves "
+                                          "(rptb_buffer_create_shard_halves)", what);
+    if (!dst->halves && halves)
+        return fail(RPTB_ERR_BAD_ARG, "the %s carry halves but dst has none: import them into a buffer with halves "
+                                      "(rptb_buffer_create_halves)", what);
     return RPTB_OK;
 }
 
@@ -1649,6 +1666,11 @@ int rptb_buffer_create_shard(rptb_scene* s, uint32_t width, uint32_t height, uin
     return buffer_create_impl(s, width, height, box_radius, out, false, true, shard_index, shard_count);
 }
 
+int rptb_buffer_create_shard_halves(rptb_scene* s, uint32_t width, uint32_t height, uint32_t box_radius, uint32_t shard_index,
+                                    uint32_t shard_count, rptb_buffer** out) {
+    return buffer_create_impl(s, width, height, box_radius, out, true, true, shard_index, shard_count);
+}
+
 void rptb_buffer_destroy(rptb_buffer* b) {
     if (b) buffer_free(b);
 }
@@ -1765,8 +1787,9 @@ static int guide_mark(rptb_buffer* f, rptb_buffer* b, const rptb_adaptive& crit,
 
 // What rptb_sample_into_guided_shard checks of `whole` (locked) once the filter runs: a one-part whole buffer on the
 // shard's device, of its size, last written by an import of all the shards at the shard's current state -- which the
-// shard still has, not having changed since its last export -- and check_guide_buffer's conditions.
-static int check_guide_whole(const rptb_buffer* shard, const rptb_buffer* whole, const rptb_camera* cam) {
+// shard still has, not having changed since its last export -- and check_guide_buffer's conditions.  `error`
+// (rptb_sample_into_guided_error_shard): whole has halves too.
+static int check_guide_whole(const rptb_buffer* shard, const rptb_buffer* whole, const rptb_camera* cam, bool error) {
     if (!whole) return fail(RPTB_ERR_BAD_ARG, "null whole buffer: the shard has reached min_entries, so the filter runs over its gathered image");
     if (whole->shard) return fail(RPTB_ERR_BAD_ARG, "whole is a shard buffer: the filter needs every shard gathered (rptb_buffer_import_shards)");
     if (whole->parts.size() != 1)
@@ -1776,6 +1799,9 @@ static int check_guide_whole(const rptb_buffer* shard, const rptb_buffer* whole,
         return fail(RPTB_ERR_BAD_ARG, "whole is on device %d but the shard on device %d", whole->parts[0].device, q.device);
     if (whole->width != shard->width || whole->height != shard->height)
         return fail(RPTB_ERR_BAD_ARG, "whole is %ux%u but the shard %ux%u", whole->width, whole->height, shard->width, shard->height);
+    if (error && !whole->halves)
+        return fail(RPTB_ERR_BAD_ARG, "whole has no halves (rptb_buffer_create_halves): no error estimate; import halves shards into a "
+                                      "whole buffer with halves");
     if (shard->exported != shard->state)
         return fail(RPTB_ERR_BAD_ARG, "the shard changed since its last export: gather it into whole first (rptb_buffer_export_shard or "
                                       "rptb_buffer_export_delta)");
@@ -1792,7 +1818,8 @@ static int check_guide_whole(const rptb_buffer* shard, const rptb_buffer* whole,
 
 // rptb_sample_into (crit null), rptb_sample_into_adaptive (crit) and rptb_sample_into_guided (crit and guide; the
 // filter runs when guide->iterations > 0).  shard_entry (rptb_sample_into_guided_shard): b is a shard buffer and the
-// filter runs over `whole`.  error (rptb_sample_into_guided_error): b has halves, and the mark tests E.
+// filter runs over `whole`.  error (rptb_sample_into_guided_error, and with shard_entry
+// rptb_sample_into_guided_error_shard): b (and `whole`) has halves, and the mark tests E.
 static int sample_into_impl(rptb_scene* s, const rptb_camera* cam, const rptb_render_params* p, const rptb_adaptive* crit,
                             const rptb_denoise* guide, rptb_buffer* b, uint64_t* out_active, rptb_stats* stats, bool shard_entry = false,
                             rptb_buffer* whole = nullptr, bool error = false) {
@@ -1818,7 +1845,7 @@ static int sample_into_impl(rptb_scene* s, const rptb_camera* cam, const rptb_re
     std::unique_lock<std::mutex> wl;
     if (marked && shard_entry) {
         if (whole && whole != b) wl = std::unique_lock<std::mutex>(whole->lock);
-        rc = check_guide_whole(b, whole, cam);
+        rc = check_guide_whole(b, whole, cam, error);
         if (rc != RPTB_OK) return rc;
     }
     uint32_t guide_launches = 0;
@@ -1945,6 +1972,16 @@ int rptb_sample_into_guided_shard(rptb_scene* s, const rptb_camera* cam, const r
     if (rc == RPTB_OK) rc = check_denoise(guide);
     if (rc != RPTB_OK) return rc;
     return sample_into_impl(s, cam, p, crit, guide, shard, out_active, stats, true, whole);
+}
+
+int rptb_sample_into_guided_error_shard(rptb_scene* s, const rptb_camera* cam, const rptb_render_params* p, const rptb_adaptive* crit,
+                                        const rptb_denoise* guide, rptb_buffer* shard, rptb_buffer* whole, uint64_t* out_active,
+                                        rptb_stats* stats) {
+    int rc = check_adaptive(crit);
+    if (rc == RPTB_OK) rc = check_denoise(guide);
+    if (rc != RPTB_OK) return rc;
+    if (guide->iterations == 0) return fail(RPTB_ERR_BAD_ARG, "iterations 0: the error estimate needs at least one filter pass");
+    return sample_into_impl(s, cam, p, crit, guide, shard, out_active, stats, true, whole, true);
 }
 
 int rptb_buffer_add_samples(rptb_buffer* b, const double* rgb) {
@@ -2217,6 +2254,7 @@ int rptb_buffer_denoise_variance(rptb_buffer* b, const rptb_denoise* d, double* 
 int rptb_buffer_half_sums(rptb_buffer* b, double* out) {
     if (!b || !out) return fail(RPTB_ERR_BAD_ARG, "null argument");
     if (!b->halves) return fail(RPTB_ERR_BAD_ARG, "the buffer has no halves (rptb_buffer_create_halves)");
+    if (b->shard) return refuse_shard("half_sums");
     std::lock_guard<std::mutex> bl(b->lock);
     BufferPart& q0 = b->parts[0];
     DeviceGuard g(q0.device);
@@ -2414,7 +2452,7 @@ int rptb_buffer_reproject_merge_shard(rptb_buffer* dst, rptb_buffer* src, const 
 
 uint64_t rptb_buffer_shard_bytes(const rptb_buffer* b, uint32_t with_features) {
     if (!b || !b->shard) return 0;
-    return shard_layout(b->width, b->height, b->parts[0].count, with_features != 0).bytes;
+    return shard_layout(b->width, b->height, b->parts[0].count, with_features != 0, b->halves).bytes;
 }
 
 int rptb_buffer_export_shard(rptb_buffer* b, void* dst_device, uint32_t with_features, void* stream) {
@@ -2425,7 +2463,7 @@ int rptb_buffer_export_shard(rptb_buffer* b, void* dst_device, uint32_t with_fea
     BufferPart& q = b->parts[0];
     DeviceGuard g(q.device);
     if (!g.ok) return fail(RPTB_ERR_CUDA, "cudaSetDevice(%d) failed", q.device);
-    const ShardLayout l = shard_layout(b->width, b->height, q.count, with_features != 0);
+    const ShardLayout l = shard_layout(b->width, b->height, q.count, with_features != 0, b->halves);
     ShardHeader h;
     std::memset(&h, 0, sizeof(h));
     h.magic = kShardMagic;
@@ -2454,13 +2492,12 @@ int rptb_buffer_import_shards(rptb_buffer* dst, const void* gathered_device, uin
     if (!dst || !gathered_device) return fail(RPTB_ERR_BAD_ARG, "null argument");
     if (shard_count == 0) return fail(RPTB_ERR_BAD_ARG, "shard_count 0");
     if (dst->shard) return fail(RPTB_ERR_BAD_ARG, "dst is a shard buffer: the shards gather into a whole buffer (rptb_buffer_create)");
-    if (dst->halves) return fail(RPTB_ERR_UNSUPPORTED, "dst has halves: shards carry no halves");
     std::lock_guard<std::mutex> bl(dst->lock);
     BufferPart& d0 = dst->parts[0];
     DeviceGuard g(d0.device);
     if (!g.ok) return fail(RPTB_ERR_CUDA, "cudaSetDevice(%d) failed", d0.device);
     const uint32_t W = dst->width, H = dst->height;
-    const ShardLayout l = shard_layout(W, H, shard_count, with_features != 0);
+    const ShardLayout l = shard_layout(W, H, shard_count, with_features != 0, dst->halves);
     const char* in = (const char*)gathered_device;
     std::vector<ShardHeader> hs;
     int rc = fetch_headers(in, shard_count, l.bytes, d0.stream, hs, [&](const ShardHeader& h0) {
@@ -2470,8 +2507,8 @@ int rptb_buffer_import_shards(rptb_buffer* dst, const void* gathered_device, uin
         if (h0.shard_count != shard_count) return fail(RPTB_ERR_BAD_ARG, "the shards are %u but shard_count is %u", h0.shard_count, shard_count);
         if (h0.with_features != (with_features ? 1u : 0u))
             return fail(RPTB_ERR_BAD_ARG, "the shards were exported %s features", h0.with_features ? "with" : "without");
-        if (h0.s.flags & ~kShardReprojected) return fail(RPTB_ERR_BAD_ARG, "block 0 carries unknown flags 0x%x", h0.s.flags);
-        return (int)RPTB_OK;
+        if (h0.s.flags & ~(kShardReprojected | kShardHalves)) return fail(RPTB_ERR_BAD_ARG, "block 0 carries unknown flags 0x%x", h0.s.flags);
+        return check_halves(h0.s, dst, "shards");
     });
     if (rc != RPTB_OK) return rc;
     const ShardHeader& h0 = hs[0];
@@ -2527,6 +2564,8 @@ int rptb_buffer_import_shards(rptb_buffer* dst, const void* gathered_device, uin
 
 uint64_t rptb_delta_bytes(uint32_t capacity) { return delta_bytes(capacity); }
 
+uint64_t rptb_delta_bytes_halves(uint32_t capacity) { return delta_bytes_halves(capacity); }
+
 int rptb_buffer_export_delta(rptb_buffer* b, void* dst_device, uint32_t capacity, void* stream, uint32_t* out_pixels) {
     if (!b || !dst_device) return fail(RPTB_ERR_BAD_ARG, "null argument");
     if (!b->shard) return fail(RPTB_ERR_BAD_ARG, "not a shard buffer (rptb_buffer_create_shard)");
@@ -2562,8 +2601,8 @@ int rptb_buffer_export_delta(rptb_buffer* b, void* dst_device, uint32_t capacity
     h.capacity = capacity;
     // pageable source: the call returns once the header is staged
     CU(cudaMemcpyAsync(dst_device, &h, sizeof(h), cudaMemcpyHostToDevice, st));
-    CU(launch_delta_export(q.mask, nelem, q.planes.sums, q.planes.m2, q.planes.counts, dst_device, capacity, (uint32_t)n, q.delta_len,
-                           q.delta_temp, q.delta_temp_bytes, st));
+    CU(launch_delta_export(q.mask, nelem, q.planes.sums, q.planes.m2, q.planes.counts, b->halves ? q.planes.half : nullptr, dst_device,
+                           capacity, (uint32_t)n, q.delta_len, q.delta_temp, q.delta_temp_bytes, st));
     // a later mark or accumulate into the part waits until the block is written
     CU(cudaEventRecord(q.done, st));
     if (!stream) CU(cudaStreamSynchronize(st));
@@ -2576,7 +2615,6 @@ int rptb_buffer_import_deltas(rptb_buffer* dst, const void* gathered_device, uin
     if (!dst || !gathered_device) return fail(RPTB_ERR_BAD_ARG, "null argument");
     if (shard_count == 0) return fail(RPTB_ERR_BAD_ARG, "shard_count 0");
     if (dst->shard) return fail(RPTB_ERR_BAD_ARG, "dst is a shard buffer: the deltas go into the shards' gathered whole buffer");
-    if (dst->halves) return fail(RPTB_ERR_UNSUPPORTED, "dst has halves: shards carry no halves");
     if (dst->parts.size() != 1)
         return fail(RPTB_ERR_UNSUPPORTED, "dst has %zu parts: deltas are imported into a one-part whole buffer", dst->parts.size());
     std::lock_guard<std::mutex> bl(dst->lock);
@@ -2584,7 +2622,7 @@ int rptb_buffer_import_deltas(rptb_buffer* dst, const void* gathered_device, uin
     DeviceGuard g(d0.device);
     if (!g.ok) return fail(RPTB_ERR_CUDA, "cudaSetDevice(%d) failed", d0.device);
     const uint32_t W = dst->width, H = dst->height;
-    const uint64_t bytes = delta_bytes(capacity);
+    const uint64_t bytes = dst->halves ? delta_bytes_halves(capacity) : delta_bytes(capacity);
     const char* in = (const char*)gathered_device;
     std::vector<DeltaHeader> hs;
     const int rc = fetch_headers(in, shard_count, bytes, d0.stream, hs, [&](const DeltaHeader& h0) {
@@ -2593,7 +2631,7 @@ int rptb_buffer_import_deltas(rptb_buffer* dst, const void* gathered_device, uin
         if (h0.shard_count != shard_count)
             return fail(RPTB_ERR_BAD_ARG, "the deltas are of %u shards but shard_count is %u", h0.shard_count, shard_count);
         if (h0.capacity != capacity) return fail(RPTB_ERR_BAD_ARG, "the deltas have capacity %u but capacity is %u", h0.capacity, capacity);
-        return (int)RPTB_OK;
+        return check_halves(h0.s, dst, "deltas");
     });
     if (rc != RPTB_OK) return rc;
     const DeltaHeader& h0 = hs[0];
@@ -2614,9 +2652,10 @@ int rptb_buffer_import_deltas(rptb_buffer* dst, const void* gathered_device, uin
     }
     // dst must hold the shards' state before the call: an import of them, untouched since.  The entry camera before the call
     // is the one after it, or none before the first entry (rptb_buffer_export_delta refuses any other change).  The state
-    // is compared as dst would record it from the header: the reprojected flag only, and each camera as its state keeps it.
+    // is compared as dst would record it from the header: the reprojected and halves flags only, and each camera as its
+    // state keeps it.
     const CameraRecord after_cam = camera_record(h0.s.entry_cam);
-    const BlockState before = {h0.entries_before, h0.s.flags & kShardReprojected, h0.s.feature_rays,
+    const BlockState before = {h0.entries_before, h0.s.flags & (kShardReprojected | kShardHalves), h0.s.feature_rays,
                                shard_camera(h0.entries_before == 0 ? CameraRecord() : after_cam), shard_camera(camera_record(h0.s.feat_cam))};
     if (dst->imported != dst->state || dst->imported_shards != shard_count)
         return fail(RPTB_ERR_BAD_ARG, "dst was not last written by an import of the %u shards (rptb_buffer_import_shards or "
@@ -2630,7 +2669,8 @@ int rptb_buffer_import_deltas(rptb_buffer* dst, const void* gathered_device, uin
     // in place in dst's compact planes; every later call on dst is ordered behind it
     dst->state++;
     CU(cudaStreamWaitEvent(d0.stream, d0.done, 0));
-    CU(launch_delta_import(in, shard_count, capacity, d0.planes.sums, d0.planes.m2, d0.planes.counts, d0.stream));
+    CU(launch_delta_import(in, shard_count, capacity, d0.planes.sums, d0.planes.m2, d0.planes.counts, dst->halves ? d0.planes.half : nullptr,
+                           d0.stream));
     CU(cudaEventRecord(d0.done, d0.stream));
     // the caller may reuse the gathered bytes when the call returns
     CU(cudaStreamSynchronize(d0.stream));

@@ -8,8 +8,11 @@
 //     m2      m doubles
 //     counts  m uint32
 //     slots   m uint32   the shard's compact slot of each pixel, ascending
-// 256 + 40 m bytes, so every plane and the next block start 8-byte aligned.  Only the header's `pixels` entries of each
-// plane are written.
+// 256 + 40 m bytes, so every plane and the next block start 8-byte aligned.  A shard with halves
+// (rptb_buffer_create_shard_halves; its header's flags hold kShardHalves) appends
+//     half    3m doubles  the sums of each pixel's odd entries (the HALF plane, planes.h)
+// at 256 + 40 m: 256 + 64 m bytes, with the prefix laid out as above.  Only the header's `pixels` entries of each plane
+// are written.
 #pragma once
 #include "../../include/rpt_b200.h"
 #include "tile.h"
@@ -25,8 +28,8 @@ struct ShardCamera {
     rptb_camera cam;
 };
 
-// A buffer's state as both exchange headers carry it, at the same offset: its entry calls, flags (kShardReprojected,
-// api.cu), feature rays per pixel and cameras.  Every byte is written (shard_camera zeroes what a state leaves unused),
+// A buffer's state as both exchange headers carry it, at the same offset: its entry calls, flags (kShardReprojected and
+// kShardHalves, api.cu), feature rays per pixel and cameras.  Every byte is written (shard_camera zeroes what a state leaves unused),
 // so two states are the same when their bytes are.
 struct BlockState {
     uint32_t entries, flags;
@@ -46,6 +49,7 @@ static_assert(offsetof(DeltaHeader, s) == 24, "the state sits where the shard he
 static_assert(offsetof(DeltaHeader, pixels) == 248, "distributed.DELTA_PIXELS_AT");
 
 RPTB_HD uint64_t delta_bytes(uint32_t capacity) { return kDeltaHeaderBytes + 40ull * capacity; }
+RPTB_HD uint64_t delta_bytes_halves(uint32_t capacity) { return kDeltaHeaderBytes + 64ull * capacity; }
 
 // The planes of the block at `block`, of capacity m.
 struct DeltaPlanes {
@@ -85,6 +89,37 @@ RPTB_HD void delta_import_one(const DeltaPlanes& d, uint32_t i, uint32_t index, 
     sums[3 * e + 2] = d.sums[3ull * i + 2];
     m2[e] = d.m2[i];
     counts[e] = d.counts[i];
+}
+
+// The planes of a halves block at `block`, of capacity m: the plain block's, then HALF.
+struct DeltaHalvesPlanes {
+    DeltaPlanes d;
+    double* half;
+};
+RPTB_HD DeltaHalvesPlanes delta_halves_planes(const void* block, uint32_t m) {
+    return {delta_planes(block, m), (double*)((char*)block + kDeltaHeaderBytes + 40ull * m)};
+}
+
+// delta_export_one, and the slot's HALF.
+RPTB_HD void delta_export_halves_one(const DeltaHalvesPlanes& d, uint32_t i, const double* __restrict__ sums,
+                                     const double* __restrict__ m2, const uint32_t* __restrict__ counts,
+                                     const double* __restrict__ half) {
+    delta_export_one(d.d, i, sums, m2, counts);
+    const uint64_t s = d.d.slots[i];
+    d.half[3ull * i] = half[3 * s];
+    d.half[3ull * i + 1] = half[3 * s + 1];
+    d.half[3ull * i + 2] = half[3 * s + 2];
+}
+
+// delta_import_one, and the element's HALF.
+RPTB_HD void delta_import_halves_one(const DeltaHalvesPlanes& d, uint32_t i, uint32_t index, uint32_t count,
+                                     double* __restrict__ sums, double* __restrict__ m2, uint32_t* __restrict__ counts,
+                                     double* __restrict__ half) {
+    delta_import_one(d.d, i, index, count, sums, m2, counts);
+    const uint64_t e = delta_whole_slot(index, count, d.d.slots[i]);
+    half[3 * e] = d.half[3ull * i];
+    half[3 * e + 1] = d.half[3ull * i + 1];
+    half[3 * e + 2] = d.half[3ull * i + 2];
 }
 
 }  // namespace rptb

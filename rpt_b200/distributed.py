@@ -33,7 +33,9 @@ other ranks' tiles, so every rank needs the whole image's state before each guid
 buffer current instead of re-gathering it: one full gather with features when the filter is first needed, then after
 every call one all-gather of delta blocks (ShardBuffer.gather_delta) -- only the pixels that call changed, with their
 new state -- applied in place.  Each rank's filter and decisions are then those of the whole buffer's call, bit for
-bit, and so are its entries.
+bit, and so are its entries.  The error estimate from two half buffers (Adaptive(estimate="halves")) runs the same
+way over shards with halves (ShardBuffer(halves=True)): their full and delta blocks carry HALF too, and the gathered
+whole buffer has halves.
 """
 from __future__ import annotations
 
@@ -174,34 +176,44 @@ def render_distributed_gather(renderer, iterations: int, first_sample: int = 0, 
 SHARD_HEADER_BYTES = 256  # must match rpt_b200/csrc/api.cu (kShardHeaderBytes)
 
 
-def shard_block_layout(width: int, height: int, shard_count: int, with_features: bool = False) -> dict:
+def shard_block_layout(width: int, height: int, shard_count: int, with_features: bool = False, halves: bool = False) -> dict:
     """Byte offsets of the planes in one shard's exchange block (rptb_buffer_export_shard), the same for every shard:
     a header, then sums (3 doubles a slot), M2 (1 double), with features the feature sums (8 doubles: normal 3, albedo
-    3, hits 1, depth 1), then counts (1 uint32).  Every plane has `slots` = shard 0's tiles * 128 slots, the padding
-    gather_tiles uses, so slot k * 128 + j of shard s's planes is pixel rptb_tile_pixel(width, height, s, shard_count,
-    k, j) and gather_permutation(width, height, shard_count) // slots / % slots finds a pixel's shard and slot."""
+    3, hits 1, depth 1), then counts (1 uint32), and from a shard with halves HALF (3 doubles: the sums of the odd
+    entries) at "half".  Every plane has `slots` = shard 0's tiles * 128 slots, the padding gather_tiles uses, so slot
+    k * 128 + j of shard s's planes is pixel rptb_tile_pixel(width, height, s, shard_count, k, j) and
+    gather_permutation(width, height, shard_count) // slots / % slots finds a pixel's shard and slot."""
     slots = shard_tiles(width, height, 0, shard_count) * TILE_W * TILE_H
     sums = SHARD_HEADER_BYTES
     m2 = sums + slots * 3 * 8
     features = m2 + slots * 8
     counts = features + (slots * 8 * 8 if with_features else 0)
-    return {"slots": slots, "sums": sums, "m2": m2, "features": features, "counts": counts, "bytes": counts + slots * 4}
+    lay = {"slots": slots, "sums": sums, "m2": m2, "features": features, "counts": counts, "bytes": counts + slots * 4}
+    if halves:
+        lay["half"] = lay["bytes"]
+        lay["bytes"] += slots * 3 * 8
+    return lay
 
 
 DELTA_HEADER_BYTES = 256  # must match rpt_b200/csrc/delta.h (kDeltaHeaderBytes)
 DELTA_PIXELS_AT = 248  # the byte offset of the header's pixel count (DeltaHeader::pixels, a uint32)
 
 
-def delta_block_layout(capacity: int) -> dict:
+def delta_block_layout(capacity: int, halves: bool = False) -> dict:
     """Byte offsets of the planes in one shard's delta block of `capacity` pixels (rptb_buffer_export_delta), the same for
     every shard: a header, then sums (3 doubles a pixel), M2 (1 double), counts (1 uint32) and slots (1 uint32: the
-    pixel's compact slot in its shard, ascending).  Only the header's pixel count of each plane is written."""
+    pixel's compact slot in its shard, ascending), and from a shard with halves HALF (3 doubles) at "half"
+    (rptb_delta_bytes_halves).  Only the header's pixel count of each plane is written."""
     m = int(capacity)
     sums = DELTA_HEADER_BYTES
     m2 = sums + 24 * m
     counts = m2 + 8 * m
     slots = counts + 4 * m
-    return {"capacity": m, "sums": sums, "m2": m2, "counts": counts, "slots": slots, "bytes": slots + 4 * m}
+    lay = {"capacity": m, "sums": sums, "m2": m2, "counts": counts, "slots": slots, "bytes": slots + 4 * m}
+    if halves:
+        lay["half"] = lay["bytes"]
+        lay["bytes"] += 24 * m
+    return lay
 
 
 def _all_gather_bytes(mine, world: int, group):
@@ -235,10 +247,12 @@ class ShardBuffer(api.DeviceBuffer):
     those tiles, with no exchange; an adaptive sample() returns this rank's active pixel count, and reproject_from
     takes this rank's pixels' history from a whole buffer.  Whole-image reads (image, variance, sums, pixel_stats,
     counts, features, denoise, add_samples) are refused: gather() first.  `entries` counts the calls (a bound on any
-    pixel's count) until the gather reads the counts."""
+    pixel's count) until the gather reads the counts.  `halves` (rptb_buffer_create_shard_halves): the shard also keeps
+    the sums of each pixel's odd entries, its blocks carry them, and gather() gives a whole buffer with halves -- what
+    Adaptive(estimate="halves") needs; a frame's reproject_from and merge_history_from refuse it."""
 
     def __init__(self, scene: "api.DeviceScene", width: int, height: int, filter: Optional["api.Filter"] = None, group=None,
-                 rank: Optional[int] = None, world: Optional[int] = None):
+                 rank: Optional[int] = None, world: Optional[int] = None, halves: bool = False):
         if rank is None or world is None:
             rank, world = _rank_world(group)
         self.width, self.height = int(width), int(height)
@@ -247,14 +261,16 @@ class ShardBuffer(api.DeviceBuffer):
         self.entries = 0
         self.feature_rays = 0
         self.shard = (int(rank), int(world))
+        self.halves = bool(halves)
         self.group = group
         self._scene = scene  # the whole buffer of gather() is created on it
         self.handle = C.c_void_p()
-        capi.check(capi.lib().rptb_buffer_create_shard(scene.handle, self.width, self.height, self.filter.radius, self.shard[0],
-                                                       self.shard[1], C.byref(self.handle)), "rptb_buffer_create_shard")
+        name = "rptb_buffer_create_shard_halves" if self.halves else "rptb_buffer_create_shard"
+        capi.check(getattr(capi.lib(), name)(scene.handle, self.width, self.height, self.filter.radius, self.shard[0], self.shard[1],
+                                             C.byref(self.handle)), name)
 
     def block_bytes(self, with_features: bool = False) -> int:
-        """The size of this shard's exchange block (rptb_buffer_shard_bytes): the same on every rank."""
+        """The size of this shard's exchange block (rptb_buffer_shard_bytes; shard_block_layout): the same on every rank."""
         return int(capi.lib().rptb_buffer_shard_bytes(self.handle, 1 if with_features else 0))
 
     def export(self, out, with_features: bool = False, stream: Optional[int] = None) -> None:
@@ -320,9 +336,10 @@ class ShardBuffer(api.DeviceBuffer):
         """All ranks call this: export every shard's block, one all_gather_into_tensor, and import the blocks into a new
         whole DeviceBuffer on this rank's device -- the same bits on every rank, and those of one whole buffer given the
         same calls.  NCCL gathers GPU to GPU; any other backend (gloo) through a host tensor.  `with_features` carries
-        the feature sums too (denoise and reproject need them), 100 instead of 36 bytes per pixel."""
+        the feature sums too (denoise and reproject need them), 100 instead of 36 bytes per pixel.  A shard with halves
+        carries HALF as well (124 or 60 bytes per pixel) and gives a whole buffer with halves."""
         gathered, _ = self._exchange(group, self.block_bytes(with_features), lambda out, stream: self.export(out, with_features, stream))
-        whole = api.DeviceBuffer(self._scene, self.width, self.height, self.filter)
+        whole = api.DeviceBuffer(self._scene, self.width, self.height, self.filter, halves=self.halves)
         capi.check(capi.lib().rptb_buffer_import_shards(whole.handle, C.c_void_p(gathered.data_ptr()), self.shard[1],
                                                         1 if with_features else 0), "rptb_buffer_import_shards")
         whole.entries = int(whole.counts().max())
@@ -330,7 +347,8 @@ class ShardBuffer(api.DeviceBuffer):
         return whole
 
     def export_delta(self, out, capacity: int, stream: Optional[int] = None) -> int:
-        """Writes this shard's delta block of `capacity` pixels (delta_block_layout; rptb_buffer_export_delta) into `out`, a
+        """Writes this shard's delta block of `capacity` pixels (delta_block_layout(capacity, self.halves);
+        rptb_buffer_export_delta) into `out`, a
         CUDA uint8 tensor on the buffer's device, on `stream` (a raw cudaStream_t; the current torch stream when None):
         the pixels this shard's last call changed, which must be an adaptive or guided call made right after an export
         (gather or gather_delta).  Returns their number."""
@@ -352,7 +370,7 @@ class ShardBuffer(api.DeviceBuffer):
         import torch
 
         world = self.shard[1]
-        lay = delta_block_layout(capacity)
+        lay = delta_block_layout(capacity, self.halves)
         gathered, staged = self._exchange(group, lay["bytes"], lambda out, stream: self.export_delta(out, capacity, stream))
         capi.check(capi.lib().rptb_buffer_import_deltas(whole.handle, C.c_void_p(gathered.data_ptr()), world, lay["capacity"]),
                    "rptb_buffer_import_deltas")
@@ -413,12 +431,12 @@ class _GuidedShard:
 def _check_guided_world(adaptive, world: int) -> None:
     """A guided loop on shards keeps a gathered whole buffer on every rank and exchanges the ranks' deltas.  On one rank
     the shard is already the whole image, so that copy and that exchange would only add work to what the whole-buffer
-    loop does: refused, before any device work or collective, with the loop to use instead.  The error estimate from two
-    half buffers (estimate="halves") is refused on any world size: a shard buffer has no halves."""
-    if adaptive is not None and adaptive.estimate == "halves":
-        raise ValueError('estimate="halves" is not supported on shards: a shard buffer has no halves; one process renders it '
-                         "on one whole buffer: Renderer.iterative_render")
+    loop does: refused, before any device work or collective, with the loop to use instead."""
     if adaptive is not None and adaptive.guide is not None and world < 2:
+        if adaptive.estimate == "halves":
+            raise ValueError('guided adaptive sampling on the error estimate (estimate="halves") on shards needs two or more '
+                             "ranks (torch.distributed initialized); one process renders it on one whole buffer with halves: "
+                             "Renderer.iterative_render")
         raise ValueError("guided adaptive sampling (Adaptive(guide=...)) on shards needs two or more ranks (torch.distributed "
                          "initialized); one process renders it on one whole buffer: Renderer.iterative_render / render_frames")
 
@@ -435,13 +453,20 @@ def render_iterative_distributed(renderer, callback_interval: int, callback: Cal
     feature rays per pixel; the first batch that runs the filter is preceded by one gather with features, and every
     batch after that by the gather_delta of the batch before, which runs right after it, ahead of the callback.  The
     active counts are all-gathered instead of all-reduced: their sum ends the loop, their largest is the delta's
-    capacity.  With one rank, a guided criterion is refused (ValueError): the whole-buffer loop does the same work."""
+    capacity.  With one rank, a guided criterion is refused (ValueError): the whole-buffer loop does the same work.
+    The error estimate (Adaptive(guide=..., estimate="halves")) needs a shard with halves: None creates one, and a given
+    buffer without halves is refused (ValueError) before any device work or collective.  The loop then gives
+    iterative_render's bits on one whole buffer with halves."""
     import torch
     import torch.distributed as dist
 
     _check_guided_world(adaptive, buffer.shard[1] if buffer is not None else _rank_world(group)[1])
+    halves = adaptive is not None and adaptive.estimate == "halves"
+    if halves and buffer is not None and not buffer.halves:
+        raise ValueError('estimate="halves" needs a shard buffer with halves: ShardBuffer(..., halves=True), or buffer=None')
     if buffer is None:
-        buffer = ShardBuffer(renderer.device_scene(), renderer._width, renderer._height, renderer._filter, group=group)
+        buffer = ShardBuffer(renderer.device_scene(), renderer._width, renderer._height, renderer._filter, group=group,
+                             halves=halves)
     if adaptive is not None and adaptive.guide is not None:
         if buffer.feature_rays == 0:
             renderer.sample_features(feature_samples, buffer)
@@ -491,7 +516,8 @@ def render_frames_distributed(renderer, cameras, entries: int = 8, feature_sampl
     gather with features before the first that runs the filter and a gather_delta after each.  The whole buffer they keep
     current is the frame's image and the next frame's source, so a frame still makes one full gather (at its end, as
     without guidance, when no entry ran the filter).  With one rank, a guided criterion is refused (ValueError), as in
-    render_iterative_distributed."""
+    render_iterative_distributed.  The error estimate (estimate="halves") is refused (ValueError), as render_frames
+    refuses it: reprojected history has no halves."""
     _check_guided_world(adaptive, _rank_world(group)[1])
     renderer._check_frames(entries, adaptive, denoise, reproject, history_test)
     with_features = reproject is not None or denoise is not None

@@ -96,7 +96,8 @@ HOSTEMU_DENOISE := tests/hostemu/_build/libhostemu_denoise.so
 HOSTEMU_SLIM := tests/hostemu/_build/libhostemu_slim.so
 # the denoiser's emulation plus the reprojection's per-pixel function (reproject.h; tests/hostemu/hostemu_reproject.cu) and
 # its per-element form for a shard's compact tiles (tests/hostemu/hostemu_reproject_part.cu), and the history test of
-# the merge, per pixel and per element (tests/hostemu/hostemu_reproject_merge.cu)
+# the merge, per pixel and per element (tests/hostemu/hostemu_reproject_merge.cu), and the history halves of both
+# (tests/hostemu/hostemu_reproject_halves.cu)
 HOSTEMU_REPROJECT := tests/hostemu/_build/libhostemu_reproject.so
 # the denoiser's emulation plus the guided adaptive criterion, per pixel and per slot of a part (guided.h;
 # tests/hostemu/hostemu_guided.cu)
@@ -120,9 +121,9 @@ $(HOSTEMU_DENOISE): tests/hostemu/hostemu_denoise.cu tests/hostemu/hostemu.cu $(
 $(HOSTEMU_SLIM): tests/hostemu/hostemu_slim.cu tests/hostemu/hostemu.cu $(CSRC)/kdbuild.cpp $(CSRC)/bvhbuild.cpp $(HDRS)
 	@mkdir -p $(dir $@)
 	nvcc -std=c++17 -O2 -DRPTB_HOST_EMU -DRPTB_BUILD_BVH8=1 -DRPTB_BUILD_BVH4=1 -gencode arch=compute_90a,code=sm_90a -Xcompiler -fPIC,-fopenmp,-ffp-contract=off -shared -Xlinker -Bsymbolic -o $@ tests/hostemu/hostemu_slim.cu $(CSRC)/kdbuild.cpp $(CSRC)/bvhbuild.cpp -lgomp
-$(HOSTEMU_REPROJECT): tests/hostemu/hostemu_reproject.cu tests/hostemu/hostemu_reproject_part.cu tests/hostemu/hostemu_reproject_merge.cu tests/hostemu/hostemu_denoise.cu tests/hostemu/hostemu.cu $(CSRC)/kdbuild.cpp $(CSRC)/bvhbuild.cpp $(HDRS)
+$(HOSTEMU_REPROJECT): tests/hostemu/hostemu_reproject.cu tests/hostemu/hostemu_reproject_part.cu tests/hostemu/hostemu_reproject_merge.cu tests/hostemu/hostemu_reproject_halves.cu tests/hostemu/hostemu_denoise.cu tests/hostemu/hostemu.cu $(CSRC)/kdbuild.cpp $(CSRC)/bvhbuild.cpp $(HDRS)
 	@mkdir -p $(dir $@)
-	nvcc -std=c++17 -O2 -DRPTB_HOST_EMU -DRPTB_BUILD_BVH8=1 -DRPTB_BUILD_BVH4=1 -gencode arch=compute_90a,code=sm_90a -Xcompiler -fPIC,-fopenmp,-ffp-contract=off -shared -Xlinker -Bsymbolic -o $@ tests/hostemu/hostemu_reproject.cu tests/hostemu/hostemu_reproject_part.cu tests/hostemu/hostemu_reproject_merge.cu $(CSRC)/kdbuild.cpp $(CSRC)/bvhbuild.cpp -lgomp
+	nvcc -std=c++17 -O2 -DRPTB_HOST_EMU -DRPTB_BUILD_BVH8=1 -DRPTB_BUILD_BVH4=1 -gencode arch=compute_90a,code=sm_90a -Xcompiler -fPIC,-fopenmp,-ffp-contract=off -shared -Xlinker -Bsymbolic -o $@ tests/hostemu/hostemu_reproject.cu tests/hostemu/hostemu_reproject_part.cu tests/hostemu/hostemu_reproject_merge.cu tests/hostemu/hostemu_reproject_halves.cu $(CSRC)/kdbuild.cpp $(CSRC)/bvhbuild.cpp -lgomp
 $(HOSTEMU_GUIDED): tests/hostemu/hostemu_guided.cu tests/hostemu/hostemu_denoise.cu tests/hostemu/hostemu.cu $(CSRC)/kdbuild.cpp $(CSRC)/bvhbuild.cpp $(HDRS)
 	@mkdir -p $(dir $@)
 	nvcc -std=c++17 -O2 -DRPTB_HOST_EMU -DRPTB_BUILD_BVH8=1 -DRPTB_BUILD_BVH4=1 -gencode arch=compute_90a,code=sm_90a -Xcompiler -fPIC,-fopenmp,-ffp-contract=off -shared -Xlinker -Bsymbolic -o $@ tests/hostemu/hostemu_guided.cu $(CSRC)/kdbuild.cpp $(CSRC)/bvhbuild.cpp -lgomp

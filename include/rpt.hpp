@@ -356,14 +356,16 @@ public:
         return out;
     }
     // Carries src's entries over a camera move into this buffer, which holds features and no entries
-    // (rptb_buffer_reproject).  Returns the number of pixels that got history.
+    // (rptb_buffer_reproject).  Returns the number of pixels that got history.  A buffer with halves needs a src with
+    // halves and takes the history's HALF too; a plain one ignores src's.
     uint64_t reproject_from(const DeviceBuffer& src, const rptb_reproject& params) {
         uint64_t n = 0;
         check(rptb_buffer_reproject(handle_, src.handle_, &params, &n));
         return n;
     }
     // Tests src's reprojected history against this buffer's own fresh entries (>= 2 calls through its feature camera)
-    // and merges it where they agree (rptb_buffer_reproject_merge).  Returns {reused, rejected} pixel counts.
+    // and merges it where they agree (rptb_buffer_reproject_merge).  Returns {reused, rejected} pixel counts.  Halves as
+    // for reproject_from.
     std::pair<uint64_t, uint64_t> merge_history_from(const DeviceBuffer& src, const rptb_reproject& params, double gamma) {
         uint64_t reused = 0, rejected = 0;
         check(rptb_buffer_reproject_merge(handle_, src.handle_, &params, gamma, &reused, &rejected));

@@ -539,8 +539,9 @@ int rptb_sample_into_guided(rptb_scene* scene, const rptb_camera* camera, const 
  * buffer, and the square of the result, remodulated, averaged over the channels and smoothed over 3x3, is E: an
  * estimate of each pixel's variance of the denoised value that accounts for the correlation between passes.
  * rpt_b200/csrc/halves.h gives every formula and its order of operations.
- * A buffer with halves is not a reprojection's or merge's dst (RPTB_ERR_UNSUPPORTED): history carries no halves.  It
- * may be a reprojection's src.  It imports the blocks of shards with halves (rptb_buffer_create_shard_halves), whose
+ * A buffer with halves may be a reprojection's or merge's src or dst.  A dst with halves needs a src with halves
+ * (RPTB_ERR_UNSUPPORTED from a plain src: its history has no halves), and then takes the history's HALF too (see
+ * rptb_buffer_reproject).  It imports the blocks of shards with halves (rptb_buffer_create_shard_halves), whose
  * exchange blocks carry HALF, and only those.
  * Arguments and refusals of create as rptb_buffer_create.                                                      */
 int rptb_buffer_create_halves(rptb_scene* scene, uint32_t width, uint32_t height, uint32_t box_radius, rptb_buffer** out);
@@ -580,7 +581,12 @@ int rptb_sample_into_guided_error(rptb_scene* scene, const rptb_camera* camera, 
  * buffers may differ in size.  The results are the same bits for any device count.  Afterwards dst's entries count
  * as rendered through its feature camera.  A reprojected buffer may hold pixels with 0 or 1 entries: its image()
  * fails ("Pixel found with no samples") while a pixel has none, denoise() while a pixel has fewer than 2, and its
- * variance() is NaN while a pixel has fewer than 2.                                                            */
+ * variance() is NaN while a pixel has fewer than 2.
+ *
+ * Halves (rptb_buffer_create_halves): a dst with halves takes history with halves from a src with halves -- each
+ * pixel's HALF scaled so that the error estimate (rptb_buffer_denoise_error) sees the variance of the mean that the
+ * capped count claims, not that of the taps' full counts -- and RPTB_ERR_UNSUPPORTED from a plain src.  A plain dst
+ * ignores a src's halves.  The sums, M2 and counts are the plain dst's bits.                                    */
 typedef struct rptb_reproject {
     double depth_tol;      /* relative depth tolerance, finite, >= 0                        */
     double normal_cos;     /* least N_p . N_q, in [-1, 1]                                  */
@@ -616,9 +622,10 @@ uint64_t rptb_buffer_shard_bytes(const rptb_buffer* buffer, uint32_t with_featur
  * count before the add) goes into HALF iff k is odd, so a shard's HALF is the whole buffer's for its tiles.  Its
  * exchange block appends HALF (3P doubles) after counts: 256 + 60 P bytes, 256 + 124 P with features, and its header's
  * flags say so.  Such blocks import into a whole buffer with halves only (RPTB_ERR_BAD_ARG into a plain one), and a
- * buffer with halves imports no plain blocks (RPTB_ERR_UNSUPPORTED).  It is not a reprojection's or merge's dst
- * (RPTB_ERR_UNSUPPORTED: history carries no halves), and its half_sums and denoise_error are refused like every other
- * whole-image read.  Arguments and refusals as rptb_buffer_create_shard.                                        */
+ * buffer with halves imports no plain blocks (RPTB_ERR_UNSUPPORTED).  It is a reprojection's or merge's dst
+ * (rptb_buffer_reproject_shard, rptb_buffer_reproject_merge_shard) from a whole src with halves (RPTB_ERR_UNSUPPORTED
+ * from a plain one), and afterwards its block's flags say reprojected and halves.  Its half_sums and denoise_error are
+ * refused like every other whole-image read.  Arguments and refusals as rptb_buffer_create_shard.                                        */
 int rptb_buffer_create_shard_halves(rptb_scene* scene, uint32_t width, uint32_t height, uint32_t box_radius, uint32_t shard_index,
                                     uint32_t shard_count, rptb_buffer** out);
 /* Writes the shard buffer's block (rptb_buffer_shard_bytes) to dst_device, on `stream` (a cudaStream_t, behind the
@@ -664,7 +671,9 @@ int rptb_buffer_reproject_shard(rptb_buffer* dst, rptb_buffer* src, const rptb_r
  * The checks and refusals are rptb_buffer_reproject's for src, the parameters and the device lists; for dst,
  * RPTB_ERR_BAD_ARG: fewer than 2 entry calls, already reprojected, or entries whose camera is not exactly its feature
  * camera (or mixed or unknown); gamma NaN or negative.  Afterwards dst is reprojected, its entry count is its fresh
- * calls plus max_history (a bound), and its entry camera is unchanged, so the next frame can reproject from it.  */
+ * calls plus max_history (a bound), and its entry camera is unchanged, so the next frame can reproject from it.  A dst
+ * with halves (from a src with halves) adds the accepted history's half that keeps "entry k goes into HALF iff k is
+ * odd" true: its B half when the pixel's fresh count is even, its A half when odd.                               */
 int rptb_buffer_reproject_merge(rptb_buffer* dst, rptb_buffer* src, const rptb_reproject* params, double gamma,
                                 uint64_t* out_reused /* nullable, forces sync: pixels whose history was merged */,
                                 uint64_t* out_rejected /* nullable, forces sync: pixels whose history was rejected */);

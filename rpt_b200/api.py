@@ -1094,7 +1094,12 @@ class DeviceBuffer:
         """Carries `src`'s entries over a camera move into this buffer, which must hold features (Renderer.sample_features
         through its camera) and no entries; `src` must hold entries and features made through one camera.  Each pixel
         takes the history of the old pixels that saw its first-hit point, or none (count 0: a disocclusion or the edge of
-        the old view, which an adaptive sample() renders first).  Returns the number of pixels that got history."""
+        the old view, which an adaptive sample() renders first).  Returns the number of pixels that got history.
+
+        A buffer with halves takes history with halves from a `src` with halves: each pixel's HALF is scaled so that
+        denoised_error and Adaptive(estimate="halves") see the variance of the mean its capped count claims
+        (rpt_b200/csrc/reproject.h).  From a plain `src` it raises RptbError (RPTB_ERR_UNSUPPORTED).  A plain buffer
+        ignores a `src`'s halves; the sums, M2 and counts are the same bits either way."""
         c = (params or Reproject()).to_c()
         n = C.c_uint64(0)
         capi.check(capi.lib().rptb_buffer_reproject(self.handle, src.handle, C.byref(c), C.byref(n)), "rptb_buffer_reproject")
@@ -1107,7 +1112,9 @@ class DeviceBuffer:
         only where they agree (rptb_buffer_reproject_merge).  This buffer must hold features and >= 2 entry calls, all
         through its feature camera, and must not be reprojected; `src` as for reproject_from.  A merged pixel holds both
         groups' entries, and the gap between their means goes into its variance; a rejected one keeps its fresh entries
-        only.  Returns (reused, rejected) pixel counts; pixels with no history are in neither."""
+        only.  Returns (reused, rejected) pixel counts; pixels with no history are in neither.  A buffer with halves needs
+        a `src` with halves, as for reproject_from, and a merged pixel's HALF takes the history's half that keeps "entry
+        k goes into HALF iff k is odd" true."""
         c = (reproject or Reproject()).to_c()
         gamma = (test or HistoryTest()).gamma
         n, j = C.c_uint64(0), C.c_uint64(0)
@@ -1349,7 +1356,8 @@ class Renderer:
         if denoise is not None and entries < 2 and adaptive is None:
             raise ValueError("a denoised frame needs entries >= 2 (or adaptive entries)")
         if adaptive is not None and adaptive.estimate == "halves":
-            raise ValueError('estimate="halves" is not supported in frame loops: reprojected history has no halves')
+            raise ValueError('estimate="halves" is not supported in frame loops: drive frames through reproject_from / '
+                             'merge_history_from on buffers with halves')
         if history_test is not None:
             if history_test.fresh_entries < 2 or history_test.fresh_entries > entries:
                 raise ValueError(f"history_test.fresh_entries {history_test.fresh_entries} must lie in [2, entries {entries}]")

@@ -89,6 +89,14 @@ cudaError_t launch_reproject_merge_part(const ReprojectView& dv, const Reproject
                                         const FeaturePlanes& f, double rays, uint32_t index, uint32_t count, uint64_t nelem,
                                         const rptb_reproject& prm, double gamma, double* sums, double* m2, uint32_t* counts,
                                         unsigned long long* tally, cudaStream_t stream);
+cudaError_t launch_reproject_halves_part(const ReprojectView& dv, const ReprojectView& sv, const ReprojectSource& s, const double* shalf,
+                                         const FeaturePlanes& f, double rays, uint32_t index, uint32_t count, uint64_t nelem,
+                                         const rptb_reproject& prm, double* sums, double* m2, uint32_t* counts, double* half,
+                                         unsigned long long* reused, cudaStream_t stream);
+cudaError_t launch_reproject_merge_halves_part(const ReprojectView& dv, const ReprojectView& sv, const ReprojectSource& s,
+                                               const double* shalf, const FeaturePlanes& f, double rays, uint32_t index, uint32_t count,
+                                               uint64_t nelem, const rptb_reproject& prm, double gamma, double* sums, double* m2,
+                                               uint32_t* counts, double* half, unsigned long long* tally, cudaStream_t stream);
 cudaError_t launch_buffer_min_count(const uint32_t* counts, uint64_t npix, uint32_t* out, cudaStream_t stream);
 int parse_obj_text(const char* text, size_t len, std::vector<double>& tris, std::string& err);
 struct ObjGroup {
@@ -2286,11 +2294,13 @@ static int check_reproject_params(const rptb_buffer* dst, const rptb_buffer* src
     return RPTB_OK;
 }
 
-// What a reprojection checks of the buffers (both locked): dst has no halves (history has none; a halves src is fine),
-// features and no entries (a merge's dst: see check_merge_dst instead), src has entries and features made through one
-// camera, and neither camera has an open aperture.
+// What a reprojection checks of the buffers (both locked): a dst with halves has a src with halves (a plain src's history
+// has none; a plain dst takes either src), dst has features and no entries (a merge's dst: see check_merge_dst instead),
+// src has entries and features made through one camera, and neither camera has an open aperture.
 static int check_reproject_buffers(const rptb_buffer* dst, const rptb_buffer* src, bool merge) {
-    if (dst->halves) return fail(RPTB_ERR_UNSUPPORTED, "dst has halves: reprojected history has no halves (a halves src is fine)");
+    if (dst->halves && !src->halves)
+        return fail(RPTB_ERR_UNSUPPORTED, "dst has halves but src has none: its history has no halves (reproject from a buffer with "
+                                          "halves, or into a plain one)");
     if (!merge && dst->entries) return fail(RPTB_ERR_BAD_ARG, "dst already holds entries");
     if (dst->feature_rays == 0) return fail(RPTB_ERR_BAD_ARG, "dst holds no features (rptb_buffer_add_features)");
     if (src->entries == 0) return fail(RPTB_ERR_BAD_ARG, "src holds no entries");
@@ -2324,11 +2334,11 @@ static int check_merge_dst(const rptb_buffer* dst, const rptb_reproject* prm) {
 }
 
 // src's state and resolved features, row-major on its parts[0]'s device (current), enqueued on that part's stream with
-// its `done` recorded behind them.
-static int reproject_source(rptb_buffer* src, ReprojectSource* out) {
+// its `done` recorded behind them.  halves: its HALF too, in src->rows.half.
+static int reproject_source(rptb_buffer* src, bool halves, ReprojectSource* out) {
     BufferPart& s0 = src->parts[0];
     const size_t snpix = (size_t)src->width * src->height;
-    const int rc = buffer_gather(src, COLOUR | FEATURES);
+    const int rc = buffer_gather(src, COLOUR | FEATURES | (halves ? 1u << HALF : 0u));
     if (rc != RPTB_OK) return rc;
     const Aov sa = buffer_aov(src);
     CU(launch_features_resolve(feature_planes(src->rows.feat, snpix), snpix, (double)src->feature_rays, sa, s0.stream));
@@ -2367,7 +2377,7 @@ static int reproject_finish(rptb_buffer* dst, const rptb_reproject* prm, bool me
 // rptb_buffer_reproject_merge_shard (*gamma the test's threshold); shard_entry: the _shard entry points, whose dst is a
 // shard buffer on src's first device.  Every dst part with tiles runs the per-element kernel over its own compact tiles
 // against src's gathered row-major state: part 0 in place, any other (on another device, no peer access assumed) through
-// the staging on parts[0]'s device.
+// the staging on parts[0]'s device.  A dst with halves (and so a src with halves) also carries the history's HALF.
 static int reproject_impl(rptb_buffer* dst, rptb_buffer* src, const rptb_reproject* prm, const double* gamma, uint64_t* out_reused,
                           uint64_t* out_rejected, bool shard_entry) {
     int rc = check_reproject_params(dst, src, prm);
@@ -2397,18 +2407,21 @@ static int reproject_impl(rptb_buffer* dst, rptb_buffer* src, const rptb_reproje
         if (out_rejected) *out_rejected = 0;
         return reproject_finish(dst, prm, gamma != nullptr, nullptr, nullptr, d0.stream);
     }
+    const bool halves = dst->halves;
+    const uint32_t half = halves ? 1u << HALF : 0u;
     size_t most = 0;  // the staging holds the largest other part
     for (size_t i = 1; i < dst->parts.size(); i++) most = std::max(most, (size_t)dst->parts[i].tiles * 128u);
-    if (most) rc = planes_alloc(dst->mem, dst->staging, most, COLOUR | FEATURES);
+    if (most) rc = planes_alloc(dst->mem, dst->staging, most, COLOUR | FEATURES | half);
     const bool count = out_reused || out_rejected;
     ReprojectSource sp;
-    if (rc == RPTB_OK) rc = reproject_source(src, &sp);
+    if (rc == RPTB_OK) rc = reproject_source(src, halves, &sp);
     if (rc != RPTB_OK) return rc;
     CU(cudaStreamWaitEvent(d0.stream, s0.done, 0));
     if (count) CU(cudaMemsetAsync(dst->reused, 0, (gamma ? 2 : 1) * sizeof(unsigned long long), d0.stream));
     const ReprojectView dv = reproject_view(dst->feat_cam.cam, dst->width, dst->height);
     const ReprojectView sv = reproject_view(src->feat_cam.cam, src->width, src->height);
-    const uint32_t in = gamma ? COLOUR | FEATURES : FEATURES;  // a merge reads the fresh colour; a reprojection writes it all
+    // a merge reads the fresh colour (and HALF); a reprojection writes it all
+    const uint32_t in = gamma ? COLOUR | FEATURES | half : FEATURES;
     for (size_t i = 0; rc == RPTB_OK && i < dst->parts.size(); i++) {
         const BufferPart& q = dst->parts[i];
         if (!q.tiles) continue;
@@ -2417,13 +2430,20 @@ static int reproject_impl(rptb_buffer* dst, rptb_buffer* src, const rptb_reproje
         if (i > 0) rc = copy_planes(p.set(in), d0.device, q.planes.set(in), q.device, q.planes.n, d0.stream);
         if (rc != RPTB_OK) return rc;
         const FeaturePlanes f = feature_planes(p.feat, p.n);
-        if (gamma)
-            CU(launch_reproject_merge_part(dv, sv, sp, f, (double)dst->feature_rays, q.index, q.count, q.planes.n, *prm, *gamma, p.sums,
-                                           p.m2, p.counts, count ? dst->reused : nullptr, d0.stream));
+        unsigned long long* tally = count ? dst->reused : nullptr;
+        const double rays = (double)dst->feature_rays;
+        if (gamma && halves)
+            CU(launch_reproject_merge_halves_part(dv, sv, sp, src->rows.half, f, rays, q.index, q.count, q.planes.n, *prm, *gamma, p.sums,
+                                                  p.m2, p.counts, p.half, tally, d0.stream));
+        else if (gamma)
+            CU(launch_reproject_merge_part(dv, sv, sp, f, rays, q.index, q.count, q.planes.n, *prm, *gamma, p.sums, p.m2, p.counts, tally,
+                                           d0.stream));
+        else if (halves)
+            CU(launch_reproject_halves_part(dv, sv, sp, src->rows.half, f, rays, q.index, q.count, q.planes.n, *prm, p.sums, p.m2,
+                                            p.counts, p.half, tally, d0.stream));
         else
-            CU(launch_reproject_part(dv, sv, sp, f, (double)dst->feature_rays, q.index, q.count, q.planes.n, *prm, p.sums, p.m2, p.counts,
-                                     count ? dst->reused : nullptr, d0.stream));
-        if (i > 0) rc = copy_planes(q.planes.set(COLOUR), q.device, p.set(COLOUR), d0.device, q.planes.n, d0.stream);
+            CU(launch_reproject_part(dv, sv, sp, f, rays, q.index, q.count, q.planes.n, *prm, p.sums, p.m2, p.counts, tally, d0.stream));
+        if (i > 0) rc = copy_planes(q.planes.set(COLOUR | half), q.device, p.set(COLOUR | half), d0.device, q.planes.n, d0.stream);
     }
     // every later call on either buffer is ordered behind this one
     if (rc == RPTB_OK) rc = buffer_order_behind(dst, d0.stream);

@@ -48,6 +48,23 @@
 // test reads the pixel's own fresh state only, no neighbourhood: a 3x3 window would cross tile borders into other shards,
 // and per pixel the shards' merges stay the whole buffer's bits with no exchange.  reproject_merge_slot is the per-element
 // form for a shard's compact tiles, as reproject_slot is reproject_pixel's.
+//
+// History halves (a dst with halves from a src with halves, rptb_buffer_create_halves).  Each src pixel q also keeps
+// H_q, the sums of its odd entries (halves.h).  Per valid tap q of a pixel with history, in tap order, with
+// n_Bq = floor(n_q / 2) and n_Aq = n_q - n_Bq:
+//     g_q = sqrt((n_Aq n_Bq) / n_q),   delta_qc = ((S_qc - H_qc) / n_Aq - H_qc / n_Bq) * g_q
+// the tap's half-mean difference in per-entry units (Var delta_q = sigma_q^2); then, in tap order,
+//     t_c = sum w^_q * delta_qc,   w2 = sum w^_q * w^_q,   d_c = t_c / sqrt(w2)
+// (for independent taps Var d is a weighted mean of the sigma_q^2), and with n_hB = floor(n_h / 2), n_hA = n_h - n_hB:
+//     H_hc = n_hB * mu_c - d_c * sqrt((n_hA n_hB) / n_h)
+// is the history's HALF.  halves_u of (mu n_h, H_h, n_h) is then u = d / sqrt(n_h) before the albedo, E[u^2] =
+// sigma^2 / n_h: the variance of the mean that the history claims through its capped count.  The taps' own half-means
+// would show the noise of up to n_q >> max_history entries, and the error estimate would call stale history converged.
+// A pixel with no history, and an element past a ragged edge, gets HALF 0.  The sums, M2 and count are reproject_pixel's.
+//
+// Merged (reproject_merge_halves): no test and a rejection leave HALF untouched; an accepted history adds H_hc to
+// HALF_c when n_f is even and (S_hc - H_hc), the history's A half, when n_f is odd.  So n_B = floor((n_f + n_h) / 2), as
+// halves_u assumes, and every later entry k still goes into HALF iff k is odd.
 #pragma once
 #include <cmath>
 
@@ -108,13 +125,17 @@ RPTB_HD void reproject_cross(const double* a, const double* b, double* o) {
 RPTB_HD bool reproject_finite(double x) { return x - x == 0.0; }
 
 // The history of destination pixel (x, y) of view dv from the source state s seen through view sv.  Np (3), zp, fp: the
-// pixel's resolved features.  Writes out_sums[3] and *out_m2, returns the count.
-RPTB_HD uint32_t reproject_pixel(const ReprojectView& dv, const ReprojectView& sv, const ReprojectSource& s, uint32_t x, uint32_t y,
-                                 const double* Np, double zp, double fp, const rptb_reproject& prm, double* out_sums, double* out_m2) {
+// pixel's resolved features.  Writes out_sums[3] and *out_m2, returns the count.  HALVES: also the history's HALF
+// out_half[3] from the source's row-major HALF shalf (3 per pixel).
+template <bool HALVES>
+RPTB_HD uint32_t reproject_history(const ReprojectView& dv, const ReprojectView& sv, const ReprojectSource& s, const double* shalf,
+                                   uint32_t x, uint32_t y, const double* Np, double zp, double fp, const rptb_reproject& prm,
+                                   double* out_sums, double* out_m2, double* out_half) {
     out_sums[0] = 0.0;
     out_sums[1] = 0.0;
     out_sums[2] = 0.0;
     *out_m2 = 0.0;
+    if constexpr (HALVES) out_half[0] = out_half[1] = out_half[2] = 0.0;
     const double xn = ((double)(2u * x + 1u) - (double)dv.width) / dv.dim;
     const double yn = ((double)(2u * (dv.height - y) - 1u) - (double)dv.height) / dv.dim;
     double r[3];
@@ -178,6 +199,7 @@ RPTB_HD uint32_t reproject_pixel(const ReprojectView& dv, const ReprojectView& s
     }
     if (!(W >= kReprojectMinWeight)) return 0u;
     double mu0 = 0.0, mu1 = 0.0, mu2 = 0.0, s2 = 0.0;
+    double t0 = 0.0, t1 = 0.0, t2 = 0.0, w2 = 0.0;  // HALVES: the weighted half-mean differences, the squared weights
     for (int t = 0; t < 4; t++) {
         if (q[t] < 0) continue;
         const int64_t i = q[t];
@@ -187,6 +209,16 @@ RPTB_HD uint32_t reproject_pixel(const ReprojectView& dv, const ReprojectView& s
         mu1 = mu1 + wh * (s.sums[3 * i + 1] / dn);
         mu2 = mu2 + wh * (s.sums[3 * i + 2] / dn);
         s2 = s2 + wh * (s.m2[i] / (double)(s.counts[i] - 1u));
+        if constexpr (HALVES) {
+            const uint32_t nb = s.counts[i] >> 1;
+            const double dB = (double)nb, dA = (double)(s.counts[i] - nb);
+            const double g = ::sqrt((dA * dB) / dn);
+            const double* hq = shalf + 3 * i;
+            t0 = t0 + wh * (((s.sums[3 * i] - hq[0]) / dA - hq[0] / dB) * g);
+            t1 = t1 + wh * (((s.sums[3 * i + 1] - hq[1]) / dA - hq[1] / dB) * g);
+            t2 = t2 + wh * (((s.sums[3 * i + 2] - hq[2]) / dA - hq[2] / dB) * g);
+            w2 = w2 + wh * wh;
+        }
     }
     const uint32_t nh = prm.max_history < nmin ? prm.max_history : nmin;
     const double dh = (double)nh;
@@ -194,27 +226,63 @@ RPTB_HD uint32_t reproject_pixel(const ReprojectView& dv, const ReprojectView& s
     out_sums[1] = mu1 * dh;
     out_sums[2] = mu2 * dh;
     *out_m2 = s2 * (double)(nh - 1u);
+    if constexpr (HALVES) {
+        const uint32_t nb = nh >> 1;
+        const double dB = (double)nb, dA = (double)(nh - nb);
+        const double sw = ::sqrt(w2), k = ::sqrt((dA * dB) / dh);
+        out_half[0] = dB * mu0 - (t0 / sw) * k;
+        out_half[1] = dB * mu1 - (t1 / sw) * k;
+        out_half[2] = dB * mu2 - (t2 / sw) * k;
+    }
     return nh;
+}
+
+RPTB_HD uint32_t reproject_pixel(const ReprojectView& dv, const ReprojectView& sv, const ReprojectSource& s, uint32_t x, uint32_t y,
+                                 const double* Np, double zp, double fp, const rptb_reproject& prm, double* out_sums, double* out_m2) {
+    return reproject_history<false>(dv, sv, s, nullptr, x, y, Np, zp, fp, prm, out_sums, out_m2, nullptr);
+}
+
+// reproject_pixel with the history's HALF out_half[3] from the source's row-major HALF shalf (see History halves above).
+RPTB_HD uint32_t reproject_pixel_halves(const ReprojectView& dv, const ReprojectView& sv, const ReprojectSource& s, const double* shalf,
+                                        uint32_t x, uint32_t y, const double* Np, double zp, double fp, const rptb_reproject& prm,
+                                        double* out_sums, double* out_m2, double* out_half) {
+    return reproject_history<true>(dv, sv, s, shalf, x, y, Np, zp, fp, prm, out_sums, out_m2, out_half);
 }
 
 // The history of element `slot` of the compact tiles of shard `index` of `count` of view dv: its pixel is
 // tile_pixel(dv.width, dv.height, index + (slot / 128) * count, slot % 128), and its features resolve from the element's
 // sums in f (the part's feature planes) over `rays` camera rays.  Writes out_sums[3] and *out_m2, returns the count; an
 // element past a ragged edge gets sums 0, M2 0 and count 0.
-RPTB_HD uint32_t reproject_slot(const ReprojectView& dv, const ReprojectView& sv, const ReprojectSource& s, const FeaturePlanes& f,
-                                double rays, uint32_t index, uint32_t count, uint64_t slot, const rptb_reproject& prm,
-                                double* out_sums, double* out_m2) {
+template <bool HALVES>
+RPTB_HD uint32_t reproject_slot_history(const ReprojectView& dv, const ReprojectView& sv, const ReprojectSource& s, const double* shalf,
+                                        const FeaturePlanes& f, double rays, uint32_t index, uint32_t count, uint64_t slot,
+                                        const rptb_reproject& prm, double* out_sums, double* out_m2, double* out_half) {
     const int64_t p = tile_pixel(dv.width, dv.height, index + (uint32_t)(slot >> 7) * count, (uint32_t)(slot & 127u));
     if (p < 0) {
         out_sums[0] = 0.0;
         out_sums[1] = 0.0;
         out_sums[2] = 0.0;
         *out_m2 = 0.0;
+        if constexpr (HALVES) out_half[0] = out_half[1] = out_half[2] = 0.0;
         return 0u;
     }
     double N[3], z, a[3], fp;
     features_resolve(f.h[slot], f.n + 3 * slot, f.z[slot], f.a + 3 * slot, rays, N, &z, a, &fp);
-    return reproject_pixel(dv, sv, s, (uint32_t)(p % dv.width), (uint32_t)(p / dv.width), N, z, fp, prm, out_sums, out_m2);
+    return reproject_history<HALVES>(dv, sv, s, shalf, (uint32_t)(p % dv.width), (uint32_t)(p / dv.width), N, z, fp, prm, out_sums,
+                                     out_m2, out_half);
+}
+
+RPTB_HD uint32_t reproject_slot(const ReprojectView& dv, const ReprojectView& sv, const ReprojectSource& s, const FeaturePlanes& f,
+                                double rays, uint32_t index, uint32_t count, uint64_t slot, const rptb_reproject& prm,
+                                double* out_sums, double* out_m2) {
+    return reproject_slot_history<false>(dv, sv, s, nullptr, f, rays, index, count, slot, prm, out_sums, out_m2, nullptr);
+}
+
+// reproject_slot with the history's HALF out_half[3] (0 past a ragged edge) from the source's row-major HALF shalf.
+RPTB_HD uint32_t reproject_slot_halves(const ReprojectView& dv, const ReprojectView& sv, const ReprojectSource& s, const double* shalf,
+                                       const FeaturePlanes& f, double rays, uint32_t index, uint32_t count, uint64_t slot,
+                                       const rptb_reproject& prm, double* out_sums, double* out_m2, double* out_half) {
+    return reproject_slot_history<true>(dv, sv, s, shalf, f, rays, index, count, slot, prm, out_sums, out_m2, out_half);
 }
 
 // Merges the history sh[3], m2h, nh into the fresh state sums[3], *m2, *count in place when the test above accepts it.
@@ -246,6 +314,28 @@ RPTB_HD int reproject_merge_slot(const ReprojectView& dv, const ReprojectView& s
     double sh[3], m2h;
     const uint32_t nh = reproject_slot(dv, sv, s, f, rays, index, count, slot, prm, sh, &m2h);
     return reproject_merge(sh, m2h, nh, gamma, sums, m2, n);
+}
+
+// reproject_merge with the history's HALF hh[3] and the fresh HALF half[3]: an accepted history adds its B half (n_f
+// even) or its A half (n_f odd) to half.  Same verdict, sums, M2 and count.
+RPTB_HD int reproject_merge_halves(const double* sh, double m2h, uint32_t nh, const double* hh, double gamma, double* sums, double* m2,
+                                   uint32_t* count, double* half) {
+    const uint32_t nf = *count;
+    const int verdict = reproject_merge(sh, m2h, nh, gamma, sums, m2, count);
+    if (verdict == 1) {
+        const bool odd = (nf & 1u) != 0u;
+        for (int k = 0; k < 3; k++) half[k] = half[k] + (odd ? sh[k] - hh[k] : hh[k]);
+    }
+    return verdict;
+}
+
+// reproject_merge_slot with the source's row-major HALF shalf and the element's fresh HALF half[3].
+RPTB_HD int reproject_merge_slot_halves(const ReprojectView& dv, const ReprojectView& sv, const ReprojectSource& s, const double* shalf,
+                                        const FeaturePlanes& f, double rays, uint32_t index, uint32_t count, uint64_t slot,
+                                        const rptb_reproject& prm, double gamma, double* sums, double* m2, uint32_t* n, double* half) {
+    double sh[3], m2h, hh[3];
+    const uint32_t nh = reproject_slot_halves(dv, sv, s, shalf, f, rays, index, count, slot, prm, sh, &m2h, hh);
+    return reproject_merge_halves(sh, m2h, nh, hh, gamma, sums, m2, n, half);
 }
 
 }  // namespace rptb

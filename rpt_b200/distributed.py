@@ -249,7 +249,8 @@ class ShardBuffer(api.DeviceBuffer):
     counts, features, denoise, add_samples) are refused: gather() first.  `entries` counts the calls (a bound on any
     pixel's count) until the gather reads the counts.  `halves` (rptb_buffer_create_shard_halves): the shard also keeps
     the sums of each pixel's odd entries, its blocks carry them, and gather() gives a whole buffer with halves -- what
-    Adaptive(estimate="halves") needs; a frame's reproject_from and merge_history_from refuse it."""
+    Adaptive(estimate="halves") needs.  Its reproject_from and merge_history_from take history with halves from a whole
+    src with halves (RptbError from a plain one)."""
 
     def __init__(self, scene: "api.DeviceScene", width: int, height: int, filter: Optional["api.Filter"] = None, group=None,
                  rank: Optional[int] = None, world: Optional[int] = None, halves: bool = False):
@@ -286,8 +287,9 @@ class ShardBuffer(api.DeviceBuffer):
     def reproject_from(self, src: "api.DeviceBuffer", params: Optional["api.Reproject"] = None) -> int:
         """DeviceBuffer.reproject_from into this shard (rptb_buffer_reproject_shard): this rank's pixels take their history
         from `src`, a whole DeviceBuffer on this rank's device -- typically the previous frame's shards gathered with
-        features, prev.gather(with_features=True).  Every pixel gets the bits a whole buffer's reprojection gives it.
-        Returns this rank's reused pixels; summed over the ranks, they are the whole call's."""
+        features, prev.gather(with_features=True).  Every pixel gets the bits a whole buffer's reprojection gives it,
+        HALF included for a shard with halves (whose `src` must have halves too).  Returns this rank's reused pixels;
+        summed over the ranks, they are the whole call's."""
         if isinstance(src, ShardBuffer):
             raise TypeError("src is a ShardBuffer: gather() the shards into a whole buffer first")
         c = (params or api.Reproject()).to_c()
@@ -301,8 +303,9 @@ class ShardBuffer(api.DeviceBuffer):
                            test: Optional["api.HistoryTest"] = None) -> tuple:
         """DeviceBuffer.merge_history_from into this shard (rptb_buffer_reproject_merge_shard): this rank's pixels test
         the history of `src`, a whole DeviceBuffer on this rank's device (the previous frame gathered with features),
-        against their own fresh entries.  Every pixel gets the bits a whole buffer's merge gives it.  Returns this rank's
-        (reused, rejected) pixels; summed over the ranks, they are the whole call's."""
+        against their own fresh entries.  Every pixel gets the bits a whole buffer's merge gives it, HALF included for a
+        shard with halves (whose `src` must have halves too).  Returns this rank's (reused, rejected) pixels; summed over
+        the ranks, they are the whole call's."""
         if isinstance(src, ShardBuffer):
             raise TypeError("src is a ShardBuffer: gather() the shards into a whole buffer first")
         c = (reproject or api.Reproject()).to_c()
@@ -517,7 +520,7 @@ def render_frames_distributed(renderer, cameras, entries: int = 8, feature_sampl
     current is the frame's image and the next frame's source, so a frame still makes one full gather (at its end, as
     without guidance, when no entry ran the filter).  With one rank, a guided criterion is refused (ValueError), as in
     render_iterative_distributed.  The error estimate (estimate="halves") is refused (ValueError), as render_frames
-    refuses it: reprojected history has no halves."""
+    refuses it: the loop makes no shards with halves yet (ShardBuffer.reproject_from and merge_history_from take them)."""
     _check_guided_world(adaptive, _rank_world(group)[1])
     renderer._check_frames(entries, adaptive, denoise, reproject, history_test)
     with_features = reproject is not None or denoise is not None

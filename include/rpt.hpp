@@ -355,6 +355,20 @@ public:
         check(rptb_buffer_denoise_error(handle_, &d, out.data()));
         return out;
     }
+    // A buffer with halves: denoise(d) with each pixel's pass count (0 .. d.iterations) chosen by the least estimated
+    // error (rptb_buffer_denoise_select).  rgb: 3 doubles per pixel, each that level's denoise output bit for bit;
+    // level: the chosen pass count; mse: the estimated squared error at it.  Row-major; d.iterations >= 1.
+    struct Selection {
+        std::vector<double> rgb;
+        std::vector<uint8_t> level;
+        std::vector<double> mse;
+    };
+    Selection denoise_select(const rptb_denoise& d) const {
+        const size_t n = (size_t)width_ * height_;
+        Selection s{std::vector<double>(n * 3), std::vector<uint8_t>(n), std::vector<double>(n)};
+        check(rptb_buffer_denoise_select(handle_, &d, s.rgb.data(), nullptr, s.level.data(), s.mse.data()));
+        return s;
+    }
     // Carries src's entries over a camera move into this buffer, which holds features and no entries
     // (rptb_buffer_reproject).  Returns the number of pixels that got history.  A buffer with halves needs a src with
     // halves and takes the history's HALF too; a plain one ignores src's.

@@ -561,6 +561,17 @@ int rptb_buffer_denoise_error(rptb_buffer* buffer, const rptb_denoise* params, d
 int rptb_sample_into_guided_error(rptb_scene* scene, const rptb_camera* camera, const rptb_render_params* params,
                                   const rptb_adaptive* criterion, const rptb_denoise* guide, rptb_buffer* buffer,
                                   uint64_t* out_active /* nullable, forces sync */, rptb_stats* stats /* nullable, forces sync */);
+/* rptb_buffer_denoise with each pixel's number of passes chosen from a half-buffer estimate of each level's error.
+ * Level k (0 .. params->iterations) is rptb_buffer_denoise's output with iterations = k.  Per pixel, m_k estimates
+ * the squared error of level k (bias included) from the two halves, M_k smooths it over 5x5, and the level with the
+ * least M_k is kept (level 0 unless a deeper one is strictly less); select.h gives every formula.  So every output pixel
+ * is rptb_buffer_denoise(iterations = level) at that pixel, bit for bit.  out_rgb: width*height*3 doubles;
+ * out_rgb8: its bytes as rptb_buffer_denoise writes them; out_level: width*height chosen levels; out_mse:
+ * width*height M at the chosen level, in the units of v' (NaN where no finite tap was left).  Refusals as
+ * rptb_buffer_denoise_error.  Allocates 9 doubles and 1 byte a pixel on first use (151 MB at 1920x1080), beside the
+ * error estimate's.                                                                                          */
+int rptb_buffer_denoise_select(rptb_buffer* buffer, const rptb_denoise* params, double* out_rgb /* nullable */,
+                               uint8_t* out_rgb8 /* nullable */, uint8_t* out_level /* nullable */, double* out_mse /* nullable */);
 
 /* ---- Reprojecting the device Buffer across a camera move ---------------------------------------------------
  * The temporal half of SVGF for a static scene: each pixel of `dst`'s view finds, through its own first-hit depth,

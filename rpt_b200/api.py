@@ -27,7 +27,7 @@ from __future__ import annotations
 
 import ctypes as C
 import math
-from typing import Callable, List, Optional, Sequence
+from typing import Callable, List, Optional, Sequence, Tuple
 
 import numpy as np
 
@@ -1090,6 +1090,29 @@ class DeviceBuffer:
                    "rptb_buffer_denoise")
         return out
 
+    def denoise_select(self, d: Optional[Denoise] = None) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+        """denoise(d) with each pixel's number of passes chosen by the estimated error of each level
+        (rptb_buffer_denoise_select): level k is denoise(Denoise(iterations=k, ...)), and each pixel keeps the level
+        whose error, estimated from the two half buffers and smoothed over 5x5, is least (DESIGN.md section 6h).
+        Returns (rgb (H, W, 3) float64, level (H, W) uint8, mse (H, W) float64): every rgb pixel is that level's denoise
+        output bit for bit, and mse is the estimated squared error (bias included) at the chosen level, in the units of
+        denoised_variance().  Needs a buffer with halves and d.iterations >= 1; otherwise refusals as denoise()."""
+        h, w = self.height, self.width
+        rgb, level, mse = np.empty((h, w, 3)), np.empty((h, w), np.uint8), np.empty((h, w))
+        c = (d or Denoise()).to_c()
+        capi.check(capi.lib().rptb_buffer_denoise_select(self.handle, C.byref(c), rgb.ctypes.data_as(capi.c_double_p), None,
+                                                         level.ctypes.data_as(capi.c_u8_p), mse.ctypes.data_as(capi.c_double_p)),
+                   "rptb_buffer_denoise_select")
+        return rgb, level, mse
+
+    def selected_image(self, d: Optional[Denoise] = None) -> np.ndarray:
+        """denoise_select()'s colour through Buffer::image's clamp, gamma and cast, as denoised_image(): (H, W, 3) uint8."""
+        out = np.empty((self.height, self.width, 3), np.uint8)
+        c = (d or Denoise()).to_c()
+        capi.check(capi.lib().rptb_buffer_denoise_select(self.handle, C.byref(c), None, out.ctypes.data_as(capi.c_u8_p), None, None),
+                   "rptb_buffer_denoise_select")
+        return out
+
     def reproject_from(self, src: "DeviceBuffer", params: Optional[Reproject] = None) -> int:
         """Carries `src`'s entries over a camera move into this buffer, which must hold features (Renderer.sample_features
         through its camera) and no entries; `src` must hold entries and features made through one camera.  Each pixel
@@ -1332,9 +1355,14 @@ class Renderer:
         buffer.feature_rays += int(iterations)
         self.last_stats = stats.as_dict() if want_stats else None
 
-    def render(self, denoise: Optional[Denoise] = None, entries: int = 8, feature_samples: int = 16) -> np.ndarray:  # :96-100
+    def render(self, denoise: Optional[Denoise] = None, entries: int = 8, feature_samples: int = 16,
+               select: bool = False) -> np.ndarray:  # :96-100
         """Renderer::render.  With `denoise`, num_samples are rendered as `entries` equal entries of a DeviceBuffer,
-        `feature_samples` camera rays per pixel give it features, and the denoised bytes are returned."""
+        `feature_samples` camera rays per pixel give it features, and the denoised bytes are returned.  With `select`
+        as well, the buffer keeps halves and each pixel takes the number of passes (0 .. denoise.iterations) whose
+        estimated error is least (DeviceBuffer.selected_image)."""
+        if select and denoise is None:
+            raise ValueError("select=True chooses each pixel's number of filter passes: it needs denoise (a Denoise)")
         if denoise is None:
             buffer = Buffer(self._width, self._height, self._filter, self._first_device())
             self.sample(self._num_samples, buffer)
@@ -1342,11 +1370,11 @@ class Renderer:
         if entries < 2 or self._num_samples % entries:
             # the entries are weighted equally: unequal ones would bias the mean
             raise ValueError(f"num_samples {self._num_samples} must be a multiple of entries {entries} (and entries >= 2)")
-        with self.device_buffer() as buf:
+        with self.device_buffer(halves=select) as buf:
             for _ in range(entries):
                 self.sample(self._num_samples // entries, buf, want_stats=False)
             self.sample_features(feature_samples, buf)
-            return buf.denoised_image(denoise)
+            return buf.selected_image(denoise) if select else buf.denoised_image(denoise)
 
     def _check_frames(self, entries: int, adaptive: Optional[Adaptive], denoise: Optional[Denoise],
                       reproject: Optional[Reproject] = None, history_test: Optional[HistoryTest] = None) -> None:

@@ -81,6 +81,11 @@ cudaError_t launch_halves_error(const double* sums, const double* m2, const doub
                                 const double* depth, const double* albedo, uint32_t width, uint32_t height, const rptb_denoise& d,
                                 double* const col[2], double* const var[2], double* const u[2], double* E, const double** out_col,
                                 cudaStream_t stream, uint32_t* launches);
+// the per-pixel choice of the filter's pass count: select.cu
+cudaError_t launch_denoise_select(const double* sums, const double* m2, const double* half, const uint32_t* counts, const double* nrm,
+                                  const double* depth, const double* albedo, uint32_t width, uint32_t height, const rptb_denoise& d,
+                                  double* const col[3], double* const var[3], double* const u[3], double* m, double* best, double* best_M,
+                                  uint8_t* level, cudaStream_t stream, uint32_t* launches);
 // the reprojection and the least count: reproject.cu
 cudaError_t launch_reproject_part(const ReprojectView& dv, const ReprojectView& sv, const ReprojectSource& s, const FeaturePlanes& f,
                                   double rays, uint32_t index, uint32_t count, uint64_t nelem, const rptb_reproject& prm, double* sums,
@@ -705,6 +710,10 @@ struct rptb_buffer {
     double* aov = nullptr;           // with the feature rows, width*height*8: the resolved features (buffer_aov)
     double* dn = nullptr;            // the denoiser's, width*height*11: colour (3) and variance ping-pong planes, then c' (3)
     double* hv = nullptr;            // the error estimate's (halves.cu), width*height*7: u (3) ping-pong planes, then E
+    // the selection's (select.cu), width*height*9: a third colour (3), variance and u (3) set for the passes, then m and M;
+    // and the chosen level, width*height bytes
+    double* sl = nullptr;
+    uint8_t* sl_level = nullptr;
     // allocated by the first guided adaptive call on a buffer of several parts: the mask and flags of parts[1..] (as many
     // tiles as the largest holds, *132 bytes) marked here before they go to the part, and their active pixel count
     uint8_t* guide_mask = nullptr;
@@ -2281,6 +2290,47 @@ int rptb_buffer_denoise_error(rptb_buffer* b, const rptb_denoise* d, double* out
     if (b->shard) return refuse_shard("denoise_error");
     if (!b->halves) return fail(RPTB_ERR_BAD_ARG, "the buffer has no halves (rptb_buffer_create_halves)");
     return denoise_read(b, *d, true, out);
+}
+
+int rptb_buffer_denoise_select(rptb_buffer* b, const rptb_denoise* d, double* out_rgb, uint8_t* out_rgb8, uint8_t* out_level,
+                               double* out_mse) {
+    if (!b) return fail(RPTB_ERR_BAD_ARG, "null argument");
+    int rc = check_denoise(d);
+    if (rc != RPTB_OK) return rc;
+    if (d->iterations == 0) return fail(RPTB_ERR_BAD_ARG, "iterations 0: the selection needs at least one filter pass to choose");
+    if (b->shard) return refuse_shard("denoise_select");
+    if (!b->halves) return fail(RPTB_ERR_BAD_ARG, "the buffer has no halves (rptb_buffer_create_halves)");
+    std::lock_guard<std::mutex> bl(b->lock);
+    BufferPart& q0 = b->parts[0];
+    DeviceGuard g(q0.device);
+    FilterPlanes f;
+    rc = check_denoise_entries(b);
+    if (rc == RPTB_OK) rc = filter_planes(b, true, &f);
+    if (rc == RPTB_OK) rc = check_denoise_counts(b);
+    if (rc != RPTB_OK) return rc;
+    const size_t npix = (size_t)b->width * b->height;
+    if (!b->sl) CU(own(b->mem, &b->sl, npix * 9 * sizeof(double)));
+    if (!b->sl_level) CU(own(b->mem, &b->sl_level, npix));
+    // level 0 in the filter's first colour and variance planes and the estimate's first u plane; the passes alternate
+    // between the filter's second set and the selection's own; the chosen colour goes to c' (f.out)
+    double* const col[3] = {f.col[0], f.col[1], b->sl};
+    double* const var[3] = {f.var[0], f.var[1], b->sl + 3 * npix};
+    double* const u[3] = {f.u[0], f.u[1], b->sl + 4 * npix};
+    double* const m = b->sl + 7 * npix;
+    double* const best_M = b->sl + 8 * npix;
+    uint32_t launches = 0;
+    CU(launch_denoise_select(b->rows.sums, b->rows.m2, b->rows.half, b->rows.counts, f.a.normal, f.a.depth, f.a.albedo, b->width, b->height,
+                             *d, col, var, u, m, f.out, best_M, b->sl_level, q0.stream, &launches));
+    if (out_rgb) CU(cudaMemcpyAsync(out_rgb, f.out, npix * 3 * sizeof(double), cudaMemcpyDeviceToHost, q0.stream));
+    if (out_rgb8) {
+        // as rptb_buffer_denoise: the film resolve of one entry at radius 0
+        CU(launch_film_resolve(f.out, 1u, b->width, b->height, 0u, b->rgb8, q0.stream));
+        CU(cudaMemcpyAsync(out_rgb8, b->rgb8, npix * 3, cudaMemcpyDeviceToHost, q0.stream));
+    }
+    if (out_level) CU(cudaMemcpyAsync(out_level, b->sl_level, npix, cudaMemcpyDeviceToHost, q0.stream));
+    if (out_mse) CU(cudaMemcpyAsync(out_mse, best_M, npix * sizeof(double), cudaMemcpyDeviceToHost, q0.stream));
+    CU(cudaStreamSynchronize(q0.stream));
+    return RPTB_OK;
 }
 
 // What a reprojection checks before it looks at the buffers: its arguments and parameters.

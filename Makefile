@@ -54,6 +54,11 @@ $(OBJDIR)/halves.o: $(CSRC)/halves.cu $(HDRS)
 $(OBJDIR)/select.o: $(CSRC)/select.cu $(HDRS)
 	@mkdir -p $(OBJDIR)
 	$(NVCC) $(NVFLAGS) -fmad=false -c $< -o $@ 2> $(OBJDIR)/select.ptxas.log || (cat $(OBJDIR)/select.ptxas.log; false)
+# the cross-filtered denoiser with a smoothed selection map (cross.h) likewise: its numpy restatement and host emulation
+# round every operation on its own
+$(OBJDIR)/cross.o: $(CSRC)/cross.cu $(HDRS)
+	@mkdir -p $(OBJDIR)
+	$(NVCC) $(NVFLAGS) -fmad=false -c $< -o $@ 2> $(OBJDIR)/cross.ptxas.log || (cat $(OBJDIR)/cross.ptxas.log; false)
 # the delta exchange (delta.h) only moves doubles; compiled like its neighbours all the same
 $(OBJDIR)/delta.o: $(CSRC)/delta.cu $(HDRS)
 	@mkdir -p $(OBJDIR)
@@ -74,7 +79,7 @@ $(OBJDIR)/objparse.o: $(CSRC)/objparse.cpp
 	@mkdir -p $(OBJDIR)
 	$(CXX) -std=c++17 -O3 -fPIC -Wall -c $< -o $@
 
-$(LIB): $(OBJDIR)/kernels_f32.o $(OBJDIR)/kernels_vx.o $(OBJDIR)/kernels_f64.o $(OBJDIR)/film.o $(OBJDIR)/adaptive.o $(OBJDIR)/denoise.o $(OBJDIR)/guided.o $(OBJDIR)/halves.o $(OBJDIR)/select.o $(OBJDIR)/delta.o $(OBJDIR)/reproject.o $(OBJDIR)/api.o $(OBJDIR)/kdbuild.o $(OBJDIR)/bvhbuild.o $(OBJDIR)/objparse.o
+$(LIB): $(OBJDIR)/kernels_f32.o $(OBJDIR)/kernels_vx.o $(OBJDIR)/kernels_f64.o $(OBJDIR)/film.o $(OBJDIR)/adaptive.o $(OBJDIR)/denoise.o $(OBJDIR)/guided.o $(OBJDIR)/halves.o $(OBJDIR)/select.o $(OBJDIR)/cross.o $(OBJDIR)/delta.o $(OBJDIR)/reproject.o $(OBJDIR)/api.o $(OBJDIR)/kdbuild.o $(OBJDIR)/bvhbuild.o $(OBJDIR)/objparse.o
 	@mkdir -p rpt_b200/lib
 	$(NVCC) -shared $(ARCH) -o $@ $^ -Xcompiler -fopenmp -lgomp -cudart shared
 
@@ -115,7 +120,9 @@ HOSTEMU_DELTA_HALVES := tests/hostemu/_build/libhostemu_delta_halves.so
 HOSTEMU_HALVES := tests/hostemu/_build/libhostemu_halves.so
 # the choice of the filter's pass count per pixel (select.h; tests/hostemu/hostemu_select.cu)
 HOSTEMU_SELECT := tests/hostemu/_build/libhostemu_select.so
-hostemu: $(HOSTEMU) $(HOSTEMU_LIST) $(HOSTEMU_DENOISE) $(HOSTEMU_SLIM) $(HOSTEMU_REPROJECT) $(HOSTEMU_GUIDED) $(HOSTEMU_DELTA) $(HOSTEMU_DELTA_HALVES) $(HOSTEMU_HALVES) $(HOSTEMU_SELECT)
+# the cross-filtered denoiser's per-pixel functions (cross.h; tests/hostemu/hostemu_cross.cu)
+HOSTEMU_CROSS := tests/hostemu/_build/libhostemu_cross.so
+hostemu: $(HOSTEMU) $(HOSTEMU_LIST) $(HOSTEMU_DENOISE) $(HOSTEMU_SLIM) $(HOSTEMU_REPROJECT) $(HOSTEMU_GUIDED) $(HOSTEMU_DELTA) $(HOSTEMU_DELTA_HALVES) $(HOSTEMU_HALVES) $(HOSTEMU_SELECT) $(HOSTEMU_CROSS)
 $(HOSTEMU): tests/hostemu/hostemu.cu $(CSRC)/kdbuild.cpp $(CSRC)/bvhbuild.cpp $(HDRS)
 	@mkdir -p $(dir $@)
 	nvcc -std=c++17 -O2 -DRPTB_HOST_EMU -DRPTB_BUILD_BVH8=1 -DRPTB_BUILD_BVH4=1 -gencode arch=compute_90a,code=sm_90a -Xcompiler -fPIC,-fopenmp,-ffp-contract=off -shared -Xlinker -Bsymbolic -o $@ tests/hostemu/hostemu.cu $(CSRC)/kdbuild.cpp $(CSRC)/bvhbuild.cpp -lgomp
@@ -146,6 +153,9 @@ $(HOSTEMU_HALVES): tests/hostemu/hostemu_halves.cu $(HDRS)
 $(HOSTEMU_SELECT): tests/hostemu/hostemu_select.cu $(HDRS)
 	@mkdir -p $(dir $@)
 	nvcc -std=c++17 -O2 -DRPTB_HOST_EMU -gencode arch=compute_90a,code=sm_90a -Xcompiler -fPIC,-fopenmp,-ffp-contract=off -shared -Xlinker -Bsymbolic -o $@ tests/hostemu/hostemu_select.cu -lgomp
+$(HOSTEMU_CROSS): tests/hostemu/hostemu_cross.cu $(HDRS)
+	@mkdir -p $(dir $@)
+	nvcc -std=c++17 -O2 -DRPTB_HOST_EMU -gencode arch=compute_90a,code=sm_90a -Xcompiler -fPIC,-fopenmp,-ffp-contract=off -shared -Xlinker -Bsymbolic -o $@ tests/hostemu/hostemu_cross.cu -lgomp
 
 clean:
 	rm -rf build $(LIB) $(ORACLE) tests/hostemu/_build

@@ -369,6 +369,16 @@ public:
         check(rptb_buffer_denoise_select(handle_, &d, s.rgb.data(), nullptr, s.level.data(), s.mse.data()));
         return s;
     }
+    // A buffer with halves, cross-filtered with a smoothed selection map (rptb_buffer_denoise_cross): each half filtered
+    // through weights from the other half's own passes, and the levels 0 .. d.iterations blended per pixel by the share
+    // of its 5x5 neighbours whose estimated error is least at each.  rgb: the blended colour; level: the pixel's own
+    // least-error level; mse: the estimated squared error blended with the colour's weights.  Row-major; d.iterations >= 1.
+    Selection denoise_cross(const rptb_denoise& d) const {
+        const size_t n = (size_t)width_ * height_;
+        Selection s{std::vector<double>(n * 3), std::vector<uint8_t>(n), std::vector<double>(n)};
+        check(rptb_buffer_denoise_cross(handle_, &d, s.rgb.data(), nullptr, s.level.data(), s.mse.data()));
+        return s;
+    }
     // Carries src's entries over a camera move into this buffer, which holds features and no entries
     // (rptb_buffer_reproject).  Returns the number of pixels that got history.  A buffer with halves needs a src with
     // halves and takes the history's HALF too; a plain one ignores src's.

@@ -572,6 +572,20 @@ int rptb_sample_into_guided_error(rptb_scene* scene, const rptb_camera* camera, 
  * error estimate's.                                                                                          */
 int rptb_buffer_denoise_select(rptb_buffer* buffer, const rptb_denoise* params, double* out_rgb /* nullable */,
                                uint8_t* out_rgb8 /* nullable */, uint8_t* out_level /* nullable */, double* out_mse /* nullable */);
+/* A buffer with halves, denoised by cross-filtering with a smoothed selection map.  Each half is filtered through
+ * params->iterations passes whose weights come from the other half's own chain of passes (not from its own entries),
+ * giving level k = 0 .. iterations: level 0 is S / n, level k the count-weighted mean of the two cross-filtered halves,
+ * remodulated.  Per pixel, m_k estimates the squared error of level k (bias included) from the halves, M_k smooths it
+ * over 5x5, k* is the level with the least M_k (level 0 unless a deeper one is strictly less), and the output blends
+ * the levels by the 5x5-smoothed share of each level among its neighbours' k*; a pixel whose 5x5 neighbourhood chose one
+ * level gets that level bit for bit.  cross.h gives every formula.  out_rgb: width*height*3 doubles; out_rgb8: its bytes
+ * as rptb_buffer_denoise writes them; out_level: width*height k*; out_mse: width*height M^, the blend of M_k with the
+ * colour's weights, in the units of v' (NaN where a blended level had no finite tap).  Refusals as
+ * rptb_buffer_denoise_select: RPTB_ERR_BAD_ARG for a buffer without halves or features, iterations == 0, or a pixel with
+ * fewer than 2 entries; RPTB_ERR_UNSUPPORTED for a shard (gather it first).  Allocates 23 doubles and 1 byte a pixel on
+ * first use (384 MB at 1920x1080), beside the error estimate's.                                                  */
+int rptb_buffer_denoise_cross(rptb_buffer* buffer, const rptb_denoise* params, double* out_rgb /* nullable */,
+                              uint8_t* out_rgb8 /* nullable */, uint8_t* out_level /* nullable */, double* out_mse /* nullable */);
 
 /* ---- Reprojecting the device Buffer across a camera move ---------------------------------------------------
  * The temporal half of SVGF for a static scene: each pixel of `dst`'s view finds, through its own first-hit depth,

@@ -304,6 +304,7 @@ SYMBOLS = [
     ("rptb_buffer_half_sums", C.c_int, [C.c_void_p, c_double_p]),
     ("rptb_buffer_denoise_error", C.c_int, [C.c_void_p, C.POINTER(Denoise), c_double_p]),
     ("rptb_buffer_denoise_select", C.c_int, [C.c_void_p, C.POINTER(Denoise), c_double_p, c_u8_p, c_u8_p, c_double_p]),
+    ("rptb_buffer_denoise_cross", C.c_int, [C.c_void_p, C.POINTER(Denoise), c_double_p, c_u8_p, c_u8_p, c_double_p]),
     ("rptb_sample_into_guided_error", C.c_int,
      [C.c_void_p, C.POINTER(Camera), C.POINTER(RenderParams), C.POINTER(Adaptive), C.POINTER(Denoise), C.c_void_p,
       C.POINTER(C.c_uint64), C.POINTER(Stats)]),

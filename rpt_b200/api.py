@@ -1113,6 +1113,31 @@ class DeviceBuffer:
                    "rptb_buffer_denoise_select")
         return out
 
+    def denoise_cross(self, d: Optional[Denoise] = None) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+        """The buffer denoised by cross-filtering with a smoothed selection map (rptb_buffer_denoise_cross): each half is
+        filtered through d.iterations passes whose weights come from the other half's own passes, level k (0 ..
+        d.iterations) is the count-weighted mean of the two filtered halves (level 0 the raw mean), and each pixel blends
+        the levels by the 5x5-smoothed share of its neighbours whose estimated error is least at each level (DESIGN.md
+        section 6i).  Returns (rgb (H, W, 3) float64, level (H, W) uint8, mse (H, W) float64): the blended colour, each
+        pixel's own least-error level, and the estimated squared error (bias included) blended with the colour's weights,
+        in the units of denoised_variance().  Needs a buffer with halves and d.iterations >= 1; otherwise refusals as
+        denoise()."""
+        h, w = self.height, self.width
+        rgb, level, mse = np.empty((h, w, 3)), np.empty((h, w), np.uint8), np.empty((h, w))
+        c = (d or Denoise()).to_c()
+        capi.check(capi.lib().rptb_buffer_denoise_cross(self.handle, C.byref(c), rgb.ctypes.data_as(capi.c_double_p), None,
+                                                        level.ctypes.data_as(capi.c_u8_p), mse.ctypes.data_as(capi.c_double_p)),
+                   "rptb_buffer_denoise_cross")
+        return rgb, level, mse
+
+    def cross_image(self, d: Optional[Denoise] = None) -> np.ndarray:
+        """denoise_cross()'s colour through Buffer::image's clamp, gamma and cast, as denoised_image(): (H, W, 3) uint8."""
+        out = np.empty((self.height, self.width, 3), np.uint8)
+        c = (d or Denoise()).to_c()
+        capi.check(capi.lib().rptb_buffer_denoise_cross(self.handle, C.byref(c), None, out.ctypes.data_as(capi.c_u8_p), None, None),
+                   "rptb_buffer_denoise_cross")
+        return out
+
     def reproject_from(self, src: "DeviceBuffer", params: Optional[Reproject] = None) -> int:
         """Carries `src`'s entries over a camera move into this buffer, which must hold features (Renderer.sample_features
         through its camera) and no entries; `src` must hold entries and features made through one camera.  Each pixel
@@ -1356,13 +1381,18 @@ class Renderer:
         self.last_stats = stats.as_dict() if want_stats else None
 
     def render(self, denoise: Optional[Denoise] = None, entries: int = 8, feature_samples: int = 16,
-               select: bool = False) -> np.ndarray:  # :96-100
+               select: bool = False, cross: bool = False) -> np.ndarray:  # :96-100
         """Renderer::render.  With `denoise`, num_samples are rendered as `entries` equal entries of a DeviceBuffer,
         `feature_samples` camera rays per pixel give it features, and the denoised bytes are returned.  With `select`
         as well, the buffer keeps halves and each pixel takes the number of passes (0 .. denoise.iterations) whose
-        estimated error is least (DeviceBuffer.selected_image)."""
+        estimated error is least (DeviceBuffer.selected_image).  With `cross` in place of `select`, the buffer keeps
+        halves and is cross-filtered with a smoothed selection map (DeviceBuffer.cross_image)."""
         if select and denoise is None:
             raise ValueError("select=True chooses each pixel's number of filter passes: it needs denoise (a Denoise)")
+        if cross and denoise is None:
+            raise ValueError("cross=True cross-filters the buffer's halves: it needs denoise (a Denoise)")
+        if cross and select:
+            raise ValueError("cross=True and select=True are two ways to choose the passes per pixel: pass one of them")
         if denoise is None:
             buffer = Buffer(self._width, self._height, self._filter, self._first_device())
             self.sample(self._num_samples, buffer)
@@ -1370,10 +1400,12 @@ class Renderer:
         if entries < 2 or self._num_samples % entries:
             # the entries are weighted equally: unequal ones would bias the mean
             raise ValueError(f"num_samples {self._num_samples} must be a multiple of entries {entries} (and entries >= 2)")
-        with self.device_buffer(halves=select) as buf:
+        with self.device_buffer(halves=select or cross) as buf:
             for _ in range(entries):
                 self.sample(self._num_samples // entries, buf, want_stats=False)
             self.sample_features(feature_samples, buf)
+            if cross:
+                return buf.cross_image(denoise)
             return buf.selected_image(denoise) if select else buf.denoised_image(denoise)
 
     def _check_frames(self, entries: int, adaptive: Optional[Adaptive], denoise: Optional[Denoise],

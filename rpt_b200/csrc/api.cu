@@ -24,6 +24,7 @@
 #include <vector>
 
 #include "../../include/rpt_b200.h"
+#include "cross.h"
 #include "delta.h"
 #include "denoise.h"
 #include "flatten.h"
@@ -86,6 +87,11 @@ cudaError_t launch_denoise_select(const double* sums, const double* m2, const do
                                   const double* depth, const double* albedo, uint32_t width, uint32_t height, const rptb_denoise& d,
                                   double* const col[3], double* const var[3], double* const u[3], double* m, double* best, double* best_M,
                                   uint8_t* level, cudaStream_t stream, uint32_t* launches);
+// the cross-filtered denoiser with a smoothed selection map: cross.cu
+cudaError_t launch_denoise_cross(const double* sums, const double* m2, const double* half, const uint32_t* counts, const double* nrm,
+                                 const double* depth, const double* albedo, uint32_t width, uint32_t height, const rptb_denoise& d,
+                                 const CrossSet set[3], double* m, double* best_M, double* out, uint8_t* level, cudaStream_t stream,
+                                 uint32_t* launches);
 // the reprojection and the least count: reproject.cu
 cudaError_t launch_reproject_part(const ReprojectView& dv, const ReprojectView& sv, const ReprojectSource& s, const FeaturePlanes& f,
                                   double rays, uint32_t index, uint32_t count, uint64_t nelem, const rptb_reproject& prm, double* sums,
@@ -714,6 +720,10 @@ struct rptb_buffer {
     // and the chosen level, width*height bytes
     double* sl = nullptr;
     uint8_t* sl_level = nullptr;
+    // the cross-filtered denoiser's (cross.cu), width*height*23: chain B's first ping-pong set (7), both chains' second
+    // (14), then m and M; and the chosen level, width*height bytes
+    double* cr = nullptr;
+    uint8_t* cr_level = nullptr;
     // allocated by the first guided adaptive call on a buffer of several parts: the mask and flags of parts[1..] (as many
     // tiles as the largest holds, *132 bytes) marked here before they go to the part, and their active pixel count
     uint8_t* guide_mask = nullptr;
@@ -2329,6 +2339,49 @@ int rptb_buffer_denoise_select(rptb_buffer* b, const rptb_denoise* d, double* ou
     }
     if (out_level) CU(cudaMemcpyAsync(out_level, b->sl_level, npix, cudaMemcpyDeviceToHost, q0.stream));
     if (out_mse) CU(cudaMemcpyAsync(out_mse, best_M, npix * sizeof(double), cudaMemcpyDeviceToHost, q0.stream));
+    CU(cudaStreamSynchronize(q0.stream));
+    return RPTB_OK;
+}
+
+int rptb_buffer_denoise_cross(rptb_buffer* b, const rptb_denoise* d, double* out_rgb, uint8_t* out_rgb8, uint8_t* out_level,
+                              double* out_mse) {
+    if (!b) return fail(RPTB_ERR_BAD_ARG, "null argument");
+    int rc = check_denoise(d);
+    if (rc != RPTB_OK) return rc;
+    if (d->iterations == 0) return fail(RPTB_ERR_BAD_ARG, "iterations 0: the cross filter needs at least one filter pass to blend");
+    if (b->shard) return refuse_shard("denoise_cross");
+    if (!b->halves) return fail(RPTB_ERR_BAD_ARG, "the buffer has no halves (rptb_buffer_create_halves)");
+    std::lock_guard<std::mutex> bl(b->lock);
+    BufferPart& q0 = b->parts[0];
+    DeviceGuard g(q0.device);
+    FilterPlanes f;
+    rc = check_denoise_entries(b);
+    if (rc == RPTB_OK) rc = filter_planes(b, true, &f);
+    if (rc == RPTB_OK) rc = check_denoise_counts(b);
+    if (rc != RPTB_OK) return rc;
+    const size_t npix = (size_t)b->width * b->height;
+    if (!b->cr) CU(own(b->mem, &b->cr, npix * 23 * sizeof(double)));
+    if (!b->cr_level) CU(own(b->mem, &b->cr_level, npix));
+    // level 0 in the filter's first colour and variance planes (A) and the estimate's first u plane and E (B); the first
+    // ping-pong set in the filter's second planes and the estimate's second u plane (chain A) and cr (chain B); the
+    // second set in cr; the blended colour goes to c' (f.out)
+    double* const c = b->cr;
+    const CrossSet set[3] = {{f.col[0], f.var[0], f.u[0], f.u[0], f.E, f.col[0]},
+                             {f.col[1], f.var[1], f.u[1], c, c + 3 * npix, c + 4 * npix},
+                             {c + 7 * npix, c + 10 * npix, c + 11 * npix, c + 14 * npix, c + 17 * npix, c + 18 * npix}};
+    double* const m = c + 21 * npix;
+    double* const M = c + 22 * npix;
+    uint32_t launches = 0;
+    CU(launch_denoise_cross(b->rows.sums, b->rows.m2, b->rows.half, b->rows.counts, f.a.normal, f.a.depth, f.a.albedo, b->width, b->height,
+                            *d, set, m, M, f.out, b->cr_level, q0.stream, &launches));
+    if (out_rgb) CU(cudaMemcpyAsync(out_rgb, f.out, npix * 3 * sizeof(double), cudaMemcpyDeviceToHost, q0.stream));
+    if (out_rgb8) {
+        // as rptb_buffer_denoise: the film resolve of one entry at radius 0
+        CU(launch_film_resolve(f.out, 1u, b->width, b->height, 0u, b->rgb8, q0.stream));
+        CU(cudaMemcpyAsync(out_rgb8, b->rgb8, npix * 3, cudaMemcpyDeviceToHost, q0.stream));
+    }
+    if (out_level) CU(cudaMemcpyAsync(out_level, b->cr_level, npix, cudaMemcpyDeviceToHost, q0.stream));
+    if (out_mse) CU(cudaMemcpyAsync(out_mse, M, npix * sizeof(double), cudaMemcpyDeviceToHost, q0.stream));
     CU(cudaStreamSynchronize(q0.stream));
     return RPTB_OK;
 }

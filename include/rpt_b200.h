@@ -479,8 +479,11 @@ int rptb_buffer_add_features(rptb_scene* scene, const rptb_camera* camera, const
 int rptb_buffer_features(rptb_buffer* buffer, double* normal, double* depth, double* albedo, double* hit_fraction);
 /* The filter's parameters (rpt_b200/csrc/denoise.h gives every formula and its order of operations).
  * iterations: a-trous passes with steps 1, 2, 4, ... (0 = the mean itself, <= 12); sigma_normal: the exponent of
- * the normal weight; sigma_depth, sigma_luminance: the depth and luminance tolerances; albedo_eps: added to the
- * albedo before the colour is divided by it.  Defaults 5, 128, 1, 4, 1e-3.                                   */
+ * the normal weight; sigma_depth, sigma_luminance: the depth and luminance tolerances (finite, >= 0); albedo_eps:
+ * added to the albedo before the colour is divided by it, finite and > 0 -- a pixel whose feature rays all hit a black
+ * material has albedo 0, and with albedo_eps 0 its colour would be divided by 0 and come back NaN.  A positive
+ * albedo_eps keeps every colour finite while mean / albedo_eps stays within the double range: a mean of 1e6 overflows
+ * below albedo_eps ~ 1e-303.  Defaults 5, 128, 1, 4, 1e-3.                                                     */
 typedef struct rptb_denoise {
     uint32_t iterations;
     uint32_t sigma_normal;
@@ -492,8 +495,8 @@ typedef struct rptb_denoise {
  * included): out_rgb (nullable) = width*height*3 linear doubles; out_rgb8 (nullable) = their bytes through the
  * film resolve of Buffer::image with one entry and radius 0 (clamp, gamma 1/2.2, truncation) -- the buffer's box
  * radius does not apply to a denoised image.  RPTB_ERR_BAD_ARG: no entries ("Pixel found with no samples"), a
- * pixel with fewer than 2 entries (no variance), no features, iterations > 12, or a sigma / albedo_eps that is
- * negative or not finite.                                                                                     */
+ * pixel with fewer than 2 entries (no variance), no features, iterations > 12, a sigma that is negative or not
+ * finite, or an albedo_eps that is not finite and > 0.                                                        */
 int rptb_buffer_denoise(rptb_buffer* buffer, const rptb_denoise* params, double* out_rgb /* nullable */,
                         uint8_t* out_rgb8 /* nullable */);
 /* Stands beside rptb_buffer_denoise: the variance v' of each pixel's denoised value, the filter's own estimate carried

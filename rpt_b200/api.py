@@ -886,8 +886,10 @@ class Denoise:
     part of SVGF, an edge-avoiding a-trous wavelet filter guided by the buffer's first-hit features (normal, depth,
     albedo) and by each pixel's variance of the mean.  `iterations` passes (0 = the mean itself, at most 12);
     sigma_normal is the exponent of the normal weight, sigma_depth and sigma_luminance the depth and luminance
-    tolerances, albedo_eps what is added to the albedo before the colour is divided by it (a black surface would
-    otherwise divide by zero).  rpt_b200/csrc/denoise.h gives every formula."""
+    tolerances, albedo_eps what is added to the albedo before the colour is divided by it.  albedo_eps must be finite and
+    > 0: a pixel whose feature rays all hit a black surface has albedo 0, and dividing by it would make that pixel NaN
+    even where its mean is 0.  A tiny albedo_eps still overflows once mean / albedo_eps leaves the double range (about
+    1e-303 for a mean of 1e6).  rpt_b200/csrc/denoise.h gives every formula."""
 
     def __init__(self, iterations: int = 5, sigma_normal: int = 128, sigma_depth: float = 1.0, sigma_luminance: float = 4.0,
                  albedo_eps: float = 1e-3):

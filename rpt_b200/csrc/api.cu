@@ -1961,10 +1961,13 @@ static int check_denoise(const rptb_denoise* d) {
     if (!d) return fail(RPTB_ERR_BAD_ARG, "null argument");
     if (d->iterations > kDenoiseMaxIterations)
         return fail(RPTB_ERR_BAD_ARG, "iterations %u > %u", d->iterations, kDenoiseMaxIterations);
-    if (!(std::isfinite(d->sigma_depth) && d->sigma_depth >= 0.0) || !(std::isfinite(d->sigma_luminance) && d->sigma_luminance >= 0.0) ||
-        !(std::isfinite(d->albedo_eps) && d->albedo_eps >= 0.0))
-        return fail(RPTB_ERR_BAD_ARG, "sigma_depth, sigma_luminance and albedo_eps must be finite and >= 0 (%g, %g, %g)", d->sigma_depth,
-                    d->sigma_luminance, d->albedo_eps);
+    if (!(std::isfinite(d->sigma_depth) && d->sigma_depth >= 0.0) || !(std::isfinite(d->sigma_luminance) && d->sigma_luminance >= 0.0))
+        return fail(RPTB_ERR_BAD_ARG, "sigma_depth and sigma_luminance must be finite and >= 0 (%g, %g)", d->sigma_depth,
+                    d->sigma_luminance);
+    // 0 would divide a black albedo's pixel by 0: its demodulated colour is NaN or inf, the filter keeps it, and the
+    // remodulation turns a raw mean of 0 into NaN
+    if (!(std::isfinite(d->albedo_eps) && d->albedo_eps > 0.0))
+        return fail(RPTB_ERR_BAD_ARG, "albedo_eps must be finite and > 0 (%g)", d->albedo_eps);
     return RPTB_OK;
 }
 

@@ -94,10 +94,19 @@ def test_denoise_struct_size_matches_header(tmp_path):
 def test_denoise_errors_before_any_device_work():
     L = capi.lib()
     bad = [capi.Denoise(13, 128, 1.0, 4.0, 1e-3), capi.Denoise(5, 128, -1.0, 4.0, 1e-3), capi.Denoise(5, 128, 1.0, float("nan"), 1e-3),
-           capi.Denoise(5, 128, 1.0, 4.0, float("inf")), capi.Denoise(5, 128, 1.0, 4.0, -1e-9)]
+           capi.Denoise(5, 128, 1.0, 4.0, float("inf")), capi.Denoise(5, 128, 1.0, 4.0, -1e-9), capi.Denoise(5, 128, 1.0, 4.0, 0.0),
+           capi.Denoise(5, 128, 1.0, 4.0, -0.0), capi.Denoise(5, 128, 1.0, 4.0, float("nan"))]
     for d in bad:  # checked before the buffer is looked at
         assert L.rptb_buffer_denoise(C.c_void_p(1), C.byref(d), None, None) == capi.ERR_BAD_ARG
         assert b"iterations" in L.rptb_last_error() or b"finite" in L.rptb_last_error()
+        assert L.rptb_buffer_denoise_variance(C.c_void_p(1), C.byref(d), _p(np.empty(1))) == capi.ERR_BAD_ARG
+    # albedo_eps 0 divides a black albedo's pixel by 0 (a NaN colour for a raw mean of 0): refused, as every value <= 0
+    for eps in (0.0, -0.0):
+        assert L.rptb_buffer_denoise(C.c_void_p(1), C.byref(capi.Denoise(5, 128, 1.0, 4.0, eps)), None, None) == capi.ERR_BAD_ARG
+        assert b"albedo_eps" in L.rptb_last_error() and b"> 0" in L.rptb_last_error()
+    tiny = capi.Denoise(5, 128, 1.0, 4.0, 5e-324)  # the least positive double passes the argument check: the buffer is next
+    assert L.rptb_buffer_denoise(None, C.byref(tiny), None, None) == capi.ERR_BAD_ARG
+    assert b"null" in L.rptb_last_error()
     good = api.Denoise().to_c()
     assert L.rptb_buffer_denoise(None, C.byref(good), None, None) == capi.ERR_BAD_ARG
     assert L.rptb_buffer_denoise(C.c_void_p(1), None, None, None) == capi.ERR_BAD_ARG

@@ -208,6 +208,9 @@ def test_errors_before_any_device_work():
     assert L.rptb_buffer_denoise_select(fake, C.byref(capi.Denoise(13, 128, 1.0, 4.0, 1e-3)), None, None, None, None) == capi.ERR_BAD_ARG
     assert L.rptb_buffer_denoise_select(fake, C.byref(capi.Denoise(0, 128, 1.0, 4.0, 1e-3)), None, None, None, None) == capi.ERR_BAD_ARG
     assert b"iterations" in L.rptb_last_error()
+    for eps in (0.0, -1e-9, float("inf")):  # albedo_eps must be finite and > 0
+        assert L.rptb_buffer_denoise_select(fake, C.byref(capi.Denoise(5, 128, 1.0, 4.0, eps)), None, None, None, None) == capi.ERR_BAD_ARG
+        assert b"albedo_eps" in L.rptb_last_error()
 
 
 def test_render_select_needs_denoise_before_device_work():

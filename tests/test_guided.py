@@ -188,7 +188,7 @@ def test_guided_errors_before_any_device_work():
         assert call(C.byref(c), C.byref(good_d), scene=fake) == capi.ERR_BAD_ARG
         assert b"min_entries" in L.rptb_last_error() or b"tolerances" in L.rptb_last_error()
     bad_d = [capi.Denoise(13, 128, 1.0, 4.0, 1e-3), capi.Denoise(5, 128, -1.0, 4.0, 1e-3), capi.Denoise(5, 128, 1.0, float("nan"), 1e-3),
-             capi.Denoise(5, 128, 1.0, 4.0, float("inf"))]
+             capi.Denoise(5, 128, 1.0, 4.0, float("inf")), capi.Denoise(5, 128, 1.0, 4.0, 0.0), capi.Denoise(0, 128, 1.0, 4.0, 0.0)]
     for d in bad_d:
         assert call(C.byref(good_c), C.byref(d), scene=fake) == capi.ERR_BAD_ARG
         assert b"iterations" in L.rptb_last_error() or b"finite" in L.rptb_last_error()

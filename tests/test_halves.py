@@ -226,6 +226,9 @@ def test_errors_before_any_device_work():
     assert L.rptb_buffer_denoise_error(fake, C.byref(good_d), None) == capi.ERR_BAD_ARG
     assert L.rptb_buffer_denoise_error(fake, C.byref(capi.Denoise(13, 128, 1.0, 4.0, 1e-3)), _p(np.empty(1))) == capi.ERR_BAD_ARG
     assert L.rptb_buffer_denoise_error(fake, C.byref(capi.Denoise(0, 128, 1.0, 4.0, 1e-3)), _p(np.empty(1))) == capi.ERR_BAD_ARG
+    for eps in (0.0, -1e-9, float("nan")):  # albedo_eps must be finite and > 0
+        assert L.rptb_buffer_denoise_error(fake, C.byref(capi.Denoise(5, 128, 1.0, 4.0, eps)), _p(np.empty(1))) == capi.ERR_BAD_ARG
+        assert b"albedo_eps" in L.rptb_last_error()
 
     def call(crit, guide, scene=fake, buf=fake):
         return L.rptb_sample_into_guided_error(scene, C.byref(cam), C.byref(p), crit, guide, buf, None, None)
@@ -236,6 +239,8 @@ def test_errors_before_any_device_work():
     assert call(C.byref(good_c), C.byref(capi.Denoise(13, 128, 1.0, 4.0, 1e-3))) == capi.ERR_BAD_ARG
     assert call(C.byref(good_c), C.byref(capi.Denoise(0, 128, 1.0, 4.0, 1e-3))) == capi.ERR_BAD_ARG
     assert b"iterations" in L.rptb_last_error()
+    assert call(C.byref(good_c), C.byref(capi.Denoise(4, 128, 1.0, 4.0, 0.0))) == capi.ERR_BAD_ARG
+    assert b"albedo_eps" in L.rptb_last_error()
     assert call(C.byref(good_c), C.byref(good_d), scene=None) == capi.ERR_BAD_ARG
     assert call(C.byref(good_c), C.byref(good_d), buf=None) == capi.ERR_BAD_ARG
 
